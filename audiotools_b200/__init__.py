@@ -1,4 +1,4 @@
-"""audiotools_b200 -- B200-native (sm_100a) engine for the AudioSignal transform/augment hot
+"""audiotools_b200 -- H100-native (sm_90a) engine for the AudioSignal transform/augment hot
 path of descriptinc/audiotools, behind the reference's own method surface::
 
     from audiotools_b200 import AudioSignal

@@ -1,5 +1,5 @@
-"""In-tree build of ``audiotools_b200/csrc/libb2a.so`` for sm_100a (nvcc cross-compiles
-without a GPU).  The .so is git-ignored but travels to the GPU box with the snapshot."""
+"""In-tree build of ``audiotools_b200/csrc/libb2a.so`` for sm_90a (H100; nvcc cross-compiles
+without a GPU).  The .so is a build product and is git-ignored."""
 import glob
 import hashlib
 import os
@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(CSRC, "libb2a.so")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",
 ]
 
@@ -36,6 +36,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
     moved into place atomically, so a concurrent importer never sees a half-written file."""
     import fcntl
 
+    if not force and _up_to_date(_deps()):  # a built tree may be read-only: take no lock unless there is work
+        return OUT
     with open(os.path.join(CSRC, ".build.lock"), "w") as lock:
         fcntl.flock(lock, fcntl.LOCK_EX)
         try:
@@ -44,14 +46,27 @@ def build(force: bool = False, verbose: bool = False) -> str:
             fcntl.flock(lock, fcntl.LOCK_UN)
 
 
+STAMP = os.path.join(CSRC, ".libb2a.stamp")
+
+
+def _deps():
+    return sorted(glob.glob(os.path.join(CSRC, "*.cu"))) + sorted(glob.glob(os.path.join(CSRC, "*.h"))) + sorted(
+        glob.glob(os.path.join(CSRC, "*.cuh"))) + [os.path.join(os.path.dirname(HERE), "include", "b2a.h")]
+
+
+def _up_to_date(deps):
+    if not (os.path.exists(OUT) and os.path.exists(STAMP)):
+        return False
+    with open(STAMP) as f:
+        return f.read() == _digest(deps)
+
+
 def _build_locked(force: bool, verbose: bool) -> str:
     srcs = sorted(glob.glob(os.path.join(CSRC, "*.cu")))
-    deps = srcs + sorted(glob.glob(os.path.join(CSRC, "*.h"))) + sorted(glob.glob(os.path.join(CSRC, "*.cuh"))) + [
-        os.path.join(os.path.dirname(HERE), "include", "b2a.h")]
-    stamp = os.path.join(CSRC, ".libb2a.stamp")
-    dig = _digest(deps)
-    if not force and os.path.exists(OUT) and os.path.exists(stamp) and open(stamp).read() == dig:
+    deps = _deps()
+    if not force and _up_to_date(deps):
         return OUT
+    dig = _digest(deps)
     nvcc = _nvcc()
     objs, procs = [], []
     for s in srcs:
@@ -66,10 +81,10 @@ def _build_locked(force: bool, verbose: bool) -> str:
         if p.returncode != 0:
             raise RuntimeError(f"nvcc failed on {s}:\n{out.decode()}")
     tmp = OUT + ".tmp.%d" % os.getpid()
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", tmp] + objs
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", tmp] + objs
     subprocess.check_call(cmd)
     os.replace(tmp, OUT)
-    with open(stamp, "w") as f:
+    with open(STAMP, "w") as f:
         f.write(dig)
     return OUT
 

@@ -1,6 +1,6 @@
 """ctypes binding of ``libb2a.so`` (C ABI declared in ``include/b2a.h``).
 
-The library is built in-tree by ``audiotools_b200/_build.py`` (nvcc, sm_100a) and
+The library is built in-tree by ``audiotools_b200/_build.py`` (nvcc, sm_90a) and
 lives next to the sources in ``audiotools_b200/csrc/``.  There is no fallback: if
 the shared object is missing or does not load, importing the engine raises.
 """
@@ -108,7 +108,7 @@ class B2ALibrary:
         if not os.path.exists(path):
             raise ImportError(
                 f"{path} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  audiotools_b200 has no CPU fallback.")
+                "(nvcc, sm_90a).  audiotools_b200 has no CPU fallback.")
         self.path = path
         self.cdll = ctypes.CDLL(path)
         for name, (res, args) in SIGNATURES.items():

@@ -1,5 +1,5 @@
 """``AudioSignal``: the batched waveform container of the hot path, with the reference's
-method surface (ref:audiotools/core/audio_signal.py) on top of the sm_100a engine.
+method surface (ref:audiotools/core/audio_signal.py) on top of the sm_90a engine.
 
 State: ``audio_data`` [B, C, T] float32, ``stft_data`` [B, C, F, N] complex64 (cache of the
 last ``stft()``), ``_loudness`` [B] (cache, cleared by the ``audio_data`` setter, kept by

@@ -1,6 +1,6 @@
 """``EffectMixin`` / ``ImpulseResponseMixin``: loudness normalisation, gain, mixing, mel-band
 equaliser, impulse-response convolution and pitch shift with the method surface of
-ref:audiotools/core/effects.py, on the sm_100a engine."""
+ref:audiotools/core/effects.py, on the sm_90a engine."""
 import numpy as np
 import torch
 

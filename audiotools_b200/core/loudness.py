@@ -1,4 +1,4 @@
-"""ITU-R BS.1770 integrated loudness on the sm_100a engine.
+"""ITU-R BS.1770 integrated loudness on the sm_90a engine.
 
 ``LoudnessMixin.loudness`` keeps the shell of ref:audiotools/core/loudness.py:268-320 (cache,
 zero-extension to 0.5 s, clamp to -70 LUFS); the measurement itself -- K-weighting IIR, 400 ms /

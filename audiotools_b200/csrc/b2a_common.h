@@ -1,7 +1,7 @@
-// b2a_common.h -- shared helpers of the sm_100a kernels behind include/b2a.h.
+// b2a_common.h -- shared helpers of the sm_90a kernels behind include/b2a.h.
 //
 // The same sources compile two ways:
-//   nvcc -gencode arch=compute_100a,code=sm_100a   -> libb2a.so (the product)
+//   nvcc -gencode arch=compute_90a,code=sm_90a     -> libb2a.so (the product)
 //   g++ -x c++ -DB2A_SIM -include tests/cusim/cusim.h -> test-only CPU execution of the
 //     identical kernel bodies (tests/cusim); inline PTX is compiled out there.
 #pragma once
@@ -16,7 +16,7 @@
 
 #include "../../include/b2a.h"
 
-#define B2A_NUM_SMS 148  // B200: 2 dies x 74 SMs
+#define B2A_NUM_SMS 132  // H100 SXM; only a fallback when the device attribute cannot be read
 
 // ---------------------------------------------------------------------------------------
 // error plumbing (thread-local message, integer codes; nothing throws)
@@ -74,50 +74,24 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
-// Packed FP32 pairs.  sm_100a issues fma / add / mul on a register PAIR as one instruction (SASS FFMA2 / FADD2 / FMUL2:
-// PTX fma.rn.f32x2 ...), each half rounded exactly like the scalar instruction, and its operands take free half swaps,
-// per-half negation and scalar broadcast (R4.F32x2.LO_HI.NP, R7.F32 ...).  The FFT kernels are bound by instruction
-// issue, not by the FP32 pipe (tests/probes/f32x2_probe.cu: FFMA2 = 2 pipe cycles, 1 issue slot), so a complex
-// butterfly written on (re, im) pairs costs half the issue slots with bit-identical results.  Under the CPU
-// simulator the same functions are two scalar operations.
+// Complex-pair helpers: fma / add / mul on (re, im) pairs, each half rounded exactly like the scalar instruction.
+// Hopper has no packed FP32 instruction, so each is two scalar operations (the compiler pairs them freely).
 __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-#ifdef B2A_SIM
   return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
-#else
-  unsigned long long A, B, C, R;
-  float2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(A) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(B) : "f"(b.x), "f"(b.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(C) : "f"(c.x), "f"(c.y));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(R) : "l"(A), "l"(B), "l"(C));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(R));
-  return r;
-#endif
 }
+// (the _rn intrinsics keep a separate multiply and add from being contracted into an fma)
 __device__ __forceinline__ float2 add2(float2 a, float2 b) {
 #ifdef B2A_SIM
   return make_float2(a.x + b.x, a.y + b.y);
 #else
-  unsigned long long A, B, R;
-  float2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(A) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(B) : "f"(b.x), "f"(b.y));
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(R) : "l"(A), "l"(B));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(R));
-  return r;
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 #endif
 }
 __device__ __forceinline__ float2 mul2(float2 a, float2 b) {
 #ifdef B2A_SIM
   return make_float2(a.x * b.x, a.y * b.y);
 #else
-  unsigned long long A, B, R;
-  float2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(A) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(B) : "f"(b.x), "f"(b.y));
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(R) : "l"(A), "l"(B));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(R));
-  return r;
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 #endif
 }
 __device__ __forceinline__ float2 neg2(float2 a) { return make_float2(-a.x, -a.y); }

@@ -1,12 +1,12 @@
-// dft.cu -- STFT / inverse STFT for window lengths the FFT kernels do not cover, as dense DFTs on sm_100a.
+// dft.cu -- STFT / inverse STFT for window lengths the FFT kernels do not cover, as dense DFTs on sm_90a.
 //
 // AudioSignal.stft accepts ANY window_length (ref:audiotools/core/audio_signal.py:1123-1212 -> torch.stft), e.g. the
 // 400 / 480 / 1200-sample (25 ms) windows of speech front-ends; spectral.cu covers the powers of two in [32, 4096].
 // Everything else runs here: the windowed real DFT of all frames of a batch is ONE real x complex matrix product
 //     X[f][k] = sum_n x[(f + drop_edge) hop + origin + n] . M[n][k],     M[n][k] = w[n] exp(-2 pi i nk / n_fft)
 // -- genuinely GEMM-shaped (64 k frames x 400 x 201 at 64 x 10 s @ 16 kHz / hop 160), computed in FP32 so that the
-// 1e-4 parity bar holds without operand splitting: a register-tiled product on packed FFMA2 (one instruction per
-// complex multiply-accumulate: the sample broadcast to both halves, the (re, im) of M as the pair).  The framing is
+// 1e-4 parity bar holds without operand splitting: a register-tiled product of complex multiply-accumulates on
+// (re, im) pairs (fma2: the sample broadcast to both halves, the (re, im) of M as the pair).  The framing is
 // implicit (A is read straight from the waveform with torch's two nested paddings resolved per sample, bit-exact in
 // the frame / sample indexing like spectral.cu), M is built once per (n_fft, window) by dft_matrix_kernel with the
 // angle reduced in integers (nk mod n_fft) and evaluated in float64.
@@ -16,7 +16,7 @@
 // the two power-of-two sizes istft.cu does not (32, 4096), which removes the last torch.istft delegation.
 //
 // Tile: 64 frames x 64 outputs per CTA (256 threads, 4 x 4 micro-tile), reduction in chunks of 16 through
-// double-buffered shared memory; 3 (forward) / 4 (inverse) 128-bit shared loads per 16 FFMA2.
+// double-buffered shared memory; 3 (forward) / 4 (inverse) 128-bit shared loads per 16 complex fma2.
 #include "b2a_common.h"
 #include "spectral_internal.h"
 

@@ -1,4 +1,4 @@
-// effects.cu -- the element-wise / per-row-peak effects of EffectMixin on sm_100a (SURVEY.md 8f.2): each is ONE pass
+// effects.cu -- the element-wise / per-row-peak effects of EffectMixin on sm_90a (SURVEY.md 8f.2): each is ONE pass
 // over the waveform (HBM-bound: read x once, write y once) instead of the reference's chain of tensor temporaries.
 //
 //   b2a_row_absmax_f32   peak[row] = max |x|                      ref:audiotools/core/effects.py:194 (ensure_max_of_audio),

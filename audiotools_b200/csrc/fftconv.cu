@@ -1,5 +1,5 @@
 // fftconv.cu -- per-row FIR / circular convolution of [rows, T] waveforms by uniformly partitioned
-// overlap-save FFT convolution on sm_100a.
+// overlap-save FFT convolution on sm_90a.
 //
 // One engine serves every "long filter" of the hot path:
 //   * DSPMixin.low_pass / high_pass   (ref:audiotools/core/dsp.py:153-215 -> julius.LowPassFilter:
@@ -225,8 +225,8 @@ struct Layout {
   int P, NB, NBX, chunk;
 };
 static inline size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
-// Spectra of one chunk of rows (X and, with several partitions, Y).  Sized to stay L2-resident between the forward
-// FFT, the spectral FIR and the inverse FFT (126 MB L2 on B200); B2A_FFTCONV_WS_MB overrides it for experiments.
+// Spectra of one chunk of rows (X and, with several partitions, Y): rows are processed in chunks whose spectra take at
+// most 256 MB, which bounds the workspace; B2A_FFTCONV_WS_MB overrides the budget for experiments.
 static size_t chunk_budget_mb() {
   static size_t mb = 0;
   if (mb == 0) {

@@ -1,4 +1,4 @@
-// fir.cu -- direct (time-domain) strided FIR for short filters on sm_100a.
+// fir.cu -- direct (time-domain) strided FIR for short filters on sm_90a.
 //
 //   out[row][m] = sum_{k<K} taps[f][k] * xv[row][m*stride + k - left[f]],   f = row / rows_per_filt, m < out_len
 //   (correlation form; xv extends x by zeros or edge replication).

@@ -1,4 +1,4 @@
-// istft.cu -- inverse STFT on sm_100a: spectra -> inverse real FFT -> window -> overlap-add -> / envelope.
+// istft.cu -- inverse STFT on sm_90a: spectra -> inverse real FFT -> window -> overlap-add -> / envelope.
 //
 // Replaces AudioSignal.istft (ref:audiotools/core/audio_signal.py:1214-1296), i.e. torch.istft(center=True,
 // onesided, window of n_fft samples):

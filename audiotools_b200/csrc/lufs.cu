@@ -1,4 +1,4 @@
-// lufs.cu -- integrated loudness (ITU-R BS.1770) for [B, C, T] float32 waveforms on sm_100a.
+// lufs.cu -- integrated loudness (ITU-R BS.1770) for [B, C, T] float32 waveforms on sm_90a.
 //
 // Replaces the device work of Meter.integrated_loudness with the exact-IIR semantics of
 // Meter.apply_filter_cpu (ref:audiotools/core/loudness.py:102-126) -- NOT the 512-tap FIR
@@ -467,7 +467,7 @@ kweight_energy_kernel(const float* __restrict__ x, int rows, int T, int Tp, int 
 // That bound is five orders of magnitude below the rounding noise the float32 recursion itself carries (each step
 // rounds at 6e-8 |y| and the feedback amplifies it by ~1/(1 - rho)), i.e. the results are those of the exact carry
 // to float32 rounding; the first warp-per-segment versions (decoupled look-back, then two passes with published
-// aggregates) were exact in the same sense and cost a serial ripple of ~35 us per wave resp. a second HBM read.
+// aggregates) were exact in the same sense and cost a serial ripple per wave resp. a second HBM read.
 // B2A_LUFS_V1=1 selects round 1's CTA-cooperative kernel with its exact look-back carry (rows whose dynamic range
 // exceeds 2^40 within 70 ms are the only inputs on which the two can differ beyond rounding).
 // =============================================================================================
@@ -478,8 +478,6 @@ constexpr int SEG = 32 * L2;        // samples per warp segment
 constexpr int CHS = L2 + 4;         // shared-memory words per lane chunk: 16 B aligned, conflict-free LDS.128
 constexpr int WPB = 12;             // warps per CTA (one CTA per SM: 12 x 17 KB of windows)
 constexpr int NBUF = 2;             // windows per warp: the next segment lands underneath the arithmetic
-// (measured, round 2: 24 warps with single windows and 4x-unrolled loops issue 70 % of the time but execute 7 % more
-//  instructions and take 116 us against 100 us for this configuration)
 constexpr int BUF = 32 * CHS;       // floats per window
 
 template <int NS>
@@ -736,21 +734,16 @@ kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp,
 }  // namespace v2
 
 // =============================================================================================
-// Chunk-pair variant (round 2, second half): the v2 algorithm with TWO lane chunks of the same row in the halves of
-// packed FP32 registers.  A segment is 64 chunks of L4 = 32 samples; lane l owns chunk l (half x) and chunk l + 32
-// (half y), so every arithmetic instruction of v2 -- the 34-tap end-state map, the affine scan, the DF-I recursion,
-// the energy accumulation -- is ONE FFMA2 / FMUL2 / FADD2 on a (chunk l, chunk l + 32) pair with the coefficient
-// broadcast (profiles/r02j: v2 executes 24.8 warp instructions per sample at 57 % issue utilisation -- instruction
-// issue and dependent-issue latency, not HBM, are the limit).  The window holds the two halves INTERLEAVED sample by
+// Chunk-pair variant: the v2 algorithm with TWO lane chunks of the same row in the halves of (x, y) register pairs.
+// A segment is 64 chunks of L4 = 32 samples; lane l owns chunk l (half x) and chunk l + 32 (half y), so every
+// arithmetic step of v2 -- the 34-tap end-state map, the affine scan, the DF-I recursion, the energy accumulation --
+// is one fma2 / mul2 / add2 (b2a_common.h) on a (chunk l, chunk l + 32) pair with the coefficient broadcast.  The
+// window holds the two halves INTERLEAVED sample by
 // sample (4-byte cp.async, coalesced 128 B per warp instruction, issued a few at a time inside the arithmetic of the
 // current segment), so one 128-bit shared load delivers two ready-made register pairs.  The scan runs on both halves
 // at once; half y is then re-based on half x's total:  c' = T_x + A^1024 carry,  carry' = T_y + A^1024 c'.
-// MEASURED (64 x 2ch x 10 s, profiles/r02n_prof_lufs_pair_*): 116 us against v2's 100 us -- 47.0 M warp instructions
-// (v2: 51.7 M; the 32-sample chunks double the per-segment scan / bookkeeping share and the boundary path runs on two
-// split points), issue-active 43 %, shared-memory data pipe 56 % busy.  A first packed version with two ROWS in the
-// halves (twice the window per warp, 6 warps per SM) took 124 us with 31.3 M instructions at 30 % issue-active.  Both
-// say the same as the packed K1: these kernels wait on dependent-issue and shared-memory latency, not on issue slots.
-// The kernel therefore stays OPT-IN (B2A_LUFS_PAIR=1); v2 is the default.
+// The 32-sample chunks double v2's per-segment scan / bookkeeping share and the boundary path runs on two split points;
+// the kernel is OPT-IN (B2A_LUFS_PAIR=1) and v2 is the default.
 // =============================================================================================
 namespace v4 {
 
@@ -1188,7 +1181,7 @@ static int use_v1() {
   return v;
 }
 
-static int use_pair() {  // B2A_LUFS_PAIR=1: the chunk-pair (packed FP32) kernel, measured slower than v2 (116 vs 100 us)
+static int use_pair() {  // B2A_LUFS_PAIR=1: the opt-in chunk-pair kernel (v4) instead of v2
   const char* e = getenv("B2A_LUFS_PAIR");  // read per call: the tests switch it
   return (e && e[0] == '1') ? 1 : 0;
 }

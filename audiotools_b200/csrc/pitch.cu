@@ -1,4 +1,4 @@
-// pitch.cu -- length-preserving pitch shift of [rows, T] waveforms on sm_100a.
+// pitch.cu -- length-preserving pitch shift of [rows, T] waveforms on sm_90a.
 //
 // Replaces EffectMixin.pitch_shift (ref:audiotools/core/effects.py:247-277), which moves the batch to the
 // CPU and runs libsox `pitch -q <cents>` + `rate` row by row.  SoX's pitch effect is WSOLA time-scale

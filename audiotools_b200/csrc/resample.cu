@@ -1,4 +1,4 @@
-// resample.cu -- windowed-sinc polyphase resampling of [rows, T] waveforms on sm_100a.
+// resample.cu -- windowed-sinc polyphase resampling of [rows, T] waveforms on sm_90a.
 //
 // Replaces julius.resample_frac as called by AudioSignal.resample (ref:audiotools/core/audio_signal.py:716-736):
 // with old/new the gcd-reduced rates and K = 2*width + old taps per output phase,

@@ -1,4 +1,4 @@
-// specmask.cu -- in-place operations on a complex STFT [rows, F, N] for the SpectralTransform family, sm_100a.
+// specmask.cu -- in-place operations on a complex STFT [rows, F, N] for the SpectralTransform family, sm_90a.
 //
 // The reference expresses every one of them through |X|, angle(X), masked_fill and mag * exp(1j * phase)
 // (ref:audiotools/core/dsp.py:217-370): about a dozen elementwise passes over the spectrogram each.  Here:

@@ -1,4 +1,4 @@
-// spectral.cu -- fused framing -> window -> real FFT -> |.| -> banded mel -> post-op on sm_100a.
+// spectral.cu -- fused framing -> window -> real FFT -> |.| -> banded mel -> post-op on sm_90a.
 //
 // Replaces the device work of AudioSignal.stft (ref:audiotools/core/audio_signal.py:1123-1212),
 // AudioSignal.mel_spectrogram (:1333-1369), the log-mel of ref:audiotools/metrics/spectral.py:187-190
@@ -602,7 +602,7 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
               const int4 sg = mseg[mm];  // (row offset, lo4, own n4, padded even n4: the same for the 4 filters of a step)
               const float4* w4 = mpk4 + sg.x;
               const float4* v4 = reinterpret_cast<const float4*>(xf + sg.y);
-              float2 a01 = make_float2(0.f, 0.f), a23 = a01;  // packed accumulator pairs (FFMA2)
+              float2 a01 = make_float2(0.f, 0.f), a23 = a01;  // packed accumulator pairs (fma on (re, im) pairs)
               for (int it = 0; it < sg.w; it += 2) {
                 const float4 wa = w4[it], wb = w4[it + 1], va = v4[it], vb = v4[it + 1];
                 a01 = fma2(make_float2(wa.x, wa.y), make_float2(va.x, va.y), a01);
@@ -794,7 +794,7 @@ extern "C" int b2a_spectral_f32(const float* x, int64_t rows, int64_t T, int n_f
   p.mel_packed_len = (mel_out && mel_packed_len > 0) ? mel_packed_len : 0;
   p.center = 1; p.origin = -(n_fft / 2) - pad; p.row_origin = nullptr;
   p.rows_per_gain = gain ? rows_per_gain : 1; p.post = post; p.post_eps = post_eps; p.post_power = post_power;
-  if (tc_supported(p)) return launch_tc(p, stream);  // tcgen05 path (spectral_tc.cu): n_fft 2048 log-mel / mel
+  if (tc_supported(p)) return launch_tc(p, stream);  // tensor-core path (spectral_tc.cu): n_fft 2048 log-mel / mel
   switch (n_fft) {
     case 32: return launch<4>(p, stream);
     case 64: return launch_warp<5>(p, stream);

@@ -53,7 +53,7 @@ __device__ __forceinline__ int src_index(int w, int T, int pad, int right_pad, i
   return (u >= 0 && u < T) ? u : -1;
 }
 
-// Tensor-core (tcgen05) variant of the fused kernel for n_fft = 2048 mel / log-mel launches (spectral_tc.cu).
+// Tensor-core (wgmma) variant of the fused kernel for n_fft = 2048 mel / log-mel launches (spectral_tc.cu).
 // tc_supported: the launch can take that path (geometry, shared memory, B2A_SPECTRAL_TC != 0).
 bool tc_supported(const Params& p);
 int launch_tc(Params& p, void* stream);

@@ -1,5 +1,6 @@
 // spectral_tc.cu -- the fused framing -> window -> real DFT -> |.| -> banded mel -> post-op kernel with the DFT's
-// first (radix-128) stage on the 5th-generation tensor cores (tcgen05.mma, accumulators in tensor memory).
+// first (radix-128) stage on the Hopper tensor cores (wgmma.mma_async, fp16 operands in shared memory, fp32
+// accumulators in registers).
 //
 // Same contract as spectral_warp_kernel<10,0> (spectral.cu): replaces torch.stft + abs + mel matmul + log of
 // ref:audiotools/core/audio_signal.py:1195-1202,1355,1367 and ref:audiotools/metrics/spectral.py:187-190 for
@@ -7,25 +8,24 @@
 //
 // Factorisation of the 2048-point real DFT, n = 16 a + b (a < 128, b < 16), k = c + 128 d (c < 128, d < 16):
 //   X[c + 128 d] = sum_b W16^{bd} . W2048^{bc} . Y_b[c],   Y_b[c] = sum_a xw[16 a + b] W128^{ac}
-// * Y_b[c] for c = 0..63 (the other half follows from xw being real) is ONE GEMM per group b on the tensor cores:
-//   D[128 x 16 frames] = F[128 x 128] . XW_b[128 x 16 frames], rows r = 2c + {0: cos, 1: -sin}; row 1 (Im Y[0] = 0)
-//   carries c = 64 instead ((-1)^a).  Operands are fp16 with an exact two-term split of BOTH sides
-//   (x = h1 + h2, F = F1 + F2; products h1 F1 + h2 F1 + h1 F2, fp32 accumulation in TMEM): measured relative error
-//   1.2e-7 (tests/probes/tc_probe.cu), i.e. fp32 quality; the samples of a tile are pre-scaled by a power of two so
-//   that max |x| lands in [512, 1024) and F by 64, which keeps both correction terms out of the fp16 subnormals.
-//   F lives in TENSOR MEMORY (A operand of tcgen05.mma "ts" form, written once per CTA with tcgen05.st); the
-//   windowed frames are the B operand in shared memory (canonical no-swizzle K-major layout).
-// * the second stage -- twiddle by W2048^{bc} and a 16-point complex DFT over b -- runs in registers, one thread per
-//   (frame, c): lanes 2c and 2c+1 hold Re / Im of the same Y and swap one of two frames with a shuffle so that each
-//   processes one whole frame.  The odd lane ends up with (Im, Re) = i conj(z): its DFT is i conj(X[-d]), whose
-//   MAGNITUDE is that of bin -d -- so it conjugates its twiddles and mirrors its store index instead of un-swapping.
-//   Outputs d >= 8 are the mirrored bins 2048 - k.  c = 0 / c = 64 (real inputs) pack the two frames of the pair
-//   into one complex DFT and separate them with the usual even/odd split.
+// * Y_b[c] for c = 0..63 (the other half follows from xw being real) is ONE GEMM on the tensor cores:
+//   D[128 rows x (16 groups x 16 frames)] = F[128 x 128] . XW[128 x 256].  Row R of F (16-row slab s = R / 16,
+//   j = R % 16) is c = 8 s + j % 8, Re for j < 8 (64 cos) and Im for j >= 8 (-64 sin); the Im row of c = 0 (Im Y[0] = 0)
+//   carries c = 64 instead (64 (-1)^a).  With this order the wgmma accumulator fragment of a thread holds Re AND Im of
+//   one c for two consecutive frames of every group b.  Operands are fp16 with an exact two-term split of BOTH sides
+//   (x = h1 + h2, F = F1 + F2; products h1 F1 + h2 F1 + h1 F2, fp32 accumulation): fp32 quality; the samples of a tile
+//   are pre-scaled by a power of two so that max |x| lands in [512, 1024) and F by 64, which keeps both correction
+//   terms out of the fp16 subnormals.  F1, F2 are the A operand (built once per CTA), the windowed frames the B
+//   operand, both in the canonical no-swizzle K-major shared-memory layout.
+// * Warpgroup g (of 4) computes rows 64 (g % 2) .. +64 for frames 8 (g / 2) .. +8 of all 16 groups; the groups are
+//   staged in two halves of 8 (one 64 KB operand buffer), 24 wgmma m64n64k16 per half and warpgroup.
+// * the second stage -- twiddle by W2048^{bc} and a 16-point complex DFT over b -- runs in registers straight from
+//   the accumulators, one thread per (c, frame).  Outputs d >= 8 are the mirrored bins 2048 - k.  c = 0 / c = 64
+//   (real inputs) pack the two frames of the thread into one complex DFT and separate them with the even/odd split.
 // * |X| of the 16 frames of a tile goes to shared memory (on top of the dead B operand), the banded FP32 mel
 //   projection + post-op + coalesced tile store are those of spectral.cu.
 //
-// Per 16-frame tile: 1 TMA-staged span (19 bulk copies, padded per 512 samples -> conflict-free strided reads),
-// 48 tcgen05.mma (M 128, N 128 = 8 groups x 16 frames, K 16).
+// Per 16-frame tile: 1 TMA-staged span (19 bulk copies, padded per 512 samples -> conflict-free strided reads).
 #ifndef B2A_SIM
 #include <cuda_fp16.h>
 #endif
@@ -52,18 +52,12 @@ constexpr int NWARP = THREADS / 32;
 constexpr int XBS = 1156;     // floats per |X| slot (1025 + band over-read slack; 1156 % 32 == 4: frames interleave)
 constexpr int BLK = 512;      // span padding granule (samples)
 constexpr int BLKP = BLK + 4; // padded granule
-constexpr int B_PART = NG * 4096;  // bytes of one fp16 part (hi or lo) of the B operand
-constexpr int TM_COLS = 512;
-constexpr int TM_D = 0, TM_F1 = 256, TM_F2 = 320;
+constexpr int B_PART = 8 * 4096;  // bytes of one fp16 part (hi or lo) of one half (8 groups) of the B operand
+constexpr int F_PART = 128 * 256;  // bytes of one fp16 part (F1 or F2) of the A operand
 
 __host__ __device__ __forceinline__ int pad_idx(int i) { return i + 4 * (i >> 9); }
 
-// ---------------------------------------------------------------------------------------------
-// tcgen05 / TMEM wrappers.  Under the CPU simulator (tests/cusim) tensor memory is a per-block array and the MMA
-// a plain loop over the same shared-memory bytes, so that the kernel's indexing is checked before any GPU time.
-// ---------------------------------------------------------------------------------------------
 #ifdef B2A_SIM
-static thread_local uint32_t g_tmem[128][TM_COLS];  // per simulator worker = per block in flight
 static inline float h2f(uint16_t h) { _Float16 v; memcpy(&v, &h, 2); return (float)v; }
 static inline uint16_t f2h(float f) { _Float16 v = (_Float16)f; uint16_t h; memcpy(&h, &v, 2); return h; }
 #endif
@@ -97,140 +91,73 @@ __device__ __forceinline__ void split2(float v0, float v1, uint32_t& hi, uint32_
   lo = pack_f16x2(v0 - f16lo_to_f32(hi), v1 - f16hi_to_f32(hi));
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot) {
-#ifdef B2A_SIM
-  *slot = 0;
-#else
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   (uint32_t)__cvta_generic_to_shared(slot)), "r"(TM_COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void tmem_free(uint32_t base) {
-#ifndef B2A_SIM
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"(TM_COLS) : "memory");
-#else
-  (void)base;
-#endif
-}
-__device__ __forceinline__ void tc_fence_before() {
-#ifndef B2A_SIM
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void tc_fence_after() {
-#ifndef B2A_SIM
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#endif
-}
 __device__ __forceinline__ void fence_async_smem() {
 #ifndef B2A_SIM
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 #endif
 }
-// 16 consecutive 32-bit columns of this thread's TMEM lane (lane = 32 * (warp % 4) + laneid)
-__device__ __forceinline__ void tmem_st16(uint32_t base, int lane_row, int col, const uint32_t (&w)[16]) {
-#ifdef B2A_SIM
-  (void)base;
-  for (int j = 0; j < 16; ++j) g_tmem[lane_row][col + j] = w[j];
-#else
-  const uint32_t addr = base + (uint32_t)col + ((uint32_t)(lane_row & ~31) << 16);
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(addr),
-               "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]), "r"(w[8]), "r"(w[9]),
-               "r"(w[10]), "r"(w[11]), "r"(w[12]), "r"(w[13]), "r"(w[14]), "r"(w[15]) : "memory");
-#endif
-}
-__device__ __forceinline__ void tmem_st_wait() {
-#ifndef B2A_SIM
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void tmem_ld2(uint32_t base, int lane_row, int col, float& v0, float& v1) {
-#ifdef B2A_SIM
-  (void)base;
-  memcpy(&v0, &g_tmem[lane_row][col], 4);
-  memcpy(&v1, &g_tmem[lane_row][col + 1], 4);
-#else
-  const uint32_t addr = base + (uint32_t)col + ((uint32_t)(lane_row & ~31) << 16);
-  uint32_t a, b;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0, %1}, [%2];" : "=r"(a), "=r"(b) : "r"(addr));
-  v0 = __uint_as_float(a);
-  v1 = __uint_as_float(b);
-#endif
-}
-// tcgen05.ld is asynchronous: the registers it names may only be read after tcgen05.wait::ld.  The values are
-// threaded THROUGH the wait ("+f") so that no consumer can be scheduled above it.
-__device__ __forceinline__ void tmem_ld_wait(float (&v)[16]) {
-#ifndef B2A_SIM
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7]), "+f"(v[8]),
-                 "+f"(v[9]), "+f"(v[10]), "+f"(v[11]), "+f"(v[12]), "+f"(v[13]), "+f"(v[14]), "+f"(v[15])
-               :
-               : "memory");
-#else
-  (void)v;
-#endif
-}
 
 #ifndef B2A_SIM
-__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version 1 (sm_100); layout type 0 = no swizzle
-  return d;
+// wgmma shared-memory matrix descriptor: canonical no-swizzle K-major layout of 8-row x 16-byte core matrices,
+// LBO = bytes between the two core matrices along K, SBO = bytes between consecutive 8-row groups
+__device__ __forceinline__ uint64_t smem_desc(const void* p, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  const uint32_t a = (uint32_t)__cvta_generic_to_shared(p);
+  return (uint64_t)((a >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);  // base offset 0, layout type 0 = no swizzle
 }
 #endif
-// D[128 x NN] (+)= A[128 x 16] (TMEM columns a_col .. a_col + 8, two halves per column) . B[NN x 16]^T (shared
-// memory, canonical no-swizzle K-major: 8-row x 16-byte core matrices, LBO = 128 B between the two K chunks, SBO =
-// 2048 B between consecutive 8-row groups); fp16 in, fp32 accumulate.  B row n' = 16 (group) + frame: the groups'
-// operand regions are 4096 B apart = two row groups, so ONE instruction with NN = 16 * (number of groups) multiplies
-// the same F slice with every group's frames and lands in D columns 16 b + n -- measured (tests/probes/
-// tc_latency_probe.cu): a tcgen05.mma costs ~60 cycles to issue whatever its N, so 48 wide instructions per tile
-// replace 384 narrow ones.  One thread issues it.
-template <int NN>
-__device__ __forceinline__ void mma_ts(uint32_t base, int d_col, int a_col, const unsigned char* b_smem, int accumulate) {
-#ifdef B2A_SIM
-  (void)base;
-  for (int m = 0; m < 128; ++m)
-    for (int n = 0; n < NN; ++n) {
-      float acc = 0.f;
-      if (accumulate) memcpy(&acc, &g_tmem[m][d_col + n], 4);
-      for (int k = 0; k < 16; ++k) {
-        const uint32_t aw = g_tmem[m][a_col + (k >> 1)];
-        const float a = h2f((uint16_t)((k & 1) ? (aw >> 16) : (aw & 0xffff)));
-        uint16_t bh;
-        memcpy(&bh, b_smem + (n >> 3) * 2048 + (k >> 3) * 128 + (n & 7) * 16 + (k & 7) * 2, 2);
-        acc += a * h2f(bh);
-      }
-      memcpy(&g_tmem[m][d_col + n], &acc, 4);
-    }
-#else
-  constexpr uint32_t idesc = (1u << 4) | ((uint32_t)(NN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);  // f16 x f16 -> f32
-  const uint64_t db = smem_desc((uint32_t)__cvta_generic_to_shared(b_smem), 128, 2048);
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-               "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}\n" ::"r"(base + (uint32_t)d_col),
-               "r"(base + (uint32_t)a_col), "l"(db), "r"(idesc), "r"((uint32_t)accumulate) : "memory");
-#endif
-}
-// one lane of a converged warp (warp-uniform control flow around it: the tcgen05.mma it guards is issued once, with
-// no per-lane serialisation loop)
-__device__ __forceinline__ bool elect_one() {
-#ifdef B2A_SIM
-  return (threadIdx.x & 31) == 0;
-#else
-  uint32_t pred;
-  asm volatile("{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(pred));
-  return pred != 0;
-#endif
-}
-__device__ __forceinline__ void mma_commit(unsigned long long* bar) {
+// Keeps the compiler from moving accesses of the accumulators across the wgmma fence / wait around them.
+__device__ __forceinline__ void fence_acc(float (&d)[32]) {
 #ifndef B2A_SIM
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   (uint32_t)__cvta_generic_to_shared(bar)) : "memory");
+#pragma unroll
+  for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
 #else
-  (void)bar;
+  (void)d;
+#endif
+}
+__device__ __forceinline__ void wgmma_fence() {
+#ifndef B2A_SIM
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#endif
+}
+__device__ __forceinline__ void wgmma_commit() {
+#ifndef B2A_SIM
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+#endif
+}
+__device__ __forceinline__ void wgmma_wait_all() {
+#ifndef B2A_SIM
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#endif
+}
+// d[64 x 64] (+)= A[64 x 16] . B[64 x 16]^T for the calling warpgroup, fp16 in, fp32 accumulate.  A: 64 rows of F at
+// a_smem (8-row groups 2048 B apart), B: 64 rows n = 8 i + r (group i, frame r) at b_smem (8-row groups 4096 B apart);
+// both K-major, the two 8-wide K chunks 128 B apart.  Thread (warp w of the group, lane l) receives
+// d[4 i + 2 h + e] = D[16 w + l / 4 + 8 h][8 i + 2 (l % 4) + e].  Under the CPU simulator each thread computes its
+// own fragment from the same shared-memory bytes.
+__device__ __forceinline__ void wgmma_64x64x16(float (&d)[32], const unsigned char* a_smem, const unsigned char* b_smem,
+                                               int accumulate) {
+#ifdef B2A_SIM
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  for (int i = 0; i < 8; ++i)
+    for (int h = 0; h < 2; ++h)
+      for (int e = 0; e < 2; ++e) {
+        const int m = 16 * w + (l >> 2) + 8 * h, n = 8 * i + 2 * (l & 3) + e;
+        float acc = accumulate ? d[4 * i + 2 * h + e] : 0.f;
+        for (int k = 0; k < 16; ++k) {
+          uint16_t ah, bh;
+          memcpy(&ah, a_smem + (m >> 3) * 2048 + (k >> 3) * 128 + (m & 7) * 16 + (k & 7) * 2, 2);
+          memcpy(&bh, b_smem + (n >> 3) * 4096 + (k >> 3) * 128 + (n & 7) * 16 + (k & 7) * 2, 2);
+          acc += h2f(ah) * h2f(bh);
+        }
+        d[4 * i + 2 * h + e] = acc;
+      }
+#else
+  const uint64_t da = smem_desc(a_smem, 128, 2048), db = smem_desc(b_smem, 128, 4096);
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "l"(da), "l"(db), "r"(accumulate));
 #endif
 }
 // arm `bar` with the byte count of the whole span, then one bulk copy per 512-sample granule (padded destination)
@@ -252,13 +179,14 @@ __device__ __forceinline__ void tma_span(float* sp, const float* src, int span, 
 }
 
 struct Smem {
-  int off_b, off_span, off_win, off_tw, off_mel, off_mpk, off_mseg, off_red, total;
+  int off_b, off_f, off_span, off_win, off_tw, off_mel, off_mpk, off_mseg, off_red, total;
 };
 static Smem smem_layout(const Params& p) {
   Smem s;
   auto al = [](int v) { return (v + 127) & ~127; };
   int o = 0;
-  s.off_b = o; o = al(o + 2 * B_PART);                       // B operand (hi, lo); later the |X| slots
+  s.off_b = o; o = al(o + max(2 * B_PART, FR * XBS * 4));   // B operand (hi, lo) of a half; later the |X| slots
+  s.off_f = o; o = al(o + 2 * F_PART);                       // A operand F1, F2
   const int nblk = (p.span + BLK - 1) / BLK;
   s.off_span = o; o = al(o + nblk * BLKP * 4);
   s.off_win = o; o = al(o + NFFT * 4);
@@ -280,6 +208,7 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
   const Params& p = kp.p;
   B2A_DYN_SMEM(smem);
   unsigned char* bop = smem + kp.s.off_b;
+  unsigned char* fop = smem + kp.s.off_f;
   float* xs = reinterpret_cast<float*>(smem + kp.s.off_b);  // |X| slots alias the B operand (dead after the MMAs)
   float* sp = reinterpret_cast<float*>(smem + kp.s.off_span);
   float* wsc = reinterpret_cast<float*>(smem + kp.s.off_win);
@@ -289,26 +218,18 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
   int4* mseg = reinterpret_cast<int4*>(smem + kp.s.off_mseg);
   float* red = reinterpret_cast<float*>(smem + kp.s.off_red);
 
-  __shared__ __align__(8) unsigned long long s_bar_tma, s_bar_mma;
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) unsigned long long s_bar_tma;
   __shared__ int s_clamp;
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int q = warp & 3;             // TMEM lane quarter this warp may access
-  const int row = 32 * q + lane;      // GEMM row = TMEM lane: r = 2c + ri
-  const int c = row >> 1, ri = row & 1;
+  const int rb = (warp >> 2) & 1, fh = warp >> 3;        // warpgroup: rows 64 rb .. +64, frames 8 fh .. +8
+  const int c = 32 * rb + 8 * (warp & 3) + (lane >> 2);  // DFT-128 bin of this thread's accumulator rows
+  const int f0 = 8 * fh + 2 * (lane & 3);                // ... and its two frames f0, f0 + 1
   const int hop = p.hop, F = NFFT / 2 + 1;
   const int total_tiles = p.rows * p.n_tiles;
 
-  if (tid == 0) {
-    mbar_init(&s_bar_tma, 1);
-    mbar_init(&s_bar_mma, 1);
-  }
-  if (warp == 0) tmem_alloc(&s_tmem);
-  tc_fence_before();
+  if (tid == 0) mbar_init(&s_bar_tma, 1);
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmb = s_tmem;
 
   // ---- first tile's span in flight while the tables are built
   int t = blockIdx.x;
@@ -329,32 +250,30 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
     return false;
   };
   if (t < total_tiles) by_tma = stage(t);
-  unsigned par_tma = 0, par_mma = 0;
+  unsigned par_tma = 0;
 
-  // ---- DFT-128 matrix rows into tensor memory: F[r][a] = 64 cos(2 pi a c / 128) (ri = 0), -64 sin(..) (ri = 1);
-  //      row 1 = 64 (-1)^a (the c = 64 component).  Warp (q, w/4) writes columns a in [32 (w/4), +32).
-  {
-    const int a0 = 32 * (warp >> 2);
-    uint32_t h[16], l[16];
+  // ---- DFT-128 matrix F (A operand, fp16 hi / lo parts): row R = (slab R / 16, j = R % 16) is bin cr = 8 slab + j % 8,
+  //      64 cos(2 pi a cr / 128) for j < 8, -64 sin(..) for j >= 8; the Im row of cr = 0 is 64 (-1)^a (bin 64)
+  for (int i = tid; i < 128 * 64; i += THREADS) {
+    const int R = i >> 6, a0 = 2 * (i & 63);
+    const int cr = 8 * (R >> 4) + (R & 7), im = (R >> 3) & 1;
+    float v[2];
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      float v[2];
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int a = a0 + 2 * j + e;
-        float sn, cs;
-        sincospif((float)((a * c) & 127) * (1.0f / 64.0f), &sn, &cs);
-        v[e] = 64.0f * (ri ? -sn : cs);
-        if (row == 1) v[e] = (a & 1) ? -64.0f : 64.0f;
-      }
-      split2(v[0], v[1], h[j], l[j]);
+    for (int e = 0; e < 2; ++e) {
+      const int a = a0 + e;
+      float sn, cs;
+      sincospif((float)((a * cr) & 127) * (1.0f / 64.0f), &sn, &cs);
+      v[e] = 64.0f * (im ? -sn : cs);
+      if (cr == 0 && im) v[e] = (a & 1) ? -64.0f : 64.0f;
     }
-    tmem_st16(tmb, row, TM_F1 + a0 / 2, h);
-    tmem_st16(tmb, row, TM_F2 + a0 / 2, l);
-    tmem_st_wait();
+    uint32_t h, l;
+    split2(v[0], v[1], h, l);
+    const int off = (R >> 3) * 2048 + (a0 >> 3) * 128 + (R & 7) * 16 + (a0 & 7) * 2;
+    *reinterpret_cast<uint32_t*>(fop + off) = h;
+    *reinterpret_cast<uint32_t*>(fop + F_PART + off) = l;
   }
-  // ---- second-stage twiddles W2048^{b c} (conjugated for the odd lane, which works on i conj(z));
-  //      row 1 (c = 64 packed pair): W2048^{64 b}, not conjugated
+  // ---- second-stage twiddles W2048^{b c} at [b][2 c]; [b][1] = W2048^{64 b} (the c = 64 packed pair).  (The odd
+  //      entries [b][2 c + 1] hold the conjugates and are not read.)
   for (int i = tid; i < NG * 128; i += THREADS) {
     const int b = i >> 7, r = i & 127;
     const int cc = (r == 1) ? 64 : (r >> 1);
@@ -395,9 +314,8 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
       }
     }
   }
-  tc_fence_before();
+  fence_async_smem();  // generic-proxy writes of F -> visible to the tensor core (async proxy)
   __syncthreads();
-  tc_fence_after();
 
 #pragma unroll 1
   for (; t < total_tiles; t += gridDim.x) {
@@ -435,12 +353,13 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
     }
     __syncthreads();
 
-    // ---- (3) + (4): windowed frames -> fp16 (hi, lo) B operand, in two halves of 8 groups; the MMAs of a half are
-    //      issued (warp 0, one elected lane) as soon as the half is in shared memory, so the tensor core works on groups
-    //      0-7 while the CUDA cores convert groups 8-15.  Unit u (64 per half) = (nh, ac, gq'): frames 8 nh + (lane & 7),
-    //      a in [8 ac, +8), groups b = 4 (2 half + gq') + e.  Sample of (n, a, b) = span[n hop + 16 a + b].
+    // ---- (3) + (4): windowed frames -> fp16 (hi, lo) B operand, in two halves of 8 groups (one operand buffer); each
+    //      warpgroup multiplies its 64 rows of F with its 8 frames of the half's groups: 3 products x 8 k-steps of
+    //      wgmma m64n64k16.  Unit u (64 per half) = (nh, ac, gq'): frames 8 nh + (lane & 7), a in [8 ac, +8),
+    //      groups b = 4 (2 half + gq') + e.  Sample of (n, a, b) = span[n hop + 16 a + b].
     const bool blk_aligned = (hop & (BLK - 1)) == 0;  // every frame starts on a padding granule
-#pragma unroll 1
+    float acc[2][32];  // [half][4 i + 2 im + e]: Re (im = 0) / Im (im = 1) of bin c, group 8 half + i, frame f0 + e
+#pragma unroll
     for (int half = 0; half < 2; ++half) {
       {
         const int u = 4 * warp + (lane >> 3);
@@ -474,7 +393,7 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
           split2(pr[0].z, pr[1].z, hw[2][jp], lw[2][jp]);
           split2(pr[0].w, pr[1].w, hw[3][jp], lw[3][jp]);
         }
-        unsigned char* dst = bop + (4 * gq) * 4096 + nh * 2048 + ac * 128 + (lane & 7) * 16;
+        unsigned char* dst = bop + (4 * (gq - 2 * half)) * 4096 + nh * 2048 + ac * 128 + (lane & 7) * 16;
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           *reinterpret_cast<int4*>(dst + e * 4096) = make_int4((int)hw[e][0], (int)hw[e][1], (int)hw[e][2], (int)hw[e][3]);
@@ -482,29 +401,26 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
         }
       }
       fence_async_smem();  // generic-proxy writes of the operand -> visible to the tensor core (async proxy)
-      tc_fence_before();
       __syncthreads();
-      if (warp == 0) {
-        // 3 products x 8 k-steps, each ONE instruction over the 8 groups of the half (N = 128 = 8 groups x 16 frames)
-        tc_fence_after();
-        if (elect_one()) {
-          const unsigned char* bh0 = bop + (8 * half) * 4096;
+      fence_acc(acc[half]);
+      wgmma_fence();
 #pragma unroll
-          for (int prod = 0; prod < 3; ++prod) {
-            const int a_col = (prod == 2) ? TM_F2 : TM_F1;
-            const unsigned char* bp = bh0 + (prod == 1 ? B_PART : 0);
+      for (int prod = 0; prod < 3; ++prod) {  // h1 F1, h2 F1, h1 F2
+        const unsigned char* ap = fop + (prod == 2 ? F_PART : 0) + rb * 16384;
+        const unsigned char* bp = bop + (prod == 1 ? B_PART : 0) + fh * 2048;
 #pragma unroll
-            for (int ks = 0; ks < 8; ++ks)
-              mma_ts<8 * FR>(tmb, TM_D + FR * 8 * half, a_col + 8 * ks, bp + ks * 256, (prod | ks) != 0);
-          }
-          if (half == 1) mma_commit(&s_bar_mma);
-        }
-        __syncwarp();
+        for (int ks = 0; ks < 8; ++ks) wgmma_64x64x16(acc[half], ap + ks * 256, bp + ks * 256, (prod | ks) != 0);
+      }
+      wgmma_commit();
+      if (half == 0) {  // the operand buffer is refilled with the second half: every warpgroup must be done reading it
+        wgmma_wait_all();
+        fence_acc(acc[0]);
+        __syncthreads();
       }
     }
-    // everybody but the issuing warp streams the scaled waveform out while the tensor core works
-    if (p.y_out && warp != 0) {  // y = g x for the samples this tile owns ([n0 hop, (n0 + FR) hop), the last tile up to T)
-      const int wt = tid - 32, WT = THREADS - 32;
+    // everybody streams the scaled waveform out while the tensor cores work on the second half
+    if (p.y_out) {  // y = g x for the samples this tile owns ([n0 hop, (n0 + FR) hop), the last tile up to T)
+      const int wt = tid, WT = THREADS;
       const int own_lo = n0 * hop;
       const int own_hi = (tile == p.n_tiles - 1) ? p.T : min(p.T, (n0 + FR) * hop);
       float* yr = p.y_out + (size_t)rw * (size_t)p.T;
@@ -529,60 +445,57 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
       const int tn = t + gridDim.x;
       by_tma = (tn < total_tiles) ? stage(tn) : false;
     }
-    mbar_wait(&s_bar_mma, par_mma);
-    par_mma ^= 1u;
-    tc_fence_after();
+    wgmma_wait_all();
+    fence_acc(acc[1]);
+    __syncthreads();  // the |X| slots below overwrite the operand buffer: every warpgroup's MMAs must be complete
 
-    // ---- (5) second stage in registers: thread (row, frame pair) -> one frame's 16 bins k = +-c + 128 d
-#pragma unroll 1
-    for (int pp = (warp >> 2); pp < FR / 2; pp += NWARP / 4) {
-      float v0[NG], v1[NG];
-#pragma unroll
-      for (int b = 0; b < NG; ++b) tmem_ld2(tmb, row, TM_D + FR * b + 2 * pp, v0[b], v1[b]);
-      tmem_ld_wait(v0);
-      tmem_ld_wait(v1);
-      float2 z[NG];
+    // ---- (5) second stage in registers: per thread two 16-point DFTs over b.  c != 0: one per frame (z = Re + i Im of
+    //      bin c), 16 bins k = +-c + 128 d each.  c = 0: the accumulator's Re rows hold Y[0], its Im rows Y[64], both
+    //      real: pass 0 packs Y[0] of frames f0 + i f1, pass 1 packs Y[64] likewise.  All 64 accumulators are moved
+    //      into z first so that they are dead before the DFTs.
+    {
+      const bool c0 = (c == 0);
+      float2 z[2][NG];
 #pragma unroll
       for (int b = 0; b < NG; ++b) {
-        const float mine = ri ? v1[b] : v0[b];
-        const float other = ri ? v0[b] : v1[b];
-        const float recv = __shfl_xor_sync(0xffffffffu, other, 1);
-        z[b] = make_float2(mine, recv);
-        if (c == 0) z[b].y = other;  // c = 0 / 64: both frames of the pair in one complex DFT (lanes 0, 1 of 4 warps)
+        const float* A = &acc[b >> 3][4 * (b & 7)];
+        z[0][b] = make_float2(A[0], c0 ? A[1] : A[2]);
+        z[1][b] = make_float2(c0 ? A[2] : A[1], A[3]);
       }
 #pragma unroll
-      for (int b = 1; b < NG; ++b) z[b] = cmul(z[b], tw[b * 128 + row]);
-      float2 o[NG];
-      DFT<NG, 1>::run(z, o);
-      const int f = 2 * pp + ri;  // even lane: frame 2 pp, odd lane: frame 2 pp + 1
-      if (c != 0) {
-        float* xf = xs + f * XBS;
-        float* P1 = ri ? xf - c : xf + c;  // d = 1..7  -> +-c + 128 d
-        float* P2 = ri ? xf + c : xf - c;  // d = 9..15 -> -+c + 128 (16 - d)
-        xf[c] = fast_sqrt(fmaf(o[0].x, o[0].x, o[0].y * o[0].y));
+      for (int pass = 0; pass < 2; ++pass) {
+        const int twi = c0 ? pass : 2 * c;
 #pragma unroll
-        for (int d = 1; d < 8; ++d) P1[128 * d] = fast_sqrt(fmaf(o[d].x, o[d].x, o[d].y * o[d].y));
-        xf[1024 - c] = fast_sqrt(fmaf(o[8].x, o[8].x, o[8].y * o[8].y));
+        for (int b = 1; b < NG; ++b) z[pass][b] = cmul(z[pass][b], tw[b * 128 + twi]);
+        float2 o[NG];
+        DFT<NG, 1>::run(z[pass], o);
+        if (!c0) {
+          float* xf = xs + (f0 + pass) * XBS;
+          float* P1 = xf + c;  // d = 1..7  -> c + 128 d
+          float* P2 = xf - c;  // d = 9..15 -> -c + 128 (16 - d)
+          xf[c] = fast_sqrt(fmaf(o[0].x, o[0].x, o[0].y * o[0].y));
 #pragma unroll
-        for (int d = 9; d < 16; ++d) P2[128 * (16 - d)] = fast_sqrt(fmaf(o[d].x, o[d].x, o[d].y * o[d].y));
-      } else {
-        // Y = DFT(u + i v) of two real-input problems u, v (the two frames of the pair):
-        //   row 0 (c = 0):  U[d] = (Y[d] + conj Y[16-d]) / 2, V[d] = (Y[d] - conj Y[16-d]) / 2i  -> bins 128 d, d = 0..8,
-        //                   u = frame 2 pp, v = frame 2 pp + 1
-        //   row 1 (c = 64): partner index 15 - d, bins 64 + 128 d, d = 0..7, u = frame 2 pp + 1 (mine), v = frame 2 pp
-        float* xu = xs + (2 * pp + ri) * XBS;
-        float* xv = xs + (2 * pp + 1 - ri) * XBS;
-        const int koff = ri ? 64 : 0;
+          for (int d = 1; d < 8; ++d) P1[128 * d] = fast_sqrt(fmaf(o[d].x, o[d].x, o[d].y * o[d].y));
+          xf[1024 - c] = fast_sqrt(fmaf(o[8].x, o[8].x, o[8].y * o[8].y));
 #pragma unroll
-        for (int d = 0; d < 9; ++d) {  // (static register indices: the partner is selected, not indexed)
-          const float2 yd = o[d];
-          const float2 ya = o[(16 - d) & 15], yb = o[(15 - d) & 15];
-          const float2 yn = ri ? yb : ya;
-          const float2 U = make_float2(0.5f * (yd.x + yn.x), 0.5f * (yd.y - yn.y));
-          const float2 V = make_float2(0.5f * (yd.y + yn.y), 0.5f * (yn.x - yd.x));
-          if (d < 8 || !ri) {
-            xu[koff + 128 * d] = sqrtf(fmaf(U.x, U.x, U.y * U.y));
-            xv[koff + 128 * d] = sqrtf(fmaf(V.x, V.x, V.y * V.y));
+          for (int d = 9; d < 16; ++d) P2[128 * (16 - d)] = fast_sqrt(fmaf(o[d].x, o[d].x, o[d].y * o[d].y));
+        } else {
+          // Y = DFT(u + i v) of two real-input problems u = frame f0, v = frame f0 + 1:
+          //   pass 0 (c = 0):  U[d] = (Y[d] + conj Y[16-d]) / 2, V[d] = (Y[d] - conj Y[16-d]) / 2i  -> bins 128 d, d = 0..8
+          //   pass 1 (c = 64): partner index 15 - d, bins 64 + 128 d, d = 0..7
+          float* xu = xs + f0 * XBS;
+          float* xv = xs + (f0 + 1) * XBS;
+          const int koff = pass ? 64 : 0;
+#pragma unroll
+          for (int d = 0; d < 9; ++d) {
+            const float2 yd = o[d];
+            const float2 yn = pass ? o[(15 - d) & 15] : o[(16 - d) & 15];
+            const float2 U = make_float2(0.5f * (yd.x + yn.x), 0.5f * (yd.y - yn.y));
+            const float2 V = make_float2(0.5f * (yd.y + yn.y), 0.5f * (yn.x - yd.x));
+            if (d < 8 || !pass) {
+              xu[koff + 128 * d] = sqrtf(fmaf(U.x, U.x, U.y * U.y));
+              xv[koff + 128 * d] = sqrtf(fmaf(V.x, V.x, V.y * V.y));
+            }
           }
         }
       }
@@ -591,7 +504,6 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
       float* xf = xs + tid * XBS;
       xf[1025] = 0.f; xf[1026] = 0.f; xf[1027] = 0.f;
     }
-    tc_fence_before();
     __syncthreads();
 
     // ---- (6) banded mel projection + post-op: warps 0-7 take frames 0-7, warps 8-15 frames 8-15
@@ -655,9 +567,6 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
     // (the barrier at the top of the next iteration orders these reads of melt / xs before they are rewritten)
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_free(tmb);
 }
 
 }  // namespace tc
@@ -665,9 +574,8 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
 static int g_tc_enabled = -1;
 static int tc_enabled() {
   if (g_tc_enabled < 0) {
-    // Opt-in: measured on B200 (profiles/README.md, round 2) this kernel runs 64 x 2ch x 10 s in 0.62 ms against 0.45 ms
-    // for the FP32 warp kernel, so the FP32 kernel stays the default; B2A_SPECTRAL_TC=1 or b2a_spectral_tc_enable(1)
-    // selects the tensor-core path.
+    // Opt-in: the FP32 warp kernel is the default; B2A_SPECTRAL_TC=1 or b2a_spectral_tc_enable(1) selects the
+    // tensor-core path.
     const char* e = getenv("B2A_SPECTRAL_TC");
     g_tc_enabled = (e && e[0] == '1') ? 1 : 0;
   }

@@ -33,8 +33,7 @@ tt = torch.tensor
 # Parameter tables.  A transform draws its parameters as PLAIN host values (python / numpy scalars, small arrays,
 # AudioSignals) -- the RNG calls and their order are the reference's, so a seed reproduces them -- and they only become
 # tensors once per batch: ``batch_instantiate`` stacks the B draws of every parameter into ONE tensor per key
-# (the reference builds B x n_keys zero-dim tensors and collates them: 250 ms per 512 items for a seven-transform
-# Compose on this host, 30 ms here), ``instantiate`` tensorises a single draw.  ``util.prepare_batch`` then uploads each
+# (the reference builds B x n_keys zero-dim tensors and collates them), ``instantiate`` tensorises a single draw.  ``util.prepare_batch`` then uploads each
 # table once and keeps its host mirror, so mask / cutoff / shift decisions never synchronise with the device.
 # ------------------------------------------------------------------------------------------
 def _tensorize(value):
@@ -76,8 +75,8 @@ class BaseTransform:
         # mask-aware: ``_transform(signal, ..., _bypass=[B] bool)`` runs on the WHOLE batch and leaves the flagged items
         # untouched inside the kernels (csrc: bypass flags / unit gains / zero shifts): no gather, no scatter
         # ... where that pays: `_bypass_pays = False` marks the FFT-convolution transforms, whose forward block FFTs run
-        # for every row of the launch -- measured on a prob-0.5 chain (128 x 10 s), flags on all five transforms 7.58 ms
-        # against 7.44 ms for the gather path, so those keep the gather (half the rows, two cheap copies)
+        # for every row of the launch, flagged or not, so those keep the gather (at prob 0.5: half the rows, two cheap
+        # copies)
         self._mask_aware = "_bypass" in params and getattr(self, "_bypass_pays", True)
         self.prob = prob
         self.name = self.__class__.__name__ if name is None else name

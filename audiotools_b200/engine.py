@@ -35,7 +35,7 @@ class Engine:
             raise TypeError(f"{name} must be a torch.Tensor")
         if self.require_cuda and not t.is_cuda:
             raise RuntimeError(
-                f"{name} is on {t.device}: audiotools_b200 runs on CUDA (sm_100a) only and has no CPU fallback")
+                f"{name} is on {t.device}: audiotools_b200 runs on CUDA (sm_90a) only and has no CPU fallback")
         if t.dtype != dtype:
             t = t.to(dtype)
         return t.contiguous()
@@ -87,7 +87,7 @@ class Engine:
         if not torch.is_complex(spec):
             raise TypeError("istft: spec must be complex")
         if self.require_cuda and not spec.is_cuda:
-            raise RuntimeError(f"stft_data is on {spec.device}: audiotools_b200 runs on CUDA (sm_100a) only and has "
+            raise RuntimeError(f"stft_data is on {spec.device}: audiotools_b200 runs on CUDA (sm_90a) only and has "
                                "no CPU fallback")
         if spec.dtype != torch.complex64:
             spec = spec.to(torch.complex64)
@@ -177,7 +177,7 @@ class Engine:
         if not torch.is_complex(spec):
             raise TypeError(f"{what}: spec must be complex")
         if self.require_cuda and not spec.is_cuda:
-            raise RuntimeError(f"stft_data is on {spec.device}: audiotools_b200 runs on CUDA (sm_100a) only and has "
+            raise RuntimeError(f"stft_data is on {spec.device}: audiotools_b200 runs on CUDA (sm_90a) only and has "
                                "no CPU fallback")
         if spec.dtype != torch.complex64 or not spec.is_contiguous():
             spec = spec.to(torch.complex64).contiguous()

@@ -2,7 +2,7 @@
 data-path collective.  The only exchange on the path is an all-gather of the per-item loudness vector
 (``[B/W] f32`` per rank -> ``[B]``), for whole-batch loudness statistics / logging; with NCCL it is issued
 on a side stream so that it overlaps the spectral kernel.  Works with any ``torch.distributed`` backend
-(NCCL over NVLink on the B200 box, gloo in the CPU tests)."""
+(NCCL over NVLink between the GPUs of one node, gloo in the CPU tests)."""
 from typing import Optional, Tuple
 
 import torch

@@ -2,7 +2,7 @@
 """bench.py -- the BASELINE.json metric: clips/sec for 10 s @ 44.1 kHz stereo clips through
 LUFS-normalise (-24) + log-mel (n_fft 2048, hop 512, 128 mels)  [BASELINE.json configs[1]].
 
-  python bench.py [--gpus N --steps K --warmup W]                    our arm (CUDA, one rank per GPU)
+  python bench.py [--gpus N --steps K --warmup W] [--dump-outputs DIR]   our arm (CUDA, one rank per GPU)
   python bench.py --impl reference [--gpus N --steps K --warmup W]    the reference's CPU path (oracle port)
 
 One "step" = one pass of the hot path over one batch of 64 clips per GPU (weak scaling): the
@@ -17,10 +17,12 @@ waveform [B,2,441000], log-mel [B,2,128,862], LUFS [B].
   cpu_baseline  the oracle (CPU port of the reference path) on this box's host cores, bounded sample
 Timing hygiene: >= 3 warm-ups plus a >= 1 s identical pre-roll, barrier, one untimed post-barrier step, then
 EXACTLY K steps between CUDA events on the launching stream (max over ranks); inputs rotate over 3 distinct
-226 MB batches (each > the 126 MB L2); nvidia-smi clocks are sampled from before the pre-roll to the end of a
+226 MB batches (each > the 50 MB L2 of an H100); nvidia-smi clocks are sampled from before the pre-roll to the end of a
 >= 2 s sustained loop of the same step (reported next to the K-step figure).  At N > 1 the per-item LUFS
 exchange (csrc/peer.cu) runs on its own stream, never waits for another rank inside a step, and is validated
 once, untimed, against an NCCL all_gather of the same vector.
+--dump-outputs DIR writes what the last timed step computed on rank 0 (see dump_outputs) as DIR/<name>.npy; the
+inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -99,7 +101,7 @@ def make_config(world, B, exchange_kind=None):
     return {"workload": WORKLOAD, "global_batch": world * B, "per_gpu_batch": B,
             "parallelism": f"batch-sharded x{world}, no data-path collective"
                            + (" (+ per-item LUFS exchange on a side stream)" if world > 1 else ""),
-            "l2": f"inputs rotate over 3 distinct {B * BYTES_X / 1e6:.0f} MB batches (> 126 MB L2)"}
+            "l2": f"inputs rotate over 3 distinct {B * BYTES_X / 1e6:.0f} MB batches (> 50 MB L2)"}
 
 
 def run_reference(args):
@@ -137,7 +139,7 @@ class ClockSampler:
     timed region, sustained loop) can be cut out afterwards."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -167,7 +169,7 @@ class ClockSampler:
                 pass
 
     def summary(self, t_lo=None, t_hi=None):
-        sm, mx, pw, reasons = [], [], [], set()
+        sm, mx, pw, lim, reasons = [], [], [], [], set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for ts, r in self.rows:
             if (t_lo is not None and ts < t_lo) or (t_hi is not None and ts > t_hi):
@@ -179,13 +181,33 @@ class ClockSampler:
                 for n, v in zip(names, r[3:7]):
                     if v.lower().startswith("active"):
                         reasons.add(n)
+                lim.append(float(r[7]))
             except Exception:
                 continue
         if not sm:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": [], "samples": 0}
         sm.sort()
         return {"sm_mhz": sm[len(sm) // 2], "sm_min_mhz": sm[0], "sm_max_mhz": max(mx), "power_w_max": max(pw),
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "power_limit_w": min(lim) if lim else None, "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def dump_outputs(out_dir, lu, out, seed=0, max_items=16, n_pos=65536):
+    """Write what one step of the timed path returned as float32 .npy files (about 22 MB at the default sizes):
+    ``lufs``, ``loud``, ``gain`` [B] in full; ``log_mel`` [k, C, n_mels, n_frames] and ``normalized`` [k, C, n_pos]
+    for k = min(B, max_items) items and n_pos time positions drawn with a fixed seed (the same for every build)."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    B, _, T_ = out["scaled"].shape
+    g = torch.Generator().manual_seed(seed)
+    items = torch.randperm(B, generator=g)[: min(B, max_items)].sort().values
+    pos = torch.randperm(T_, generator=g)[: min(T_, n_pos)].sort().values
+    arrays = {"lufs": lu["lufs"], "loud": lu["loud"], "gain": lu["gain"],
+              "log_mel": out["mel"][items.to(out["mel"].device)],
+              "normalized": out["scaled"][items.to(out["scaled"].device)][..., pos.to(out["scaled"].device)]}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.detach().float().cpu().numpy())
 
 
 # ----------------------------------------------------------------------------------------------
@@ -201,7 +223,7 @@ def run_ours(args):
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py (our arm) needs a B200: there is no CPU fallback. Use --impl reference "
+        raise SystemExit("bench.py (our arm) needs an H100: there is no CPU fallback. Use --impl reference "
                          "for the CPU path.")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
@@ -303,11 +325,20 @@ def run_ours(args):
         xl0 = exchange.launches if exchange is not None else 0
         t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         t0.record()
+        last = None
         for i in range(args.steps):
-            step(args.warmup + i, timed=True)
+            res = step(args.warmup + i, timed=True)
+            # only the final step's outputs are kept: holding every step's until the next one returns would make the
+            # first timed step allocate a second set of output buffers (cudaMalloc) inside the timed region
+            if i == args.steps - 1:
+                last = res
+            del res
         t1.record()
         torch.cuda.synchronize()
         w_timed1 = time.perf_counter()
+        if args.dump_outputs and rank == 0 and last is not None:
+            dump_outputs(args.dump_outputs, last[1], last[0])
+            w_timed1 = time.perf_counter()
         ms_rank = t0.elapsed_time(t1)
         launches = eng.launches - launches0 + (exchange.launches - xl0 if exchange is not None else 0)
         # sustained figure: the same step for >= args.sustain seconds (SM clocks settle under the power cap)
@@ -435,28 +466,14 @@ def run_ours(args):
         return 0
 
     # ---- roofline of the dominant kernel
-    peaks_path = os.path.join(REPO, "MEASURED_PEAKS.json")
-    if os.path.exists(peaks_path):
-        peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+    peak, peak_src = 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
     alg_bytes = B * (2 * BYTES_X + BYTES_MEL)  # read x + write y + write log-mel, each once
     achieved = alg_bytes / (spec_ms * 1e-3) / 1e9
     lufs_ms = ms / args.steps - spec_ms
     kernel_name = eng.spectral_kernel_name(N_FFT, HOP) if hasattr(eng, "spectral_kernel_name") else \
         "spectral_warp_kernel<10,0>"
-    # DRAM traffic of one launch: from the committed `ncu --set full` capture of THIS kernel at B = 64 (bench.py cannot
-    # run under ncu); null when no capture of the kernel in use has been committed
-    traffic, traffic_src = None, None
-    tpath = os.path.join(REPO, "profiles", "spectral_traffic.json")
-    if os.path.exists(tpath):
-        rec = json.load(open(tpath)).get(kernel_name.split("<")[0])
-        if rec:
-            traffic = (rec["dram_bytes_read"] + rec["dram_bytes_write"]) * B / rec["batch"]
-            traffic_src = rec["source"]
     roof = {"kernel": kernel_name + " (gain + STFT + |.| + mel + log10, fused)", "bound": "hbm",
             "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": traffic, "traffic_source": traffic_src,
             "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_bytes, "ms_per_launch": spec_ms,
             "rest_of_step_ms": lufs_ms,
             "rest_of_step": "lufs kernels (read x once: %.0f GB/s algorithmic)" % (B * BYTES_X / max(lufs_ms, 1e-9) / 1e6),
@@ -490,7 +507,7 @@ def run_ours(args):
                 "result_d2h": "log-mel + LUFS" + (" + normalised waveform" if full_d2h else ""),
                 "api": "AudioSignal(x).normalize(-24).mel_spectrogram(..., log=True)"},
         "sustained": sus_line, "exchange": exchange_line,
-        "gpu_launches": launches, "clocks": clk,
+        "gpu_launches": launches, "clocks": clk, "device": torch.cuda.get_device_name(dev),
     }
     print(json.dumps(line))
     if world > 1:
@@ -509,6 +526,8 @@ def main():
     ap.add_argument("--preroll", type=float, default=1.0, help="seconds of identical untimed steps before the barrier")
     ap.add_argument("--sustain", type=float, default=2.0, help="seconds of the sustained loop after the timed steps")
     ap.add_argument("--tc", action="store_true", help="use the opt-in tensor-core spectral kernel (A/B measurements)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's outputs (sampled) to DIR/<name>.npy")
     ap.add_argument("--e2e-features-only", action="store_true",
                     help="e2e leg copies back log-mel + LUFS only (not the normalised waveform)")
     args = ap.parse_args()

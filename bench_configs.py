@@ -95,10 +95,7 @@ def main():
     from oracle import signal_path as sp
 
     dev = f"cuda:{LOCAL}"
-    peak = 6576.1
-    pp = os.path.join(REPO, "MEASURED_PEAKS.json")
-    if os.path.exists(pp):
-        peak = float(json.load(open(pp))["hbm_gbs"])
+    peak = 3350.0  # GB/s: H100 SXM data sheet (HBM3), not measured
     torch.set_num_threads(os.cpu_count() or 1)
     only = set(args.only.split(","))
 
@@ -227,8 +224,8 @@ def main():
         macs = B * nfr * 400 * 201  # complex-real multiply-accumulates = FFMA2 instructions x 32 lanes
         emit({"config": "dense DFT 64 x 1ch x 10s@16k window 400 hop 160 (+ 80-mel log-mel, inverse)", "ms_stft": ms_stft,
               "ms_logmel": ms_mel, "ms_istft": ms_inv, "ms_torch_stft_cufft": ms_torch, "clips_per_s": B / ms_mel * 1e3,
-              "gflops_stft": 4 * macs / ms_stft / 1e6, "fp32_peak_gflops": 2 * 148 * 128 * 1.965,
-              "frac_of_fp32_peak": 4 * macs / ms_stft / 1e6 / (2 * 148 * 128 * 1.965)})
+              "gflops_stft": 4 * macs / ms_stft / 1e6, "fp32_peak_gflops": 67000.0,  # H100 SXM data sheet
+              "frac_of_fp32_peak": 4 * macs / ms_stft / 1e6 / 67000.0})
 
     if "gate" in only:  # SpectralGate (csrc/specmask.cu) at 64 x 2ch x 10 s: stft x2 + gate + istft
         from audiotools_b200.ml.layers import SpectralGate

@@ -1,4 +1,4 @@
-/* b2a.h -- C ABI of libb2a.so, the B200-native (sm_100a) engine behind the
+/* b2a.h -- C ABI of libb2a.so, the H100-native (sm_90a) engine behind the
  * AudioSignal transform/augment hot path of descriptinc/audiotools.
  *
  * The reference is 100% Python and has NO plugin/FFI interface (SURVEY.md §8b): the
@@ -95,7 +95,7 @@ int b2a_istft_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, 
 /* ---- STFT / inverse STFT for ANY window length (dense DFT, csrc/dft.cu) ---------------------------------------
  * AudioSignal.stft / istft accept any window_length (audiotools/core/audio_signal.py:1123-1212, 1214-1296 -> torch.stft /
  * torch.istft), e.g. 400 / 480 / 1200-sample speech windows; b2a_spectral_f32 / b2a_istft_f32 cover the powers of two.
- * Everything else is ONE real x complex matrix product over all frames of the batch (FP32, packed FFMA2):
+ * Everything else is ONE real x complex matrix product over all frames of the batch (FP32 FMA):
  *   b2a_dft_matrix_f32     builds the matrix of (n_fft, window) once: inverse 0 -> M[n][k] = w[n] exp(-2 pi i nk/n_fft)
  *                          for b2a_stft_dense_f32, inverse 1 -> c_k/n_fft . w[n] exp(-2 pi i nk/n_fft) (c = 1 for DC and
  *                          Nyquist, else 2) for b2a_istft_dense_f32; `matrix`: b2a_dft_matrix_floats(n_fft, inverse)
@@ -290,11 +290,10 @@ int b2a_alter_drr_f32(const float* ir, float* out, int64_t rows, int64_t T, int 
 int b2a_pack_rows_f32(const float* const* src_ptrs, const int64_t* src_len, const int64_t* src_stride,
                       const int64_t* src_off, int64_t n_items, int C, int64_t T_out, float* out, void* stream);
 
-/* 1 when b2a_spectral_f32 runs a launch of this geometry on the tensor-core kernel (csrc/spectral_tc.cu: tcgen05.mma,
- * accumulators in tensor memory): window_length 2048, hop <= 512, mel / log-mel output without the complex STFT, and
- * the path switched on (environment variable B2A_SPECTRAL_TC=1, or b2a_spectral_tc_enable(1)).  It is opt-in because
- * the FP32 warp kernel of spectral.cu is currently the faster of the two on B200; every other launch uses the FP32
- * kernels. */
+/* 1 when b2a_spectral_f32 runs a launch of this geometry on the tensor-core kernel (csrc/spectral_tc.cu: wgmma,
+ * accumulators in registers): window_length 2048, hop <= 512, mel / log-mel output without the complex STFT, and
+ * the path switched on (environment variable B2A_SPECTRAL_TC=1, or b2a_spectral_tc_enable(1)).  It is opt-in: the FP32 warp kernel of
+ * spectral.cu is the default; every other launch uses the FP32 kernels. */
 int b2a_spectral_uses_tensor_cores(int n_fft, int hop, int want_mel, int want_stft);
 /* Switch the tensor-core path on / off for this process (A/B measurements, parity tests of both kernels); returns the
  * previous setting. */

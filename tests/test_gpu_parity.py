@@ -1,5 +1,5 @@
-"""GPU parity tests proper (run with ``-m gpu`` on a B200): the product path -- AudioSignal API ->
-ctypes -> C ABI of libb2a.so -> sm_100a kernels -- against (a) the golden vectors produced by the
+"""GPU parity tests proper (run with ``-m gpu`` on an H100): the product path -- AudioSignal API ->
+ctypes -> C ABI of libb2a.so -> sm_90a kernels -- against (a) the golden vectors produced by the
 REAL reference, (b) the oracle on the same seeded inputs, and (c) at BASELINE.json's full sizes,
 size-independent properties (linearity, batch == per-item, normalise-then-measure, round trips).
 
@@ -647,7 +647,7 @@ def test_host_mirror_follows_in_place_writes(at):
 
 
 # ------------------------------------------------------------------------------------------
-# tensor-core spectral kernel (csrc/spectral_tc.cu): same launches on tcgen05 and on the FP32 warp kernel, both
+# tensor-core spectral kernel (csrc/spectral_tc.cu): same launches on the tensor cores (wgmma) and on the FP32 warp kernel, both
 # against the oracle, per cell (elementwise_ok) and globally; then BASELINE cfg2 at its full size
 # ------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("hop,T,n_mels,wtype", [(512, 60000, 128, "hann"), (256, 20000, 80, "hann"),

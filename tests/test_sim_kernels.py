@@ -676,7 +676,7 @@ def test_fftconv_random_geometries(eng):
 
 
 # ------------------------------------------------------------------------------------------
-# tensor-core spectral kernel (csrc/spectral_tc.cu) under the simulator: tensor memory and tcgen05.mma are emulated
+# tensor-core spectral kernel (csrc/spectral_tc.cu) under the simulator: each thread computes its wgmma accumulator fragment
 # (same operand bytes, same layouts), everything else is the shipped source
 # ------------------------------------------------------------------------------------------
 from tests.conftest import elementwise_ok as _elementwise_ok  # noqa: E402

@@ -1,5 +1,5 @@
 """The AudioSignal / transforms layer driven end to end ON THE CPU: the product's host code with the engine swapped for
-the CPU-simulated build of the same kernel sources (tests/cusim).  This is what the `-m gpu` tests check on a B200,
+the CPU-simulated build of the same kernel sources (tests/cusim).  This is what the `-m gpu` tests check on an H100,
 repeated here at the goldens' small sizes so that host-side regressions (argument plumbing, deferred gains, masks,
 match_stride trimming, per-item grouping) show up without a GPU."""
 import numpy as np
