@@ -458,8 +458,9 @@ class AudioSignal(EffectMixin, LoudnessMixin, ImpulseResponseMixin, DSPMixin):
     def istft(self, window_length: int = None, hop_length: int = None, window_type: str = None,
               match_stride: bool = None, length: int = None):
         """Inverse STFT of ``stft_data`` into ``audio_data`` (ref :1214-1296): one fused kernel (inverse real FFT,
-        window, overlap-add, envelope division; ``csrc/istft.cu``) for power-of-two windows in [64, 2048]; every other
-        window length runs as a dense inverse DFT + overlap-add fold (``csrc/dft.cu``).  No ``torch.istft`` on the path."""
+        window, overlap-add, envelope division; ``csrc/istft.cu``) for power-of-two windows in [64, 2048]; powers of two
+        in [4096, 32768] run a per-frame inverse FFT (``csrc/fft_large.cu``) and every other window length a dense
+        inverse DFT (``csrc/dft.cu``), both followed by the overlap-add fold of dft.cu.  No ``torch.istft`` on the path."""
         if self.stft_data is None:
             raise RuntimeError("Cannot do inverse STFT without self.stft_data!")
         window_length, hop_length, window_type, match_stride, _ = self._resolve_stft(

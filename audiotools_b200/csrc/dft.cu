@@ -18,6 +18,7 @@
 // Tile: 64 frames x 64 outputs per CTA (256 threads, 4 x 4 micro-tile), reduction in chunks of 16 through
 // double-buffered shared memory; 3 (forward) / 4 (inverse) 128-bit shared loads per 16 complex fma2.
 #include "b2a_common.h"
+#include "dft_internal.h"
 #include "spectral_internal.h"
 
 namespace b2a {
@@ -422,11 +423,16 @@ extern "C" int b2a_istft_dense_f32(const float* spec, int64_t rows, int64_t n_fr
   const int64_t gx = rows * p.tiles_f;
   B2A_REQUIRE(gx < (int64_t)2147483647, B2A_E_UNSUPPORTED, "istft_dense: too many tiles");
   B2A_LAUNCH(dft_inverse_kernel, dim3((unsigned)gx, (unsigned)(p.Np / BN)), dim3(256), 0, stream, p);
+  B2A_CUDA_OK(cudaGetLastError());
+  return launch_fold(p.frames, window, rows, (int)n_frames, n_fft, hop, pad_frames, start, out_len, out, stream);
+}
+
+int b2a::dft::launch_fold(const float* frames, const float* window, int64_t rows, int n_frames, int n_fft, int hop,
+                          int pad_frames, int64_t start, int64_t out_len, float* out, void* stream) {
   const long long expected = (long long)(n_frames + 2 * pad_frames - 1) * hop + n_fft;
   const long long want = (out_len + 255) / 256;
-  B2A_LAUNCH(fold_kernel, dim3((unsigned)(want < 2048 ? want : 2048), (unsigned)rows), dim3(256), 0, stream,
-             (const float*)p.frames, window, (int)n_frames, n_fft, hop, pad_frames, (long long)start, (long long)out_len,
-             expected, out);
+  B2A_LAUNCH(fold_kernel, dim3((unsigned)(want < 2048 ? want : 2048), (unsigned)rows), dim3(256), 0, stream, frames,
+             window, n_frames, n_fft, hop, pad_frames, (long long)start, (long long)out_len, expected, out);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }

@@ -94,9 +94,10 @@ class Engine:
         spec = spec.contiguous()
         B, C, F, N = spec.shape
         assert F == n_fft // 2 + 1, (F, n_fft)
-        dense = not self.lib.b2a_istft_supported(int(n_fft), int(hop))
+        large = bool(self.lib.b2a_stft_large_supported(int(n_fft), int(hop), 1))
+        dense = not large and not self.lib.b2a_istft_supported(int(n_fft), int(hop))
         if dense and not (self.lib.b2a_dft_supported(int(n_fft), int(hop)) and hop <= n_fft):
-            raise NotImplementedError(f"istft: n_fft={n_fft} hop={hop}")
+            raise NotImplementedError(f"istft: n_fft={n_fft} hop={hop}" + self._large_limit(int(n_fft)))
         window = self._prep(window, "window")
         assert window.numel() == n_fft
         start = n_fft // 2 + int(trim)
@@ -113,7 +114,16 @@ class Engine:
         if self._packed_cache[key][1] < 1e-11:
             raise RuntimeError("istft: window overlap add min: 1 (the window envelope vanishes inside the output)")
         out = torch.empty(B, C, int(length), dtype=torch.float32, device=spec.device)
-        if dense:  # any other window length (and 32 / 4096): transposed dense DFT + overlap-add fold (csrc/dft.cu)
+        if large:  # powers of two 4096 .. 32768: per-frame inverse FFT (csrc/fft_large.cu) + the overlap-add fold of dft.cu
+            nbytes = int(self.lib.b2a_istft_large_workspace_bytes(B * C, N, int(n_fft)))
+            ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=spec.device)
+            rc = self.lib.b2a_istft_large_f32(_dptr(torch.view_as_real(spec)), B * C, N, int(n_fft), int(hop), _dptr(window),
+                                              int(pad_frames), start, int(length), _dptr(out), _dptr(ws), nbytes,
+                                              self._stream(spec))
+            self.lib.check(rc)
+            self.launches += 2
+            return out
+        if dense:  # any other window length (and 32): transposed dense DFT + overlap-add fold (csrc/dft.cu)
             imat = self.dft_matrix(window, int(n_fft), inverse=True)
             nbytes = int(self.lib.b2a_istft_dense_workspace_bytes(B * C, N, int(n_fft)))
             ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=spec.device)
@@ -134,6 +144,14 @@ class Engine:
     def fft_window_length(n_fft: int) -> bool:
         """Window lengths the fused FFT kernel (csrc/spectral.cu) covers: powers of two in [32, 4096]."""
         return 32 <= n_fft <= 4096 and (n_fft & (n_fft - 1)) == 0
+
+    LARGE_FFT_MAX = 32768  # longest window of csrc/fft_large.cu (one frame per CTA in shared memory)
+
+    def _large_limit(self, n_fft: int) -> str:
+        """The error-message suffix for a power-of-two window beyond the large-window FFT kernels."""
+        if n_fft > self.LARGE_FFT_MAX and (n_fft & (n_fft - 1)) == 0:
+            return f": power-of-two windows run on the FFT kernels up to {self.LARGE_FFT_MAX}"
+        return ""
 
     def dft_matrix(self, window: torch.Tensor, n_fft: int, inverse: bool = False) -> torch.Tensor:
         """The windowed DFT matrix of csrc/dft.cu for (n_fft, window), built on the device once and cached (the cache
@@ -456,6 +474,9 @@ class Engine:
 
     def spectral_kernel_name(self, n_fft: int, hop: int, want_mel: bool = True, want_stft: bool = False) -> str:
         """Name of the kernel ``spectral`` launches for this geometry (bench.py / profiles label their numbers with it)."""
+        if self.lib.b2a_stft_large_supported(int(n_fft), int(hop), 0):
+            name = f"stft_large_kernel<{int(math.log2(n_fft))}>"
+            return name + " + mel_from_stft_kernel" if want_mel else name
         if self.lib.b2a_spectral_uses_tensor_cores(int(n_fft), int(hop), int(want_mel), int(want_stft)):
             return "spectral_tc_kernel"
         if n_fft in (32, 4096):
@@ -530,22 +551,30 @@ class Engine:
 
     def _spectral_dense(self, x, n_fft, hop, window, pad, right_pad, pad_mode, drop_edge, gain, want_scaled, mel_fb,
                         mel_lo, mel_hi, post, post_eps, post_power, want_stft, N):
-        """``spectral`` for window lengths outside the FFT kernel's set: gain pass (if any) -> dense DFT of all frames
-        (one matrix product, csrc/dft.cu) -> optional |X| -> banded mel -> post-op from the materialised STFT."""
+        """``spectral`` for window lengths outside the fused FFT kernel's set: gain pass (if any) -> the STFT of all
+        frames, materialised -> optional |X| -> banded mel -> post-op from it.  The STFT is a per-frame FFT for the
+        powers of two 8192 .. 32768 (csrc/fft_large.cu) and one dense DFT matrix product otherwise (csrc/dft.cu)."""
         B, C, T = x.shape
         F = n_fft // 2 + 1
-        if not self.lib.b2a_dft_supported(n_fft, hop):
-            raise NotImplementedError(f"stft: window_length {n_fft} hop {hop}: the dense DFT path covers 2..8192")
+        large = bool(self.lib.b2a_stft_large_supported(n_fft, hop, 0))
+        if not large and not self.lib.b2a_dft_supported(n_fft, hop):
+            raise NotImplementedError(f"stft: window_length {n_fft} hop {hop}: the dense DFT path covers 2..8192"
+                                      + self._large_limit(n_fft))
         scaled = None
         if gain is not None:
             gain = self._prep(gain.reshape(-1), "gain")
             assert gain.numel() == B
             x = scaled = self.gain(x, gain)
-        mat = self.dft_matrix(window, n_fft, inverse=False)
         stft = torch.empty(B, C, F, N, dtype=torch.complex64, device=x.device)
-        rc = self.lib.b2a_stft_dense_f32(_dptr(x), B * C, T, n_fft, hop, _dptr(mat), pad, right_pad,
-                                         _lib.PAD_MODES[pad_mode], drop_edge, _dptr(torch.view_as_real(stft)),
-                                         self._stream(x))
+        if large:
+            rc = self.lib.b2a_stft_large_f32(_dptr(x), B * C, T, n_fft, hop, _dptr(window), pad, right_pad,
+                                             _lib.PAD_MODES[pad_mode], drop_edge, _dptr(torch.view_as_real(stft)),
+                                             self._stream(x))
+        else:
+            mat = self.dft_matrix(window, n_fft, inverse=False)
+            rc = self.lib.b2a_stft_dense_f32(_dptr(x), B * C, T, n_fft, hop, _dptr(mat), pad, right_pad,
+                                             _lib.PAD_MODES[pad_mode], drop_edge, _dptr(torch.view_as_real(stft)),
+                                             self._stream(x))
         self.lib.check(rc)
         self.launches += 1
         mel = None

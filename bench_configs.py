@@ -3,7 +3,7 @@
 bench.py, which measures configs[1]).  One JSON line per config: device-resident throughput (CUDA events,
 >= 3 warm-ups, inputs larger than L2 or rotated), algorithmic bytes, and the CPU oracle on a bounded sample.
 
-    python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,gate,masked] [--no-cpu]
+    python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,largewin,gate,masked] [--no-cpu]
 
 Multi-GPU (BASELINE configs[3] = 512 items on 4 GPUs, configs[4] = 2048 items on 8 GPUs): one process per GPU,
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 4 --master-addr 127.0.0.1 --master-port 29511 \
@@ -226,6 +226,63 @@ def main():
               "ms_logmel": ms_mel, "ms_istft": ms_inv, "ms_torch_stft_cufft": ms_torch, "clips_per_s": B / ms_mel * 1e3,
               "gflops_stft": 4 * macs / ms_stft / 1e6, "fp32_peak_gflops": 67000.0,  # H100 SXM data sheet
               "frac_of_fp32_peak": 4 * macs / ms_stft / 1e6 / 67000.0})
+
+    if "largewin" in only:  # large power-of-two windows (csrc/fft_large.cu): the default 8192 window at 192 kHz
+        import ctypes
+        import subprocess
+
+        from audiotools_b200.engine import get_engine
+
+        B, C, T, sr = 64, 2, 1_920_000, 192000
+        g = torch.Generator().manual_seed(0)
+        x = torch.empty(B, C, T)
+        for i in range(0, B, 8):
+            x[i:i + 8] = 0.1 * torch.randn(8, C, T, generator=g)
+        x = x.to(dev)  # 983 MB > L2
+        sig = AudioSignal(x, sr)
+        eng = get_engine()
+        ms_stft = timed(lambda: sig.stft(), steps=5)  # default stft_params: 8192 / 2048, hann
+        ms_logmel = timed(lambda: sig.mel_spectrogram(n_mels=128, log=True), steps=5)
+        sig.stft()
+        X = sig.stft_data
+        ms_istft = timed(lambda: sig.istft(), steps=5)
+        ms_32k = timed(lambda: AudioSignal(x, sr).stft(window_length=32768, hop_length=8192), steps=3)
+        # the dense route these sizes took before (csrc/dft.cu): the engine's matrix + product, called directly
+        w = sig.get_window("hann", 8192, x.device)
+        mat = eng.dft_matrix(w, 8192)
+        dense_out = torch.empty_like(X)
+        xs = x.reshape(B * C, T)
+
+        def dense():
+            eng.lib.check(eng.lib.b2a_stft_dense_f32(ctypes.c_void_p(xs.data_ptr()), B * C, T, 8192, 2048,
+                                                     ctypes.c_void_p(mat.data_ptr()), 0, 0, 0, 0,
+                                                     ctypes.c_void_p(torch.view_as_real(dense_out).data_ptr()),
+                                                     ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
+
+        ms_dense = timed(dense, warmup=1, steps=2)
+        dense_rel = float((dense_out - X).abs().max() / X.abs().max())
+        del dense_out, mat
+        for k in [k for k in eng._packed_cache if k[0] == "dft"]:  # release the 270 MB matrix
+            del eng._packed_cache[k]
+        wt = torch.hann_window(8192, periodic=True, device=dev)
+        ms_torch = timed(lambda: torch.stft(xs, 8192, 2048, window=wt, center=True, return_complex=True), steps=5)
+        Xr = X.reshape(B * C, 4097, -1)
+        ms_torch_inv = timed(lambda: torch.istft(Xr, 8192, 2048, window=wt, center=True, length=T), steps=5)
+        alg = x.numel() * 4 + X.numel() * 8  # x read + STFT written
+        try:
+            plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(LOCAL)],
+                                  capture_output=True, text=True, timeout=30).stdout.strip()
+        except Exception:  # noqa: BLE001 (informational field)
+            plim = "unknown"
+        emit({"config": "largewin 64x2ch 10s@192k default window 8192 hop 2048 (stft, log-mel, istft; stft 32768)",
+              "kernel": eng.spectral_kernel_name(8192, 2048, want_mel=False, want_stft=True),
+              "ms_stft": ms_stft, "ms_logmel": ms_logmel, "ms_istft": ms_istft, "ms_stft_32768": ms_32k,
+              "ms_dense_dft_stft_8192": ms_dense, "dense_vs_fft_rel_err": dense_rel,
+              "ms_torch_stft_cufft": ms_torch, "ms_torch_istft_cufft": ms_torch_inv,
+              "clips_per_s_stft": B / ms_stft * 1e3, "alg_bytes_stft": alg, "achieved_GBps": alg / ms_stft / 1e6,
+              "frac_of_hbm_peak": alg / ms_stft / 1e6 / peak, "gpu": torch.cuda.get_device_name(LOCAL),
+              "power_limit": plim})
+        del X, Xr, sig, x
 
     if "gate" in only:  # SpectralGate (csrc/specmask.cu) at 64 x 2ch x 10 s: stft x2 + gate + istft
         from audiotools_b200.ml.layers import SpectralGate

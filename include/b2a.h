@@ -105,7 +105,8 @@ int b2a_istft_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, 
  *   b2a_mel_from_stft_f32  |X| -> banded mel -> post-op from a materialised STFT (AudioSignal.mel_spectrogram :1333-1369
  *                          for these window lengths; the FFT kernel fuses it)
  *   b2a_istft_dense_f32    the arguments of b2a_istft_f32 + the inverse matrix + ws (b2a_istft_dense_workspace_bytes:
- *                          the windowed frames) -> out; also serves n_fft 32 and 4096, which istft.cu does not. */
+ *                          the windowed frames) -> out; also accepts n_fft 32 and 4096, which istft.cu does not
+ *                          (the engine routes 4096 to b2a_istft_large_f32 below). */
 int b2a_dft_supported(int n_fft, int hop);
 size_t b2a_dft_matrix_floats(int n_fft, int inverse);
 int b2a_dft_matrix_f32(const float* window, int n_fft, int inverse, float* matrix, void* stream);
@@ -122,6 +123,25 @@ size_t b2a_istft_dense_workspace_bytes(int64_t rows, int64_t n_frames, int n_fft
 int b2a_istft_dense_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,
                         const float* imatrix, int pad_frames, int64_t start, int64_t out_len, float* out, void* ws,
                         size_t ws_bytes, void* stream);
+
+/* ---- STFT / inverse STFT for LARGE power-of-two windows (FFT, one CTA per frame, csrc/fft_large.cu) -----------
+ * The window lengths b2a_spectral_f32 / b2a_istft_f32 leave to the dense DFT or do not cover at all: the default
+ * window of AudioSignal.stft_params is 2^ceil(log2(0.032 sr)) = 4096 at 88.2 / 96 kHz and 8192 at 176.4 / 192 kHz;
+ * 16384 / 32768 serve fine frequency resolution.  FP32; no matrix, no table to build.
+ *   b2a_stft_large_supported   (n_fft, hop, inverse): inverse 0 -> n_fft in {8192, 16384, 32768}, hop >= 1;
+ *                              inverse 1 -> n_fft in {4096 .. 32768}, 1 <= hop <= n_fft.  65536 and above: 0.
+ *   b2a_stft_large_f32         the arguments of b2a_stft_dense_f32 with the window instead of the matrix (same framing /
+ *                              padding semantics, bit-exact frame indexing) -> stft_out [rows, n_fft/2+1, n_frames]
+ *   b2a_istft_large_f32        the arguments of b2a_istft_f32 + ws (b2a_istft_large_workspace_bytes: the windowed
+ *                              frames, 8-byte aligned) -> out; the overlap-add / envelope division is the fold of
+ *                              b2a_istft_dense_f32. */
+int b2a_stft_large_supported(int n_fft, int hop, int inverse);
+int b2a_stft_large_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window, int pad,
+                       int right_pad, int pad_mode, int drop_edge, float* stft_out, void* stream);
+size_t b2a_istft_large_workspace_bytes(int64_t rows, int64_t n_frames, int n_fft);
+int b2a_istft_large_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,
+                        int pad_frames, int64_t start, int64_t out_len, float* out, void* ws, size_t ws_bytes,
+                        void* stream);
 
 /* ---- SpecAugment band masks on a complex STFT, in place -------------------------------------------------
  * DSPMixin.mask_frequencies / mask_timesteps (audiotools/core/dsp.py:217-306): cells whose axis value v satisfies
