@@ -20,6 +20,7 @@ from collections import namedtuple
 import numpy as np
 import torch
 
+from . import grad as _grad
 from . import mel as _mel
 from . import util
 from .dsp import DSPMixin
@@ -340,6 +341,14 @@ class AudioSignal(EffectMixin, LoudnessMixin, ImpulseResponseMixin, DSPMixin):
         can ride along the next kernel that reads the samples (ref:audiotools/core/effects.py:219,237).
         Same observable state as the reference's assignment: the loudness cache is dropped."""
         gain = gain.reshape(-1).float()
+        if _grad.wants_grad(gain):
+            raise NotImplementedError("normalize / volume_change: db requires a gradient; gradients reach audio_data "
+                                      "only (the gain is a constant, as the reference's loudness is not differentiable)")
+        if _grad.wants_grad(self._audio_data) and _on_engine(self._audio_data):
+            # a signal that carries a gradient is scaled at once, by the differentiable gain op (after any gain that
+            # was deferred while grad mode was off)
+            self.audio_data = _grad.Gain.apply(self._materialized(), gain)
+            return
         if not self._audio_data.is_cuda:  # plain container arithmetic, like ``signal * x``
             self.audio_data = self._audio_data * gain.to(self._audio_data.device)[:, None, None]
             return
@@ -350,7 +359,10 @@ class AudioSignal(EffectMixin, LoudnessMixin, ImpulseResponseMixin, DSPMixin):
         """The sample tensor with any deferred gain applied."""
         if self._pending_gain is not None:
             g, self._pending_gain = self._pending_gain, None
-            self._audio_data = _engine().gain(self._audio_data, g)
+            if _grad.wants_grad(self._audio_data):
+                self._audio_data = _grad.Gain.apply(self._audio_data, g)
+            else:
+                self._audio_data = _engine().gain(self._audio_data, g)
         return self._audio_data
 
     samples = audio_data
@@ -432,10 +444,23 @@ class AudioSignal(EffectMixin, LoudnessMixin, ImpulseResponseMixin, DSPMixin):
                 sp.match_stride if match_stride is None else match_stride,
                 sp.padding_type if padding_type is None else padding_type)
 
-    def _spectral(self, stft_args, **engine_kwargs):
+    def _spectral(self, stft_args, method="stft", **engine_kwargs):
         window_length, hop_length, window_type, match_stride, padding_type = self._resolve_stft(*stft_args)
         window = self.get_window(window_type, window_length, self._audio_data.device)
         right_pad, pad = self.compute_stft_padding(window_length, hop_length, match_stride)
+        if _grad.wants_grad(self._audio_data):
+            fb = engine_kwargs.get("mel_fb")
+            _grad.check_supported(method, window_length, hop_length, self.batch_size * self.num_channels,
+                                  0 if fb is None else fb.shape[0])
+            mel = None
+            if engine_kwargs.get("mel_fb") is not None:
+                mel = (engine_kwargs["mel_fb"], engine_kwargs["mel_lo"], engine_kwargs["mel_hi"],
+                       engine_kwargs.get("post", 0), engine_kwargs.get("post_eps", 0.0),
+                       engine_kwargs.get("post_power", 1.0))
+            x = self._materialized()  # a gain deferred while grad mode was off is applied first, differentiably
+            stft, mel_out = _grad.Spectral.apply(x, window_length, hop_length, window, pad, right_pad, padding_type,
+                                                 2 if match_stride else 0, mel, engine_kwargs.get("want_stft", True))
+            return {"stft": stft, "mel": mel_out, "scaled": None}
         gain = self._pending_gain
         if gain is not None and (pad or right_pad or match_stride):
             gain = None
@@ -470,6 +495,12 @@ class AudioSignal(EffectMixin, LoudnessMixin, ImpulseResponseMixin, DSPMixin):
         if length is None:
             length = self.original_signal_length + 2 * pad + right_pad
         eng = _engine()  # (the engine refuses CPU tensors)
+        if _grad.wants_grad(self.stft_data):
+            _grad.check_supported("istft", window_length, hop_length, self.stft_data.shape[0] * self.stft_data.shape[1])
+            pad_frames, trim, out_len = (2, pad, length - 2 * pad - right_pad) if match_stride else (0, 0, length)
+            self.audio_data = _grad.ISTFT.apply(self.stft_data, window_length, hop_length, window, out_len, pad_frames,
+                                                trim)
+            return self
         if match_stride:
             # the reference pads 2 zero frames on either side, inverts to `length`, then keeps
             # [pad : length - (pad + right_pad)] (:1276-1292)
@@ -505,7 +536,7 @@ class AudioSignal(EffectMixin, LoudnessMixin, ImpulseResponseMixin, DSPMixin):
         fb, lo, hi = self._mel_tables(self.sample_rate, n_fft, n_mels, mel_fmin, mel_fmax, self._audio_data.device)
         from .. import _lib
 
-        out = self._spectral(args, want_stft=False, mel_fb=fb, mel_lo=lo, mel_hi=hi,
+        out = self._spectral(args, method="mel_spectrogram", want_stft=False, mel_fb=fb, mel_lo=lo, mel_hi=hi,
                              post=_lib.POST_LOG10 if log else _lib.POST_NONE, post_eps=clamp_eps, post_power=pow)
         return out["mel"]
 
@@ -533,9 +564,11 @@ class AudioSignal(EffectMixin, LoudnessMixin, ImpulseResponseMixin, DSPMixin):
         fb, lo, hi = self._mel_tables(self.sample_rate, n_fft, n_mels, mel_fmin, mel_fmax, self._audio_data.device)
         from .. import _lib
 
-        logmel = self._spectral(args, want_stft=False, mel_fb=fb, mel_lo=lo, mel_hi=hi, post=_lib.POST_LN,
-                                post_eps=log_offset)["mel"]
+        logmel = self._spectral(args, method="mfcc", want_stft=False, mel_fb=fb, mel_lo=lo, mel_hi=hi,
+                                post=_lib.POST_LN, post_eps=log_offset)["mel"]
         dct = self.get_dct(n_mfcc, n_mels, "ortho", self.device)
+        if _grad.wants_grad(logmel):
+            return _grad.MelDCT.apply(logmel, dct)
         return _engine().mel_dct(logmel, dct)
 
     @property

@@ -102,7 +102,8 @@ class EffectMixin:
             padded = T
             if self.signal_duration < 0.5:
                 padded = T + int((0.5 - self.signal_duration) * self.sample_rate)
-            out = _engine().lufs(self._audio_data, self.sample_rate, padded_length=padded, target_db=db)
+            # the gain is a constant: gradients reach audio_data through the gain op, not the loudness
+            out = _engine().lufs(self._audio_data.detach(), self.sample_rate, padded_length=padded, target_db=db)
             gain = out["gain"]
             measured = out["loud"]
         else:

@@ -63,6 +63,8 @@ class LoudnessMixin:
         if self.signal_duration < 0.5:  # zero-extend to 0.5 s (ref :302-305); no copy: the kernel reads zeros
             padded = T + int((0.5 - self.signal_duration) * self.sample_rate)
         kweighting.design(float(self.sample_rate), filter_class)
-        out = _engine().lufs(self._materialized(), self.sample_rate, filter_class, block_size, padded_length=padded)
+        # detached: the loudness is not differentiable (nor is the reference's, ref:tests/core/test_grad.py:70)
+        out = _engine().lufs(self._materialized().detach(), self.sample_rate, filter_class, block_size,
+                             padded_length=padded)
         self._loudness = out["loud"]
         return self._loudness.to(self.device)

@@ -19,6 +19,7 @@
 // double-buffered shared memory; 3 (forward) / 4 (inverse) 128-bit shared loads per 16 complex fma2.
 #include "b2a_common.h"
 #include "dft_internal.h"
+#include "grad_internal.h"
 #include "spectral_internal.h"
 
 namespace b2a {
@@ -35,6 +36,7 @@ __host__ __device__ inline int round_up(int v, int m) { return (v + m - 1) / m *
 // matrices.  forward: Mt[n][k] (k fastest, [Np][Fp]) = w[n] (cos, -sin)(2 pi nk / N), zero padded.
 //            inverse: Mi[k][n] (n fastest, [Fq][Np]) = c_k / N . w[n] (cos, -sin)(2 pi nk / N), c = 1 for k = 0 and
 //            k = N/2 (N even), else 2 (the Hermitian half folded in); y[n] = sum_k Xr Mi.x + Xi Mi.y.
+//            adjoint (kind 2): the inverse layout with weight 1 on every bin -- the STFT's adjoint (gradient wrt x).
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void unit(int n, int k, int N, double* cs, double* sn) {
   const long long r = ((long long)n * (long long)k) % (long long)N;
@@ -58,7 +60,7 @@ __global__ void __launch_bounds__(256) dft_matrix_kernel(const float* __restrict
       double cs, sn;
       unit(n, k, N, &cs, &sn);
       double s = (double)window[n];
-      if (inverse) s *= ((k == 0 || 2 * k == N) ? 1.0 : 2.0) / (double)N;
+      if (inverse == 1) s *= ((k == 0 || 2 * k == N) ? 1.0 : 2.0) / (double)N;
       v = make_float2((float)(s * cs), (float)(-s * sn));
     }
     M[i] = v;
@@ -73,6 +75,7 @@ struct FwdParams {
   const float2* Mt;
   float2* out;
   int rows, T, n_fft, hop, pad, right_pad, pad_mode, drop_edge, n_frames, F, Np, Fp, tiles_f;
+  int origin, center;  // frame f starts at x-coordinate (f + drop_edge) hop + origin; center: src_index's framing flag
 };
 
 __global__ void __launch_bounds__(256) dft_forward_kernel(FwdParams p) {
@@ -82,7 +85,7 @@ __global__ void __launch_bounds__(256) dft_forward_kernel(FwdParams p) {
   const int row = blockIdx.x / p.tiles_f, f0 = (blockIdx.x - row * p.tiles_f) * BM;
   const int k0 = blockIdx.y * BN;
   const float* xr = p.x + (size_t)row * (size_t)p.T;
-  const int origin = -(p.n_fft / 2) - p.pad;
+  const int origin = p.origin;
   // interior tile: every sample the tile touches is inside [0, T) -> no index resolution
   const long long lo = (long long)(f0 + p.drop_edge) * p.hop + origin;
   const long long hi = (long long)(min(f0 + BM, p.n_frames) - 1 + p.drop_edge) * p.hop + origin + p.n_fft;
@@ -102,7 +105,7 @@ __global__ void __launch_bounds__(256) dft_forward_kernel(FwdParams p) {
         if (n < p.n_fft) v = __ldg(xr + (size_t)((long long)(f0 + ff + p.drop_edge) * p.hop + origin + n));
       } else if (n < p.n_fft && f0 + ff < p.n_frames) {
         const long long w = (long long)(f0 + ff + p.drop_edge) * p.hop + origin + n;
-        const int u = spectral::src_index((int)w, p.T, p.pad, p.right_pad, p.pad_mode, 1);
+        const int u = spectral::src_index((int)w, p.T, p.pad, p.right_pad, p.pad_mode, p.center);
         if (u >= 0) v = __ldg(xr + u);
       }
       ra[j] = v;
@@ -303,7 +306,8 @@ __global__ void __launch_bounds__(256) dft_inverse_kernel(InvParams p) {
 // overlap-add (gather) + window envelope: out[row][i] = y[start + i] / env[start + i] for start + i < expected, else 0
 __global__ void __launch_bounds__(256) fold_kernel(const float* __restrict__ frames, const float* __restrict__ window,
                                                    int n_frames, int n_fft, int hop, int pad_frames, long long start,
-                                                   long long out_len, long long expected, float* __restrict__ out) {
+                                                   long long out_len, long long expected, int divide,
+                                                   float* __restrict__ out) {
   const int row = blockIdx.y;
   const float* fr = frames + (size_t)row * n_frames * (size_t)n_fft;
   float* o = out + (size_t)row * (size_t)out_len;
@@ -325,7 +329,7 @@ __global__ void __launch_bounds__(256) fold_kernel(const float* __restrict__ fra
         const long long f = g - pad_frames;
         if (f >= 0 && f < n_frames) acc += fr[(size_t)f * n_fft + n];
       }
-      v = acc / env;
+      v = divide ? acc / env : acc;
     }
     o[i] = v;
   }
@@ -343,21 +347,24 @@ static inline int fq_of(int n_fft) { return round_up(n_fft / 2 + 1, BK); }  // b
 extern "C" int b2a_dft_supported(int n_fft, int hop) { return n_fft >= 2 && n_fft <= 8192 && hop >= 1; }
 
 extern "C" size_t b2a_dft_matrix_floats(int n_fft, int inverse) {
-  if (n_fft < 2 || n_fft > 8192) return 0;
+  if (n_fft < 2 || n_fft > 8192 || inverse < 0 || inverse > 2) return 0;
   return 2 * (inverse ? (size_t)fq_of(n_fft) * np_of(n_fft) : (size_t)np_of(n_fft) * fp_of(n_fft));
 }
 
 extern "C" int b2a_dft_matrix_f32(const float* window, int n_fft, int inverse, float* matrix, void* stream) {
   B2A_REQUIRE(window && matrix, B2A_E_INVALID, "dft_matrix: null pointer");
   B2A_REQUIRE(n_fft >= 2 && n_fft <= 8192, B2A_E_UNSUPPORTED, "dft_matrix: window_length %d (2..8192)", n_fft);
+  B2A_REQUIRE(inverse >= 0 && inverse <= 2, B2A_E_INVALID, "dft_matrix: kind %d (0 forward, 1 inverse, 2 adjoint)", inverse);
   const int F = n_fft / 2 + 1;
   const size_t total = b2a_dft_matrix_floats(n_fft, inverse) / 2;
   const unsigned grid = (unsigned)((total + 255) / 256 < 4096 ? (total + 255) / 256 : 4096);
   B2A_LAUNCH(dft_matrix_kernel, dim3(grid), dim3(256), 0, stream, window, n_fft, F, np_of(n_fft), fp_of(n_fft),
-             fq_of(n_fft), inverse ? 1 : 0, reinterpret_cast<float2*>(matrix));
+             fq_of(n_fft), inverse, reinterpret_cast<float2*>(matrix));
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }
+
+static int launch_forward(FwdParams& p, int64_t rows, void* stream);
 
 extern "C" int b2a_stft_dense_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* matrix,
                                   int pad, int right_pad, int pad_mode, int drop_edge, float* stft_out, void* stream) {
@@ -378,12 +385,31 @@ extern "C" int b2a_stft_dense_f32(const float* x, int64_t rows, int64_t T, int n
   p.x = x; p.Mt = reinterpret_cast<const float2*>(matrix); p.out = reinterpret_cast<float2*>(stft_out);
   p.rows = (int)rows; p.T = (int)T; p.n_fft = n_fft; p.hop = hop; p.pad = pad; p.right_pad = right_pad;
   p.pad_mode = pad_mode; p.drop_edge = drop_edge; p.n_frames = (int)nfr; p.F = n_fft / 2 + 1;
-  p.Np = np_of(n_fft); p.Fp = fp_of(n_fft); p.tiles_f = (int)((nfr + BM - 1) / BM);
+  p.origin = -(n_fft / 2) - pad; p.center = 1;
+  return launch_forward(p, rows, stream);
+}
+
+static int launch_forward(FwdParams& p, int64_t rows, void* stream) {
+  p.Np = np_of(p.n_fft); p.Fp = fp_of(p.n_fft); p.tiles_f = (p.n_frames + BM - 1) / BM;
   const int64_t gx = rows * p.tiles_f;
   B2A_REQUIRE(gx < (int64_t)2147483647, B2A_E_UNSUPPORTED, "stft_dense: too many tiles");
   B2A_LAUNCH(dft_forward_kernel, dim3((unsigned)gx, (unsigned)(p.Fp / BN)), dim3(256), 0, stream, p);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
+}
+
+int b2a::dft::forward_raw(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* matrix,
+                          int64_t origin, int64_t n_frames, float* out, void* stream) {
+  B2A_REQUIRE(b2a_dft_supported(n_fft, hop), B2A_E_UNSUPPORTED, "stft_dense: window_length %d hop %d", n_fft, hop);
+  B2A_REQUIRE(T < (int64_t)1 << 30 && n_frames < (int64_t)1 << 30 && origin > -((int64_t)1 << 30) &&
+                  origin < ((int64_t)1 << 30),
+              B2A_E_UNSUPPORTED, "stft_dense: too large");
+  FwdParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = x; p.Mt = reinterpret_cast<const float2*>(matrix); p.out = reinterpret_cast<float2*>(out);
+  p.rows = (int)rows; p.T = (int)T; p.n_fft = n_fft; p.hop = hop; p.pad_mode = B2A_PAD_CONSTANT;
+  p.n_frames = (int)n_frames; p.F = n_fft / 2 + 1; p.origin = (int)origin; p.center = 0;
+  return launch_forward(p, rows, stream);
 }
 
 extern "C" int b2a_mel_from_stft_f32(const float* stft, int64_t rows, int F, int64_t n_frames, const float* mel_fb,
@@ -415,24 +441,32 @@ extern "C" int b2a_istft_dense_f32(const float* spec, int64_t rows, int64_t n_fr
   B2A_REQUIRE(ws_bytes >= b2a_istft_dense_workspace_bytes(rows, n_frames, n_fft), B2A_E_INVALID,
               "istft_dense: workspace too small");
   B2A_REQUIRE(((uintptr_t)spec & 7) == 0, B2A_E_INVALID, "istft_dense: spectra must be 8-byte aligned");
+  float* frames = reinterpret_cast<float*>(ws);
+  const int rc = inverse_frames(spec, rows, n_frames, n_fft, imatrix, frames, stream);
+  if (rc != B2A_OK) return rc;
+  return launch_fold(frames, window, rows, (int)n_frames, n_fft, hop, pad_frames, start, out_len, 1, out, stream);
+}
+
+int b2a::dft::inverse_frames(const float* spec, int64_t rows, int64_t n_frames, int n_fft, const float* imatrix,
+                             float* frames, void* stream) {
   InvParams p;
   p.spec = reinterpret_cast<const float2*>(spec); p.Mi = reinterpret_cast<const float2*>(imatrix);
-  p.frames = reinterpret_cast<float*>(ws);
+  p.frames = frames;
   p.rows = (int)rows; p.n_frames = (int)n_frames; p.n_fft = n_fft; p.F = n_fft / 2 + 1; p.Fq = fq_of(n_fft);
   p.Np = np_of(n_fft); p.tiles_f = (int)((n_frames + BM - 1) / BM);
   const int64_t gx = rows * p.tiles_f;
   B2A_REQUIRE(gx < (int64_t)2147483647, B2A_E_UNSUPPORTED, "istft_dense: too many tiles");
   B2A_LAUNCH(dft_inverse_kernel, dim3((unsigned)gx, (unsigned)(p.Np / BN)), dim3(256), 0, stream, p);
   B2A_CUDA_OK(cudaGetLastError());
-  return launch_fold(p.frames, window, rows, (int)n_frames, n_fft, hop, pad_frames, start, out_len, out, stream);
+  return B2A_OK;
 }
 
 int b2a::dft::launch_fold(const float* frames, const float* window, int64_t rows, int n_frames, int n_fft, int hop,
-                          int pad_frames, int64_t start, int64_t out_len, float* out, void* stream) {
+                          int pad_frames, int64_t start, int64_t out_len, int divide, float* out, void* stream) {
   const long long expected = (long long)(n_frames + 2 * pad_frames - 1) * hop + n_fft;
   const long long want = (out_len + 255) / 256;
   B2A_LAUNCH(fold_kernel, dim3((unsigned)(want < 2048 ? want : 2048), (unsigned)rows), dim3(256), 0, stream, frames,
-             window, n_frames, n_fft, hop, pad_frames, (long long)start, (long long)out_len, expected, out);
+             window, n_frames, n_fft, hop, pad_frames, (long long)start, (long long)out_len, expected, divide, out);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }

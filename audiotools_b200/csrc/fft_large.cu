@@ -20,6 +20,7 @@
 #include "b2a_common.h"
 #include "dft_internal.h"
 #include "fft_warp.cuh"
+#include "grad_internal.h"
 #include "spectral_internal.h"
 
 namespace b2a {
@@ -99,6 +100,7 @@ struct FwdParams {
   const float* window;
   float2* out;
   int T, hop, pad, right_pad, pad_mode, drop_edge, n_frames;
+  int origin, center;  // frame f starts at x-coordinate (f + drop_edge) hop + origin; center: src_index's framing flag
 };
 
 template <int LOG2_NFFT>
@@ -114,11 +116,11 @@ __global__ void __launch_bounds__(Geo<LOG2_NFFT>::NT, 1) stft_large_kernel(const
   spectral::warp_fft_tables<10, 1>(tw, tw + 10 * 32);
 
   const float* xr = p.x + (size_t)row * (size_t)p.T;
-  const long long base = (long long)(f + p.drop_edge) * p.hop - NFFT / 2 - p.pad;  // x-coordinate of sample 0
+  const long long base = (long long)(f + p.drop_edge) * p.hop + p.origin;  // x-coordinate of sample 0
   const bool interior = base >= 0 && base + NFFT <= (long long)p.T;
   auto sample = [&](int n) -> float {
     if (interior) return __ldg(xr + (base + n));
-    const int u = spectral::src_index((int)(base + n), p.T, p.pad, p.right_pad, p.pad_mode, 1);
+    const int u = spectral::src_index((int)(base + n), p.T, p.pad, p.right_pad, p.pad_mode, p.center);
     return u >= 0 ? __ldg(xr + u) : 0.f;
   };
   // framing + window: point q = x[2q] + i x[2q+1] at row q / N2, column q mod N2
@@ -152,6 +154,7 @@ struct InvParams {
   const float* window;
   float* frames;
   int n_frames;
+  int adjoint;  // 1: bin weights 1 instead of c_k / n_fft (the STFT's adjoint; the fold then skips the envelope)
 };
 
 template <int LOG2_NFFT>
@@ -170,10 +173,13 @@ __global__ void __launch_bounds__(Geo<LOG2_NFFT>::NT, 1) istft_large_kernel(cons
   // conj(Z) / N (the forward FFT of the conjugate is N conj(z)).  The imaginary parts of DC and Nyquist do not
   // enter, as in a C2R transform.
   const float2* sp = p.spec + (size_t)row * (size_t)(N + 1) * (size_t)p.n_frames + f;
-  constexpr float inv_n = 1.0f / (float)N;
+  const float inv_n = p.adjoint ? 1.0f : 1.0f / (float)N;  // adjoint: n_fft/2 x the inverse, DC / Nyquist doubled
   for (int k = tid; k <= N / 2; k += G::NT) {
     float2 xk = sp[(size_t)k * p.n_frames], xn = sp[(size_t)(N - k) * p.n_frames];
-    if (k == 0) { xk.y = 0.f; xn.y = 0.f; }
+    if (k == 0) {
+      xk.y = 0.f; xn.y = 0.f;
+      if (p.adjoint) { xk.x *= 2.f; xn.x *= 2.f; }
+    }
     const float2 e = make_float2(0.5f * (xk.x + xn.x), 0.5f * (xk.y - xn.y));
     const float2 d = make_float2(0.5f * (xk.x - xn.x), 0.5f * (xk.y + xn.y));
     float sn, cs;
@@ -235,6 +241,8 @@ extern "C" int b2a_stft_large_supported(int n_fft, int hop, int inverse) {
   return inverse ? (l >= 12 && hop <= n_fft) : l >= 13;
 }
 
+static int launch_fwd_any(const FwdParams& p, int64_t rows, int n_fft, void* stream);
+
 extern "C" int b2a_stft_large_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window,
                                   int pad, int right_pad, int pad_mode, int drop_edge, float* stft_out, void* stream) {
   B2A_REQUIRE(x && window && stft_out, B2A_E_INVALID, "stft_large: null pointer");
@@ -255,11 +263,44 @@ extern "C" int b2a_stft_large_f32(const float* x, int64_t rows, int64_t T, int n
   FwdParams p;
   p.x = x; p.window = window; p.out = reinterpret_cast<float2*>(stft_out);
   p.T = (int)T; p.hop = hop; p.pad = pad; p.right_pad = right_pad; p.pad_mode = pad_mode; p.drop_edge = drop_edge;
-  p.n_frames = (int)nfr;
+  p.n_frames = (int)nfr; p.origin = -(n_fft / 2) - pad; p.center = 1;
+  return launch_fwd_any(p, rows, n_fft, stream);
+}
+
+static int launch_fwd_any(const FwdParams& p, int64_t rows, int n_fft, void* stream) {
   switch (n_fft) {
+    case 4096: return launch_fwd<12>(p, rows, stream);
     case 8192: return launch_fwd<13>(p, rows, stream);
     case 16384: return launch_fwd<14>(p, rows, stream);
     default: return launch_fwd<15>(p, rows, stream);
+  }
+}
+
+int b2a::large::forward_raw(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window,
+                            int64_t origin, int64_t n_frames, float* out, void* stream) {
+  B2A_REQUIRE(b2a_stft_large_supported(n_fft, hop, 1), B2A_E_UNSUPPORTED, "stft_large: window_length %d hop %d", n_fft,
+              hop);
+  B2A_REQUIRE(T < (int64_t)1 << 30 && rows * n_frames < (int64_t)2147483647 && origin > -((int64_t)1 << 30) &&
+                  origin < ((int64_t)1 << 30),
+              B2A_E_UNSUPPORTED, "stft_large: too large");
+  FwdParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = x; p.window = window; p.out = reinterpret_cast<float2*>(out);
+  p.T = (int)T; p.hop = hop; p.pad_mode = B2A_PAD_CONSTANT; p.n_frames = (int)n_frames; p.origin = (int)origin;
+  p.center = 0;
+  return launch_fwd_any(p, rows, n_fft, stream);
+}
+
+int b2a::large::inverse_frames(const float* spec, int64_t rows, int64_t n_frames, int n_fft, const float* window,
+                               float* frames, int adjoint, void* stream) {
+  InvParams p;
+  p.spec = reinterpret_cast<const float2*>(spec); p.window = window; p.frames = frames;
+  p.n_frames = (int)n_frames; p.adjoint = adjoint ? 1 : 0;
+  switch (n_fft) {
+    case 4096: return launch_inv<12>(p, rows, stream);
+    case 8192: return launch_inv<13>(p, rows, stream);
+    case 16384: return launch_inv<14>(p, rows, stream);
+    default: return launch_inv<15>(p, rows, stream);
   }
 }
 
@@ -281,16 +322,9 @@ extern "C" int b2a_istft_large_f32(const float* spec, int64_t rows, int64_t n_fr
   B2A_REQUIRE(((uintptr_t)spec & 7) == 0 && ((uintptr_t)ws & 7) == 0, B2A_E_INVALID,
               "istft_large: spectra and workspace must be 8-byte aligned");
   B2A_REQUIRE(rows * n_frames < (int64_t)2147483647, B2A_E_UNSUPPORTED, "istft_large: too many frames");
-  InvParams p;
-  p.spec = reinterpret_cast<const float2*>(spec); p.window = window; p.frames = reinterpret_cast<float*>(ws);
-  p.n_frames = (int)n_frames;
-  int rc;
-  switch (n_fft) {
-    case 4096: rc = launch_inv<12>(p, rows, stream); break;
-    case 8192: rc = launch_inv<13>(p, rows, stream); break;
-    case 16384: rc = launch_inv<14>(p, rows, stream); break;
-    default: rc = launch_inv<15>(p, rows, stream); break;
-  }
+  float* frames = reinterpret_cast<float*>(ws);
+  const int rc = b2a::large::inverse_frames(spec, rows, n_frames, n_fft, window, frames, 0, stream);
   if (rc != B2A_OK) return rc;
-  return b2a::dft::launch_fold(p.frames, window, rows, (int)n_frames, n_fft, hop, pad_frames, start, out_len, out, stream);
+  return b2a::dft::launch_fold(frames, window, rows, (int)n_frames, n_fft, hop, pad_frames, start, out_len, 1, out,
+                               stream);
 }

@@ -1,0 +1,30 @@
+// grad_internal.h -- the pieces of the STFT / inverse STFT kernels that grad.cu reuses for the backward passes.
+#pragma once
+#include "b2a_common.h"
+
+namespace b2a {
+namespace istft {
+// The fused inverse of istft.cu (b2a_istft_f32's arguments).  adjoint = 1: the STFT's adjoint instead -- bin weights 1
+// (not c_k / n_fft) and no envelope division, so out[i] = sum over frames of w[n] sum_k Re(X_k e^{2 pi i kn / n_fft}).
+int run(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window, int pad_frames,
+        int64_t start, int64_t out_len, float* out, int adjoint, void* stream);
+}  // namespace istft
+
+namespace large {
+// Windowed inverse frames of fft_large.cu -> frames [rows, n_frames, n_fft] (n_fft 4096 .. 32768); adjoint as above.
+int inverse_frames(const float* spec, int64_t rows, int64_t n_frames, int n_fft, const float* window, float* frames,
+                   int adjoint, void* stream);
+// Forward FFT of raw (un-centred) frames: frame f covers x-coordinates [f hop + origin, + n_fft), zeros outside [0, T).
+int forward_raw(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window, int64_t origin,
+                int64_t n_frames, float* out, void* stream);
+}  // namespace large
+
+namespace dft {
+// Dense inverse frames of dft.cu with a kind 1 (inverse) or kind 2 (adjoint) matrix -> frames [rows, n_frames, n_fft].
+int inverse_frames(const float* spec, int64_t rows, int64_t n_frames, int n_fft, const float* imatrix, float* frames,
+                   void* stream);
+// Dense forward DFT (kind 0 matrix) of raw frames, framed as large::forward_raw.
+int forward_raw(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* matrix, int64_t origin,
+                int64_t n_frames, float* out, void* stream);
+}  // namespace dft
+}  // namespace b2a

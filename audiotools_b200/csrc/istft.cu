@@ -24,6 +24,7 @@
 // Bytes: read spectra 8 F N + write 4 T per row -- the algorithmic minimum.
 #include "b2a_common.h"
 #include "fft_warp.cuh"
+#include "grad_internal.h"
 
 namespace b2a {
 namespace istft {
@@ -35,6 +36,7 @@ struct Params {
   const float* window;  // [n_fft]
   float* out;           // [rows, out_len]
   int rows, n_frames, pad_frames, hop;
+  int adjoint;          // 1: the STFT's adjoint (bin weights 1, no envelope division), see b2a::istft::run
   int groups_total;     // groups that cover every sample below `expected`
   int seg_groups, segs_per_row, warm;
   long long start, out_len, expected;
@@ -59,7 +61,9 @@ __global__ void __launch_bounds__(256, 2) istft_kernel(const Params p) {
   const int NP = p.n_frames + 2 * p.pad_frames;  // frames incl. the zero frames of match_stride
   const int g_own = warp * FPW + lane / LPF, l = lane % LPF;
   float* slot = reg + g_own * FS;
-  const float inv_n = 0.5f / (float)N;  // 1/N of the transform and the 1/2 of the even/odd split
+  // 1/N of the transform and the 1/2 of the even/odd split; the adjoint wants sum_k Re(G_k e^{i theta}) = n_fft/2 times
+  // the inverse of the DC / Nyquist-doubled spectrum
+  const float inv_n = p.adjoint ? 0.5f : 0.5f / (float)N;
   const int src_lane = (lane & ~(LPF - 1)) | ((LPF - l) & (LPF - 1));  // holder of the partner element N - k
   const int tail = NFFT - hop;                   // samples a group hands to the next one
   const int items = p.rows * p.segs_per_row;
@@ -89,7 +93,10 @@ __global__ void __launch_bounds__(256, 2) istft_kernel(const Params p) {
         const int n = g0 + g - p.pad_frames;
         float2 v = make_float2(0.f, 0.f);
         if (n >= 0 && n < p.n_frames) v = __ldg(srow + (size_t)k * p.n_frames + n);
-        if (k == 0 || k == N) v.y = 0.f;  // a C2R transform ignores the imaginary parts of DC and Nyquist
+        if (k == 0 || k == N) {
+          v.y = 0.f;  // a C2R transform ignores the imaginary parts of DC and Nyquist
+          if (p.adjoint) v.x *= 2.f;  // weight 1 on every bin: DC / Nyquist get 2x the 1/2 of the interior pairs
+        }
         reinterpret_cast<float2*>(reg + g * FS)[k] = v;
       }
       __syncthreads();
@@ -158,7 +165,8 @@ __global__ void __launch_bounds__(256, 2) istft_kernel(const Params p) {
             ef.x = fmaf(wv.x, wv.x, ef.x); ef.y = fmaf(wv.y, wv.y, ef.y);
             ef.z = fmaf(wv.z, wv.z, ef.z); ef.w = fmaf(wv.w, wv.w, ef.w);
           }
-          const float4 inv_ef = make_float4(1.0f / ef.x, 1.0f / ef.y, 1.0f / ef.z, 1.0f / ef.w);
+          const float4 inv_ef = p.adjoint ? make_float4(1.f, 1.f, 1.f, 1.f)
+                                          : make_float4(1.0f / ef.x, 1.0f / ef.y, 1.0f / ef.z, 1.0f / ef.w);
           for (int q = q4_first; q < qn; q += QL4) {
             const int trel = q * hop + r;
             float4 acc = trel < tail ? *reinterpret_cast<const float4*>(cin + trel) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -194,7 +202,7 @@ __global__ void __launch_bounds__(256, 2) istft_kernel(const Params p) {
                   } else {
                     float env = 0.f;
                     for (int d = dlo; d <= dhi; ++d) { const float wv = win[d * hop + r + u]; env = fmaf(wv, wv, env); }
-                    v = a4[u] / env;
+                    v = p.adjoint ? a4[u] : a4[u] / env;
                   }
                 }
                 orow[iu] = v;
@@ -209,7 +217,7 @@ __global__ void __launch_bounds__(256, 2) istft_kernel(const Params p) {
         // envelope of residue r where all dmax+1 covering frames exist (everywhere but the signal's two ends)
         float env_full = 0.f;
         for (int d = 0; d <= dmax; ++d) { const float wv = win[d * hop + r]; env_full = fmaf(wv, wv, env_full); }
-        const float inv_env_full = 1.0f / env_full;
+        const float inv_env_full = p.adjoint ? 1.f : 1.0f / env_full;
         for (int q = q_first; q < qn; q += QL) {
           const int trel = q * hop + r;
           float acc = trel < tail ? cin[trel] : 0.f;
@@ -229,7 +237,7 @@ __global__ void __launch_bounds__(256, 2) istft_kernel(const Params p) {
                   } else {
                     float env = 0.f;
                     for (int d = dlo; d <= dhi; ++d) { const float wv = win[d * hop + r]; env = fmaf(wv, wv, env); }
-                    v = acc / env;
+                    v = p.adjoint ? acc : acc / env;
                   }
                 }
                 orow[i] = v;
@@ -317,10 +325,8 @@ extern "C" int b2a_istft_supported(int n_fft, int hop) {
   return hop >= 1 && hop <= n_fft;
 }
 
-extern "C" int b2a_istft_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop,
-                             const float* window, int pad_frames, int64_t start, int64_t out_len, float* out,
-                             void* stream) {
-  using namespace b2a::istft;
+int b2a::istft::run(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,
+                    int pad_frames, int64_t start, int64_t out_len, float* out, int adjoint, void* stream) {
   B2A_REQUIRE(spec && window && out, B2A_E_INVALID, "istft: null pointer");
   B2A_REQUIRE(rows >= 1 && n_frames >= 1 && out_len >= 1 && pad_frames >= 0 && start >= 0, B2A_E_INVALID,
               "istft: bad argument");
@@ -333,7 +339,7 @@ extern "C" int b2a_istft_f32(const float* spec, int64_t rows, int64_t n_frames, 
   memset(&p, 0, sizeof(p));
   p.spec = reinterpret_cast<const float2*>(spec);
   p.window = window; p.out = out;
-  p.rows = (int)rows; p.n_frames = (int)n_frames; p.pad_frames = pad_frames; p.hop = hop;
+  p.rows = (int)rows; p.n_frames = (int)n_frames; p.pad_frames = pad_frames; p.hop = hop; p.adjoint = adjoint ? 1 : 0;
   p.start = start; p.out_len = out_len;
   p.expected = (long long)(n_frames + 2 * pad_frames - 1) * hop + n_fft;
   switch (n_fft) {
@@ -344,4 +350,10 @@ extern "C" int b2a_istft_f32(const float* spec, int64_t rows, int64_t n_frames, 
     case 1024: return launch<9>(p, stream);
     default: return launch<10>(p, stream);
   }
+}
+
+extern "C" int b2a_istft_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop,
+                             const float* window, int pad_frames, int64_t start, int64_t out_len, float* out,
+                             void* stream) {
+  return b2a::istft::run(spec, rows, n_frames, n_fft, hop, window, pad_frames, start, out_len, out, 0, stream);
 }

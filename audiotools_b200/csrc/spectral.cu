@@ -733,7 +733,7 @@ static int launch_warp(Params& p, void* stream) {
   return B2A_OK;
 }
 
-// raw-framing forward FFT of blocks (used by the FFT convolution): out[rows, F, n_frames]
+// raw-framing forward FFT of blocks (the FFT convolution, the inverse STFT's backward): out[rows, F, n_frames]
 int frames_fft(const float* x, int rows, int T, int n_fft, int hop, const float* window, int origin,
                const int32_t* row_origin, int pad_mode, int n_frames, float2* out, void* stream) {
   Params p;
@@ -741,8 +741,15 @@ int frames_fft(const float* x, int rows, int T, int n_fft, int hop, const float*
   p.x = x; p.window = window; p.stft_out = out;
   p.rows = rows; p.T = T; p.n_fft = n_fft; p.hop = hop; p.pad_mode = pad_mode; p.n_frames = n_frames;
   p.rows_per_gain = 1; p.center = 0; p.origin = origin; p.row_origin = row_origin;
-  B2A_REQUIRE(n_fft == 2048, B2A_E_UNSUPPORTED, "frames_fft: block size %d", n_fft);
-  return launch_warp<10>(p, stream);
+  switch (n_fft) {
+    case 64: return launch_warp<5>(p, stream);
+    case 128: return launch_warp<6>(p, stream);
+    case 256: return launch_warp<7>(p, stream);
+    case 512: return launch_warp<8>(p, stream);
+    case 1024: return launch_warp<9>(p, stream);
+    case 2048: return launch_warp<10>(p, stream);
+  }
+  return b2a::fail(B2A_E_UNSUPPORTED, "frames_fft: block size %d", n_fft);
 }
 
 }  // namespace spectral

@@ -61,6 +61,7 @@ int launch_tc(Params& p, void* stream);
 // Forward real FFT of raw (un-centred) blocks: block n of row r covers x-coordinates
 // [n*hop + origin + row_origin[r], +n_fft), out of range samples resolved by pad_mode
 // (B2A_PAD_CONSTANT zero / B2A_PAD_REPLICATE / 3 = circular).  out: [rows, n_fft/2+1, n_frames] (re,im).
+// n_fft: power of two in [64, 2048] (the warp kernel).
 int frames_fft(const float* x, int rows, int T, int n_fft, int hop, const float* window, int origin,
                const int32_t* row_origin, int pad_mode, int n_frames, float2* out, void* stream);
 

@@ -9,6 +9,7 @@ the kernels; the module-level engine is always built with ``require_cuda=True``.
 """
 import ctypes
 import math
+import sys
 from typing import Optional
 
 import numpy as np
@@ -30,9 +31,23 @@ class Engine:
         self._packed_cache = {}
 
     # ------------------------------------------------------------------ helpers
+    DIFFERENTIABLE = ("AudioSignal.stft", "istft", "mel_spectrogram", "mfcc", "normalize", "volume_change",
+                      "and magnitude / phase / log_magnitude through stft_data")
+
+    @classmethod
+    def _refuse_grad(cls, t: torch.Tensor, name: str, depth: int = 2):
+        """A tensor that requires a gradient while grad mode is on reaches a kernel without a backward: raise instead
+        of returning a silently detached result.  The message names the engine method that was called."""
+        if t.requires_grad and torch.is_grad_enabled():
+            method = sys._getframe(depth).f_code.co_name
+            raise NotImplementedError(
+                f"{method}: {name} requires a gradient, and this method has no backward.  Differentiable: "
+                f"{', '.join(cls.DIFFERENTIABLE)}.  Call it under torch.no_grad() or on a detached signal.")
+
     def _prep(self, t: torch.Tensor, name: str, dtype=torch.float32) -> torch.Tensor:
         if not torch.is_tensor(t):
             raise TypeError(f"{name} must be a torch.Tensor")
+        self._refuse_grad(t, name)
         if self.require_cuda and not t.is_cuda:
             raise RuntimeError(
                 f"{name} is on {t.device}: audiotools_b200 runs on CUDA (sm_90a) only and has no CPU fallback")
@@ -86,6 +101,7 @@ class Engine:
         on either side and ``trim`` extra leading samples are dropped (the reference's match_stride handling)."""
         if not torch.is_complex(spec):
             raise TypeError("istft: spec must be complex")
+        self._refuse_grad(spec, "spec", depth=1)
         if self.require_cuda and not spec.is_cuda:
             raise RuntimeError(f"stft_data is on {spec.device}: audiotools_b200 runs on CUDA (sm_90a) only and has "
                                "no CPU fallback")
@@ -139,6 +155,90 @@ class Engine:
         self.launches += 1
         return out
 
+    # ------------------------------------------------------------------ backward passes (csrc/grad.cu)
+    def backward_supported(self, n_fft: int, hop: int) -> bool:
+        return bool(self.lib.b2a_stft_backward_supported(int(n_fft), int(hop)))
+
+    def _dense_backward(self, n_fft: int, hop: int) -> bool:
+        """The backward of this geometry runs on the dense DFT (needs a matrix): not a power of two in [64, 32768]."""
+        return not (self.lib.b2a_istft_supported(int(n_fft), int(hop))
+                    or self.lib.b2a_stft_large_supported(int(n_fft), int(hop), 1))
+
+    def stft_backward(self, grad_spec: torch.Tensor, T: int, n_fft: int, hop: int, window: torch.Tensor, pad: int = 0,
+                      right_pad: int = 0, pad_mode: str = "reflect", drop_edge: int = 0) -> torch.Tensor:
+        """Gradient wrt x [B, C, T] of ``spectral``'s STFT from grad_spec [B, C, F, N] (complex, torch's convention)."""
+        grad_spec = grad_spec.to(torch.complex64).contiguous()
+        B, C, F, N = grad_spec.shape
+        window = self._prep(window, "window")
+        nbytes = int(self.lib.b2a_stft_backward_workspace_bytes(B * C, int(T), int(n_fft), int(hop), int(pad),
+                                                                int(right_pad), int(drop_edge)))
+        if nbytes == 0:
+            raise NotImplementedError(f"stft backward: window_length {n_fft} hop {hop}")
+        amat = self.dft_matrix(window, int(n_fft), inverse=2) if self._dense_backward(n_fft, hop) else None
+        ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=grad_spec.device)
+        gx = torch.empty(B, C, int(T), dtype=torch.float32, device=grad_spec.device)
+        rc = self.lib.b2a_stft_backward_f32(_dptr(torch.view_as_real(grad_spec)), B * C, int(T), int(n_fft), int(hop),
+                                            _dptr(window), _dptr(amat), int(pad), int(right_pad),
+                                            _lib.PAD_MODES[pad_mode], int(drop_edge), _dptr(gx), _dptr(ws), nbytes,
+                                            self._stream(grad_spec))
+        self.lib.check(rc)
+        self.launches += 2 if self.lib.b2a_istft_supported(int(n_fft), int(hop)) else 3
+        return gx
+
+    def istft_backward(self, grad_out: torch.Tensor, n_frames: int, n_fft: int, hop: int, window: torch.Tensor,
+                       pad_frames: int = 0, trim: int = 0) -> torch.Tensor:
+        """Gradient wrt spec [B, C, F, n_frames] (complex64) of ``istft`` from grad_out [B, C, length]."""
+        grad_out = grad_out.to(torch.float32).contiguous()
+        B, C, L = grad_out.shape
+        window = self._prep(window, "window")
+        mat = self.dft_matrix(window, int(n_fft), inverse=0) if self._dense_backward(n_fft, hop) else None
+        nbytes = int(self.lib.b2a_istft_backward_workspace_bytes(B * C, L))
+        ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=grad_out.device)
+        gs = torch.empty(B, C, n_fft // 2 + 1, int(n_frames), dtype=torch.complex64, device=grad_out.device)
+        rc = self.lib.b2a_istft_backward_f32(_dptr(grad_out), B * C, int(n_frames), int(n_fft), int(hop), _dptr(window),
+                                             _dptr(mat), int(pad_frames), n_fft // 2 + int(trim), L,
+                                             _dptr(torch.view_as_real(gs)), _dptr(ws), nbytes, self._stream(grad_out))
+        self.lib.check(rc)
+        self.launches += 3
+        return gs
+
+    def _bin_table(self, mel_lo: torch.Tensor, mel_hi: torch.Tensor, F: int):
+        """[F] int32 (bin_lo, bin_hi): the filters whose band may hold bin k lie in [bin_lo[k], bin_hi[k]) -- the
+        transposed band table of the mel backward, built on the host once per filterbank (the entry keeps both alive)."""
+        key = ("bins", mel_lo.data_ptr(), mel_hi.data_ptr(), mel_lo.numel(), int(F))
+        if key not in self._packed_cache:
+            lo, hi = mel_lo.cpu().numpy().astype("int64"), mel_hi.cpu().numpy().astype("int64")
+            blo = np.full(F, len(lo), dtype=np.int32)
+            bhi = np.zeros(F, dtype=np.int32)
+            for m in range(len(lo)):
+                if hi[m] > lo[m]:
+                    blo[lo[m]:hi[m]] = np.minimum(blo[lo[m]:hi[m]], m)
+                    bhi[lo[m]:hi[m]] = np.maximum(bhi[lo[m]:hi[m]], m + 1)
+            blo = np.minimum(blo, bhi)
+            dev = mel_lo.device
+            self._packed_cache[key] = (torch.from_numpy(blo).to(dev), torch.from_numpy(bhi).to(dev), mel_lo, mel_hi)
+        return self._packed_cache[key][:2]
+
+    def mel_backward(self, stft: torch.Tensor, grad_mel: torch.Tensor, mel_fb: torch.Tensor, mel_lo: torch.Tensor,
+                     mel_hi: torch.Tensor, post: int = _lib.POST_NONE, post_eps: float = 0.0,
+                     post_power: float = 1.0) -> torch.Tensor:
+        """Gradient wrt the complex STFT [B, C, F, N] of ``spectral``'s mel output from grad_mel [B, C, n_mels, N]."""
+        stft = stft.to(torch.complex64).contiguous()
+        B, C, F, N = stft.shape
+        grad_mel = grad_mel.to(torch.float32).contiguous()
+        mel_fb = self._prep(mel_fb, "mel_fb")
+        mel_lo = self._prep(mel_lo, "mel_lo", torch.int32)
+        mel_hi = self._prep(mel_hi, "mel_hi", torch.int32)
+        bin_lo, bin_hi = self._bin_table(mel_lo, mel_hi, F)
+        out = torch.empty_like(stft)
+        rc = self.lib.b2a_mel_backward_f32(_dptr(torch.view_as_real(stft)), B * C, F, N, _dptr(mel_fb), _dptr(mel_lo),
+                                           _dptr(mel_hi), mel_fb.shape[0], _dptr(bin_lo), _dptr(bin_hi), int(post),
+                                           float(post_eps), float(post_power), _dptr(grad_mel),
+                                           _dptr(torch.view_as_real(out)), self._stream(stft))
+        self.lib.check(rc)
+        self.launches += 1
+        return out
+
     # ------------------------------------------------------------------ dense DFT (any window length)
     @staticmethod
     def fft_window_length(n_fft: int) -> bool:
@@ -153,10 +253,11 @@ class Engine:
             return f": power-of-two windows run on the FFT kernels up to {self.LARGE_FFT_MAX}"
         return ""
 
-    def dft_matrix(self, window: torch.Tensor, n_fft: int, inverse: bool = False) -> torch.Tensor:
+    def dft_matrix(self, window: torch.Tensor, n_fft: int, inverse: int = 0) -> torch.Tensor:
         """The windowed DFT matrix of csrc/dft.cu for (n_fft, window), built on the device once and cached (the cache
-        entry holds the window tensor, so its address / version identify it)."""
-        key = ("dft", window.data_ptr(), int(window._version), int(n_fft), bool(inverse))
+        entry holds the window tensor, so its address / version identify it).  ``inverse``: 0 forward, 1 inverse
+        (c_k / n_fft weights), 2 the STFT's adjoint (the inverse layout, weight 1)."""
+        key = ("dft", window.data_ptr(), int(window._version), int(n_fft), int(inverse))
         hit = self._packed_cache.get(key)
         if hit is None:
             n = int(self.lib.b2a_dft_matrix_floats(int(n_fft), int(inverse)))
@@ -194,6 +295,7 @@ class Engine:
     def _spec_ok(self, spec: torch.Tensor, what: str) -> torch.Tensor:
         if not torch.is_complex(spec):
             raise TypeError(f"{what}: spec must be complex")
+        self._refuse_grad(spec, "spec")
         if self.require_cuda and not spec.is_cuda:
             raise RuntimeError(f"stft_data is on {spec.device}: audiotools_b200 runs on CUDA (sm_90a) only and has "
                                "no CPU fallback")

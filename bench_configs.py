@@ -3,7 +3,7 @@
 bench.py, which measures configs[1]).  One JSON line per config: device-resident throughput (CUDA events,
 >= 3 warm-ups, inputs larger than L2 or rotated), algorithmic bytes, and the CPU oracle on a bounded sample.
 
-    python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,largewin,gate,masked] [--no-cpu]
+    python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,largewin,grad,gate,masked] [--no-cpu]
 
 Multi-GPU (BASELINE configs[3] = 512 items on 4 GPUs, configs[4] = 2048 items on 8 GPUs): one process per GPU,
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 4 --master-addr 127.0.0.1 --master-port 29511 \
@@ -283,6 +283,94 @@ def main():
               "frac_of_hbm_peak": alg / ms_stft / 1e6 / peak, "gpu": torch.cuda.get_device_name(LOCAL),
               "power_limit": plim})
         del X, Xr, sig, x
+
+    if "grad" in only:  # forward + backward through the spectral front end (csrc/grad.cu) next to torch autograd
+        import subprocess
+
+        import torch.nn.functional as F
+
+        from audiotools_b200.engine import get_engine
+
+        eng = get_engine()
+        sr = 44100
+
+        def l1_log(a, b, pw):
+            return F.l1_loss(a.clamp(1e-5).pow(pw).log10(), b.clamp(1e-5).pow(pw).log10())
+
+        # the reference's losses (ref:audiotools/metrics/spectral.py:70-95, 159-192): (kind, n_mels, windows, mag, pow)
+        losses = [("mel", [150, 80], [2048, 512], 1.0, 2.0), ("stft", None, [2048, 512], 1.0, 2.0),
+                  ("mel", [5, 10, 20, 40, 80, 160, 320], [32, 64, 128, 256, 512, 1024, 2048], 0.0, 1.0)]
+        fbs = {}
+
+        def torch_mel(x, nm, wl):  # the reference's arithmetic on the GPU: torch.stft (cuFFT) + abs + matmul (cuBLAS)
+            if (nm, wl) not in fbs:
+                fbs[nm, wl] = torch.from_numpy(np.asarray(AudioSignal.get_mel_filters(sr, wl, nm), np.float32)).to(dev)
+            return (torch_mag(x, wl).transpose(2, -1) @ fbs[nm, wl].T).transpose(-1, 2)
+
+        def torch_mag(x, wl):
+            w = AudioSignal.get_window("hann", wl, x.device)
+            X = torch.stft(x.reshape(-1, x.shape[-1]), wl, wl // 4, window=w, center=True, return_complex=True)
+            return X.reshape(*x.shape[:2], *X.shape[1:]).abs()
+
+        def loss_of(x, y, cfg, ours):
+            kind, nms, wls, mag, pw = cfg
+            loss = 0.0
+            for i, wl in enumerate(wls):
+                if kind == "mel":
+                    if ours:
+                        a = AudioSignal(x, sr).mel_spectrogram(nms[i], window_length=wl, hop_length=wl // 4)
+                        b = AudioSignal(y, sr).mel_spectrogram(nms[i], window_length=wl, hop_length=wl // 4)
+                    else:
+                        a, b = torch_mel(x, nms[i], wl), torch_mel(y, nms[i], wl)
+                else:
+                    if ours:
+                        sa, sb = AudioSignal(x, sr), AudioSignal(y, sr)
+                        sa.stft(wl, wl // 4, "hann")
+                        sb.stft(wl, wl // 4, "hann")
+                        a, b = sa.magnitude, sb.magnitude
+                    else:
+                        a, b = torch_mag(x, wl), torch_mag(y, wl)
+                loss = loss + l1_log(a, b, pw) + mag * F.l1_loss(a, b)
+            return loss
+
+        g = torch.Generator().manual_seed(0)
+        x = (0.1 * torch.randn(16, 1, sr, generator=g)).to(dev)
+        y = (0.1 * torch.randn(16, 1, sr, generator=g)).to(dev)
+        res = {}
+        for name, cfg in zip(["mel_default", "stft_default", "mel_7scale"], losses):
+            for ours in (True, False):
+                def step():
+                    xg = x.clone().requires_grad_()
+                    loss_of(xg, y, cfg, ours).backward()
+
+                res[name + ("_ms" if ours else "_torch_ms")] = timed(step, steps=20)
+        # cfg2 size: 64 x 2 ch x 10 s, 2048 / 512, 128 mels -- the backward alone (forward done once, untimed)
+        B, C, T = 64, 2, 441000
+        xb = (0.1 * torch.randn(B, C, T, generator=g)).to(dev)
+        xg = xb.clone().requires_grad_()
+        mel = AudioSignal(xg, sr).mel_spectrogram(128, window_length=2048, hop_length=512)
+        gm = torch.randn_like(mel)
+        ms_bwd = timed(lambda: torch.autograd.grad(mel, xg, gm, retain_graph=True), steps=5)
+        xt = xb.clone().requires_grad_()
+        melt = torch_mel(xt, 128, 2048)
+        ms_bwd_torch = timed(lambda: torch.autograd.grad(melt, xt, gm, retain_graph=True), steps=5)
+        F_, N = 1025, mel.shape[-1]
+        Lpp = T + 2048
+        # mel backward: STFT read twice, dmel read, dX written; STFT adjoint: dX read, padded range written; pad
+        # adjoint: padded range read, dx written
+        alg = B * C * (3 * 8 * F_ * N + 4 * 128 * N + 8 * F_ * N + 4 * Lpp + 4 * Lpp + 4 * T)
+        try:
+            plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(LOCAL)],
+                                  capture_output=True, text=True, timeout=30).stdout.strip()
+        except Exception:  # noqa: BLE001 (informational field)
+            plim = "unknown"
+        emit({"config": "grad: forward+backward of the reference's 3 spectral losses at 16x1ch x 1s@44.1k; "
+                        "mel backward at 64x2ch x 10s@44.1k (2048/512, 128 mels)",
+              **res, "ms_mel_backward_cfg2": ms_bwd, "ms_mel_backward_cfg2_torch_autograd": ms_bwd_torch,
+              "alg_bytes_mel_backward_cfg2": alg, "achieved_GBps_mel_backward_cfg2": alg / ms_bwd / 1e6,
+              "frac_of_hbm_peak": alg / ms_bwd / 1e6 / peak, "launches_total": eng.launches,
+              "gpu": torch.cuda.get_device_name(LOCAL), "power_limit": plim})
+        del xb, xg, xt, mel, melt, gm
 
     if "gate" in only:  # SpectralGate (csrc/specmask.cu) at 64 x 2ch x 10 s: stft x2 + gate + istft
         from audiotools_b200.ml.layers import SpectralGate

@@ -98,7 +98,8 @@ int b2a_istft_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, 
  * Everything else is ONE real x complex matrix product over all frames of the batch (FP32 FMA):
  *   b2a_dft_matrix_f32     builds the matrix of (n_fft, window) once: inverse 0 -> M[n][k] = w[n] exp(-2 pi i nk/n_fft)
  *                          for b2a_stft_dense_f32, inverse 1 -> c_k/n_fft . w[n] exp(-2 pi i nk/n_fft) (c = 1 for DC and
- *                          Nyquist, else 2) for b2a_istft_dense_f32; `matrix`: b2a_dft_matrix_floats(n_fft, inverse)
+ *                          Nyquist, else 2) for b2a_istft_dense_f32, inverse 2 -> the layout of 1 with weight 1 on every
+ *                          bin for b2a_stft_backward_f32; `matrix`: b2a_dft_matrix_floats(n_fft, inverse)
  *                          floats, 16-byte aligned; angles reduced in integers (nk mod n_fft), evaluated in float64
  *   b2a_stft_dense_f32     the arguments of b2a_spectral_f32 (same framing / padding semantics, bit-exact frame
  *                          indexing) -> stft_out [rows, n_fft/2+1, n_frames] (re,im)
@@ -142,6 +143,47 @@ size_t b2a_istft_large_workspace_bytes(int64_t rows, int64_t n_frames, int n_fft
 int b2a_istft_large_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,
                         int pad_frames, int64_t start, int64_t out_len, float* out, void* ws, size_t ws_bytes,
                         void* stream);
+
+/* ---- backward passes of the spectral front end (csrc/grad.cu) ---------------------------------------------------
+ * Gradients of AudioSignal.stft / istft / mel_spectrogram / mfcc (audiotools/core/audio_signal.py:1123-1296, 1333-1426;
+ * differentiable through torch there, tests/core/test_grad.py).  A complex gradient is G = dL/dRe + i dL/dIm (torch's
+ * convention); every pass is deterministic (no atomics, fixed summation order).
+ *   b2a_stft_backward_supported  (n_fft, hop): 1 when both backward passes exist: 1 <= hop <= n_fft and n_fft a power of
+ *                                two up to 32768 or any length 2 .. 8192.
+ *   b2a_stft_backward_f32        grad_spec [rows, n_fft/2+1, n_frames] (re,im) -> grad_x [rows, T], for the STFT that
+ *                                b2a_spectral_f32 / b2a_stft_dense_f32 / b2a_stft_large_f32 computed with the same
+ *                                (T, n_fft, hop, window, pad, right_pad, pad_mode, drop_edge): per frame
+ *                                w[n] sum_k Re(G_k e^{2 pi i kn/n_fft}), overlap-added without envelope division over the
+ *                                padded range, folded back through both paddings (each padded position's gradient is
+ *                                added to the sample it was read from).  amatrix: the kind 2 matrix of b2a_dft_matrix_f32,
+ *                                required for the dense window lengths (not a power of two in [64, 32768]), else unused.
+ *                                ws: b2a_stft_backward_workspace_bytes(...) bytes, 8-byte aligned.
+ *   b2a_istft_backward_f32       grad_out [rows, out_len] -> grad_spec [rows, n_fft/2+1, n_frames] for the inverse that
+ *                                b2a_istft_f32 / _dense_ / _large_ computed with the same arguments: grad_out / envelope
+ *                                framed with the window, forward real FFT, bin k scaled by c_k / n_fft (c = 1 at DC and
+ *                                Nyquist, else 2), imaginary parts of DC / Nyquist 0.  matrix: the kind 0 (forward) matrix
+ *                                of b2a_dft_matrix_f32 for the dense window lengths.  ws: b2a_istft_backward_workspace_bytes.
+ *   b2a_mel_backward_f32         grad_mel [rows, n_mels, n_frames] -> grad_stft [rows, F, n_frames] (re,im) from the
+ *                                complex STFT `stft` the mel came from: recomputes mel from the banded filters, applies the
+ *                                post-op's derivative (B2A_POST_LOG10: post_power / (ln10 mel) where mel >= post_eps, else
+ *                                0; B2A_POST_LN: 1 / (mel + post_eps)), projects back through fb^T and multiplies by
+ *                                X / |X| (0 where |X| = 0).  bin_lo / bin_hi [F] int32: the filters m that may hold bin k
+ *                                lie in [bin_lo[k], bin_hi[k]) (mel_lo[m] <= k < mel_hi[m] is checked per filter).
+ * The mfcc DCT's backward is b2a_mel_dct_f32 with the transposed basis; the gain's is b2a_gain_f32. */
+int b2a_stft_backward_supported(int n_fft, int hop);
+size_t b2a_stft_backward_workspace_bytes(int64_t rows, int64_t T, int n_fft, int hop, int pad, int right_pad,
+                                         int drop_edge);
+int b2a_stft_backward_f32(const float* grad_spec, int64_t rows, int64_t T, int n_fft, int hop, const float* window,
+                          const float* amatrix, int pad, int right_pad, int pad_mode, int drop_edge, float* grad_x,
+                          void* ws, size_t ws_bytes, void* stream);
+size_t b2a_istft_backward_workspace_bytes(int64_t rows, int64_t out_len);
+int b2a_istft_backward_f32(const float* grad_out, int64_t rows, int64_t n_frames, int n_fft, int hop,
+                           const float* window, const float* matrix, int pad_frames, int64_t start, int64_t out_len,
+                           float* grad_spec, void* ws, size_t ws_bytes, void* stream);
+int b2a_mel_backward_f32(const float* stft, int64_t rows, int F, int64_t n_frames, const float* mel_fb,
+                         const int32_t* mel_lo, const int32_t* mel_hi, int n_mels, const int32_t* bin_lo,
+                         const int32_t* bin_hi, int post, float post_eps, float post_power, const float* grad_mel,
+                         float* grad_stft, void* stream);
 
 /* ---- SpecAugment band masks on a complex STFT, in place -------------------------------------------------
  * DSPMixin.mask_frequencies / mask_timesteps (audiotools/core/dsp.py:217-306): cells whose axis value v satisfies
