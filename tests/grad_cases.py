@@ -78,15 +78,57 @@ MEL_LOSS_7SCALE = dict(n_mels=[5, 10, 20, 40, 80, 160, 320], window_lengths=[32,
                        log_weight=1.0, mag_weight=0.0, pow=1.0)
 
 
-def mel_loss(x_mel, y_mel, n_mels, window_lengths, log_weight, mag_weight, pow, clamp_eps=1e-5):
+def mel_loss(x_mel, y_mel, n_mels, window_lengths, log_weight, mag_weight, pow, clamp_eps=1e-5, keep=None):
     """MelSpectrogramLoss.forward (spectral.py:159-192), loss_fn = L1, hop = window // 4, hann, fmin 0, fmax None.
-    x_mel(n_mels, wl, hop) / y_mel(...) return the mel spectrograms of the estimate / the reference."""
+    x_mel(n_mels, wl, hop) / y_mel(...) return the mel spectrograms of the estimate / the reference.  ``keep`` (one
+    boolean mask per scale, see ``fp32_resolution_keep``) drops cells from the log term; the mean still divides by
+    every cell, so the kept cells' gradients are those of the unmasked loss."""
     loss = 0.0
-    for nm, wl in zip(n_mels, window_lengths):
+    for i, (nm, wl) in enumerate(zip(n_mels, window_lengths)):
         xm, ym = x_mel(nm, wl, wl // 4), y_mel(nm, wl, wl // 4)
-        loss = loss + log_weight * F.l1_loss(xm.clamp(clamp_eps).pow(pow).log10(), ym.clamp(clamp_eps).pow(pow).log10())
+        xl, yl = xm.clamp(clamp_eps).pow(pow).log10(), ym.clamp(clamp_eps).pow(pow).log10()
+        if keep is None:
+            loss = loss + log_weight * F.l1_loss(xl, yl)
+        else:
+            loss = loss + log_weight * ((xl - yl).abs() * keep[i]).sum() / xl.numel()
         loss = loss + mag_weight * F.l1_loss(xm, ym)
     return loss
+
+
+def fp32_resolution_keep(x, y, sr, n_mels, window_lengths, pow=2.0, tol=1e-4, clamp_eps=1e-5, **_):
+    """The mel cells of MelSpectrogramLoss whose log-term gradient FP32 arithmetic can resolve, from the float64 mels
+    of x and y: one boolean mask per scale, and the number of cells dropped for each reason.  A cell is dropped when
+      - "sign":  |log10 x_mel - log10 y_mel| <= 2^-20 (four FP32 spacings of log10 values in [2, 4), about the mels'
+                 own FP32 error): the L1 term's sign(x - y) is decided below FP32 resolution.  An FP32 log10 of two mels
+                 3e-7 apart can return the same value, and the cell's gradient is then 0 instead of +-1 / (mel ln10 n);
+      - "clamp": log10 x_mel is within 2^-20 of log10 clamp_eps: the clamp's step lies inside FP32 resolution;
+      - "zero":  a filter of the cell holds a bin with |X_k| / rms_k |X_k| < C u log2(n_fft) / tol (C = 2: the FP32 FFT
+                 error budget of tests/spectral64.py) and that bin carries at least half of the mel: d|X|/dX = X / |X|
+                 is discontinuous at X = 0, so its direction is known to no better than tol.  A frame that reflect
+                 padding makes symmetric (the first and last) has a real spectrum, where such bins are common."""
+    keep, dropped = [], {"sign": 0, "clamp": 0, "zero": 0, "cells": 0}
+    tau = 2.0 ** -20
+    for nm, wl in zip(n_mels, window_lengths):
+        hop = wl // 4
+        fb = torch.from_numpy(np.asarray(AudioSignal.get_mel_filters(sr, wl, nm), dtype=np.float64)).to(x.device)
+        X = stft64(x.double(), wl, hop).abs()
+        xm = (X.transpose(2, -1) @ fb.T).transpose(-1, 2)
+        ym = mel64(y.double(), sr, nm, wl, hop)
+        xl, yl = xm.clamp(clamp_eps).log10(), ym.clamp(clamp_eps).log10()
+        both_clamped = (xm < clamp_eps) & (ym < clamp_eps)  # no gradient either way
+        sign = ((xl - yl).abs() <= tau) & ~both_clamped
+        clamp = (xm.log10() - math.log10(clamp_eps)).abs() <= tau
+        rms = X.pow(2).mean(-2, keepdim=True).sqrt()
+        small = X < (2.0 * 2.0 ** -24 * math.log2(wl) / tol) * rms  # [B, C, F, N]
+        share = ((X * small).transpose(2, -1) @ fb.T).transpose(-1, 2)  # the mel of the small bins
+        zero = share >= 0.5 * xm
+        k = ~(sign | clamp | zero)
+        keep.append(k)
+        dropped["sign"] += int(sign.sum())
+        dropped["clamp"] += int((clamp & ~sign).sum())
+        dropped["zero"] += int((zero & ~sign & ~clamp).sum())
+        dropped["cells"] += k.numel()
+    return keep, dropped
 
 
 def stft_loss(x_mag, y_mag, window_lengths=(2048, 512), clamp_eps=1e-5, pow=2.0, log_weight=1.0, mag_weight=1.0):
@@ -99,9 +141,9 @@ def stft_loss(x_mag, y_mag, window_lengths=(2048, 512), clamp_eps=1e-5, pow=2.0,
     return loss
 
 
-def signal_losses(x: torch.Tensor, y: torch.Tensor, sr: int):
+def signal_losses(x: torch.Tensor, y: torch.Tensor, sr: int, keep=(None, None)):
     """(mel default, 7-scale mel, multi-scale STFT) losses over this package's AudioSignal, each a fresh signal of x
-    (which requires grad) and of y."""
+    (which requires grad) and of y; ``keep``: the cell masks of the two mel losses (``mel_loss``)."""
     def sig_mel(t):
         return lambda nm, wl, hop: AudioSignal(t, sr).mel_spectrogram(nm, window_length=wl, hop_length=hop,
                                                                       window_type="hann")
@@ -113,12 +155,12 @@ def signal_losses(x: torch.Tensor, y: torch.Tensor, sr: int):
             return s.magnitude
         return f
 
-    return (mel_loss(sig_mel(x), sig_mel(y), **MEL_LOSS_DEFAULT),
-            mel_loss(sig_mel(x), sig_mel(y), **MEL_LOSS_7SCALE),
+    return (mel_loss(sig_mel(x), sig_mel(y), **MEL_LOSS_DEFAULT, keep=keep[0]),
+            mel_loss(sig_mel(x), sig_mel(y), **MEL_LOSS_7SCALE, keep=keep[1]),
             stft_loss(sig_mag(x), sig_mag(y)))
 
 
-def oracle_losses(x: torch.Tensor, y: torch.Tensor, sr: int):
+def oracle_losses(x: torch.Tensor, y: torch.Tensor, sr: int, keep=(None, None)):
     """The same three losses through torch.stft in x's precision (float64: the exact reference; float32: the real
     reference's arithmetic)."""
     def o_mel(t):
@@ -127,8 +169,8 @@ def oracle_losses(x: torch.Tensor, y: torch.Tensor, sr: int):
     def o_mag(t):
         return lambda wl, hop: stft64(t, wl, hop).abs()
 
-    return (mel_loss(o_mel(x), o_mel(y), **MEL_LOSS_DEFAULT),
-            mel_loss(o_mel(x), o_mel(y), **MEL_LOSS_7SCALE),
+    return (mel_loss(o_mel(x), o_mel(y), **MEL_LOSS_DEFAULT, keep=keep[0]),
+            mel_loss(o_mel(x), o_mel(y), **MEL_LOSS_7SCALE, keep=keep[1]),
             stft_loss(o_mag(x), o_mag(y)))
 
 
