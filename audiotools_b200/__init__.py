@@ -13,5 +13,6 @@ from .core import STFTParams
 from .core import Meter
 from .core import util
 from . import data
+from . import metrics
 from . import ml
 from .data import transforms

@@ -98,6 +98,11 @@ SIGNATURES = {
                                        c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
     "b2a_mel_backward_f32": (c_int, [c_void_p, c_int64, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                      c_void_p, c_int, c_float, c_float, c_void_p, c_void_p, c_void_p]),
+    "b2a_spectral_loss_supported": (c_int, [c_int, c_int, c_int]),
+    "b2a_spectral_loss_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "b2a_spectral_loss_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_int, c_int, c_int,
+                                      c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_float,
+                                      c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "b2a_istft_supported": (c_int, [c_int, c_int]),
     "b2a_istft_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_int, c_int64, c_int64, c_void_p,
                               c_void_p]),

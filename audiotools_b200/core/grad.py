@@ -102,6 +102,38 @@ class Gain(torch.autograd.Function):
         return _engine().gain(g, ctx.gain), None
 
 
+class SpectralLoss(torch.autograd.Function):
+    """(x, y) [B, C, T] -> one scale of the reference's L1 spectral loss, a 0-dim tensor (``Engine.spectral_loss``: one
+    launch plus the partials' sum).  The forward writes dL/dX (and dL/dY when y requires a gradient) of the two STFTs;
+    the backward is the STFT adjoint of that buffer, scaled by the upstream gradient on the device."""
+
+    @staticmethod
+    def forward(ctx, x, y, n_fft, hop, window, pad, right_pad, pad_mode, drop_edge, mel, clamp_eps, pow, log_weight,
+                mag_weight):
+        loss, gx, gy = _engine().spectral_loss(
+            x, y, n_fft, hop, window, pad=pad, right_pad=right_pad, pad_mode=pad_mode, drop_edge=drop_edge, mel=mel,
+            clamp_eps=clamp_eps, pow=pow, log_weight=log_weight, mag_weight=mag_weight,
+            want_grad_x=ctx.needs_input_grad[0], want_grad_y=ctx.needs_input_grad[1])
+        ctx.geo = (x.shape[-1], n_fft, hop, window, pad, right_pad, pad_mode, drop_edge)
+        ctx.grads = (gx, gy)
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        eng = _engine()
+        T, n_fft, hop, window, pad, right_pad, pad_mode, drop_edge = ctx.geo
+        out = []
+        for gs in ctx.grads:
+            if gs is None:
+                out.append(None)
+                continue
+            gw = eng.stft_backward(gs, T, n_fft, hop, window, pad, right_pad, pad_mode, drop_edge)
+            out.append(eng.gain(gw, g.reshape(1).expand(gw.shape[0])))
+        ctx.grads = None
+        return (out[0], out[1]) + (None,) * 12
+
+
 def wants_grad(t) -> bool:
     return t is not None and t.requires_grad and torch.is_grad_enabled()
 

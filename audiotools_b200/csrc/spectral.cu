@@ -120,30 +120,6 @@ __device__ __forceinline__ void stage_span(const Params& p, float* sp, int row, 
   }
 }
 
-// ---- asynchronous staging (warp kernel): raw x -> shared memory by the TMA engine, so that the copy overlaps
-// the per-CTA table set-up and, later, the previous tile's FFTs; the gain is applied after the (linear) mel
-// projection and the scaled waveform x*g is written back from shared memory.
-// Returns true when the span was handed to the TMA engine (completion on `bar`), false when it was staged with
-// cp.async / plain stores (completion by cp_async_wait_all + the CTA barrier).  The choice is CTA-uniform.
-__device__ __forceinline__ bool stage_span_async(const Params& p, float* sp, int row, int ws, unsigned long long* bar) {
-  const int tid = threadIdx.x, T = p.T, span = p.span;
-  const float* xr = p.x + (size_t)row * (size_t)T;
-  const bool interior = (ws >= 0) && (ws + span <= T);
-  if (interior && ((((uintptr_t)(xr + ws)) & 15) == 0) && ((span & 3) == 0)) {
-    // interior tile: its (FR-1)*hop + n_fft samples are one contiguous, 16 B aligned run of the row -> ONE bulk copy
-    if (tid == 0) tma_load_1d(sp, xr + ws, (unsigned)span * 4u, bar);
-    return true;
-  } else if (interior) {
-    for (int i = tid; i < span; i += (int)blockDim.x) sp[i] = __ldg(xr + ws + i);
-  } else {
-    for (int i = tid; i < span; i += (int)blockDim.x) {
-      const int u = src_index(ws + i, T, p.pad, p.right_pad, p.pad_mode, p.center);
-      sp[i] = (u >= 0) ? __ldg(xr + u) : 0.f;
-    }
-  }
-  return false;
-}
-
 // y_out[w] = x[w] * g for the samples this CTA owns (requires pad == drop_edge == 0, so span[i] = x[ws+i])
 __device__ __forceinline__ void writeback_scaled(const Params& p, const float* sp, int row, int tile, int n0, int FR,
                                                  int ws, float g) {
@@ -676,7 +652,7 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
   }
 }
 
-static int num_sms() {
+int num_sms() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;

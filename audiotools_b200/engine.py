@@ -239,6 +239,55 @@ class Engine:
         self.launches += 1
         return out
 
+    # ------------------------------------------------------------------ spectral L1 losses (csrc/loss.cu)
+    def spectral_loss_supported(self, n_fft: int, hop: int, n_mels: int = 0) -> bool:
+        return bool(self.lib.b2a_spectral_loss_supported(int(n_fft), int(hop), int(n_mels)))
+
+    def spectral_loss(self, x: torch.Tensor, y: torch.Tensor, n_fft: int, hop: int, window: torch.Tensor, pad: int = 0,
+                      right_pad: int = 0, pad_mode: str = "reflect", drop_edge: int = 0, mel=None,
+                      clamp_eps: float = 1e-5, pow: float = 2.0, log_weight: float = 1.0, mag_weight: float = 1.0,
+                      want_grad_x: bool = False, want_grad_y: bool = False):
+        """One scale of the reference's L1 spectral losses (MultiScaleSTFTLoss, or MelSpectrogramLoss with
+        ``mel=(fb, lo, hi)``) between x and y [B, C, T] -> (loss, dL/dX, dL/dY): a 0-dim float32 tensor and, when asked
+        for, the gradients wrt the two STFTs [B, C, F, N] complex64 (``stft_backward`` takes them to the waveforms)."""
+        x = self._prep(x, "x")
+        y = self._prep(y, "y")
+        assert x.ndim == 3 and x.shape == y.shape, (x.shape, y.shape)
+        B, C, T = x.shape
+        if pad_mode not in _lib.PAD_MODES:
+            raise NotImplementedError(f"padding_type {pad_mode!r} (supported: {sorted(_lib.PAD_MODES)})")
+        window = self._prep(window, "window")
+        assert window.numel() == n_fft
+        N = self.num_frames(T, n_fft, hop, pad, right_pad, drop_edge)
+        F = n_fft // 2 + 1
+        fb = lo = hi = blo = bhi = None
+        n_mels = 0
+        if mel is not None:
+            fb, lo, hi = mel
+            fb = self._prep(fb, "mel_fb")
+            assert fb.shape[1] == F, (fb.shape, F)
+            n_mels = fb.shape[0]
+            lo = self._prep(lo, "mel_lo", torch.int32)
+            hi = self._prep(hi, "mel_hi", torch.int32)
+            blo, bhi = self._bin_table(lo, hi, F)
+        nbytes = int(self.lib.b2a_spectral_loss_workspace_bytes(int(n_fft), int(hop), n_mels))
+        if nbytes == 0:
+            raise NotImplementedError(f"spectral_loss: window_length {n_fft} hop {hop} n_mels {n_mels}")
+        dev = x.device
+        ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        gx = torch.empty(B, C, F, max(N, 1), dtype=torch.complex64, device=dev) if want_grad_x else None
+        gy = torch.empty(B, C, F, max(N, 1), dtype=torch.complex64, device=dev) if want_grad_y else None
+        rc = self.lib.b2a_spectral_loss_f32(
+            _dptr(x), _dptr(y), B * C, T, int(n_fft), int(hop), _dptr(window), int(pad), int(right_pad),
+            _lib.PAD_MODES[pad_mode], int(drop_edge), _dptr(fb), _dptr(lo), _dptr(hi), _dptr(blo), _dptr(bhi), n_mels,
+            float(clamp_eps), float(pow), float(log_weight), float(mag_weight), _dptr(loss),
+            _dptr(torch.view_as_real(gx)) if gx is not None else None,
+            _dptr(torch.view_as_real(gy)) if gy is not None else None, _dptr(ws), nbytes, self._stream(x))
+        self.lib.check(rc)
+        self.launches += 2
+        return loss, gx, gy
+
     # ------------------------------------------------------------------ dense DFT (any window length)
     @staticmethod
     def fft_window_length(n_fft: int) -> bool:

@@ -3,7 +3,7 @@
 bench.py, which measures configs[1]).  One JSON line per config: device-resident throughput (CUDA events,
 >= 3 warm-ups, inputs larger than L2 or rotated), algorithmic bytes, and the CPU oracle on a bounded sample.
 
-    python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,largewin,grad,gate,masked] [--no-cpu]
+    python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,largewin,grad,loss,gate,masked] [--no-cpu]
 
 Multi-GPU (BASELINE configs[3] = 512 items on 4 GPUs, configs[4] = 2048 items on 8 GPUs): one process per GPU,
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 4 --master-addr 127.0.0.1 --master-port 29511 \
@@ -371,6 +371,94 @@ def main():
               "frac_of_hbm_peak": alg / ms_bwd / 1e6 / peak, "launches_total": eng.launches,
               "gpu": torch.cuda.get_device_name(LOCAL), "power_limit": plim})
         del xb, xg, xt, mel, melt, gm
+
+    if "loss" in only:  # audiotools_b200.metrics: fused losses (csrc/loss.cu) vs the reference's code vs torch autograd
+        import subprocess
+
+        import torch.nn.functional as F
+
+        from audiotools_b200 import metrics
+
+        sr = 44100
+        # the reference's code (ref:audiotools/metrics/spectral.py:70-95, 159-192) over this package's AudioSignal, and
+        # the same arithmetic on torch.stft (cuFFT) + abs + matmul (cuBLAS)
+        cfgs = {"mel_default": dict(n_mels=[150, 80], window_lengths=[2048, 512]),
+                "stft_default": dict(window_lengths=[2048, 512]),
+                "mel_7scale": dict(n_mels=[5, 10, 20, 40, 80, 160, 320],
+                                   window_lengths=[32, 64, 128, 256, 512, 1024, 2048], mag_weight=0.0, pow=1.0,
+                                   mel_fmin=[0.0] * 7, mel_fmax=[None] * 7)}
+        fbs = {}
+
+        def t_mag(x, wl):
+            w = AudioSignal.get_window("hann", wl, x.device)
+            X = torch.stft(x.reshape(-1, x.shape[-1]), wl, wl // 4, window=w, center=True, return_complex=True)
+            return X.reshape(*x.shape[:2], *X.shape[1:]).abs()
+
+        def composed(x, y, cfg, on_torch):
+            loss, mw, pw = 0.0, cfg.get("mag_weight", 1.0), cfg.get("pow", 2.0)
+            for i, wl in enumerate(cfg["window_lengths"]):
+                nm = cfg["n_mels"][i] if "n_mels" in cfg else None
+                if on_torch:
+                    a, b = t_mag(x, wl), t_mag(y, wl)
+                    if nm is not None:
+                        if (nm, wl) not in fbs:
+                            fbs[nm, wl] = torch.from_numpy(
+                                np.asarray(AudioSignal.get_mel_filters(sr, wl, nm), np.float32)).to(dev)
+                        a = (a.transpose(2, -1) @ fbs[nm, wl].T).transpose(-1, 2)
+                        b = (b.transpose(2, -1) @ fbs[nm, wl].T).transpose(-1, 2)
+                elif nm is not None:
+                    a = AudioSignal(x, sr).mel_spectrogram(nm, window_length=wl, hop_length=wl // 4)
+                    b = AudioSignal(y, sr).mel_spectrogram(nm, window_length=wl, hop_length=wl // 4)
+                else:
+                    sa, sb = AudioSignal(x, sr), AudioSignal(y, sr)
+                    sa.stft(wl, wl // 4, "hann")
+                    sb.stft(wl, wl // 4, "hann")
+                    a, b = sa.magnitude, sb.magnitude
+                loss = loss + F.l1_loss(a.clamp(1e-5).pow(pw).log10(), b.clamp(1e-5).pow(pw).log10())
+                loss = loss + mw * F.l1_loss(a, b)
+            return loss
+
+        def path(name, cfg):
+            if name == "fused":
+                mod = (metrics.MelSpectrogramLoss if "n_mels" in cfg else metrics.MultiScaleSTFTLoss)(**cfg)
+                return lambda x, y: mod(AudioSignal(x, sr), AudioSignal(y, sr))
+            return lambda x, y: composed(x, y, cfg, name == "torch")
+
+        try:
+            plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(LOCAL)],
+                                  capture_output=True, text=True, timeout=30).stdout.strip()
+        except Exception:  # noqa: BLE001 (informational field)
+            plim = "unknown"
+        g = torch.Generator().manual_seed(0)
+        for size, (B, C, secs, steps) in {"16x1chx1s": (16, 1, 1, 20), "64x2chx10s": (64, 2, 10, 5)}.items():
+            x = (0.1 * torch.randn(B, C, secs * sr, generator=g)).to(dev)
+            y = (0.1 * torch.randn(B, C, secs * sr, generator=g)).to(dev)
+            res = {}
+            for lname, cfg in cfgs.items():
+                for pname in ("fused", "composed", "torch"):
+                    fn = path(pname, cfg)
+
+                    def fwd_bwd():
+                        xg = x.clone().requires_grad_()
+                        fn(xg, y).backward()
+
+                    def fwd():
+                        with torch.no_grad():
+                            fn(x, y)
+
+                    for mode, step in (("fwd_bwd", fwd_bwd), ("fwd_nograd", fwd)):
+                        torch.cuda.synchronize()
+                        torch.cuda.empty_cache()
+                        torch.cuda.reset_peak_memory_stats(dev)
+                        base = torch.cuda.memory_allocated(dev)
+                        ms = timed(step, steps=steps)
+                        res[f"{lname}_{pname}_{mode}_ms"] = ms
+                        res[f"{lname}_{pname}_{mode}_peak_MB"] = (torch.cuda.max_memory_allocated(dev) - base) / 2**20
+            emit({"config": f"loss: forward+backward / no_grad forward of the reference's spectral losses at {size}@44.1k; "
+                            "fused = audiotools_b200.metrics (csrc/loss.cu), composed = the reference's code over "
+                            "AudioSignal, torch = the same arithmetic on torch.stft; peak_MB above the inputs",
+                  **res, "gpu": torch.cuda.get_device_name(LOCAL), "power_limit": plim})
+            del x, y
 
     if "gate" in only:  # SpectralGate (csrc/specmask.cu) at 64 x 2ch x 10 s: stft x2 + gate + istft
         from audiotools_b200.ml.layers import SpectralGate

@@ -185,6 +185,29 @@ int b2a_mel_backward_f32(const float* stft, int64_t rows, int F, int64_t n_frame
                          const int32_t* bin_hi, int post, float post_eps, float post_power, const float* grad_mel,
                          float* grad_stft, void* stream);
 
+/* ---- spectral L1 losses with their gradient (csrc/loss.cu) --------------------------------------------------------
+ * One scale of MultiScaleSTFTLoss / MelSpectrogramLoss with loss_fn = nn.L1Loss() (audiotools/metrics/spectral.py:70-95,
+ * 159-192) for the estimate x and the target y [rows, T] of the same geometry (the framing arguments of
+ * b2a_spectral_f32, no gain), with lg(v) = log10(max(v, clamp_eps)^pow):
+ *   mel_fb == NULL   L = log_weight mean |lg|X| - lg|Y|| + mag_weight mean ||X| - |Y||        over [rows, F, n_frames]
+ *   mel_fb != NULL   the same over mel = fb |.| [rows, n_mels, n_frames]; mel_lo / mel_hi: the band table of
+ *                    b2a_spectral_f32, bin_lo / bin_hi: the transposed one of b2a_mel_backward_f32.
+ *   loss_out         one device float, written by a second one-warp launch that adds per-CTA partials in a fixed order
+ *                    (float64): no atomics, reruns are bit-identical.
+ *   grad_x / grad_y  nullable [rows, F, n_frames] (re,im): dL/dX, dL/dY of the two STFTs with torch's derivatives
+ *                    (sign(0) = 0, the gradient passes the clamp where v >= clamp_eps, X / |X| is 0 at X = 0); feed them
+ *                    to b2a_stft_backward_f32.  A weight of 0 removes its term and its gradient.
+ *   b2a_spectral_loss_supported  (n_fft, hop, n_mels; 0 for the STFT loss): n_fft a power of two in [64, 2048],
+ *                                1 <= hop <= n_fft, and the launch fits shared memory.
+ *   workspace        b2a_spectral_loss_workspace_bytes(n_fft, hop, n_mels) bytes, 8-byte aligned (the partials). */
+int b2a_spectral_loss_supported(int n_fft, int hop, int n_mels);
+size_t b2a_spectral_loss_workspace_bytes(int n_fft, int hop, int n_mels);
+int b2a_spectral_loss_f32(const float* x, const float* y, int64_t rows, int64_t T, int n_fft, int hop,
+                          const float* window, int pad, int right_pad, int pad_mode, int drop_edge, const float* mel_fb,
+                          const int32_t* mel_lo, const int32_t* mel_hi, const int32_t* bin_lo, const int32_t* bin_hi,
+                          int n_mels, float clamp_eps, float pow, float log_weight, float mag_weight, float* loss_out,
+                          float* grad_x, float* grad_y, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- SpecAugment band masks on a complex STFT, in place -------------------------------------------------
  * DSPMixin.mask_frequencies / mask_timesteps (audiotools/core/dsp.py:217-306): cells whose axis value v satisfies
  * lo[item] <= v < hi[item] (float32, as the reference compares) become fill = val * exp(1j * val); all other
