@@ -371,6 +371,21 @@ static int launch(Params& p, void* stream) {
 // MODE 0: no STFT output (mel / log-mel only: the bench path; the per-bin store code is compiled out);
 // MODE 1: STFT-only launch that parks the complex frames in shared memory and writes them transposed;
 // MODE 2: generic (STFT straight from registers, with or without mel).
+
+// B2A_K1_PROBE (tests/probes/k1_phase_probe.py only): lane 0 of every warp stamps clock64() at the 11 phase boundaries
+// of its first K1_PROBE_TILES tiles.  Without the macro the stamps compile to nothing.
+#ifdef B2A_K1_PROBE
+__device__ unsigned long long* g_k1_probe;  // [grid][8 warps][K1_PROBE_TILES][11] clock64 stamps of lane 0
+#define K1_PROBE_TILES 64
+#define K1_STAMP(k)                                                                                   \
+  do {                                                                                                \
+    if (g_k1_probe && lane == 0 && it_probe < K1_PROBE_TILES)                                         \
+      g_k1_probe[(((size_t)blockIdx.x * 8 + warp) * K1_PROBE_TILES + it_probe) * 11 + (k)] = clock64(); \
+  } while (0)
+#else
+#define K1_STAMP(k) do { } while (0)
+#endif
+
 template <int LOG2N, int MODE>
 __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
   using PL = WPlan<LOG2N>;
@@ -383,7 +398,6 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
   float2* tw = reinterpret_cast<float2*>(smem + p.off_tw);   // [NTW][LPF]
   float2* ut = reinterpret_cast<float2*>(smem + p.off_ut);   // [16][LPF]
   float* xbs = reinterpret_cast<float*>(smem + p.off_buf);   // [G][XB]
-  float* melt = reinterpret_cast<float*>(smem + p.off_mel);  // [n_mels][FR+1]
   float* mpk = reinterpret_cast<float*>(smem + p.off_mpk);
   int4* mseg = reinterpret_cast<int4*>(smem + p.off_mseg);   // (offset, lo4, n4, -)
 
@@ -454,6 +468,10 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
   float* xb = xbs + (warp * FPW + fw) * p.xb_stride;
   const int src_lane = (lane & ~(LPF - 1)) | ((LPF - l) & (LPF - 1));  // holder of Z[N - k]
 
+#ifdef B2A_K1_PROBE
+  int it_probe = 0;
+#endif
+  bool first = true;
 #pragma unroll 1
   for (; t < total_tiles; t += gridDim.x) {
     const int row = t / p.n_tiles, tile = t - row * p.n_tiles;
@@ -461,11 +479,24 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
     const int ws = (n0 + p.drop_edge) * hop + p.origin + (p.row_origin ? __ldg(p.row_origin + row) : 0);
     const float g = p.gain ? __ldg(p.gain + row / p.rows_per_gain) : 1.0f;
     const float ga = fabsf(g);
+    K1_STAMP(0);
     // this tile's span was issued by the previous iteration (or the prologue)
     if (by_tma) { mbar_wait(&s_bar, tma_parity); tma_parity ^= 1u; }
+    K1_STAMP(1);
+    // a TMA span is visible to each thread once its wait returns; a span staged with plain stores (and, on the first
+    // tile, the tables) needs the CTA barrier.  Nothing else is ordered here: the |X| slots the previous tile's mel
+    // phase reads are rewritten only after this tile's barrier before its TMA issue.  (The simulator's copy is
+    // synchronous and its wait a no-op, so there the barrier is what orders the copy before the reads.)
+#ifdef B2A_SIM
     __syncthreads();
+#else
+    if (!by_tma || first) __syncthreads();
+#endif
+    first = false;
+    K1_STAMP(2);
     if (p.y_out) writeback_scaled(p, sp, row, tile, n0, FR, ws, g);  // (sp is re-filled only after the barrier
                                                                       //  inside the last round, below)
+    K1_STAMP(3);
 
 #pragma unroll 1
     for (int rd = 0; rd < FR / G; ++rd) {
@@ -500,6 +531,7 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
           z[m + 16] = make_float2(fmaf(-sx, wx, ax), fmaf(-sy, wy, ay));
         }
       }
+      K1_STAMP(4);
       if (rd == FR / G - 1) {
         // every warp holds its last frame in registers: the span buffer is dead, so the next tile's
         // samples stream in (one TMA bulk copy) underneath this round's FFTs and mel projection
@@ -513,6 +545,7 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
               &s_bar);
         }
       }
+      K1_STAMP(5);
       warp_fft<LOG2N, true>(z, xb, tw, l);  // z[m] = Z[l + LPF m]
 
       // ---- untangle -> real-FFT bins k = l + LPF m (m < 16) and N - k ; magnitudes into xb
@@ -562,10 +595,17 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
       __syncwarp();
 
     }
+    K1_STAMP(6);
 
     // ---- mel phase of the tile: |X| of all FR frames sit in the xb slots (slot = frame within the tile)
+    //      Each lane stores its cells straight from registers: the 8 lanes of a filter write 8 consecutive frames (the
+    //      same 32-byte runs a staged tile store would write), so no tile buffer, and no barrier after the projection:
+    //      the next tile's barrier before its TMA issue already orders these |X| reads before the slots are rewritten.
+    const int nf = min(FR, p.n_frames - n0);
+    float* mo = p.mel_out ? p.mel_out + (size_t)row * p.n_mels * p.n_frames + n0 : nullptr;
     if (p.mel_out) {
       __syncthreads();
+      K1_STAMP(7);
       const int fl = lane & 7, jq = lane >> 3;
       const float lscale = p.post_power * 0.30102999566398120f;  // log10(c^power) = power * log10(2) * log2(c)
       if (packed) {
@@ -589,7 +629,7 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
               float acc = ((a01.x + a01.y) + (a23.x + a23.y)) * ga;
               if (p.post == B2A_POST_LOG10) acc = lscale * fast_log2(fmaxf(acc, p.post_eps));
               else if (p.post == B2A_POST_LN) acc = logf(acc + p.post_eps);
-              melt[mm * (FR + 1) + f] = acc;
+              if (f < nf) mo[(size_t)mm * p.n_frames + f] = acc;
             }
           } else {  // a zero-padded row would read past the slot: clamp the index
             const int lim = PL::XB - 4;
@@ -606,7 +646,7 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
               float acc = (a0 + a1) * ga;
               if (p.post == B2A_POST_LOG10) acc = lscale * fast_log2(fmaxf(acc, p.post_eps));
               else if (p.post == B2A_POST_LN) acc = logf(acc + p.post_eps);
-              melt[mm * (FR + 1) + f] = acc;
+              if (f < nf) mo[(size_t)mm * p.n_frames + f] = acc;
             }
           }
         }
@@ -622,14 +662,15 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
             acc *= ga;
             if (p.post == B2A_POST_LOG10) acc = lscale * fast_log2(fmaxf(acc, p.post_eps));
             else if (p.post == B2A_POST_LN) acc = logf(acc + p.post_eps);
-            melt[mm * (FR + 1) + f] = acc;
+            if (f < nf) mo[(size_t)mm * p.n_frames + f] = acc;
           }
         }
       }
     }
 
-    __syncthreads();  // all frames of the tile are done: melt complete, sp free for the next tile
+    K1_STAMP(8);
     if constexpr (STAGED) {
+      __syncthreads();  // all frames of the tile are parked in their slots
       // transposed write of the tile's complex frames: 32 lanes = 32/FR bins x FR consecutive frames, i.e. runs of
       // FR * 8 bytes instead of one 8-byte store per sector (the layout is [rows, F, n_frames], frame fastest)
       const int nf = min(FR, p.n_frames - n0);
@@ -640,15 +681,11 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
       }
       // (the next iteration's barrier, after its span wait, orders these reads before the slots are reused)
     }
-    if (p.mel_out) {
-      const int nf = min(FR, p.n_frames - n0);
-      float* o = p.mel_out + (size_t)row * p.n_mels * p.n_frames + n0;
-      for (int i = tid; i < p.n_mels * FR; i += 256) {
-        const int m = i / FR, f = i - m * FR;
-        if (f < nf) o[(size_t)m * p.n_frames + f] = melt[m * (FR + 1) + f];
-      }
-      __syncthreads();  // melt is rewritten by the next tile
-    }
+    K1_STAMP(9);
+    K1_STAMP(10);
+#ifdef B2A_K1_PROBE
+    ++it_probe;
+#endif
   }
 }
 
@@ -661,6 +698,10 @@ int num_sms() {
   }
   return n;
 }
+
+#ifdef B2A_K1_PROBE
+static int g_k1_last[3];  // occupancy (CTAs / SM), grid and dynamic shared memory of the last n_fft 2048 mel launch
+#endif
 
 template <int LOG2N>
 static int launch_warp(Params& p, void* stream) {
@@ -681,7 +722,7 @@ static int launch_warp(Params& p, void* stream) {
   }
   p.off_buf = o; o = align16(o + PL::G * p.xb_stride * 4);
   p.off_mag = o;
-  p.off_mel = o; o = align16(o + (p.mel_out ? p.n_mels * (PL::FR + 1) * 4 : 0));
+  p.off_mel = o;  // (mel cells are stored from registers: no tile buffer)
   const int base = o;
   p.off_mpk = o; p.off_mseg = o;
   if (p.mel_out && p.mel_packed_len > 0) {
@@ -704,6 +745,9 @@ static int launch_warp(Params& p, void* stream) {
   if (per_sm < 1) per_sm = 1;
   const int64_t cap = (int64_t)num_sms() * per_sm;
   const unsigned grid = (unsigned)(total < cap ? total : cap);
+#ifdef B2A_K1_PROBE
+  if (LOG2N == 10 && !p.stft_out) { g_k1_last[0] = per_sm; g_k1_last[1] = (int)grid; g_k1_last[2] = o; }
+#endif
   B2A_LAUNCH(kern, dim3(grid), dim3(256), (size_t)o, stream, p);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
@@ -790,3 +834,17 @@ extern "C" int b2a_spectral_f32(const float* x, int64_t rows, int64_t T, int n_f
   }
   return b2a::fail(B2A_E_UNSUPPORTED, "spectral: n_fft %d", n_fft);
 }
+
+#ifdef B2A_K1_PROBE
+// Phase-clock probe of spectral_warp_kernel<10, *> (tests/probes/k1_phase_probe.py): not part of include/b2a.h and
+// compiled only with -DB2A_K1_PROBE.  `buf` (device, or null to stop recording): [grid][8][K1_PROBE_TILES][11] u64.
+extern "C" int b2a_k1_probe_set(void* buf) {
+  B2A_CUDA_OK(cudaMemcpyToSymbol(b2a::spectral::g_k1_probe, &buf, sizeof(buf)));
+  return B2A_OK;
+}
+extern "C" int b2a_k1_probe_tiles() { return K1_PROBE_TILES; }
+// (occupancy in CTAs per SM, grid, dynamic shared memory bytes) of the last n_fft 2048 mel launch
+extern "C" void b2a_k1_probe_last(int* out) {
+  for (int i = 0; i < 3; ++i) out[i] = b2a::spectral::g_k1_last[i];
+}
+#endif
