@@ -96,24 +96,6 @@ __device__ __forceinline__ float2 mul2(float2 a, float2 b) {
 }
 __device__ __forceinline__ float2 neg2(float2 a) { return make_float2(-a.x, -a.y); }
 __device__ __forceinline__ float2 bcast2(float v) { return make_float2(v, v); }
-// acquire / release on a 32-bit flag in global memory (decoupled look-back)
-__device__ __forceinline__ void st_release(int* p, int v) {
-#ifdef B2A_SIM
-  __atomic_store_n(p, v, __ATOMIC_RELEASE);
-#else
-  asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-#endif
-}
-__device__ __forceinline__ int ld_acquire(const int* p) {
-#ifdef B2A_SIM
-  cusim::yield();  // polled in spin loops
-  return __atomic_load_n(p, __ATOMIC_ACQUIRE);
-#else
-  int v;
-  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-#endif
-}
 
 // ---------------------------------------------------------------------------------------
 // TMA bulk copy (1-D, global -> shared) completing on an mbarrier: one elected thread arms the barrier with

@@ -18,8 +18,6 @@
 //   3. Y[row][f][b]    = sum_p H[f][p] * X[f][b-p]       a complex FIR along the block index, per bin
 //   4. out[b*1024 ..]  = irFFT_2048(Y[.][b])[1024:]      warp-per-block inverse FFT + epilogue
 // Rows are processed in chunks so that X and Y stay L2-friendly (<= 256 MB of workspace).
-#include <stdlib.h>
-
 #include "b2a_common.h"
 #include "fft_warp.cuh"
 #include "spectral_internal.h"
@@ -226,16 +224,8 @@ struct Layout {
 };
 static inline size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
 // Spectra of one chunk of rows (X and, with several partitions, Y): rows are processed in chunks whose spectra take at
-// most 256 MB, which bounds the workspace; B2A_FFTCONV_WS_MB overrides the budget for experiments.
-static size_t chunk_budget_mb() {
-  static size_t mb = 0;
-  if (mb == 0) {
-    const char* e = getenv("B2A_FFTCONV_WS_MB");
-    const long v = e ? atol(e) : 0;
-    mb = (v >= 8 && v <= 65536) ? (size_t)v : 256;
-  }
-  return mb;
-}
+// most 256 MB, which bounds the workspace.
+constexpr size_t CHUNK_BUDGET_MB = 256;
 
 static Layout layout(int64_t rows, int64_t T, int64_t n_filt, int64_t L) {
   Layout w;
@@ -244,7 +234,7 @@ static Layout layout(int64_t rows, int64_t T, int64_t n_filt, int64_t L) {
   w.NBX = w.NB + w.P - 1;
   // one partition: the product is formed inside the inverse kernel, Y is never written (see run())
   const size_t per_row = (size_t)NF * (w.NBX + (w.P > 1 ? w.NB : 0)) * 8;
-  int64_t chunk = (int64_t)((chunk_budget_mb() << 20) / per_row);
+  int64_t chunk = (int64_t)((CHUNK_BUDGET_MB << 20) / per_row);
   if (chunk < 1) chunk = 1;
   if (chunk > rows) chunk = rows;
   if (chunk > 65535) chunk = 65535;

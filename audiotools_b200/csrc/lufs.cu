@@ -5,68 +5,63 @@
 // approximation the reference falls back to on CUDA (:69-100) -- followed by the 400 ms / 75 %
 // block energies (:164-174, 214) and the two-pass gating (:208-247).
 //
-// Kernel 1  kweight_energy_kernel   (HBM-bound: reads x exactly once, 4 B/sample)
-//   The cascade of NS biquads is a linear recurrence with a 2*NS-dim state.  Each row is cut
-//   into tiles of 256 threads x 32 samples.  Every thread runs the float32 direct-form-I
-//   recursion over its 32 samples from a ZERO state (phase A); the per-chunk end states are
-//   combined with an affine scan (state' = A^32 state + e): warp shuffles, then warp totals,
-//   then a decoupled look-back across the tiles of the row (exact carry, no truncation of the
-//   38 Hz high-pass tail whose pole radius is 0.9946 @44.1k).  The look-back runs in a ninth
-//   "carry" warp concurrently with phase A; tile records are 8-byte {value, tag} words, so one
-//   round trip fetches and validates a predecessor's state.  With its true start state each
-//   thread re-runs the recursion (phase B) and accumulates y^2 into "elementary interval" bins:
+// Kernel 1  kweight_energy_warp_kernel   (HBM-bound: 4 B/sample, plus the warm-up reads)
+//   The cascade of NS biquads is a linear recurrence with a 2*NS-dim state.  A row is cut into RUNS of run_len
+//   consecutive segments (segment = 32 lanes x L2 = 64 samples = 2048 samples); a WARP owns a run and walks it segment
+//   by segment, with no CTA barrier and no inter-warp communication: samples -> warp-private, double-buffered
+//   shared-memory window (cp.async; the next segment lands underneath the arithmetic of the current one), zero-state
+//   end state of every lane chunk (a 66-tap linear map read from the window), affine shuffle scan over the 32 chunks
+//   (state' = A^64 state + e), true lane start states from the state carried in registers, float32 DF-I recursion
+//   (second read of the window), y^2 into "elementary interval" bins:
 //   with K = q*stride + r, interval A_j = [j*stride, j*stride+r), B_j = [j*stride+r, (j+1)*stride),
 //   so that block i = sum_{j=i}^{i+q-1}(A_j + B_j) + A_{i+q} -- bit-exact block indexing for any
 //   rate (K is not always 4*stride, e.g. 11025 Hz).  Warp partials are added into float64 bins.
-// Kernel 2  lufs_gate_kernel        (tiny: one CTA per item)
+//
+//   The state entering a run comes from a WARM-UP, not from an exact carry across runs (which would need a serial
+//   hand-off from the warp of the previous run, or a second pass over x): the warp first runs the carry part (no
+//   energies) over the n_warm segments in front of its run, starting from zero.  The K-weighting poles have radius
+//   rho < 1 (0.9946 for the 38 Hz high-pass at 44.1 kHz), so whatever happened before the warm-up reaches the run
+//   attenuated by rho^(n_warm * 2048); the host picks n_warm with rho^(n_warm * 2048) <= 2^-40 (3 segments at
+//   44.1 kHz, 18 % extra reads at run_len 17).  That bound is five orders of magnitude below the rounding noise the
+//   float32 recursion itself carries (each step rounds at 6e-8 |y| and the feedback amplifies it by ~1/(1 - rho)),
+//   i.e. the results are those of the exact carry to float32 rounding; only a row whose level drops by more than
+//   2^40 across one warm-up can tell the two apart.
+// Kernel 2  lufs_gate_kernel             (tiny: one CTA per item)
 //   z -> l -> absolute gate -> relative gate -> LUFS, with the reference's dtypes (float32 z,
 //   float64 logs) and its NaN / inf scrubbing; optionally max(.,-70) and normalize()'s gain.
-#include <stdlib.h>
-
 #include "b2a_common.h"
 
 namespace b2a {
 namespace lufs {
 
-constexpr int L = 32;              // samples per thread chunk
-constexpr int WORKERS = 256;       // filter threads per CTA
-constexpr int THREADS = WORKERS + 32;  // + one carry warp (decoupled look-back)
-constexpr int NW = WORKERS / 32;   // worker warps per CTA
-constexpr int TILE = L * WORKERS;  // samples per tile (8192)
-constexpr int CH = 36;             // shared-memory words per 32-sample chunk: 16 B aligned, conflict-free LDS.128
+constexpr int L2 = 64;              // samples per lane
+constexpr int SEG = 32 * L2;        // samples per warp segment
+constexpr int CHS = L2 + 4;         // shared-memory words per lane chunk: 16 B aligned, conflict-free LDS.128
+constexpr int WPB = 12;             // warps per CTA (one CTA per SM: 12 x 17 KB of windows)
+constexpr int NBUF = 2;             // windows per warp: the next segment lands underneath the arithmetic
+constexpr int BUF = 32 * CHS;       // floats per window
 constexpr int MAX_STAGES = 2;
+// Unit of the input range b2a_lufs_f32 accepts: rows shorter than 2^31 - 2 TILE samples (every sample index the
+// kernels form, including the segment that runs past a row's end, fits an int), fewer than 2^31 tiles per batch.
+constexpr int TILE = 8192;
 
 template <int NS>
 struct Coef {  // float32-rounded, a0-normalised, stage gain folded into b
   float b0[NS], b1[NS], b2[NS], a1[NS], a2[NS];
 };
 
-template <int NS>
-struct Tables {
-  static constexpr int D = 2 * NS;
-  float Mlane[32][D * D];     // A^(L*l), l = 0..31   (chunk-start state from the warp carry)
-  float Mscan[5][D * D];      // A^(L*2^k)            (warp shuffle scan)
-  float MwPow[NW + 1][D * D]; // A^(L*32*v), v = 0..NW (carry of warp v's total into later warps)
-  float Mtile[D * D];         // A^(TILE)             (look-back across tiles)
-  float Wa[L + 2][D];         // zero-state end state of a chunk as a linear map of its 34 inputs (phase A)
-};
-
 __host__ __device__ inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 struct WsLayout {
-  size_t ticket, recs, bins, zeroed_bytes, tables, zws, prefix, total;
+  size_t bins, zeroed_bytes, zws, total;
 };
-// tile records: per (tile,row) 2*D 8-byte words {float value, uint tag}: [0,D) aggregate, [D,2D) inclusive
-__host__ inline WsLayout ws_layout(int64_t rows, int64_t ntile, int64_t nbins, int64_t nblk, int D) {
+// the interval bins are accumulated with atomics and come first: the call zeroes [0, zeroed_bytes)
+__host__ inline WsLayout ws_layout(int64_t rows, int64_t nbins, int64_t nblk) {
   WsLayout w;
   size_t o = 0;
-  w.ticket = o; o += 256;
-  w.recs = o; o = align256(o + sizeof(unsigned long long) * 2 * D * rows * ntile);
   w.bins = o; o = align256(o + sizeof(double) * rows * nbins);
   w.zeroed_bytes = o;
-  w.tables = o; o = align256(o + sizeof(Tables<MAX_STAGES>));
   w.zws = o; o = align256(o + sizeof(float) * rows * nblk);
-  w.prefix = o;
   w.total = o;
   return w;
 }
@@ -87,7 +82,7 @@ __host__ __device__ __forceinline__ F cascade_step(const F (&b0)[NS], const F (&
 }
 
 // ---------------------------------------------------------------------------------------------
-// tables: state-transition matrix powers and the phase-A map, float64 on the host (a few microseconds),
+// tables: state-transition matrix powers and the lane-chunk end-state map, float64 on the host (a few microseconds),
 // handed to the kernel as a __grid_constant__ parameter -- no set-up launch, no device buffer
 // ---------------------------------------------------------------------------------------------
 template <int D>
@@ -103,385 +98,7 @@ static void matmul(const double* a, const double* b, double* c) {
 }
 
 template <int NS>
-static void build_tables(const Coef<NS>& cf, Tables<NS>* tb) {
-  constexpr int D = 2 * NS;
-  double b0[NS], b1[NS], b2[NS], a1[NS], a2[NS];
-  for (int s = 0; s < NS; ++s) {
-    b0[s] = cf.b0[s]; b1[s] = cf.b1[s]; b2[s] = cf.b2[s]; a1[s] = cf.a1[s]; a2[s] = cf.a2[s];
-  }
-  double A[D * D];
-  for (int k = 0; k < D; ++k) {  // column k = one zero-input step applied to basis vector e_k
-    double y1[NS], y2[NS];
-    for (int s = 0; s < NS; ++s) { y1[s] = (k == 2 * s) ? 1.0 : 0.0; y2[s] = (k == 2 * s + 1) ? 1.0 : 0.0; }
-    cascade_step<NS, double>(b0, b1, b2, a1, a2, 0.0, 0.0, 0.0, y1, y2);
-    for (int s = 0; s < NS; ++s) { A[(2 * s) * D + k] = y1[s]; A[(2 * s + 1) * D + k] = y2[s]; }
-  }
-  double P[D * D];  // A^L
-  for (int i = 0; i < D * D; ++i) P[i] = A[i];
-  for (int l = 1; l < L; l <<= 1) matmul<D>(P, P, P);
-  double Q[D * D];
-  for (int i = 0; i < D * D; ++i) Q[i] = (i / D == i % D) ? 1.0 : 0.0;
-  for (int l = 0; l < 32; ++l) {
-    for (int i = 0; i < D * D; ++i) tb->Mlane[l][i] = (float)Q[i];
-    matmul<D>(P, Q, Q);
-  }
-  // Q == P^32 == transition over one warp (1024 samples)
-  double S[D * D];
-  for (int i = 0; i < D * D; ++i) S[i] = P[i];
-  for (int k = 0; k < 5; ++k) {
-    for (int i = 0; i < D * D; ++i) tb->Mscan[k][i] = (float)S[i];
-    matmul<D>(S, S, S);
-  }
-  double W[D * D];
-  for (int i = 0; i < D * D; ++i) W[i] = (i / D == i % D) ? 1.0 : 0.0;
-  for (int v = 0; v <= NW; ++v) {
-    for (int i = 0; i < D * D; ++i) tb->MwPow[v][i] = (float)W[i];
-    matmul<D>(Q, W, W);
-  }
-  for (int i = 0; i < D * D; ++i) tb->Mtile[i] = tb->MwPow[NW][i];
-  // Wa[j] = end state after the chunk when the only non-zero input is xs[j] = 1 (xs[0], xs[1] = history)
-  for (int j = 0; j < L + 2; ++j) {
-    double y1[NS], y2[NS];
-    for (int s = 0; s < NS; ++s) { y1[s] = 0.0; y2[s] = 0.0; }
-    for (int i = 0; i < L; ++i) {
-      const double in0 = (i + 2 == j) ? 1.0 : 0.0, in1 = (i + 1 == j) ? 1.0 : 0.0, in2 = (i == j) ? 1.0 : 0.0;
-      cascade_step<NS, double>(b0, b1, b2, a1, a2, in0, in1, in2, y1, y2);
-    }
-    for (int s = 0; s < NS; ++s) { tb->Wa[j][2 * s] = (float)y1[s]; tb->Wa[j][2 * s + 1] = (float)y2[s]; }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// main streaming kernel
-// ---------------------------------------------------------------------------------------------
-// 8-byte tile-record words {float value, uint32 tag}: one relaxed 64-bit access is atomic, so a
-// word is either absent (tag 0, the workspace is zeroed per call) or complete.
-__device__ __forceinline__ void rec_store(unsigned long long* p, float v) {
-  const unsigned long long w = ((unsigned long long)1u << 32) | (unsigned long long)(unsigned)__float_as_int(v);
-#ifdef B2A_SIM
-  __atomic_store_n(p, w, __ATOMIC_RELEASE);
-#else
-  asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(w) : "memory");
-#endif
-}
-__device__ __forceinline__ unsigned long long rec_load(const unsigned long long* p) {
-#ifdef B2A_SIM
-  cusim::yield();  // polled in spin loops: let the other fibers of the block (and the scheduler) run
-  return __atomic_load_n(p, __ATOMIC_ACQUIRE);
-#else
-  unsigned long long w;
-  asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(w) : "l"(p) : "memory");
-  return w;
-#endif
-}
-
-// cp.async (16 B) global -> shared; plain copy under the CPU simulator
-__device__ __forceinline__ void cp_async16(float* smem_dst, const float* gmem_src) {
-#ifdef B2A_SIM
-  *reinterpret_cast<float4*>(smem_dst) = *reinterpret_cast<const float4*>(gmem_src);
-#else
-  const unsigned sa = (unsigned)__cvta_generic_to_shared(smem_dst);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(sa), "l"(gmem_src) : "memory");
-#endif
-}
-__device__ __forceinline__ void cp_async_wait_all() {
-#ifndef B2A_SIM
-  asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
-#endif
-}
-
-// Stage tile `tk` of the ticket order into sx (32-sample chunks of CH words) and its 2 history samples into
-// hist.  Called by the WORKERS threads only.  Interior, 16 B aligned tiles go through cp.async (no registers,
-// completes in the background); the others (row tails, unaligned rows) through plain loads.
-__device__ __forceinline__ void stage_tile(const float* __restrict__ x, int tk, int rows, int T, float* sx,
-                                           float* hist, int tid) {
-  const int tile = tk / rows, row = tk - tile * rows;
-  const int t0 = tile * TILE;
-  const float* xr = x + (size_t)row * (size_t)T;
-  if ((t0 + TILE <= T) && ((((uintptr_t)(xr + t0)) & 15) == 0)) {
-#pragma unroll
-    for (int i = 0; i < L / 4; ++i) {
-      const int v = tid + WORKERS * i;  // float4 index within the tile
-      cp_async16(&sx[CH * (v >> 3) + 4 * (v & 7)], xr + t0 + 4 * v);
-    }
-  } else {
-#pragma unroll 4
-    for (int pp = tid; pp < TILE; pp += WORKERS) {
-      const int n = t0 + pp;
-      sx[CH * (pp >> 5) + (pp & 31)] = (n < T) ? __ldg(xr + n) : 0.f;
-    }
-  }
-  if (tid < 2) {
-    const int n = t0 - 2 + tid;
-    hist[tid] = (n >= 0 && n < T) ? __ldg(xr + n) : 0.f;
-  }
-}
-
-template <int D>
-__device__ __forceinline__ float row_dot(const float* M, int i, const float* v) {
-  float a = 0.f;
-#pragma unroll
-  for (int j = 0; j < D; ++j) a = fmaf(M[i * D + j], v[j], a);
-  return a;
-}
-
-template <int NS>
-__global__ void __launch_bounds__(THREADS, 3)
-kweight_energy_kernel(const float* __restrict__ x, int rows, int T, int Tp, int ntile, Coef<NS> cf,
-                      const B2A_GRID_CONSTANT Tables<NS> tbv, int* __restrict__ ticket,
-                      unsigned long long* __restrict__ recs, double* __restrict__ bins, int stride, int r,
-                      int nbins) {
-  constexpr int D = 2 * NS;
-  __shared__ __align__(16) float sx[WORKERS * CH];
-  __shared__ float s_hist[2][2];   // history samples of the current / prefetched tile
-  __shared__ float s_mlane[32][D * D];
-  __shared__ float s_mscan[5][D * D];
-  __shared__ float s_mwpow[NW + 1][D * D];
-  __shared__ float s_mt[D * D];
-  __shared__ float s_tot[NW][D];
-  __shared__ float s_c0[NW + 1][D];  // carry into warp w for a ZERO incoming tile state; [NW] = tile aggregate
-  __shared__ float s_sin[D];         // incoming tile state (from the look-back)
-  __shared__ __align__(16) float s_wa[L + 2][D];
-  __shared__ int s_cur, s_next;    // ticket of this tile and of the next one (its samples are prefetched)
-
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const Tables<NS>* tb = &tbv;
-  for (int i = tid; i < 32 * D * D; i += THREADS) (&s_mlane[0][0])[i] = (&tb->Mlane[0][0])[i];
-  for (int i = tid; i < 5 * D * D; i += THREADS) (&s_mscan[0][0])[i] = (&tb->Mscan[0][0])[i];
-  for (int i = tid; i < (NW + 1) * D * D; i += THREADS) (&s_mwpow[0][0])[i] = (&tb->MwPow[0][0])[i];
-  for (int i = tid; i < (L + 2) * D; i += THREADS) (&s_wa[0][0])[i] = (&tb->Wa[0][0])[i];
-  if (tid < D * D) s_mt[tid] = tb->Mtile[tid];
-  const int total_tiles = rows * ntile;
-
-  // persistent CTA: tables are loaded once; tiles are claimed through a global ticket so that the tile a
-  // look-back waits for always belongs to a CTA that is already running (tile-major order).  Tickets
-  // 0 .. gridDim.x-1 are the CTAs' first tiles; later ones come from the global counter.  The carry warp fetches
-  // tickets TWO tiles ahead, so the next tile is always known and its samples stream in (cp.async) underneath
-  // the current tile's phases A/B -- the staging buffer is dead once every worker holds its chunk in registers.
-  if (tid == 0) {
-    s_cur = blockIdx.x;
-    s_next = (int)gridDim.x + atomicAdd(ticket, 1);
-  }
-  __syncthreads();
-  if (warp < NW && s_cur < total_tiles) stage_tile(x, s_cur, rows, T, sx, s_hist[0], tid);
-  int par = 0;  // which history slot belongs to the current tile
-#pragma unroll 1
-  for (;; par ^= 1) {
-  cp_async_wait_all();
-  __syncthreads();
-  const int tk = s_cur, nxt = s_next;
-  if (tk >= total_tiles) return;
-  const int tile = tk / rows, row = tk - tile * rows;  // tile-major: predecessors hold smaller tickets
-  const int t0 = tile * TILE;
-  unsigned long long* myrec = recs + ((size_t)tile * rows + row) * (2 * D);
-
-  if (warp == NW) {
-    // ================= carry warp: decoupled look-back, concurrent with phase A of the workers
-    // lanes [0,D): inclusive words of the predecessor, lanes [D,2D): its aggregate words
-    int ticket2 = 0;  // two tiles ahead; its round trip overlaps the look-back
-    if (lane == 0) ticket2 = (int)gridDim.x + atomicAdd(ticket, 1);
-    float sin_i = 0.f;  // lane i < D: component i of the incoming state
-    if (tile > 0) {
-      float prow[D];  // lane i < D: row i of P = Mtile^j
-#pragma unroll
-      for (int j = 0; j < D; ++j) prow[j] = (lane == j) ? 1.f : 0.f;
-      for (int tj = tile - 1; tj >= 0; --tj) {
-        const unsigned long long* rec = recs + ((size_t)tj * rows + row) * (2 * D);
-        unsigned incl_ok, agg_ok;
-        unsigned long long w = 0;
-        do {
-          if (lane < 2 * D) w = rec_load(rec + (lane < D ? D + lane : lane - D));
-          const unsigned ok = __ballot_sync(0xffffffffu, (lane < 2 * D) && (w >> 32) != 0);
-          incl_ok = (ok & ((1u << D) - 1)) == ((1u << D) - 1);
-          agg_ok = ((ok >> D) & ((1u << D) - 1)) == ((1u << D) - 1);
-        } while (!incl_ok && !agg_ok);
-        const float val = __int_as_float((int)(unsigned)(w & 0xffffffffu));
-        float v[D];  // the predecessor's inclusive state if present, else its aggregate
-#pragma unroll
-        for (int j = 0; j < D; ++j) v[j] = __shfl_sync(0xffffffffu, val, incl_ok ? j : D + j);
-        if (lane < D) {
-#pragma unroll
-          for (int j = 0; j < D; ++j) sin_i = fmaf(prow[j], v[j], sin_i);
-        }
-        if (incl_ok) break;
-        float pn[D];  // P <- P * Mtile (row-wise)
-#pragma unroll
-        for (int j = 0; j < D; ++j) {
-          float a = 0.f;
-#pragma unroll
-          for (int k = 0; k < D; ++k) a = fmaf(prow[k], s_mt[k * D + j], a);
-          pn[j] = a;
-        }
-#pragma unroll
-        for (int j = 0; j < D; ++j) prow[j] = pn[j];
-      }
-    }
-    if (lane < D) s_sin[lane] = sin_i;
-    B2A_BAR_SYNC(2, THREADS);  // S_in is ready (every thread has read s_cur / s_next long ago)
-    if (lane == 0) { s_cur = nxt; s_next = ticket2; }
-    continue;
-  }
-
-  // ================= worker warps: this tile's samples are already in sx (prologue / previous iteration)
-  float xs[L + 2];
-  {
-    const float4* c4 = reinterpret_cast<const float4*>(&sx[CH * tid]);
-#pragma unroll
-    for (int i = 0; i < L / 4; ++i) {
-      const float4 q = c4[i];
-      xs[2 + 4 * i] = q.x; xs[3 + 4 * i] = q.y; xs[4 + 4 * i] = q.z; xs[5 + 4 * i] = q.w;
-    }
-    if (tid == 0) {
-      xs[0] = s_hist[par][0]; xs[1] = s_hist[par][1];
-    } else {
-      const float2 h = *reinterpret_cast<const float2*>(&sx[CH * (tid - 1) + 30]);
-      xs[0] = h.x; xs[1] = h.y;
-    }
-  }
-  B2A_BAR_SYNC(1, WORKERS);  // every worker holds its chunk: sx is free
-  if (nxt < total_tiles) stage_tile(x, nxt, rows, T, sx, s_hist[par ^ 1], tid);  // lands under phases A / B
-
-  // ---- phase A: zero-state end state of this thread's chunk, e = Wa^T xs (a 34-tap linear map per state
-  //      component: the same numbers the recursion would produce, without its serial dependency)
-  float g[D];
-#pragma unroll
-  for (int i = 0; i < D; ++i) g[i] = 0.f;
-#pragma unroll
-  for (int j = 0; j < L + 2; ++j) {
-#pragma unroll
-    for (int i = 0; i < D; ++i) g[i] = fmaf(s_wa[j][i], xs[j], g[i]);
-  }
-  // ---- inclusive affine scan over the warp's 32 chunks
-#pragma unroll
-  for (int k = 0; k < 5; ++k) {
-    float o[D];
-#pragma unroll
-    for (int j = 0; j < D; ++j) o[j] = __shfl_up_sync(0xffffffffu, g[j], 1u << k);
-    if (lane >= (1 << k)) {
-#pragma unroll
-      for (int i = 0; i < D; ++i) g[i] += row_dot<D>(s_mscan[k], i, o);
-    }
-  }
-  float ex[D];  // exclusive prefix within the warp
-#pragma unroll
-  for (int j = 0; j < D; ++j) {
-    ex[j] = __shfl_up_sync(0xffffffffu, g[j], 1);
-    if (lane == 0) ex[j] = 0.f;
-  }
-  if (lane == 31) {
-#pragma unroll
-    for (int j = 0; j < D; ++j) s_tot[warp][j] = g[j];
-  }
-  B2A_BAR_SYNC(1, WORKERS);
-
-  // ---- carries for a zero incoming state: c0[w] = sum_{v<w} MwPow[w-1-v] tot[v]  (each warp its own)
-  if (lane < D) {
-    float c = 0.f;
-    for (int v = 0; v < warp; ++v) c += row_dot<D>(s_mwpow[warp - 1 - v], lane, s_tot[v]);
-    s_c0[warp][lane] = c;
-    if (warp == 0) {  // tile aggregate = c0[NW]; publish it at once so successors need not wait for our look-back
-      float e = 0.f;
-      for (int v = 0; v < NW; ++v) e += row_dot<D>(s_mwpow[NW - 1 - v], lane, s_tot[v]);
-      s_c0[NW][lane] = e;
-      if (tile > 0) rec_store(myrec + lane, e);
-    }
-  }
-  B2A_BAR_SYNC(2, THREADS);  // S_in from the carry warp (also orders s_c0 within each warp: same lanes)
-  if (warp == 0 && lane < D)  // inclusive tile state = Mtile S_in + aggregate
-    rec_store(myrec + D + lane, s_c0[NW][lane] + row_dot<D>(s_mt, lane, s_sin));
-
-  // ---- phase B: true start state, recursion again, energies into bins
-  float y1[NS], y2[NS];
-  {
-    float cw[D], st[D];
-#pragma unroll
-    for (int i = 0; i < D; ++i) cw[i] = s_c0[warp][i] + row_dot<D>(s_mwpow[warp], i, s_sin);
-#pragma unroll
-    for (int i = 0; i < D; ++i) st[i] = ex[i] + row_dot<D>(s_mlane[lane], i, cw);
-#pragma unroll
-    for (int s = 0; s < NS; ++s) { y1[s] = st[2 * s]; y2[s] = st[2 * s + 1]; }
-  }
-  const int n0 = t0 + tid * L;
-  const int nv = min(L, max(0, Tp - n0));  // samples of this chunk that exist in the padded signal
-  // bin of a sample n: j = n / stride, rem = n - j*stride -> 2j + (rem >= r); A_j is empty when r == 0
-  int j0 = n0 / stride, rem0 = n0 - j0 * stride;
-  int b0 = 2 * j0 + (rem0 >= r ? 1 : 0);
-  int end0 = (b0 & 1) ? (j0 + 1) * stride : j0 * stride + r;  // first sample after bin b0
-  int s1 = min(end0 - n0, L);
-  const bool simple = (s1 >= L) && (nv == L);
-  const int b0_first = __shfl_sync(0xffffffffu, b0, 0), b0_last = __shfl_sync(0xffffffffu, b0, 31);
-  const bool fast = __all_sync(0xffffffffu, simple) && (b0_first == b0_last);
-  double* rb = bins + (size_t)row * (size_t)nbins;
-  if (fast) {
-    float acc = 0.f;
-#pragma unroll
-    for (int i = 0; i < L; ++i) {
-      float y = cascade_step<NS, float>(cf.b0, cf.b1, cf.b2, cf.a1, cf.a2, xs[i + 2], xs[i + 1], xs[i], y1, y2);
-      acc = fmaf(y, y, acc);
-    }
-    acc = warp_sum(acc);
-    if (lane == 0) atomicAdd(rb + b0, (double)acc);
-  } else {
-    int s2 = L, b1 = b0, b2 = b0;
-    if (s1 < L) {
-      int n1 = n0 + s1, j1 = n1 / stride, rem1 = n1 - j1 * stride;
-      b1 = 2 * j1 + (rem1 >= r ? 1 : 0);
-      int end1 = (b1 & 1) ? (j1 + 1) * stride : j1 * stride + r;
-      s2 = min(end1 - n0, L);
-      if (s2 < L) {
-        int n2 = n0 + s2, j2 = n2 / stride, rem2 = n2 - j2 * stride;
-        b2 = 2 * j2 + (rem2 >= r ? 1 : 0);
-      }
-    }
-    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-#pragma unroll
-    for (int i = 0; i < L; ++i) {
-      float y = cascade_step<NS, float>(cf.b0, cf.b1, cf.b2, cf.a1, cf.a2, xs[i + 2], xs[i + 1], xs[i], y1, y2);
-      float e = (i < nv) ? y * y : 0.f;
-      a0 += (i < s1) ? e : 0.f;
-      a1 += (i >= s1 && i < s2) ? e : 0.f;
-      a2 += (i >= s2) ? e : 0.f;
-    }
-    if (nv > 0) {
-      atomicAdd(rb + b0, (double)a0);
-      if (s1 < nv) atomicAdd(rb + b1, (double)a1);
-      if (s2 < nv) atomicAdd(rb + b2, (double)a2);
-    }
-  }
-  }  // persistent tile loop
-}
-
-// =============================================================================================
-// Warp-autonomous variant (round 2): no CTA barrier, no inter-warp communication, ONE pass over the samples.
-//
-// A row is cut into RUNS of run_len consecutive segments (segment = 32 lanes x L2 = 64 samples = 2048 samples); a warp
-// owns a run and walks it segment by segment: samples -> warp-private, double-buffered shared-memory window (cp.async;
-// the next segment lands underneath the arithmetic of the current one), zero-state end state of every lane chunk
-// (a 66-tap linear map read from the window), affine shuffle scan, true lane start states from the state carried in
-// registers, float32 DF-I recursion (second read of the window), energies into the float64 interval bins.
-//
-// The state entering a run comes from a WARM-UP: the warp first runs the carry part (no energies) over the n_warm
-// segments in front of its run, starting from zero.  The K-weighting poles have radius rho < 1 (0.9946 for the 38 Hz
-// high-pass at 44.1 kHz), so whatever happened before the warm-up reaches the run attenuated by rho^(n_warm * 2048);
-// the host picks n_warm with rho^(n_warm * 2048) <= 2^-40 (3 segments at 44.1 kHz, 18 % extra reads at run_len 17).
-// That bound is five orders of magnitude below the rounding noise the float32 recursion itself carries (each step
-// rounds at 6e-8 |y| and the feedback amplifies it by ~1/(1 - rho)), i.e. the results are those of the exact carry
-// to float32 rounding; the first warp-per-segment versions (decoupled look-back, then two passes with published
-// aggregates) were exact in the same sense and cost a serial ripple per wave resp. a second HBM read.
-// B2A_LUFS_V1=1 selects round 1's CTA-cooperative kernel with its exact look-back carry (rows whose dynamic range
-// exceeds 2^40 within 70 ms are the only inputs on which the two can differ beyond rounding).
-// =============================================================================================
-namespace v2 {
-
-constexpr int L2 = 64;              // samples per lane
-constexpr int SEG = 32 * L2;        // samples per warp segment
-constexpr int CHS = L2 + 4;         // shared-memory words per lane chunk: 16 B aligned, conflict-free LDS.128
-constexpr int WPB = 12;             // warps per CTA (one CTA per SM: 12 x 17 KB of windows)
-constexpr int NBUF = 2;             // windows per warp: the next segment lands underneath the arithmetic
-constexpr int BUF = 32 * CHS;       // floats per window
-
-template <int NS>
-struct Tables2 {
+struct Tables {
   static constexpr int D = 2 * NS;
   float Wa[L2 + 2][D];        // zero-state end state of a lane chunk as a linear map of its 66 inputs
   float Mlane[32][D * D];     // A^(L2 l)
@@ -489,10 +106,8 @@ struct Tables2 {
   float Mseg[D * D];          // A^SEG
 };
 
-// L = samples per lane chunk (<= L2): Wa = end-state map of a chunk, Mlane[l] = A^(L l), Mscan[k] = A^(L 2^k),
-// Mseg = A^(32 L)
 template <int NS>
-static void build_tables2(const Coef<NS>& cf, Tables2<NS>* tb, int L = L2) {
+static void build_tables(const Coef<NS>& cf, Tables<NS>* tb) {
   constexpr int D = 2 * NS;
   double b0[NS], b1[NS], b2[NS], a1[NS], a2[NS];
   for (int s = 0; s < NS; ++s) {
@@ -507,24 +122,24 @@ static void build_tables2(const Coef<NS>& cf, Tables2<NS>* tb, int L = L2) {
   }
   double P[D * D];  // A^L2
   for (int i = 0; i < D * D; ++i) P[i] = A[i];
-  for (int l = 1; l < L; l <<= 1) matmul<D>(P, P, P);
+  for (int l = 1; l < L2; l <<= 1) matmul<D>(P, P, P);
   double Q[D * D];
   for (int i = 0; i < D * D; ++i) Q[i] = (i / D == i % D) ? 1.0 : 0.0;
   for (int l = 0; l < 32; ++l) {
     for (int i = 0; i < D * D; ++i) tb->Mlane[l][i] = (float)Q[i];
     matmul<D>(P, Q, Q);
   }
-  for (int i = 0; i < D * D; ++i) tb->Mseg[i] = (float)Q[i];  // Q == A^(32 L)
+  for (int i = 0; i < D * D; ++i) tb->Mseg[i] = (float)Q[i];  // Q == A^SEG
   double S[D * D];
   for (int i = 0; i < D * D; ++i) S[i] = P[i];
   for (int k = 0; k < 5; ++k) {
     for (int i = 0; i < D * D; ++i) tb->Mscan[k][i] = (float)S[i];
     matmul<D>(S, S, S);
   }
-  for (int j = 0; j < L + 2; ++j) {
+  for (int j = 0; j < L2 + 2; ++j) {
     double y1[NS], y2[NS];
     for (int s = 0; s < NS; ++s) { y1[s] = 0.0; y2[s] = 0.0; }
-    for (int i = 0; i < L; ++i) {
+    for (int i = 0; i < L2; ++i) {
       const double in0 = (i + 2 == j) ? 1.0 : 0.0, in1 = (i + 1 == j) ? 1.0 : 0.0, in2 = (i == j) ? 1.0 : 0.0;
       cascade_step<NS, double>(b0, b1, b2, a1, a2, in0, in1, in2, y1, y2);
     }
@@ -544,6 +159,29 @@ static double max_pole_radius(const Coef<NS>& cf) {
     if (r > rho) rho = r;
   }
   return rho;
+}
+
+// cp.async (16 B) global -> shared; plain copy under the CPU simulator
+__device__ __forceinline__ void cp_async16(float* smem_dst, const float* gmem_src) {
+#ifdef B2A_SIM
+  *reinterpret_cast<float4*>(smem_dst) = *reinterpret_cast<const float4*>(gmem_src);
+#else
+  const unsigned sa = (unsigned)__cvta_generic_to_shared(smem_dst);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(sa), "l"(gmem_src) : "memory");
+#endif
+}
+__device__ __forceinline__ void cp_async_wait_all() {
+#ifndef B2A_SIM
+  asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
+#endif
+}
+
+template <int D>
+__device__ __forceinline__ float row_dot(const float* M, int i, const float* v) {
+  float a = 0.f;
+#pragma unroll
+  for (int j = 0; j < D; ++j) a = fmaf(M[i * D + j], v[j], a);
+  return a;
 }
 
 // Stage segment `seg` of row `xr` into a warp window (cp.async when the 8 KB are inside the row and 16 B aligned).
@@ -566,7 +204,7 @@ __device__ __forceinline__ void stage_segment(const float* __restrict__ xr, int 
 template <int NS>
 __global__ void __launch_bounds__(32 * WPB, 1)
 kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp, int nseg, int run_len, int n_runs,
-                           int n_warm, Coef<NS> cf, const B2A_GRID_CONSTANT Tables2<NS> tbv,
+                           int n_warm, Coef<NS> cf, const B2A_GRID_CONSTANT Tables<NS> tbv,
                            double* __restrict__ bins, int stride, int r, int nbins) {
   constexpr int D = 2 * NS;
   B2A_DYN_SMEM(smem);
@@ -731,301 +369,6 @@ kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp,
   cp_async_wait_all();
 }
 
-}  // namespace v2
-
-// =============================================================================================
-// Chunk-pair variant: the v2 algorithm with TWO lane chunks of the same row in the halves of (x, y) register pairs.
-// A segment is 64 chunks of L4 = 32 samples; lane l owns chunk l (half x) and chunk l + 32 (half y), so every
-// arithmetic step of v2 -- the 34-tap end-state map, the affine scan, the DF-I recursion, the energy accumulation --
-// is one fma2 / mul2 / add2 (b2a_common.h) on a (chunk l, chunk l + 32) pair with the coefficient broadcast.  The
-// window holds the two halves INTERLEAVED sample by
-// sample (4-byte cp.async, coalesced 128 B per warp instruction, issued a few at a time inside the arithmetic of the
-// current segment), so one 128-bit shared load delivers two ready-made register pairs.  The scan runs on both halves
-// at once; half y is then re-based on half x's total:  c' = T_x + A^1024 carry,  carry' = T_y + A^1024 c'.
-// The 32-sample chunks double v2's per-segment scan / bookkeeping share and the boundary path runs on two split points;
-// the kernel is OPT-IN (B2A_LUFS_PAIR=1) and v2 is the default.
-// =============================================================================================
-namespace v4 {
-
-constexpr int L4 = 32;                 // samples per chunk
-constexpr int SEG = 64 * L4;           // samples per warp segment (2048, as v2)
-constexpr int HALF = 32 * L4;          // samples between the two chunks of a lane
-constexpr int CHS = 2 * L4 + 4;        // words per lane (both chunks interleaved): 16 B aligned, conflict-free LDS.128
-constexpr int WPB = 12;                // warps per CTA (one CTA per SM)
-constexpr int NBUF = 2;
-constexpr int BUF = 32 * CHS;          // floats per window (8.7 KB)
-constexpr int NST = SEG / 32;          // 4-byte copies per lane and segment
-
-__device__ __forceinline__ void cp_async4(float* smem_dst, const float* gmem_src) {
-#ifdef B2A_SIM
-  *smem_dst = *gmem_src;
-#else
-  const unsigned sa = (unsigned)__cvta_generic_to_shared(smem_dst);
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(sa), "l"(gmem_src) : "memory");
-#endif
-}
-
-// copy e (0 .. NST-1) of a segment: sample s = 32 e + lane -> win[CHS * (chunk & 31) + 2 * (s & 31) + (chunk >> 5)]
-__device__ __forceinline__ float* stage_dst(float* win, int e, int lane) { return &win[CHS * (e & 31) + 2 * lane + (e >> 5)]; }
-
-// Stage copies [e0, e1) of segment `seg` of row `xr` (interior segments: asynchronous, no registers).
-__device__ __forceinline__ void stage_some(const float* __restrict__ xr, int t0, bool interior, int T, float* win, int lane,
-                                           int e0, int e1) {
-  if (interior) {
-#pragma unroll
-    for (int e = e0; e < e1; ++e) cp_async4(stage_dst(win, e, lane), xr + t0 + 32 * e + lane);
-  } else {
-#pragma unroll
-    for (int e = e0; e < e1; ++e) {
-      const int n = t0 + 32 * e + lane;
-      *stage_dst(win, e, lane) = (n < T) ? __ldg(xr + n) : 0.f;
-    }
-  }
-}
-
-template <int D>
-__device__ __forceinline__ float2 row_dot2(const float* M, int i, const float2* v) {
-  float2 a = make_float2(0.f, 0.f);
-#pragma unroll
-  for (int j = 0; j < D; ++j) a = fma2(bcast2(M[i * D + j]), v[j], a);
-  return a;
-}
-
-// one step of the cascade on a pair of chunks: the operation order of cascade_step, every product fused
-template <int NS>
-__device__ __forceinline__ float2 cascade_step2(const Coef<NS>& cf, float2 in0, float2 in1, float2 in2, float2 (&y1)[NS],
-                                                float2 (&y2)[NS]) {
-#pragma unroll
-  for (int s = 0; s < NS; ++s) {
-    const float2 f = fma2(bcast2(cf.b0[s]), in0, fma2(bcast2(cf.b1[s]), in1, mul2(bcast2(cf.b2[s]), in2)));
-    const float2 y0 = fma2(bcast2(-cf.a1[s]), y1[s], fma2(bcast2(-cf.a2[s]), y2[s], f));
-    in0 = y0; in1 = y1[s]; in2 = y2[s];
-    y2[s] = y1[s]; y1[s] = y0;
-  }
-  return in0;
-}
-
-// interval bookkeeping of one chunk [n0, n0 + L4): first interval b0, split points s1 <= s2 (L4 = none), the
-// intervals b1, b2 behind them
-struct Split { int b0, b1, b2, s1, s2, nv; };
-__device__ __forceinline__ Split split_of(int n0, int Tp, int stride, int r) {
-  Split sp;
-  sp.nv = min(L4, max(0, Tp - n0));
-  const int j0 = n0 / stride, rem0 = n0 - j0 * stride;
-  sp.b0 = 2 * j0 + (rem0 >= r ? 1 : 0);
-  const int end0 = (sp.b0 & 1) ? (j0 + 1) * stride : j0 * stride + r;
-  sp.s1 = min(end0 - n0, L4);
-  sp.s2 = L4; sp.b1 = sp.b0; sp.b2 = sp.b0;
-  if (sp.s1 < L4) {
-    const int n1 = n0 + sp.s1, j1 = n1 / stride, rem1 = n1 - j1 * stride;
-    sp.b1 = 2 * j1 + (rem1 >= r ? 1 : 0);
-    const int end1 = (sp.b1 & 1) ? (j1 + 1) * stride : j1 * stride + r;
-    sp.s2 = min(end1 - n0, L4);
-    if (sp.s2 < L4) {
-      const int n2 = n0 + sp.s2, j2 = n2 / stride, rem2 = n2 - j2 * stride;
-      sp.b2 = 2 * j2 + (rem2 >= r ? 1 : 0);
-    }
-  }
-  return sp;
-}
-
-// energies of one half into the row's interval bins: one atomic per interval the warp touched
-__device__ __forceinline__ void flush_half(double* rb, int nbins, const Split& sp, float a0, float a1, float a2, bool clean,
-                                           int lane) {
-  const int blast = (sp.s2 < L4) ? sp.b2 : ((sp.s1 < L4) ? sp.b1 : sp.b0);
-  const int bf = __shfl_sync(0xffffffffu, sp.b0, 0), bl = __shfl_sync(0xffffffffu, blast, 31);
-  for (int id = bf; id <= bl; ++id) {
-    float v = (sp.b0 == id) ? a0 : 0.f;
-    if (!clean) v += ((sp.s1 < L4 && sp.b1 == id) ? a1 : 0.f) + ((sp.s2 < L4 && sp.b2 == id) ? a2 : 0.f);
-    v = warp_sum(v);
-    if (lane == 0 && id < nbins) atomicAdd(rb + id, (double)v);
-  }
-}
-
-template <int NS>
-__global__ void __launch_bounds__(32 * WPB, 1)
-kweight_energy_pair_kernel(const float* __restrict__ x, int rows, int T, int Tp, int nseg, int run_len, int n_runs,
-                           int n_warm, Coef<NS> cf, const B2A_GRID_CONSTANT v2::Tables2<NS> tbv,
-                           double* __restrict__ bins, int stride, int r, int nbins) {
-  constexpr int D = 2 * NS;
-  B2A_DYN_SMEM(smem);
-  float* wins = reinterpret_cast<float*>(smem);  // [WPB][NBUF][BUF]
-  __shared__ __align__(16) float s_wa[L4 + 2][D];
-  __shared__ float s_mlane[32][D * D];
-  __shared__ float s_mscan[5][D * D];
-  __shared__ float s_mhalf[D * D];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int i = tid; i < (L4 + 2) * D; i += blockDim.x) (&s_wa[0][0])[i] = (&tbv.Wa[0][0])[i];
-  for (int i = tid; i < 32 * D * D; i += blockDim.x) (&s_mlane[0][0])[i] = (&tbv.Mlane[0][0])[i];
-  for (int i = tid; i < 5 * D * D; i += blockDim.x) (&s_mscan[0][0])[i] = (&tbv.Mscan[0][0])[i];
-  if (tid < D * D) s_mhalf[tid] = tbv.Mseg[tid];  // A^(32 L4): one half segment
-  __syncthreads();  // the only CTA barrier: tables
-  const int total = rows * n_runs;
-  float* win0 = wins + (size_t)warp * NBUF * BUF;
-
-#pragma unroll 1
-  for (int cur = (int)blockIdx.x * WPB + warp; cur < total; cur += (int)gridDim.x * WPB) {
-    const int run = cur / rows, row = cur - run * rows;
-    const int seg0 = run * run_len, seg1 = min(nseg, seg0 + run_len);
-    const int segw = max(0, seg0 - n_warm);  // warm-up starts here, from a zero state
-    const float* xr = x + (size_t)row * (size_t)T;
-    double* rb = bins + (size_t)row * (size_t)nbins;
-    float carry[D];  // state entering the current segment (all lanes hold it)
-#pragma unroll
-    for (int j = 0; j < D; ++j) carry[j] = 0.f;
-    stage_some(xr, segw * SEG, segw * SEG + SEG <= T, T, win0, lane, 0, NST);
-    int par = 0;
-#pragma unroll 1
-    for (int seg = segw; seg < seg1; ++seg, par ^= (NBUF - 1)) {
-      cp_async_wait_all();
-      __syncwarp();
-      const float* win = win0 + par * BUF;
-      float* wnext = win0 + (par ^ 1) * BUF;
-      const bool more = seg + 1 < seg1;
-      const int tn = (seg + 1) * SEG;
-      const bool next_in = tn + SEG <= T;
-      const int t0 = seg * SEG;
-      float2 h0, h1;  // the two samples in front of each of this lane's chunks
-      {
-        const float4 q = *reinterpret_cast<const float4*>(&win[CHS * ((lane + 31) & 31) + 2 * (L4 - 2)]);
-        if (lane == 0) {  // chunk 0 continues the previous segment, chunk 32 continues chunk 31 (half x of lane 31)
-          const float g0 = (t0 >= 2 && t0 - 2 < T) ? __ldg(xr + t0 - 2) : 0.f;
-          const float g1 = (t0 >= 1 && t0 - 1 < T) ? __ldg(xr + t0 - 1) : 0.f;
-          h0 = make_float2(g0, q.x); h1 = make_float2(g1, q.z);
-        } else {
-          h0 = make_float2(q.x, q.y); h1 = make_float2(q.z, q.w);
-        }
-      }
-      const float4* c4 = reinterpret_cast<const float4*>(&win[CHS * lane]);
-      const float4* wa4 = reinterpret_cast<const float4*>(&s_wa[0][0]);  // D == 4: one 128-bit broadcast load per tap
-      // ---- zero-state end state of the two chunks as a linear map of their 34 inputs (two partial sums: ILP); the
-      //      next segment's copies are issued four at a time in between
-      float2 g[D], ge[D];
-#pragma unroll
-      for (int i = 0; i < D; ++i) {
-        g[i] = mul2(bcast2(s_wa[0][i]), h0);
-        ge[i] = mul2(bcast2(s_wa[1][i]), h1);
-      }
-#pragma unroll
-      for (int i4 = 0; i4 < L4 / 2; ++i4) {
-        if (more) stage_some(xr, tn, next_in, T, wnext, lane, 4 * i4, 4 * i4 + 4);
-        const float4 q = c4[i4];  // (x[2 i4], y[2 i4], x[2 i4 + 1], y[2 i4 + 1])
-        const float2 q0 = make_float2(q.x, q.y), q1 = make_float2(q.z, q.w);
-        if constexpr (D == 4) {
-          const float4 w0 = wa4[2 + 2 * i4], w1 = wa4[3 + 2 * i4];
-          g[0] = fma2(bcast2(w0.x), q0, g[0]); g[1] = fma2(bcast2(w0.y), q0, g[1]);
-          g[2] = fma2(bcast2(w0.z), q0, g[2]); g[3] = fma2(bcast2(w0.w), q0, g[3]);
-          ge[0] = fma2(bcast2(w1.x), q1, ge[0]); ge[1] = fma2(bcast2(w1.y), q1, ge[1]);
-          ge[2] = fma2(bcast2(w1.z), q1, ge[2]); ge[3] = fma2(bcast2(w1.w), q1, ge[3]);
-        } else {
-#pragma unroll
-          for (int i = 0; i < D; ++i) {
-            g[i] = fma2(bcast2(s_wa[2 + 2 * i4][i]), q0, g[i]);
-            ge[i] = fma2(bcast2(s_wa[3 + 2 * i4][i]), q1, ge[i]);
-          }
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < D; ++i) g[i] = add2(g[i], ge[i]);
-#pragma unroll
-      for (int k = 0; k < 5; ++k) {  // inclusive affine scan over the 32 chunks of each half
-        float2 o[D];
-#pragma unroll
-        for (int j = 0; j < D; ++j) {
-          o[j].x = __shfl_up_sync(0xffffffffu, g[j].x, 1u << k);
-          o[j].y = __shfl_up_sync(0xffffffffu, g[j].y, 1u << k);
-        }
-        if (lane >= (1 << k)) {
-#pragma unroll
-          for (int i = 0; i < D; ++i) g[i] = add2(g[i], row_dot2<D>(s_mscan[k], i, o));
-        }
-      }
-      float2 ex[D];
-      float tx[D], ty[D];  // zero-state totals of the two halves
-#pragma unroll
-      for (int j = 0; j < D; ++j) {
-        ex[j].x = __shfl_up_sync(0xffffffffu, g[j].x, 1);
-        ex[j].y = __shfl_up_sync(0xffffffffu, g[j].y, 1);
-        if (lane == 0) ex[j] = make_float2(0.f, 0.f);
-        tx[j] = __shfl_sync(0xffffffffu, g[j].x, 31);
-        ty[j] = __shfl_sync(0xffffffffu, g[j].y, 31);
-      }
-      float cmid[D];  // state entering half y:  T_x + A^HALF carry
-#pragma unroll
-      for (int i = 0; i < D; ++i) cmid[i] = tx[i] + row_dot<D>(s_mhalf, i, carry);
-      if (seg >= seg0) {
-        // ---- true start states, recursion, energies into the interval bins
-        float2 y1[NS], y2[NS];
-        {
-          float2 cv[D];
-#pragma unroll
-          for (int j = 0; j < D; ++j) cv[j] = make_float2(carry[j], cmid[j]);
-#pragma unroll
-          for (int s = 0; s < NS; ++s) {
-            y1[s] = add2(ex[2 * s], row_dot2<D>(s_mlane[lane], 2 * s, cv));
-            y2[s] = add2(ex[2 * s + 1], row_dot2<D>(s_mlane[lane], 2 * s + 1, cv));
-          }
-        }
-        const Split sx = split_of(t0 + lane * L4, Tp, stride, r);
-        const Split sy = split_of(t0 + HALF + lane * L4, Tp, stride, r);
-        const bool simple = (sx.s1 >= L4) && (sx.nv == L4) && (sy.s1 >= L4) && (sy.nv == L4);
-        const bool clean = __all_sync(0xffffffffu, simple);  // warp-uniform: no chunk straddles an interval boundary
-        const float2 zero2 = make_float2(0.f, 0.f);
-        float2 a0 = zero2, a1 = zero2, a2 = zero2;
-        float2 xm2 = h0, xm1 = h1;
-        if (clean) {
-          float2 acc = zero2;
-#pragma unroll
-          for (int i4 = 0; i4 < L4 / 2; ++i4) {
-            const float4 q = c4[i4];
-            const float2 qs[2] = {make_float2(q.x, q.y), make_float2(q.z, q.w)};
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const float2 y = cascade_step2<NS>(cf, qs[e], xm1, xm2, y1, y2);
-              xm2 = xm1; xm1 = qs[e];
-              acc = fma2(y, y, acc);
-            }
-          }
-          a0 = acc;
-        } else {
-          float2 acc = zero2, p1 = zero2, p2 = zero2;  // running energy and its value at the two interval boundaries
-#pragma unroll
-          for (int i4 = 0; i4 < L4 / 2; ++i4) {
-            const float4 q = c4[i4];
-            const float2 qs[2] = {make_float2(q.x, q.y), make_float2(q.z, q.w)};
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int i = 2 * i4 + e;
-              p1.x = (i == sx.s1) ? acc.x : p1.x; p1.y = (i == sy.s1) ? acc.y : p1.y;
-              p2.x = (i == sx.s2) ? acc.x : p2.x; p2.y = (i == sy.s2) ? acc.y : p2.y;
-              const float2 y = cascade_step2<NS>(cf, qs[e], xm1, xm2, y1, y2);
-              xm2 = xm1; xm1 = qs[e];
-              const float2 an = fma2(y, y, acc);
-              acc.x = (i < sx.nv) ? an.x : acc.x; acc.y = (i < sy.nv) ? an.y : acc.y;
-            }
-          }
-          if (sx.s1 >= L4) p1.x = acc.x;
-          if (sy.s1 >= L4) p1.y = acc.y;
-          if (sx.s2 >= L4) p2.x = acc.x;
-          if (sy.s2 >= L4) p2.y = acc.y;
-          a0 = p1; a1 = add2(p2, neg2(p1)); a2 = add2(acc, neg2(p2));
-        }
-        flush_half(rb, nbins, sx, a0.x, a1.x, a2.x, clean, lane);
-        flush_half(rb, nbins, sy, a0.y, a1.y, a2.y, clean, lane);
-      }
-      // ---- carry into the next segment: A^HALF (state entering half y) + (zero-state end state of half y)
-#pragma unroll
-      for (int i = 0; i < D; ++i) tx[i] = ty[i] + row_dot<D>(s_mhalf, i, cmid);
-#pragma unroll
-      for (int i = 0; i < D; ++i) carry[i] = tx[i];
-      __syncwarp();  // every lane is done with this window before it is refilled
-    }
-  }
-  cp_async_wait_all();
-}
-
-}  // namespace v4
-
 // ---------------------------------------------------------------------------------------------
 // gating: ref:audiotools/core/loudness.py:208-247 (+ :315-320 clamp, effects.py:214-217 gain)
 // ---------------------------------------------------------------------------------------------
@@ -1155,7 +498,7 @@ gain_kernel(const float* __restrict__ x, float* __restrict__ out, int64_t per_it
 }
 
 struct Geometry {
-  int K, stride, q, r, nblk, nbins, ntile, nseg;
+  int K, stride, q, r, nblk, nbins, nseg;
 };
 static int geometry(int64_t Tp, double rate, double block_s, Geometry* g) {
   double kf = block_s * rate;
@@ -1167,23 +510,8 @@ static int geometry(int64_t Tp, double rate, double block_s, Geometry* g) {
   g->K = (int)K; g->stride = (int)stride; g->q = (int)(K / stride); g->r = (int)(K % stride);
   g->nblk = (int)nblk;
   g->nbins = 2 * (int)(nblk + g->q);
-  g->ntile = (int)((Tp + TILE - 1) / TILE);
-  g->nseg = (int)((Tp + v2::SEG - 1) / v2::SEG);  // segments of the warp-autonomous kernel (>= ntile)
+  g->nseg = (int)((Tp + SEG - 1) / SEG);  // warp segments per row
   return 0;
-}
-
-static int use_v1() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B2A_LUFS_V1");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v;
-}
-
-static int use_pair() {  // B2A_LUFS_PAIR=1: the opt-in chunk-pair kernel (v4) instead of v2
-  const char* e = getenv("B2A_LUFS_PAIR");  // read per call: the tests switch it
-  return (e && e[0] == '1') ? 1 : 0;
 }
 
 template <int NS>
@@ -1192,7 +520,7 @@ static int run(const float* x, int64_t B, int C, int64_t T, int64_t Tp, const Ge
                float* z_blocks, float* lufs_out, float* loud_out, const float* target_db, int n_target,
                float* gain_out, void* ws, size_t ws_bytes, void* stream) {
   const int64_t rows = B * C;
-  WsLayout w = ws_layout(rows, g.nseg, g.nbins, g.nblk, 2 * MAX_STAGES);
+  WsLayout w = ws_layout(rows, g.nbins, g.nblk);
   B2A_REQUIRE(ws_bytes >= w.total, B2A_E_INVALID, "lufs: workspace too small (%zu < %zu)", ws_bytes, w.total);
   Coef<NS> cf;
   for (int s = 0; s < NS; ++s) {
@@ -1209,61 +537,36 @@ static int run(const float* x, int64_t B, int C, int64_t T, int64_t Tp, const Ge
   int sms = B2A_NUM_SMS, dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
     sms = B2A_NUM_SMS;
-  if (use_v1()) {  // the CTA-cooperative kernel of round 1 (B2A_LUFS_V1=1): kept for A/B measurements
-    Tables<NS> tbh;
-    build_tables<NS>(cf, &tbh);
-    int per_sm = 1;
-    B2A_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kweight_energy_kernel<NS>, THREADS, 0));
+  // runs per row: as many as there are resident warps for (one CTA of 12 warps per SM), but long enough that the
+  // warm-up (n_warm segments in front of every run but the first) stays a small fraction of the work
 #ifdef B2A_SIM
-    const int64_t resident = 1;  // the CPU simulator runs CTAs one after another: no co-resident predecessors
+  const int64_t resident = 1;
 #else
-    const int64_t resident = (int64_t)sms * (per_sm < 1 ? 1 : per_sm);
+  const int64_t resident = sms;
 #endif
-    const int64_t tiles_all = rows * g.ntile;
-    B2A_LAUNCH(kweight_energy_kernel<NS>, dim3((unsigned)(tiles_all < resident ? tiles_all : resident)), dim3(THREADS), 0, stream, x, (int)rows,
-               (int)T, (int)Tp, g.ntile, cf, tbh, (int*)(base + w.ticket),
-               (unsigned long long*)(base + w.recs), (double*)(base + w.bins), g.stride, g.r, g.nbins);
-  } else {
-    // runs per row: as many as there are resident warps for (one CTA of 12 warps per SM), but long enough that the
-    // warm-up (n_warm segments in front of every run but the first) stays a small fraction of the work
-#ifdef B2A_SIM
-    const int64_t resident = 1;
-#else
-    const int64_t resident = sms;
-#endif
-    const double rho = v2::max_pole_radius<NS>(cf);
-    B2A_REQUIRE(rho < 1.0, B2A_E_UNSUPPORTED, "lufs: unstable filter (pole radius %g)", rho);
-    int n_warm = 1;
-    if (rho > 0.0) {
-      const double n_tail = 40.0 * 0.6931471805599453 / -log(rho);  // rho^n_tail = 2^-40
-      n_warm = (int)((n_tail + v2::SEG - 1) / v2::SEG);
-      if (n_warm < 1) n_warm = 1;
-    }
-    const bool pairs = use_pair() != 0;
-    const int wpb = pairs ? v4::WPB : v2::WPB;
-    int64_t rpr = (resident * wpb) / rows;
-    if (rpr < 1) rpr = 1;
-    int run_len = (int)((g.nseg + rpr - 1) / rpr);
-    if (run_len < 4 * n_warm) run_len = 4 * n_warm;  // at most 25 % warm-up
-    if (run_len > g.nseg) run_len = g.nseg;
-    const int n_runs = (g.nseg + run_len - 1) / run_len;
-    v2::Tables2<NS> tb2;
-    v2::build_tables2<NS>(cf, &tb2, pairs ? v4::L4 : v2::L2);
-    const int64_t runs_all = rows * n_runs;
-    const int64_t want = (runs_all + wpb - 1) / wpb;
-    const unsigned grid = (unsigned)(want < resident ? want : resident);
-    if (pairs) {
-      const size_t smem = (size_t)v4::WPB * v4::NBUF * v4::BUF * sizeof(float);
-      B2A_CUDA_OK(cudaFuncSetAttribute(v4::kweight_energy_pair_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      B2A_LAUNCH(v4::kweight_energy_pair_kernel<NS>, dim3(grid), dim3(32 * v4::WPB), smem, stream, x, (int)rows, (int)T,
-                 (int)Tp, g.nseg, run_len, n_runs, n_warm, cf, tb2, (double*)(base + w.bins), g.stride, g.r, g.nbins);
-    } else {
-      const size_t smem = (size_t)v2::WPB * v2::NBUF * v2::BUF * sizeof(float);
-      B2A_CUDA_OK(cudaFuncSetAttribute(v2::kweight_energy_warp_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      B2A_LAUNCH(v2::kweight_energy_warp_kernel<NS>, dim3(grid), dim3(32 * v2::WPB), smem, stream, x, (int)rows, (int)T,
-                 (int)Tp, g.nseg, run_len, n_runs, n_warm, cf, tb2, (double*)(base + w.bins), g.stride, g.r, g.nbins);
-    }
+  const double rho = max_pole_radius<NS>(cf);
+  B2A_REQUIRE(rho < 1.0, B2A_E_UNSUPPORTED, "lufs: unstable filter (pole radius %g)", rho);
+  int n_warm = 1;
+  if (rho > 0.0) {
+    const double n_tail = 40.0 * 0.6931471805599453 / -log(rho);  // rho^n_tail = 2^-40
+    n_warm = (int)((n_tail + SEG - 1) / SEG);
+    if (n_warm < 1) n_warm = 1;
   }
+  int64_t rpr = (resident * WPB) / rows;
+  if (rpr < 1) rpr = 1;
+  int run_len = (int)((g.nseg + rpr - 1) / rpr);
+  if (run_len < 4 * n_warm) run_len = 4 * n_warm;  // at most 25 % warm-up
+  if (run_len > g.nseg) run_len = g.nseg;
+  const int n_runs = (g.nseg + run_len - 1) / run_len;
+  Tables<NS> tb;
+  build_tables<NS>(cf, &tb);
+  const int64_t runs_all = rows * n_runs;
+  const int64_t want = (runs_all + WPB - 1) / WPB;
+  const unsigned grid = (unsigned)(want < resident ? want : resident);
+  const size_t smem = (size_t)WPB * NBUF * BUF * sizeof(float);
+  B2A_CUDA_OK(cudaFuncSetAttribute(kweight_energy_warp_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B2A_LAUNCH(kweight_energy_warp_kernel<NS>, dim3(grid), dim3(32 * WPB), smem, stream, x, (int)rows, (int)T, (int)Tp,
+             g.nseg, run_len, n_runs, n_warm, cf, tb, (double*)(base + w.bins), g.stride, g.r, g.nbins);
   GateParams gp;
   for (int c = 0; c < 8; ++c) gp.G[c] = c < C ? chan_gain_h[c] : 0.0;
   gp.scale = (float)(1.0 / (block_s * rate));
@@ -1288,7 +591,7 @@ extern "C" int64_t b2a_lufs_num_blocks(int64_t T_padded, double rate, double blo
 extern "C" size_t b2a_lufs_workspace_bytes(int64_t B, int C, int64_t T_padded, double rate, double block_s) {
   Geometry g;
   if (B < 1 || C < 1 || T_padded < 1 || geometry(T_padded, rate, block_s, &g) != 0) return 0;
-  return ws_layout(B * C, g.nseg, g.nbins, g.nblk, 2 * MAX_STAGES).total;
+  return ws_layout(B * C, g.nbins, g.nblk).total;
 }
 
 extern "C" int b2a_lufs_f32(const float* x, int64_t B, int C, int64_t T, int64_t T_padded, double rate,

@@ -81,7 +81,7 @@ __device__ __forceinline__ bool stage_span_async(const Params& p, float* sp, int
 int num_sms();
 
 // Tensor-core (wgmma) variant of the fused kernel for n_fft = 2048 mel / log-mel launches (spectral_tc.cu).
-// tc_supported: the launch can take that path (geometry, shared memory, B2A_SPECTRAL_TC != 0).
+// tc_supported: the launch can take that path (geometry, shared memory, switched on by b2a_spectral_tc_enable).
 bool tc_supported(const Params& p);
 int launch_tc(Params& p, void* stream);
 

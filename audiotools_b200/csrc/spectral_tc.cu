@@ -34,10 +34,6 @@
 #include "fft_warp.cuh"
 #include "spectral_internal.h"
 
-#ifndef B2A_SIM
-#include <cstdlib>
-#endif
-
 namespace b2a {
 namespace spectral {
 
@@ -571,16 +567,8 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
 
 }  // namespace tc
 
-static int g_tc_enabled = -1;
-static int tc_enabled() {
-  if (g_tc_enabled < 0) {
-    // Opt-in: the FP32 warp kernel is the default; B2A_SPECTRAL_TC=1 or b2a_spectral_tc_enable(1) selects the
-    // tensor-core path.
-    const char* e = getenv("B2A_SPECTRAL_TC");
-    g_tc_enabled = (e && e[0] == '1') ? 1 : 0;
-  }
-  return g_tc_enabled;
-}
+// Opt-in: the FP32 warp kernel is the default; b2a_spectral_tc_enable(1) selects the tensor-core path.
+static int g_tc_enabled = 0;
 
 static int tc_num_sms() {
   int n = 0, dev = 0;
@@ -590,7 +578,7 @@ static int tc_num_sms() {
 }
 
 bool tc_supported(const Params& p) {
-  if (!tc_enabled()) return false;
+  if (!g_tc_enabled) return false;
   if (p.n_fft != tc::NFFT || !p.mel_out || p.stft_out) return false;
   if (p.hop < 1 || p.hop > 512) return false;
   if (!p.center || p.row_origin) return false;
@@ -640,7 +628,7 @@ extern "C" int b2a_spectral_uses_tensor_cores(int n_fft, int hop, int want_mel, 
 }
 
 extern "C" int b2a_spectral_tc_enable(int on) {
-  const int prev = b2a::spectral::tc_enabled();
+  const int prev = b2a::spectral::g_tc_enabled;
   b2a::spectral::g_tc_enabled = on ? 1 : 0;
   return prev;
 }

@@ -377,7 +377,7 @@ int b2a_pack_rows_f32(const float* const* src_ptrs, const int64_t* src_len, cons
 
 /* 1 when b2a_spectral_f32 runs a launch of this geometry on the tensor-core kernel (csrc/spectral_tc.cu: wgmma,
  * accumulators in registers): window_length 2048, hop <= 512, mel / log-mel output without the complex STFT, and
- * the path switched on (environment variable B2A_SPECTRAL_TC=1, or b2a_spectral_tc_enable(1)).  It is opt-in: the FP32 warp kernel of
+ * the path switched on with b2a_spectral_tc_enable(1).  It is opt-in: the FP32 warp kernel of
  * spectral.cu is the default; every other launch uses the FP32 kernels. */
 int b2a_spectral_uses_tensor_cores(int n_fft, int hop, int want_mel, int want_stft);
 /* Switch the tensor-core path on / off for this process (A/B measurements, parity tests of both kernels); returns the

@@ -748,14 +748,11 @@ def test_pitch_shift_and_time_stretch_match_spec_oracle(at):
                                g, f"stretch_{fac:g}")
 
 
-@pytest.mark.parametrize("pair", ["0", "1"])
 @pytest.mark.parametrize("sr,T,B,C", [(44100, 441000, 1, 1), (48000, 600001, 2, 1), (11025, 90001, 3, 2), (16000, 200000, 200, 1)])
-def test_lufs_warp_kernel_run_geometries(at, sp, sr, T, B, C, pair, monkeypatch):
-    """csrc/lufs.cu (namespace v2, and the opt-in packed chunk-pair kernel v4): one row cut into hundreds of
-    one-segment runs, a rate with r != 0, and more rows than a launch has resident warps for."""
+def test_lufs_warp_kernel_run_geometries(at, sp, sr, T, B, C):
+    """csrc/lufs.cu: one row cut into hundreds of one-segment runs, a rate with r != 0, and more rows than a launch
+    has resident warps for."""
     from audiotools_b200.engine import get_engine
-
-    monkeypatch.setenv("B2A_LUFS_PAIR", pair)
 
     g = torch.Generator().manual_seed(sr + T)
     x = 0.2 * torch.randn(min(B, 4), C, T, generator=g) * (0.1 + torch.rand(min(B, 4), 1, 1, generator=g))

@@ -757,14 +757,12 @@ def test_pitch_shift_and_time_stretch_match_spec_oracle(eng):
 
 
 # ------------------------------------------------------------------------------------------
-# warp-autonomous K-weighting kernel (csrc/lufs.cu, namespace v2): rates with r != 0, rows of unequal phase, the
-# multi-window look-back (> 64 segments per row), short rows, unaligned lengths
+# warp-autonomous K-weighting kernel (csrc/lufs.cu): rates with r != 0, rows of unequal phase, rows cut into several
+# runs that each start with a warm-up (> 64 segments per row), short rows, unaligned lengths
 # ------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("pair", ["0", "1"])
 @pytest.mark.parametrize("sr,T,B,C", [(11025, 30001, 2, 1), (48000, 70000, 1, 2), (16000, 140001, 1, 1), (44100, 5000, 3, 2),
                                       (22050, 33333, 2, 2)])
-def test_lufs_warp_kernel_block_energies_and_loudness(eng, sr, T, B, C, pair, monkeypatch):
-    monkeypatch.setenv("B2A_LUFS_PAIR", pair)  # "1": the opt-in packed chunk-pair kernel (csrc/lufs.cu, namespace v4)
+def test_lufs_warp_kernel_block_energies_and_loudness(eng, sr, T, B, C):
     g = torch.Generator().manual_seed(sr + T)
     x = 0.2 * torch.randn(B, C, T, generator=g) * torch.rand(B, 1, 1, generator=g)
     x[0, 0, : T // 3] += 0.3  # DC step: exercises the long tail of the 38 Hz high-pass across many segments
