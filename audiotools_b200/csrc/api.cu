@@ -1,7 +1,22 @@
-// api.cu -- version + thread-local error message of libb2a.so (include/b2a.h).
+// api.cu -- version + thread-local error message of libb2a.so (include/b2a.h), and the SM count the persistent grids
+// are sized by.
+#include <atomic>
+
 #include "b2a_common.h"
 
 namespace b2a {
+int num_sms() {
+  constexpr int MAX_DEVICES = 64;
+  static std::atomic<int> cached[MAX_DEVICES];  // 0: not queried yet
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return B2A_NUM_SMS;
+  const bool cacheable = dev >= 0 && dev < MAX_DEVICES;
+  if (cacheable && (n = cached[dev].load(std::memory_order_relaxed)) > 0) return n;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = B2A_NUM_SMS;
+  if (cacheable) cached[dev].store(n, std::memory_order_relaxed);
+  return n;
+}
+
 char* err_buf() {
   static thread_local char buf[512] = {0};
   return buf;

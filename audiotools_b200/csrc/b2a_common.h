@@ -63,6 +63,25 @@ int fail(int code, const char* fmt, ...);
 
 namespace b2a {
 
+// SMs of the current device (cached per device ordinal; B2A_NUM_SMS when the attribute cannot be read)
+int num_sms();
+
+// shared-memory offsets are kept 16 B aligned (float4 / TMA access)
+inline int align16(int v) { return (v + 15) & ~15; }
+
+// Grid of a persistent 256-thread kernel: the CTAs resident at once with `smem` bytes of dynamic shared memory (at most
+// `max_per_sm` per SM when > 0) on every SM, but no more than `work` items, each CTA looping over the rest.
+template <class Kernel>
+int persistent_grid(Kernel kern, int smem, int64_t work, int64_t* grid, int max_per_sm = 0) {
+  int per_sm = 1;
+  B2A_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, (size_t)smem));
+  if (per_sm < 1) per_sm = 1;
+  if (max_per_sm > 0 && per_sm > max_per_sm) per_sm = max_per_sm;
+  const int64_t cap = (int64_t)num_sms() * per_sm;
+  *grid = work < cap ? work : cap;
+  return B2A_OK;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

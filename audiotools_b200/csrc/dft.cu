@@ -372,15 +372,9 @@ extern "C" int b2a_stft_dense_f32(const float* x, int64_t rows, int64_t T, int n
   B2A_REQUIRE(rows >= 1 && T >= 1, B2A_E_INVALID, "stft_dense: empty input");
   B2A_REQUIRE(T < (int64_t)1 << 30, B2A_E_UNSUPPORTED, "stft_dense: rows longer than 2^30 samples");
   B2A_REQUIRE(b2a_dft_supported(n_fft, hop), B2A_E_UNSUPPORTED, "stft_dense: window_length %d hop %d", n_fft, hop);
-  B2A_REQUIRE(pad >= 0 && right_pad >= 0 && drop_edge >= 0, B2A_E_INVALID, "stft_dense: negative padding");
-  B2A_REQUIRE(pad_mode >= 0 && pad_mode <= 2, B2A_E_UNSUPPORTED, "stft_dense: pad mode %d", pad_mode);
-  const int64_t Lp = T + 2 * (int64_t)pad + right_pad;
-  B2A_REQUIRE(n_fft / 2 < Lp, B2A_E_INVALID, "stft_dense: n_fft/2 (%d) must be < padded length (%lld)", n_fft / 2,
-              (long long)Lp);
-  B2A_REQUIRE(pad_mode != B2A_PAD_REFLECT || (pad + right_pad) < T || (pad + right_pad) == 0, B2A_E_INVALID,
-              "stft_dense: reflect padding (%d) must be < signal length (%lld)", pad + right_pad, (long long)T);
-  const int64_t nfr = b2a_stft_num_frames(T, n_fft, hop, pad, right_pad, drop_edge);
-  B2A_REQUIRE(nfr >= 1, B2A_E_INVALID, "stft_dense: no frames");
+  int64_t nfr;
+  const int rc = b2a::spectral::check_framing("stft_dense", T, n_fft, hop, pad, right_pad, pad_mode, drop_edge, &nfr);
+  if (rc != B2A_OK) return rc;
   FwdParams p;
   p.x = x; p.Mt = reinterpret_cast<const float2*>(matrix); p.out = reinterpret_cast<float2*>(stft_out);
   p.rows = (int)rows; p.T = (int)T; p.n_fft = n_fft; p.hop = hop; p.pad = pad; p.right_pad = right_pad;

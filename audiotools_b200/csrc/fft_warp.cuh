@@ -5,6 +5,8 @@
 //                      per frame, 32 points per lane, passes = radix 32 then radix LPF
 //   warp_fft           the forward N-point transform of a frame held by LPF lanes of one warp
 //   warp_fft_tables    its role-constant twiddle tables (shared memory, [slot][lane])
+//   load_frame         the windowed frame load in front of warp_fft (spectral.cu, loss.cu)
+//   partner_lane       the lane holding Z[N - k] (the real-FFT untangles of spectral.cu, loss.cu, istft.cu)
 #pragma once
 #include "b2a_common.h"
 
@@ -260,6 +262,45 @@ __device__ __forceinline__ float2 untangle_twiddle_m(const float2* ut, float2 u0
     case 13: return untangle_twiddle<LOG2N, 13>(ut, u0, l);
     case 14: return untangle_twiddle<LOG2N, 14>(ut, u0, l);
     default: return untangle_twiddle<LOG2N, 15>(ut, u0, l);
+  }
+}
+
+// ---- front end of a warp frame (spectral_warp_kernel and spectral_loss_kernel load it with the same instructions, so
+//      the fused loss transforms exactly the frames stft() does)
+
+// lane of the same frame that holds Z[N - k] for this lane's Z[k] (l = lane % LPF <-> LPF - l; lane 0 holds both itself)
+template <int LPF>
+__device__ __forceinline__ int partner_lane(int lane) {
+  return (lane & ~(LPF - 1)) | ((LPF - (lane & (LPF - 1))) & (LPF - 1));
+}
+
+// windowed frame, element e = l + LPF m; the first butterfly stage of the radix-32 pass (elements m and m + 16) is
+// formed right here with the window multiply fused in: a = s_m w_m, sum = fma(s_n, w_n, a), difference =
+// fma(-s_n, w_n, a)  (3 instead of 4 instructions per component pair).  Feeds warp_fft<LOG2N, true>.
+template <int LOG2N>
+__device__ __forceinline__ void load_frame(const float* fs, const float* win, int hop, float2 (&z)[32], int l) {
+  constexpr int LPF = WPlan<LOG2N>::LPF;
+  if ((hop & 1) == 0) {
+#pragma unroll
+    for (int m = 0; m < 16; ++m) {
+      const int e0 = l + LPF * m, e1 = e0 + LPF * 16;
+      const float2 s0 = *reinterpret_cast<const float2*>(fs + 2 * e0);
+      const float2 w0 = *reinterpret_cast<const float2*>(win + 2 * e0);
+      const float2 s1 = *reinterpret_cast<const float2*>(fs + 2 * e1);
+      const float2 w1 = *reinterpret_cast<const float2*>(win + 2 * e1);
+      const float2 a = mul2(s0, w0);
+      z[m] = fma2(s1, w1, a);
+      z[m + 16] = fma2(neg2(s1), w1, a);
+    }
+  } else {
+#pragma unroll
+    for (int m = 0; m < 16; ++m) {
+      const int e0 = l + LPF * m, e1 = e0 + LPF * 16;
+      const float ax = fs[2 * e0] * win[2 * e0], ay = fs[2 * e0 + 1] * win[2 * e0 + 1];
+      const float sx = fs[2 * e1], sy = fs[2 * e1 + 1], wx = win[2 * e1], wy = win[2 * e1 + 1];
+      z[m] = make_float2(fmaf(sx, wx, ax), fmaf(sy, wy, ay));
+      z[m + 16] = make_float2(fmaf(-sx, wx, ax), fmaf(-sy, wy, ay));
+    }
   }
 }
 

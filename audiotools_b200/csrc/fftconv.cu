@@ -252,13 +252,6 @@ static Layout layout(int64_t rows, int64_t T, int64_t n_filt, int64_t L) {
   return w;
 }
 
-static int num_sms() {
-  int dev = 0, n = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-    n = B2A_NUM_SMS;
-  return n;
-}
-
 static int run(const float* x, int64_t rows, int64_t T, const float* g, int64_t n_filt, int64_t L, int rows_per_filt,
                const int32_t* offset, int offset0, int pad_mode, const float* post_scale, int subtract,
                const int32_t* bypass, float* out, char* ws, const Layout& w, void* stream) {

@@ -218,28 +218,21 @@ extern "C" int b2a_stft_backward_f32(const float* grad_spec, int64_t rows, int64
                                      int drop_edge, float* grad_x, void* ws, size_t ws_bytes, void* stream) {
   B2A_REQUIRE(grad_spec && window && grad_x && ws, B2A_E_INVALID, "stft_backward: null pointer");
   B2A_REQUIRE(rows >= 1 && rows <= 65535 && T >= 1 && T < ((int64_t)1 << 30), B2A_E_INVALID, "stft_backward: bad shape");
-  B2A_REQUIRE(pad >= 0 && right_pad >= 0 && drop_edge >= 0, B2A_E_INVALID, "stft_backward: negative padding");
-  B2A_REQUIRE(pad_mode >= 0 && pad_mode <= 2, B2A_E_UNSUPPORTED, "stft_backward: pad mode %d", pad_mode);
   const Route r = route(n_fft, hop);
   B2A_REQUIRE(r != NONE, B2A_E_UNSUPPORTED,
               "stft_backward: window_length %d hop %d (hop <= window_length; powers of two up to 32768, any other length "
               "up to 8192)", n_fft, hop);
   B2A_REQUIRE(r != DENSE || amatrix, B2A_E_INVALID, "stft_backward: window_length %d needs the adjoint DFT matrix", n_fft);
-  const int64_t Lp = T + 2 * (int64_t)pad + right_pad;
-  B2A_REQUIRE(n_fft / 2 < Lp, B2A_E_INVALID, "stft_backward: n_fft/2 (%d) must be < padded length (%lld)", n_fft / 2,
-              (long long)Lp);
-  B2A_REQUIRE(pad_mode != B2A_PAD_REFLECT || (pad + right_pad) < T || (pad + right_pad) == 0, B2A_E_INVALID,
-              "stft_backward: reflect padding (%d) must be < signal length (%lld)", pad + right_pad, (long long)T);
-  const int64_t nfr = b2a_stft_num_frames(T, n_fft, hop, pad, right_pad, drop_edge);
-  B2A_REQUIRE(nfr >= 1, B2A_E_INVALID, "stft_backward: no frames");
+  int64_t nfr;
+  int rc = b2a::spectral::check_framing("stft_backward", T, n_fft, hop, pad, right_pad, pad_mode, drop_edge, &nfr);
+  if (rc != B2A_OK) return rc;
   B2A_REQUIRE(ws_bytes >= b2a_stft_backward_workspace_bytes(rows, T, n_fft, hop, pad, right_pad, drop_edge),
               B2A_E_INVALID, "stft_backward: workspace too small");
   B2A_REQUIRE(((uintptr_t)grad_spec & 7) == 0 && ((uintptr_t)ws & 7) == 0, B2A_E_INVALID,
               "stft_backward: spectra and workspace must be 8-byte aligned");
   const int half = n_fft / 2;
-  const int64_t Lpp = Lp + 2 * (int64_t)half;
+  const int64_t Lpp = T + 2 * ((int64_t)half + pad) + right_pad;  // the padded signal and the centre padding
   float* gp = reinterpret_cast<float*>(ws);
-  int rc;
   // 1. adjoint transform + overlap-add (no envelope) over the whole padded range; the dropped frames are zero frames
   if (r == WARP) {
     rc = b2a::istft::run(grad_spec, rows, nfr, n_fft, hop, window, drop_edge, 0, Lpp, gp, 1, stream);

@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(256, 2) istft_kernel(const Params p) {
   // 1/N of the transform and the 1/2 of the even/odd split; the adjoint wants sum_k Re(G_k e^{i theta}) = n_fft/2 times
   // the inverse of the DC / Nyquist-doubled spectrum
   const float inv_n = p.adjoint ? 0.5f : 0.5f / (float)N;
-  const int src_lane = (lane & ~(LPF - 1)) | ((LPF - l) & (LPF - 1));  // holder of the partner element N - k
+  const int src_lane = partner_lane<LPF>(lane);  // holder of the partner element N - k
   const int tail = NFFT - hop;                   // samples a group hands to the next one
   const int items = p.rows * p.segs_per_row;
   // gather roles: RL residue lanes x QL hop lanes (hop >= 256: every thread owns residues and walks all hops)
@@ -259,19 +259,6 @@ __global__ void __launch_bounds__(256, 2) istft_kernel(const Params p) {
   }
 }
 
-static int num_sms() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess ||
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = B2A_NUM_SMS;
-  }
-  return n;
-}
-
-static inline int align16(int v) { return (v + 15) & ~15; }
-
 template <int LOG2N>
 static int launch(Params& p, void* stream) {
   using PL = WPlan<LOG2N>;
@@ -288,10 +275,9 @@ static int launch(Params& p, void* stream) {
   p.off_reg = o; o = align16(o + G * FS * 4);
   B2A_REQUIRE(o <= 227 * 1024, B2A_E_UNSUPPORTED, "istft: n_fft=%d needs %d bytes of shared memory", NFFT, o);
   B2A_CUDA_OK(cudaFuncSetAttribute(istft_kernel<LOG2N>, cudaFuncAttributeMaxDynamicSharedMemorySize, o));
-  int per_sm = 1;
-  B2A_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, istft_kernel<LOG2N>, 256, (size_t)o));
-  if (per_sm < 1) per_sm = 1;
-  const int64_t cap = (int64_t)num_sms() * per_sm;
+  int64_t cap;  // resident CTAs: the work list below is sized from them
+  const int rc = persistent_grid(istft_kernel<LOG2N>, o, INT64_MAX, &cap);
+  if (rc != B2A_OK) return rc;
   // groups: every sample below `expected` (and below start + out_len) must be finalised by some group
   const int NP = p.n_frames + 2 * p.pad_frames;
   long long need = p.start + p.out_len;

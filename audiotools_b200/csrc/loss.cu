@@ -92,13 +92,9 @@ __device__ __forceinline__ float2 along(float d, float2 v) {
   return make_float2(v.x * r, v.y * r);
 }
 
-// mel of filter m from the frame's magnitudes (the banded FP32 sum of spectral.cu, ascending k)
+// mel of filter m from the frame's magnitudes (the banded FP32 sum of spectral.cu)
 __device__ __forceinline__ float project(const LossParams& q, int F, int m, const float* mag) {
-  const int lo = __ldg(q.mel_lo + m), hi = __ldg(q.mel_hi + m);
-  const float* w = q.mel_fb + (size_t)m * F;
-  float acc = 0.f;
-  for (int k = lo; k < hi; ++k) acc = fmaf(__ldg(w + k), mag[k], acc);
-  return acc;
+  return spectral::mel_band(q.mel_fb, q.mel_lo, q.mel_hi, F, m, mag);
 }
 
 // sum over the filters whose band holds bin k of fb[m][k] g[m] (mel_backward_kernel's transposed projection)
@@ -113,29 +109,7 @@ __device__ __forceinline__ float back_project(const LossParams& q, int F, int k,
 template <int LOG2N>
 __device__ __forceinline__ void frame_fft(const float* fs, const float* win, int hop, float2 (&z)[32], float* xb,
                                           const float2* tw, int l) {
-  constexpr int LPF = WPlan<LOG2N>::LPF;
-  if ((hop & 1) == 0) {
-#pragma unroll
-    for (int m = 0; m < 16; ++m) {
-      const int e0 = l + LPF * m, e1 = e0 + LPF * 16;
-      const float2 s0 = *reinterpret_cast<const float2*>(fs + 2 * e0);
-      const float2 w0 = *reinterpret_cast<const float2*>(win + 2 * e0);
-      const float2 s1 = *reinterpret_cast<const float2*>(fs + 2 * e1);
-      const float2 w1 = *reinterpret_cast<const float2*>(win + 2 * e1);
-      const float2 a = mul2(s0, w0);
-      z[m] = fma2(s1, w1, a);
-      z[m + 16] = fma2(neg2(s1), w1, a);
-    }
-  } else {
-#pragma unroll
-    for (int m = 0; m < 16; ++m) {
-      const int e0 = l + LPF * m, e1 = e0 + LPF * 16;
-      const float ax = fs[2 * e0] * win[2 * e0], ay = fs[2 * e0 + 1] * win[2 * e0 + 1];
-      const float sx = fs[2 * e1], sy = fs[2 * e1 + 1], wx = win[2 * e1], wy = win[2 * e1 + 1];
-      z[m] = make_float2(fmaf(sx, wx, ax), fmaf(sy, wy, ay));
-      z[m + 16] = make_float2(fmaf(-sx, wx, ax), fmaf(-sy, wy, ay));
-    }
-  }
+  spectral::load_frame<LOG2N>(fs, win, hop, z, l);
   spectral::warp_fft<LOG2N, true>(z, xb, tw, l);
 }
 
@@ -178,7 +152,7 @@ __global__ void __launch_bounds__(256, 2) spectral_loss_kernel(LossParams q) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int hop = p.hop, F = N + 1, nf = p.n_frames;
   const int l = lane & (LPF - 1), fw = lane / LPF;
-  const int src_lane = (lane & ~(LPF - 1)) | ((LPF - l) & (LPF - 1));  // holder of Z[N - k]
+  const int src_lane = spectral::partner_lane<LPF>(lane);           // holder of Z[N - k]
   const int f = warp * FPW + fw;                                         // frame within the tile = its slot
   float* xb = reinterpret_cast<float*>(smem + q.off_slot) + f * q.slot;  // exchange plane, then |.| of the frame
   float* mel_y = xb + LPlan<LOG2N>::EX;                                   // mel: mel_y, then dL/dmel_y
@@ -343,8 +317,6 @@ __global__ void __launch_bounds__(32) loss_finalize_kernel(const double* __restr
   if (lane == 0) out[0] = (float)(wl * sl + wm * sm);
 }
 
-static inline int align16(int v) { return (v + 15) & ~15; }
-
 constexpr int MAX_CTAS_PER_SM = 8;  // 256-thread CTAs: the partials buffer holds this many per SM
 
 // shared-memory layout of one launch; returns the bytes
@@ -391,14 +363,12 @@ static int launch(LossParams& q, int64_t numel, double log_weight, double mag_we
   B2A_REQUIRE(total < (int64_t)2147483647, B2A_E_UNSUPPORTED, "spectral_loss: too many tiles");
   auto kern = q.mel_fb ? spectral_loss_kernel<LOG2N, true> : spectral_loss_kernel<LOG2N, false>;
   B2A_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, o));
-  int per_sm = 1;
-  B2A_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, (size_t)o));
-  per_sm = per_sm < 1 ? 1 : (per_sm > MAX_CTAS_PER_SM ? MAX_CTAS_PER_SM : per_sm);
-  const int64_t cap = (int64_t)spectral::num_sms() * per_sm;
-  const int grid = (int)(total < cap ? total : cap);
+  int64_t grid;
+  const int rc = persistent_grid(kern, o, total, &grid, MAX_CTAS_PER_SM);
+  if (rc != B2A_OK) return rc;
   B2A_LAUNCH(kern, dim3((unsigned)grid), dim3(256), (size_t)o, stream, q);
   B2A_CUDA_OK(cudaGetLastError());
-  B2A_LAUNCH(loss_finalize_kernel, dim3(1), dim3(32), 0, stream, q.partial, grid, log_weight / (double)numel,
+  B2A_LAUNCH(loss_finalize_kernel, dim3(1), dim3(32), 0, stream, q.partial, (int)grid, log_weight / (double)numel,
              mag_weight / (double)numel, loss_out);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
@@ -418,7 +388,7 @@ extern "C" int b2a_spectral_loss_supported(int n_fft, int hop, int n_mels) {
 
 extern "C" size_t b2a_spectral_loss_workspace_bytes(int n_fft, int hop, int n_mels) {
   if (!b2a_spectral_loss_supported(n_fft, hop, n_mels)) return 0;
-  return (size_t)b2a::spectral::num_sms() * MAX_CTAS_PER_SM * 2 * sizeof(double);
+  return (size_t)b2a::num_sms() * MAX_CTAS_PER_SM * 2 * sizeof(double);
 }
 
 extern "C" int b2a_spectral_loss_f32(const float* x, const float* y, int64_t rows, int64_t T, int n_fft, int hop,
@@ -433,19 +403,13 @@ extern "C" int b2a_spectral_loss_f32(const float* x, const float* y, int64_t row
   B2A_REQUIRE(hop >= 1 && hop <= n_fft, B2A_E_INVALID, "spectral_loss: hop_length must be in [1, window_length]");
   B2A_REQUIRE(pow2_window(n_fft), B2A_E_UNSUPPORTED,
               "spectral_loss: window_length must be a power of two in [64, 2048] (got %d)", n_fft);
-  B2A_REQUIRE(pad >= 0 && right_pad >= 0 && drop_edge >= 0, B2A_E_INVALID, "spectral_loss: negative padding");
-  B2A_REQUIRE(pad_mode >= 0 && pad_mode <= 2, B2A_E_UNSUPPORTED, "spectral_loss: pad mode %d", pad_mode);
   const bool mel = mel_fb != nullptr;
   B2A_REQUIRE(!mel || (mel_lo && mel_hi && bin_lo && bin_hi && n_mels >= 1), B2A_E_INVALID,
               "spectral_loss: mel arguments");
   B2A_REQUIRE(clamp_eps > 0.f && power > 0.f, B2A_E_INVALID, "spectral_loss: clamp_eps and pow must be > 0");
-  const int64_t Lp = T + 2 * (int64_t)pad + right_pad;
-  B2A_REQUIRE(n_fft / 2 < Lp, B2A_E_INVALID, "spectral_loss: n_fft/2 (%d) must be < padded length (%lld)", n_fft / 2,
-              (long long)Lp);
-  B2A_REQUIRE(pad_mode != B2A_PAD_REFLECT || (pad + right_pad) < T || (pad + right_pad) == 0, B2A_E_INVALID,
-              "spectral_loss: reflect padding (%d) must be < signal length (%lld)", pad + right_pad, (long long)T);
-  const int64_t nfr = b2a_stft_num_frames(T, n_fft, hop, pad, right_pad, drop_edge);
-  B2A_REQUIRE(nfr >= 1, B2A_E_INVALID, "spectral_loss: no frames");
+  int64_t nfr;
+  const int rc = b2a::spectral::check_framing("spectral_loss", T, n_fft, hop, pad, right_pad, pad_mode, drop_edge, &nfr);
+  if (rc != B2A_OK) return rc;
   B2A_REQUIRE(workspace_bytes >= b2a_spectral_loss_workspace_bytes(n_fft, hop, mel ? n_mels : 0) &&
                   ((uintptr_t)workspace & 7) == 0,
               B2A_E_INVALID, "spectral_loss: workspace too small or not 8-byte aligned");

@@ -534,15 +534,12 @@ static int run(const float* x, int64_t B, int C, int64_t T, int64_t Tp, const Ge
   }
   char* base = (char*)ws;
   B2A_CUDA_OK(cudaMemsetAsync(base, 0, w.zeroed_bytes, (cudaStream_t)stream));
-  int sms = B2A_NUM_SMS, dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-    sms = B2A_NUM_SMS;
   // runs per row: as many as there are resident warps for (one CTA of 12 warps per SM), but long enough that the
   // warm-up (n_warm segments in front of every run but the first) stays a small fraction of the work
 #ifdef B2A_SIM
   const int64_t resident = 1;
 #else
-  const int64_t resident = sms;
+  const int64_t resident = num_sms();
 #endif
   const double rho = max_pole_radius<NS>(cf);
   B2A_REQUIRE(rho < 1.0, B2A_E_UNSUPPORTED, "lufs: unstable filter (pole radius %g)", rho);

@@ -327,8 +327,6 @@ __global__ void __launch_bounds__(THREADS) spectral_kernel(Params p) {
   }
 }
 
-static inline int align16(int v) { return (v + 15) & ~15; }
-
 template <int LOG2N>
 static int launch(Params& p, void* stream) {
   using PL = Plan<LOG2N>;
@@ -466,7 +464,7 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
   }
 
   float* xb = xbs + (warp * FPW + fw) * p.xb_stride;
-  const int src_lane = (lane & ~(LPF - 1)) | ((LPF - l) & (LPF - 1));  // holder of Z[N - k]
+  const int src_lane = partner_lane<LPF>(lane);  // holder of Z[N - k]
 
 #ifdef B2A_K1_PROBE
   int it_probe = 0;
@@ -505,32 +503,9 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
       const bool live = n < p.n_frames;
       const float* fs = sp + f * hop;
 
-      // ---- windowed frame, element e = l + LPF m; the first butterfly stage of the radix-32 pass (elements m and
-      //      m + 16) is formed right here with the window multiply fused in: a = s_m w_m, sum = fma(s_n, w_n, a),
-      //      difference = fma(-s_n, w_n, a)  (3 instead of 4 instructions per component pair)
+      // ---- windowed frame with the first radix-32 butterfly fused in
       float2 z[32];
-      if ((hop & 1) == 0) {
-#pragma unroll
-        for (int m = 0; m < 16; ++m) {
-          const int e0 = l + LPF * m, e1 = e0 + LPF * 16;
-          const float2 s0 = *reinterpret_cast<const float2*>(fs + 2 * e0);
-          const float2 w0 = *reinterpret_cast<const float2*>(win + 2 * e0);
-          const float2 s1 = *reinterpret_cast<const float2*>(fs + 2 * e1);
-          const float2 w1 = *reinterpret_cast<const float2*>(win + 2 * e1);
-          const float2 a = mul2(s0, w0);
-          z[m] = fma2(s1, w1, a);
-          z[m + 16] = fma2(neg2(s1), w1, a);
-        }
-      } else {
-#pragma unroll
-        for (int m = 0; m < 16; ++m) {
-          const int e0 = l + LPF * m, e1 = e0 + LPF * 16;
-          const float ax = fs[2 * e0] * win[2 * e0], ay = fs[2 * e0 + 1] * win[2 * e0 + 1];
-          const float sx = fs[2 * e1], sy = fs[2 * e1 + 1], wx = win[2 * e1], wy = win[2 * e1 + 1];
-          z[m] = make_float2(fmaf(sx, wx, ax), fmaf(sy, wy, ay));
-          z[m + 16] = make_float2(fmaf(-sx, wx, ax), fmaf(-sy, wy, ay));
-        }
-      }
+      load_frame<LOG2N>(fs, win, hop, z, l);
       K1_STAMP(4);
       if (rd == FR / G - 1) {
         // every warp holds its last frame in registers: the span buffer is dead, so the next tile's
@@ -655,11 +630,7 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
           const int f = fc + fl;
           const float* xf = xbs + f * p.xb_stride;
           for (int mm = 4 * warp + jq; mm < p.n_mels; mm += 32) {
-            const int lo = __ldg(p.mel_lo + mm), hi = __ldg(p.mel_hi + mm);
-            const float* wrow = p.mel_fb + (size_t)mm * F;
-            float acc = 0.f;
-            for (int k = lo; k < hi; ++k) acc = fmaf(__ldg(wrow + k), xf[k], acc);
-            acc *= ga;
+            float acc = mel_band(p.mel_fb, p.mel_lo, p.mel_hi, F, mm, xf) * ga;
             if (p.post == B2A_POST_LOG10) acc = lscale * fast_log2(fmaxf(acc, p.post_eps));
             else if (p.post == B2A_POST_LN) acc = logf(acc + p.post_eps);
             if (f < nf) mo[(size_t)mm * p.n_frames + f] = acc;
@@ -687,16 +658,6 @@ __global__ void __launch_bounds__(256, 2) spectral_warp_kernel(Params p) {
     ++it_probe;
 #endif
   }
-}
-
-int num_sms() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = B2A_NUM_SMS;
-  }
-  return n;
 }
 
 #ifdef B2A_K1_PROBE
@@ -740,15 +701,16 @@ static int launch_warp(Params& p, void* stream) {
                            : (p.stft_out ? spectral_warp_kernel<LOG2N, 2> : spectral_warp_kernel<LOG2N, 0>);
   B2A_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, o));
   // persistent: as many CTAs as are resident at once (2 per SM by registers / shared memory), each loops over tiles
-  int per_sm = 1;
-  B2A_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, (size_t)o));
-  if (per_sm < 1) per_sm = 1;
-  const int64_t cap = (int64_t)num_sms() * per_sm;
-  const unsigned grid = (unsigned)(total < cap ? total : cap);
+  int64_t grid;
+  const int rc = persistent_grid(kern, o, total, &grid);
+  if (rc != B2A_OK) return rc;
 #ifdef B2A_K1_PROBE
-  if (LOG2N == 10 && !p.stft_out) { g_k1_last[0] = per_sm; g_k1_last[1] = (int)grid; g_k1_last[2] = o; }
+  if (LOG2N == 10 && !p.stft_out) {
+    B2A_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&g_k1_last[0], kern, 256, (size_t)o));
+    g_k1_last[1] = (int)grid; g_k1_last[2] = o;
+  }
 #endif
-  B2A_LAUNCH(kern, dim3(grid), dim3(256), (size_t)o, stream, p);
+  B2A_LAUNCH(kern, dim3((unsigned)grid), dim3(256), (size_t)o, stream, p);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }
@@ -770,6 +732,21 @@ int frames_fft(const float* x, int rows, int T, int n_fft, int hop, const float*
     case 2048: return launch_warp<10>(p, stream);
   }
   return b2a::fail(B2A_E_UNSUPPORTED, "frames_fft: block size %d", n_fft);
+}
+
+int check_framing(const char* who, int64_t T, int n_fft, int hop, int pad, int right_pad, int pad_mode, int drop_edge,
+                  int64_t* n_frames) {
+  B2A_REQUIRE(pad >= 0 && right_pad >= 0 && drop_edge >= 0, B2A_E_INVALID, "%s: negative padding", who);
+  B2A_REQUIRE(pad_mode >= 0 && pad_mode <= 2, B2A_E_UNSUPPORTED, "%s: pad mode %d", who, pad_mode);
+  const int64_t Lp = T + 2 * (int64_t)pad + right_pad;
+  // torch raises for these (reflect padding wider than the signal)
+  B2A_REQUIRE(n_fft / 2 < Lp, B2A_E_INVALID, "%s: n_fft/2 (%d) must be < padded length (%lld)", who, n_fft / 2,
+              (long long)Lp);
+  B2A_REQUIRE(pad_mode != B2A_PAD_REFLECT || (pad + right_pad) < T || (pad + right_pad) == 0, B2A_E_INVALID,
+              "%s: reflect padding (%d) must be < signal length (%lld)", who, pad + right_pad, (long long)T);
+  *n_frames = b2a_stft_num_frames(T, n_fft, hop, pad, right_pad, drop_edge);
+  B2A_REQUIRE(*n_frames >= 1, B2A_E_INVALID, "%s: no frames", who);
+  return B2A_OK;
 }
 
 }  // namespace spectral
@@ -796,16 +773,9 @@ extern "C" int b2a_spectral_f32(const float* x, int64_t rows, int64_t T, int n_f
   B2A_REQUIRE(n_fft >= 32 && n_fft <= 4096 && (n_fft & (n_fft - 1)) == 0, B2A_E_UNSUPPORTED,
               "spectral: window_length must be a power of two in [32, 4096] (got %d)", n_fft);
   B2A_REQUIRE(hop >= 1, B2A_E_INVALID, "spectral: hop_length must be >= 1");
-  B2A_REQUIRE(pad >= 0 && right_pad >= 0 && drop_edge >= 0, B2A_E_INVALID, "spectral: negative padding");
-  B2A_REQUIRE(pad_mode >= 0 && pad_mode <= 2, B2A_E_UNSUPPORTED, "spectral: pad mode %d", pad_mode);
-  const int64_t Lp = T + 2 * (int64_t)pad + right_pad;
-  // torch raises for these (reflect padding wider than the signal)
-  B2A_REQUIRE(n_fft / 2 < Lp, B2A_E_INVALID, "spectral: n_fft/2 (%d) must be < padded length (%lld)", n_fft / 2,
-              (long long)Lp);
-  B2A_REQUIRE(pad_mode != B2A_PAD_REFLECT || (pad + right_pad) < T || (pad + right_pad) == 0, B2A_E_INVALID,
-              "spectral: reflect padding (%d) must be < signal length (%lld)", pad + right_pad, (long long)T);
-  const int64_t nfr = b2a_stft_num_frames(T, n_fft, hop, pad, right_pad, drop_edge);
-  B2A_REQUIRE(nfr >= 1, B2A_E_INVALID, "spectral: no frames");
+  int64_t nfr;
+  const int rc = check_framing("spectral", T, n_fft, hop, pad, right_pad, pad_mode, drop_edge, &nfr);
+  if (rc != B2A_OK) return rc;
   B2A_REQUIRE(!y_out || (pad == 0 && right_pad == 0 && drop_edge == 0), B2A_E_UNSUPPORTED,
               "spectral: y_out needs pad == right_pad == drop_edge == 0");
   B2A_REQUIRE(!gain || rows_per_gain >= 1, B2A_E_INVALID, "spectral: rows_per_gain");

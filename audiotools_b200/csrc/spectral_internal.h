@@ -77,8 +77,22 @@ __device__ __forceinline__ bool stage_span_async(const Params& p, float* sp, int
   return false;
 }
 
-// SMs of the current device (persistent grids)
-int num_sms();
+// banded mel projection of filter m: sum over its band k in [mel_lo[m], mel_hi[m]) of fb[m][k] mag[k], ascending k, so
+// that the fused loss projects exactly as the forward kernels do
+__device__ __forceinline__ float mel_band(const float* fb, const int32_t* mel_lo, const int32_t* mel_hi, int F, int m,
+                                          const float* mag) {
+  const int lo = __ldg(mel_lo + m), hi = __ldg(mel_hi + m);
+  const float* w = fb + (size_t)m * F;
+  float acc = 0.f;
+  for (int k = lo; k < hi; ++k) acc = fmaf(__ldg(w + k), mag[k], acc);
+  return acc;
+}
+
+// torch's stft(center=True) framing of the explicitly padded signal (F.pad(pad, pad + right_pad, pad_mode), then the
+// centre reflect), shared by every STFT entry point: B2A_OK and the frame count, or the error code with the message
+// prefixed by `who`.
+int check_framing(const char* who, int64_t T, int n_fft, int hop, int pad, int right_pad, int pad_mode, int drop_edge,
+                  int64_t* n_frames);
 
 // Tensor-core (wgmma) variant of the fused kernel for n_fft = 2048 mel / log-mel launches (spectral_tc.cu).
 // tc_supported: the launch can take that path (geometry, shared memory, switched on by b2a_spectral_tc_enable).

@@ -540,11 +540,7 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
         }
       } else {
         for (int mm = 4 * w8 + jq; mm < p.n_mels; mm += 32) {
-          const int lo = __ldg(p.mel_lo + mm), hi = __ldg(p.mel_hi + mm);
-          const float* wrow = p.mel_fb + (size_t)mm * F;
-          float acc = 0.f;
-          for (int k = lo; k < hi; ++k) acc = fmaf(__ldg(wrow + k), xf[k], acc);
-          acc *= ga;
+          float acc = mel_band(p.mel_fb, p.mel_lo, p.mel_hi, F, mm, xf) * ga;
           if (p.post == B2A_POST_LOG10) acc = lscale * fast_log2(fmaxf(acc, p.post_eps));
           else if (p.post == B2A_POST_LN) acc = logf(acc + p.post_eps);
           melt[mm * (FR + 1) + f] = acc;
@@ -569,13 +565,6 @@ __global__ void __launch_bounds__(THREADS, 1) spectral_tc_kernel(const B2A_GRID_
 
 // Opt-in: the FP32 warp kernel is the default; b2a_spectral_tc_enable(1) selects the tensor-core path.
 static int g_tc_enabled = 0;
-
-static int tc_num_sms() {
-  int n = 0, dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-    n = B2A_NUM_SMS;
-  return n;
-}
 
 bool tc_supported(const Params& p) {
   if (!g_tc_enabled) return false;
@@ -608,7 +597,7 @@ int launch_tc(Params& p, void* stream) {
   const int64_t total = (int64_t)p.rows * p.n_tiles;
   B2A_REQUIRE(total < (int64_t)2147483647, B2A_E_UNSUPPORTED, "spectral_tc: too many tiles");
   B2A_CUDA_OK(cudaFuncSetAttribute(tc::spectral_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kp.s.total));
-  const int64_t cap = tc_num_sms();
+  const int64_t cap = num_sms();
   const unsigned grid = (unsigned)(total < cap ? total : cap);
   B2A_LAUNCH(tc::spectral_tc_kernel, dim3(grid), dim3(tc::THREADS), (size_t)kp.s.total, stream, kp);
   B2A_CUDA_OK(cudaGetLastError());

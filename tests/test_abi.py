@@ -65,6 +65,54 @@ def test_bad_arguments_return_codes_not_crashes(lib):
         lib.check(rc)
 
 
+# every forward / backward STFT entry point checks torch's stft(center=True) framing of the padded signal with the
+# same codes and messages, before any CUDA call
+FRAMING_ENTRY_POINTS = {  # prefix of the message, n_fft, hop
+    "spectral": (512, 128),
+    "stft_large": (8192, 2048),
+    "stft_dense": (500, 125),
+    "stft_backward": (512, 128),
+    "spectral_loss": (512, 128),
+}
+FRAMING_FAILURES = {  # (T, pad, right_pad, pad_mode, drop_edge) as functions of n_fft -> (code, message)
+    "negative_padding": (lambda n: (n, -1, 0, 0, 0), lambda n: (-1, "negative padding")),
+    "pad_mode": (lambda n: (n, 0, 0, 5, 0), lambda n: (-2, "pad mode 5")),
+    "short_signal": (lambda n: (n // 4, 0, 0, 0, 0),
+                     lambda n: (-1, f"n_fft/2 ({n // 2}) must be < padded length ({n // 4})")),
+    "reflect_padding": (lambda n: (n, n, 0, 0, 0), lambda n: (-1, f"reflect padding ({n}) must be < signal length ({n})")),
+    "no_frames": (lambda n: (n, 0, 0, 0, 100), lambda n: (-1, "no frames")),
+}
+
+
+def _call_framed(lib, who, T, n_fft, hop, pad, right_pad, pad_mode, drop_edge):
+    buf = (ctypes.c_float * 1024)()
+    p = ctypes.cast(buf, ctypes.c_void_p)
+    if who == "spectral":
+        return lib.b2a_spectral_f32(p, 1, T, n_fft, hop, p, pad, right_pad, pad_mode, drop_edge, None, 1, None, None,
+                                    None, None, 0, 0, 0, 0.0, 1.0, None, p, None)
+    if who == "stft_large":
+        return lib.b2a_stft_large_f32(p, 1, T, n_fft, hop, p, pad, right_pad, pad_mode, drop_edge, p, None)
+    if who == "stft_dense":
+        return lib.b2a_stft_dense_f32(p, 1, T, n_fft, hop, p, pad, right_pad, pad_mode, drop_edge, p, None)
+    if who == "stft_backward":
+        return lib.b2a_stft_backward_f32(p, 1, T, n_fft, hop, p, None, pad, right_pad, pad_mode, drop_edge, p, p, 4096,
+                                         None)
+    return lib.b2a_spectral_loss_f32(p, p, 1, T, n_fft, hop, p, pad, right_pad, pad_mode, drop_edge, None, None, None,
+                                     None, None, 0, 1e-5, 2.0, 1.0, 1.0, p, None, None, p, 4096, None)
+
+
+@pytest.mark.parametrize("failure", sorted(FRAMING_FAILURES))
+@pytest.mark.parametrize("who", sorted(FRAMING_ENTRY_POINTS))
+def test_framing_failures_have_one_code_and_message(lib, who, failure):
+    n_fft, hop = FRAMING_ENTRY_POINTS[who]
+    shape, expect = FRAMING_FAILURES[failure]
+    T, pad, right_pad, pad_mode, drop_edge = shape(n_fft)
+    code, msg = expect(n_fft)
+    rc = _call_framed(lib, who, T, n_fft, hop, pad, right_pad, pad_mode, drop_edge)
+    assert rc == code
+    assert lib.b2a_last_error() == f"{who}: {msg}".encode()
+
+
 def test_missing_library_fails_loudly(tmp_path):
     with pytest.raises(ImportError, match="no CPU fallback"):
         _lib.B2ALibrary(str(tmp_path / "libb2a.so"))
