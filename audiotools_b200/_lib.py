@@ -14,6 +14,7 @@ LIB_PATH = os.environ.get("B2A_LIB_PATH") or os.path.join(HERE, "csrc", "libb2a.
 B2A_OK = 0
 PAD_MODES = {"reflect": 0, "constant": 1, "replicate": 2}
 POST_NONE, POST_LOG10, POST_LN = 0, 1, 2
+ROUTE_NONE, ROUTE_FFT, ROUTE_LARGE, ROUTE_DENSE = 0, 1, 2, 3  # b2a_stft_route
 
 # name -> (restype, argtypes); must list every symbol include/b2a.h declares
 SIGNATURES = {
@@ -72,7 +73,6 @@ SIGNATURES = {
     "b2a_spec_gate_f32": (c_int, [c_void_p, c_int64, c_int, c_int64, c_void_p, c_int64, c_int64, c_float, c_void_p, c_int,
                                   POINTER(c_float), c_int, POINTER(c_float), c_int, c_void_p, c_void_p, c_void_p]),
     "b2a_alter_drr_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_float, c_void_p]),
-    "b2a_dft_supported": (c_int, [c_int, c_int]),
     "b2a_dft_matrix_floats": (c_size_t, [c_int, c_int]),
     "b2a_dft_matrix_f32": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "b2a_stft_dense_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int,
@@ -80,16 +80,12 @@ SIGNATURES = {
     "b2a_mel_from_stft_f32": (c_int, [c_void_p, c_int64, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                       c_float, c_float, c_void_p, c_void_p]),
     "b2a_mel_dct_f32": (c_int, [c_void_p, c_int64, c_int, c_int64, c_void_p, c_int, c_void_p, c_void_p]),
-    "b2a_istft_dense_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int]),
-    "b2a_istft_dense_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_int, c_int64,
-                                    c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "b2a_stft_large_supported": (c_int, [c_int, c_int, c_int]),
+    "b2a_stft_route": (c_int, [c_int, c_int, c_int]),
+    "b2a_istft_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_int]),
+    "b2a_istft_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_int, c_int64, c_int64,
+                              c_void_p, c_void_p, c_size_t, c_void_p]),
     "b2a_stft_large_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int,
                                    c_void_p, c_void_p]),
-    "b2a_istft_large_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int]),
-    "b2a_istft_large_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_int, c_int64, c_int64,
-                                    c_void_p, c_void_p, c_size_t, c_void_p]),
-    "b2a_stft_backward_supported": (c_int, [c_int, c_int]),
     "b2a_stft_backward_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_int, c_int, c_int, c_int]),
     "b2a_stft_backward_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                       c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
@@ -103,9 +99,6 @@ SIGNATURES = {
     "b2a_spectral_loss_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_int, c_int, c_int,
                                       c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_float,
                                       c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "b2a_istft_supported": (c_int, [c_int, c_int]),
-    "b2a_istft_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_int, c_int64, c_int64, c_void_p,
-                              c_void_p]),
     "b2a_fir_direct_supported": (c_int, [c_int64, c_int, c_int]),
     "b2a_fir_direct_f32": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int, c_int, c_void_p, c_int, c_int,
                                    c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),

@@ -144,10 +144,9 @@ MAX_MELS = 1600      # mel filters of the mel backward (their gradients for 32 f
 
 def check_supported(method: str, n_fft: int, hop: int, rows: int, n_mels: int = 0):
     """Raise at forward time, not inside backward(), for a geometry without a backward pass."""
-    if not _engine().backward_supported(n_fft, hop):
-        raise NotImplementedError(
-            f"{method}: no backward for window_length {n_fft} hop {hop}: gradients through the STFT need "
-            "hop <= window_length and a window of any length up to 8192 or a power of two up to 32768")
+    eng = _engine()
+    if not eng.backward_supported(n_fft, hop):
+        raise eng.route_error(n_fft, hop, 1, backward_of=method)
     if rows > MAX_ROWS or n_mels > MAX_MELS:
         raise NotImplementedError(f"{method}: no backward for {rows} rows (items x channels) / {n_mels} mel filters: "
                                   f"gradients support up to {MAX_ROWS} rows and {MAX_MELS} mel filters")

@@ -344,7 +344,8 @@ static inline int np_of(int n_fft) { return round_up(n_fft, BN); }          // s
 static inline int fp_of(int n_fft) { return round_up(n_fft / 2 + 1, BN); }  // bins, padded for the forward tile
 static inline int fq_of(int n_fft) { return round_up(n_fft / 2 + 1, BK); }  // bins, padded for the inverse reduction
 
-extern "C" int b2a_dft_supported(int n_fft, int hop) { return n_fft >= 2 && n_fft <= 8192 && hop >= 1; }
+// the window lengths of the dense DFT: any n_fft in [2, 8192], powers of two included (the inverse: 1 <= hop <= n_fft)
+static bool supported(int n_fft, int hop) { return n_fft >= 2 && n_fft <= 8192 && hop >= 1; }
 
 extern "C" size_t b2a_dft_matrix_floats(int n_fft, int inverse) {
   if (n_fft < 2 || n_fft > 8192 || inverse < 0 || inverse > 2) return 0;
@@ -371,7 +372,7 @@ extern "C" int b2a_stft_dense_f32(const float* x, int64_t rows, int64_t T, int n
   B2A_REQUIRE(x && matrix && stft_out, B2A_E_INVALID, "stft_dense: null pointer");
   B2A_REQUIRE(rows >= 1 && T >= 1, B2A_E_INVALID, "stft_dense: empty input");
   B2A_REQUIRE(T < (int64_t)1 << 30, B2A_E_UNSUPPORTED, "stft_dense: rows longer than 2^30 samples");
-  B2A_REQUIRE(b2a_dft_supported(n_fft, hop), B2A_E_UNSUPPORTED, "stft_dense: window_length %d hop %d", n_fft, hop);
+  B2A_REQUIRE(supported(n_fft, hop), B2A_E_UNSUPPORTED, "stft_dense: window_length %d hop %d", n_fft, hop);
   int64_t nfr;
   const int rc = b2a::spectral::check_framing("stft_dense", T, n_fft, hop, pad, right_pad, pad_mode, drop_edge, &nfr);
   if (rc != B2A_OK) return rc;
@@ -394,7 +395,7 @@ static int launch_forward(FwdParams& p, int64_t rows, void* stream) {
 
 int b2a::dft::forward_raw(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* matrix,
                           int64_t origin, int64_t n_frames, float* out, void* stream) {
-  B2A_REQUIRE(b2a_dft_supported(n_fft, hop), B2A_E_UNSUPPORTED, "stft_dense: window_length %d hop %d", n_fft, hop);
+  B2A_REQUIRE(supported(n_fft, hop), B2A_E_UNSUPPORTED, "stft_dense: window_length %d hop %d", n_fft, hop);
   B2A_REQUIRE(T < (int64_t)1 << 30 && n_frames < (int64_t)1 << 30 && origin > -((int64_t)1 << 30) &&
                   origin < ((int64_t)1 << 30),
               B2A_E_UNSUPPORTED, "stft_dense: too large");
@@ -420,19 +421,14 @@ extern "C" int b2a_mel_from_stft_f32(const float* stft, int64_t rows, int F, int
   return B2A_OK;
 }
 
-extern "C" size_t b2a_istft_dense_workspace_bytes(int64_t rows, int64_t n_frames, int n_fft) {
-  if (rows < 1 || n_frames < 1 || n_fft < 2) return 0;
-  return (size_t)rows * (size_t)n_frames * (size_t)n_fft * sizeof(float);
-}
-
-extern "C" int b2a_istft_dense_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop,
-                                   const float* window, const float* imatrix, int pad_frames, int64_t start,
-                                   int64_t out_len, float* out, void* ws, size_t ws_bytes, void* stream) {
+int b2a::dft::istft(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,
+                    const float* imatrix, int pad_frames, int64_t start, int64_t out_len, float* out, void* ws,
+                    size_t ws_bytes, void* stream) {
   B2A_REQUIRE(spec && window && imatrix && out && ws, B2A_E_INVALID, "istft_dense: null pointer");
   B2A_REQUIRE(rows >= 1 && rows <= 65535 && n_frames >= 1 && out_len >= 1 && pad_frames >= 0 && start >= 0, B2A_E_INVALID,
               "istft_dense: bad argument");
-  B2A_REQUIRE(b2a_dft_supported(n_fft, hop) && hop <= n_fft, B2A_E_UNSUPPORTED, "istft_dense: n_fft=%d hop=%d", n_fft, hop);
-  B2A_REQUIRE(ws_bytes >= b2a_istft_dense_workspace_bytes(rows, n_frames, n_fft), B2A_E_INVALID,
+  B2A_REQUIRE(supported(n_fft, hop) && hop <= n_fft, B2A_E_UNSUPPORTED, "istft_dense: n_fft=%d hop=%d", n_fft, hop);
+  B2A_REQUIRE(ws_bytes >= (size_t)rows * (size_t)n_frames * (size_t)n_fft * sizeof(float), B2A_E_INVALID,
               "istft_dense: workspace too small");
   B2A_REQUIRE(((uintptr_t)spec & 7) == 0, B2A_E_INVALID, "istft_dense: spectra must be 8-byte aligned");
   float* frames = reinterpret_cast<float*>(ws);

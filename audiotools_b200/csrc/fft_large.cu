@@ -235,9 +235,10 @@ static inline int log2_pow2(int n) {
   return (1 << l) == n ? l : -1;
 }
 
-extern "C" int b2a_stft_large_supported(int n_fft, int hop, int inverse) {
+// the window lengths of these kernels: forward 8192 .. 32768, hop >= 1; inverse 4096 .. 32768, 1 <= hop <= n_fft
+static bool supported(int n_fft, int hop, int inverse) {
   const int l = n_fft >= 2 ? log2_pow2(n_fft) : -1;
-  if (hop < 1 || l > 15) return 0;
+  if (hop < 1 || l > 15) return false;
   return inverse ? (l >= 12 && hop <= n_fft) : l >= 13;
 }
 
@@ -248,7 +249,7 @@ extern "C" int b2a_stft_large_f32(const float* x, int64_t rows, int64_t T, int n
   B2A_REQUIRE(x && window && stft_out, B2A_E_INVALID, "stft_large: null pointer");
   B2A_REQUIRE(rows >= 1 && T >= 1, B2A_E_INVALID, "stft_large: empty input");
   B2A_REQUIRE(T < (int64_t)1 << 30, B2A_E_UNSUPPORTED, "stft_large: rows longer than 2^30 samples");
-  B2A_REQUIRE(b2a_stft_large_supported(n_fft, hop, 0), B2A_E_UNSUPPORTED,
+  B2A_REQUIRE(supported(n_fft, hop, 0), B2A_E_UNSUPPORTED,
               "stft_large: window_length %d hop %d (powers of two 8192 .. 32768, hop >= 1)", n_fft, hop);
   int64_t nfr;
   const int rc = b2a::spectral::check_framing("stft_large", T, n_fft, hop, pad, right_pad, pad_mode, drop_edge, &nfr);
@@ -272,8 +273,7 @@ static int launch_fwd_any(const FwdParams& p, int64_t rows, int n_fft, void* str
 
 int b2a::large::forward_raw(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window,
                             int64_t origin, int64_t n_frames, float* out, void* stream) {
-  B2A_REQUIRE(b2a_stft_large_supported(n_fft, hop, 1), B2A_E_UNSUPPORTED, "stft_large: window_length %d hop %d", n_fft,
-              hop);
+  B2A_REQUIRE(supported(n_fft, hop, 1), B2A_E_UNSUPPORTED, "stft_large: window_length %d hop %d", n_fft, hop);
   B2A_REQUIRE(T < (int64_t)1 << 30 && rows * n_frames < (int64_t)2147483647 && origin > -((int64_t)1 << 30) &&
                   origin < ((int64_t)1 << 30),
               B2A_E_UNSUPPORTED, "stft_large: too large");
@@ -298,20 +298,15 @@ int b2a::large::inverse_frames(const float* spec, int64_t rows, int64_t n_frames
   }
 }
 
-extern "C" size_t b2a_istft_large_workspace_bytes(int64_t rows, int64_t n_frames, int n_fft) {
-  if (rows < 1 || n_frames < 1 || !b2a_stft_large_supported(n_fft, 1, 1)) return 0;
-  return (size_t)rows * (size_t)n_frames * (size_t)n_fft * sizeof(float);
-}
-
-extern "C" int b2a_istft_large_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop,
-                                   const float* window, int pad_frames, int64_t start, int64_t out_len, float* out,
-                                   void* ws, size_t ws_bytes, void* stream) {
+int b2a::large::istft(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,
+                      int pad_frames, int64_t start, int64_t out_len, float* out, void* ws, size_t ws_bytes,
+                      void* stream) {
   B2A_REQUIRE(spec && window && out && ws, B2A_E_INVALID, "istft_large: null pointer");
   B2A_REQUIRE(rows >= 1 && rows <= 65535 && n_frames >= 1 && out_len >= 1 && pad_frames >= 0 && start >= 0,
               B2A_E_INVALID, "istft_large: bad argument");
-  B2A_REQUIRE(b2a_stft_large_supported(n_fft, hop, 1), B2A_E_UNSUPPORTED,
+  B2A_REQUIRE(supported(n_fft, hop, 1), B2A_E_UNSUPPORTED,
               "istft_large: n_fft=%d hop=%d (powers of two 4096 .. 32768, 1 <= hop <= n_fft)", n_fft, hop);
-  B2A_REQUIRE(ws_bytes >= b2a_istft_large_workspace_bytes(rows, n_frames, n_fft), B2A_E_INVALID,
+  B2A_REQUIRE(ws_bytes >= (size_t)rows * (size_t)n_frames * (size_t)n_fft * sizeof(float), B2A_E_INVALID,
               "istft_large: workspace too small");
   B2A_REQUIRE(((uintptr_t)spec & 7) == 0 && ((uintptr_t)ws & 7) == 0, B2A_E_INVALID,
               "istft_large: spectra and workspace must be 8-byte aligned");

@@ -177,17 +177,6 @@ __global__ void __launch_bounds__(256) mel_backward_kernel(const float2* __restr
   }
 }
 
-// routes of the backward passes, by window length (the inverse routes of the engine)
-enum Route { NONE = 0, WARP = 1, LARGE = 2, DENSE = 3 };
-
-static Route route(int n_fft, int hop) {
-  if (hop < 1 || hop > n_fft) return NONE;
-  if (b2a_istft_supported(n_fft, hop)) return WARP;
-  if (b2a_stft_large_supported(n_fft, hop, 1)) return LARGE;
-  if (b2a_dft_supported(n_fft, hop)) return DENSE;
-  return NONE;
-}
-
 static inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 static unsigned grid_for(long long n) {
@@ -200,16 +189,14 @@ static unsigned grid_for(long long n) {
 
 using namespace b2a::grad;
 
-extern "C" int b2a_stft_backward_supported(int n_fft, int hop) { return route(n_fft, hop) != NONE; }
-
 extern "C" size_t b2a_stft_backward_workspace_bytes(int64_t rows, int64_t T, int n_fft, int hop, int pad, int right_pad,
                                                     int drop_edge) {
-  const Route r = route(n_fft, hop);
+  const int r = b2a_stft_route(n_fft, hop, 1);
   const int64_t nfr = b2a_stft_num_frames(T, n_fft, hop, pad, right_pad, drop_edge);
-  if (r == NONE || rows < 1 || nfr < 1) return 0;
+  if (r == B2A_ROUTE_NONE || rows < 1 || nfr < 1) return 0;
   const int64_t Lpp = T + 2 * (int64_t)(n_fft / 2 + pad) + right_pad;
   size_t b = align256((size_t)rows * (size_t)Lpp * sizeof(float));
-  if (r != WARP) b += (size_t)rows * (size_t)nfr * (size_t)n_fft * sizeof(float);
+  if (r != B2A_ROUTE_FFT) b += (size_t)rows * (size_t)nfr * (size_t)n_fft * sizeof(float);
   return b;
 }
 
@@ -218,11 +205,12 @@ extern "C" int b2a_stft_backward_f32(const float* grad_spec, int64_t rows, int64
                                      int drop_edge, float* grad_x, void* ws, size_t ws_bytes, void* stream) {
   B2A_REQUIRE(grad_spec && window && grad_x && ws, B2A_E_INVALID, "stft_backward: null pointer");
   B2A_REQUIRE(rows >= 1 && rows <= 65535 && T >= 1 && T < ((int64_t)1 << 30), B2A_E_INVALID, "stft_backward: bad shape");
-  const Route r = route(n_fft, hop);
-  B2A_REQUIRE(r != NONE, B2A_E_UNSUPPORTED,
+  const int r = b2a_stft_route(n_fft, hop, 1);
+  B2A_REQUIRE(r != B2A_ROUTE_NONE, B2A_E_UNSUPPORTED,
               "stft_backward: window_length %d hop %d (hop <= window_length; powers of two up to 32768, any other length "
               "up to 8192)", n_fft, hop);
-  B2A_REQUIRE(r != DENSE || amatrix, B2A_E_INVALID, "stft_backward: window_length %d needs the adjoint DFT matrix", n_fft);
+  B2A_REQUIRE(r != B2A_ROUTE_DENSE || amatrix, B2A_E_INVALID,
+              "stft_backward: window_length %d needs the adjoint DFT matrix", n_fft);
   int64_t nfr;
   int rc = b2a::spectral::check_framing("stft_backward", T, n_fft, hop, pad, right_pad, pad_mode, drop_edge, &nfr);
   if (rc != B2A_OK) return rc;
@@ -234,12 +222,12 @@ extern "C" int b2a_stft_backward_f32(const float* grad_spec, int64_t rows, int64
   const int64_t Lpp = T + 2 * ((int64_t)half + pad) + right_pad;  // the padded signal and the centre padding
   float* gp = reinterpret_cast<float*>(ws);
   // 1. adjoint transform + overlap-add (no envelope) over the whole padded range; the dropped frames are zero frames
-  if (r == WARP) {
+  if (r == B2A_ROUTE_FFT) {
     rc = b2a::istft::run(grad_spec, rows, nfr, n_fft, hop, window, drop_edge, 0, Lpp, gp, 1, stream);
   } else {
     float* frames = reinterpret_cast<float*>(reinterpret_cast<char*>(ws) + align256((size_t)rows * Lpp * sizeof(float)));
-    rc = (r == LARGE) ? b2a::large::inverse_frames(grad_spec, rows, nfr, n_fft, window, frames, 1, stream)
-                      : b2a::dft::inverse_frames(grad_spec, rows, nfr, n_fft, amatrix, frames, stream);
+    rc = (r == B2A_ROUTE_LARGE) ? b2a::large::inverse_frames(grad_spec, rows, nfr, n_fft, window, frames, 1, stream)
+                                : b2a::dft::inverse_frames(grad_spec, rows, nfr, n_fft, amatrix, frames, stream);
     if (rc == B2A_OK)
       rc = b2a::dft::launch_fold(frames, window, rows, (int)nfr, n_fft, hop, drop_edge, 0, Lpp, 0, gp, stream);
   }
@@ -263,11 +251,12 @@ extern "C" int b2a_istft_backward_f32(const float* grad_out, int64_t rows, int64
   B2A_REQUIRE(rows >= 1 && rows <= 65535 && n_frames >= 1 && out_len >= 1 && out_len < ((int64_t)1 << 30) &&
                   pad_frames >= 0 && start >= 0,
               B2A_E_INVALID, "istft_backward: bad argument");
-  const Route r = route(n_fft, hop);
-  B2A_REQUIRE(r != NONE, B2A_E_UNSUPPORTED,
+  const int r = b2a_stft_route(n_fft, hop, 1);
+  B2A_REQUIRE(r != B2A_ROUTE_NONE, B2A_E_UNSUPPORTED,
               "istft_backward: window_length %d hop %d (hop <= window_length; powers of two up to 32768, any other "
               "length up to 8192)", n_fft, hop);
-  B2A_REQUIRE(r != DENSE || matrix, B2A_E_INVALID, "istft_backward: window_length %d needs the forward DFT matrix", n_fft);
+  B2A_REQUIRE(r != B2A_ROUTE_DENSE || matrix, B2A_E_INVALID,
+              "istft_backward: window_length %d needs the forward DFT matrix", n_fft);
   B2A_REQUIRE(ws_bytes >= b2a_istft_backward_workspace_bytes(rows, out_len), B2A_E_INVALID,
               "istft_backward: workspace too small");
   B2A_REQUIRE(((uintptr_t)grad_spec & 7) == 0, B2A_E_INVALID, "istft_backward: spectra must be 8-byte aligned");
@@ -281,12 +270,12 @@ extern "C" int b2a_istft_backward_f32(const float* grad_out, int64_t rows, int64
   // (f + pad_frames) hop - start on: raw framing with that origin, zeros outside [0, out_len)
   const int64_t origin = (int64_t)pad_frames * hop - start;
   int rc;
-  if (r == WARP) {
+  if (r == B2A_ROUTE_FFT) {
     B2A_REQUIRE(origin > -((int64_t)1 << 30) && origin < ((int64_t)1 << 30) && n_frames < ((int64_t)1 << 30),
                 B2A_E_UNSUPPORTED, "istft_backward: too large");
     rc = b2a::spectral::frames_fft(u, (int)rows, (int)out_len, n_fft, hop, window, (int)origin, nullptr,
                                    B2A_PAD_CONSTANT, (int)n_frames, reinterpret_cast<float2*>(grad_spec), stream);
-  } else if (r == LARGE) {
+  } else if (r == B2A_ROUTE_LARGE) {
     rc = b2a::large::forward_raw(u, rows, out_len, n_fft, hop, window, origin, n_frames, grad_spec, stream);
   } else {
     rc = b2a::dft::forward_raw(u, rows, out_len, n_fft, hop, matrix, origin, n_frames, grad_spec, stream);

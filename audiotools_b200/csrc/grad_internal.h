@@ -1,4 +1,5 @@
-// grad_internal.h -- the pieces of the STFT / inverse STFT kernels that grad.cu reuses for the backward passes.
+// grad_internal.h -- the pieces of the STFT / inverse STFT kernels that other translation units reuse: the inverse
+// routes of b2a_istft_f32 (istft.cu) and the backward passes (grad.cu).
 #pragma once
 #include "b2a_common.h"
 
@@ -11,6 +12,9 @@ int run(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, c
 }  // namespace istft
 
 namespace large {
+// b2a_istft_f32 on B2A_ROUTE_LARGE: inverse_frames into ws (rows * n_frames * n_fft floats), then dft.cu's fold.
+int istft(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window, int pad_frames,
+          int64_t start, int64_t out_len, float* out, void* ws, size_t ws_bytes, void* stream);
 // Windowed inverse frames of fft_large.cu -> frames [rows, n_frames, n_fft] (n_fft 4096 .. 32768); adjoint as above.
 int inverse_frames(const float* spec, int64_t rows, int64_t n_frames, int n_fft, const float* window, float* frames,
                    int adjoint, void* stream);
@@ -20,6 +24,11 @@ int forward_raw(const float* x, int64_t rows, int64_t T, int n_fft, int hop, con
 }  // namespace large
 
 namespace dft {
+// b2a_istft_f32 on B2A_ROUTE_DENSE (also runs n_fft 32 and 4096): inverse_frames with the kind 1 matrix into ws, then
+// the fold.
+int istft(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,
+          const float* imatrix, int pad_frames, int64_t start, int64_t out_len, float* out, void* ws, size_t ws_bytes,
+          void* stream);
 // Dense inverse frames of dft.cu with a kind 1 (inverse) or kind 2 (adjoint) matrix -> frames [rows, n_frames, n_fft].
 int inverse_frames(const float* spec, int64_t rows, int64_t n_frames, int n_fft, const float* imatrix, float* frames,
                    void* stream);

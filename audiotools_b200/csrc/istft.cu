@@ -303,20 +303,20 @@ static int launch(Params& p, void* stream) {
   return B2A_OK;
 }
 
-}  // namespace istft
-}  // namespace b2a
-
-extern "C" int b2a_istft_supported(int n_fft, int hop) {
-  if (n_fft < 64 || n_fft > 2048 || (n_fft & (n_fft - 1))) return 0;
+static bool supported(int n_fft, int hop) {
+  if (n_fft < 64 || n_fft > 2048 || (n_fft & (n_fft - 1))) return false;
   return hop >= 1 && hop <= n_fft;
 }
+
+}  // namespace istft
+}  // namespace b2a
 
 int b2a::istft::run(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,
                     int pad_frames, int64_t start, int64_t out_len, float* out, int adjoint, void* stream) {
   B2A_REQUIRE(spec && window && out, B2A_E_INVALID, "istft: null pointer");
   B2A_REQUIRE(rows >= 1 && n_frames >= 1 && out_len >= 1 && pad_frames >= 0 && start >= 0, B2A_E_INVALID,
               "istft: bad argument");
-  B2A_REQUIRE(b2a_istft_supported(n_fft, hop), B2A_E_UNSUPPORTED,
+  B2A_REQUIRE(supported(n_fft, hop), B2A_E_UNSUPPORTED,
               "istft: n_fft=%d hop=%d (power-of-two n_fft in [64, 2048], 1 <= hop <= n_fft)", n_fft, hop);
   B2A_REQUIRE(rows < ((int64_t)1 << 24) && n_frames < ((int64_t)1 << 28) && out_len < ((int64_t)1 << 40),
               B2A_E_UNSUPPORTED, "istft: too large");
@@ -338,8 +338,26 @@ int b2a::istft::run(const float* spec, int64_t rows, int64_t n_frames, int n_fft
   }
 }
 
+extern "C" size_t b2a_istft_workspace_bytes(int64_t rows, int64_t n_frames, int n_fft, int hop) {
+  const int r = b2a_stft_route(n_fft, hop, 1);
+  if (rows < 1 || n_frames < 1 || r == B2A_ROUTE_NONE || r == B2A_ROUTE_FFT) return 0;
+  return (size_t)rows * (size_t)n_frames * (size_t)n_fft * sizeof(float);
+}
+
 extern "C" int b2a_istft_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop,
-                             const float* window, int pad_frames, int64_t start, int64_t out_len, float* out,
-                             void* stream) {
-  return b2a::istft::run(spec, rows, n_frames, n_fft, hop, window, pad_frames, start, out_len, out, 0, stream);
+                             const float* window, const float* matrix, int pad_frames, int64_t start, int64_t out_len,
+                             float* out, void* ws, size_t ws_bytes, void* stream) {
+  switch (b2a_stft_route(n_fft, hop, 1)) {
+    case B2A_ROUTE_FFT:
+      return b2a::istft::run(spec, rows, n_frames, n_fft, hop, window, pad_frames, start, out_len, out, 0, stream);
+    case B2A_ROUTE_LARGE:
+      return b2a::large::istft(spec, rows, n_frames, n_fft, hop, window, pad_frames, start, out_len, out, ws, ws_bytes,
+                               stream);
+    case B2A_ROUTE_DENSE:
+      return b2a::dft::istft(spec, rows, n_frames, n_fft, hop, window, matrix, pad_frames, start, out_len, out, ws,
+                             ws_bytes, stream);
+  }
+  return b2a::fail(B2A_E_UNSUPPORTED,
+                   "istft: n_fft=%d hop=%d (1 <= hop <= n_fft; powers of two up to 32768, any other length up to 8192)",
+                   n_fft, hop);
 }

@@ -760,6 +760,16 @@ extern "C" int64_t b2a_stft_num_frames(int64_t T, int n_fft, int hop, int pad, i
   return n;
 }
 
+// The one route table (include/b2a.h).  Each family's entry points keep their own, wider or equal, range checks.
+extern "C" int b2a_stft_route(int n_fft, int hop, int inverse) {
+  if (n_fft < 2 || hop < 1 || (inverse && hop > n_fft)) return B2A_ROUTE_NONE;
+  if ((n_fft & (n_fft - 1)) == 0) {
+    if (n_fft >= (inverse ? 64 : 32) && n_fft <= (inverse ? 2048 : 4096)) return B2A_ROUTE_FFT;
+    if (n_fft >= 4096 && n_fft <= 32768) return B2A_ROUTE_LARGE;
+  }
+  return n_fft <= 8192 ? B2A_ROUTE_DENSE : B2A_ROUTE_NONE;
+}
+
 extern "C" int b2a_spectral_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window,
                                 int pad, int right_pad, int pad_mode, int drop_edge, const float* gain,
                                 int rows_per_gain, float* y_out, const float* mel_fb, const int32_t* mel_lo,

@@ -29,6 +29,7 @@ class Engine:
         self.require_cuda = require_cuda
         self.launches = 0  # kernels of libb2a launched through this engine (bench.py reports it)
         self._packed_cache = {}
+        self._routes = {}
 
     # ------------------------------------------------------------------ helpers
     DIFFERENTIABLE = ("AudioSignal.stft", "istft", "mel_spectrogram", "mfcc", "normalize", "volume_change",
@@ -99,21 +100,12 @@ class Engine:
         """``torch.istft(spec, n_fft, hop, window=window, length=..., center=True)`` for spec [B, C, F, N] complex64
         (ref:audiotools/core/audio_signal.py:1214-1296) -> [B, C, length].  ``pad_frames`` zero frames are put back
         on either side and ``trim`` extra leading samples are dropped (the reference's match_stride handling)."""
-        if not torch.is_complex(spec):
-            raise TypeError("istft: spec must be complex")
-        self._refuse_grad(spec, "spec", depth=1)
-        if self.require_cuda and not spec.is_cuda:
-            raise RuntimeError(f"stft_data is on {spec.device}: audiotools_b200 runs on CUDA (sm_90a) only and has "
-                               "no CPU fallback")
-        if spec.dtype != torch.complex64:
-            spec = spec.to(torch.complex64)
-        spec = spec.contiguous()
+        spec = self._spec_ok(spec, "istft")
         B, C, F, N = spec.shape
         assert F == n_fft // 2 + 1, (F, n_fft)
-        large = bool(self.lib.b2a_stft_large_supported(int(n_fft), int(hop), 1))
-        dense = not large and not self.lib.b2a_istft_supported(int(n_fft), int(hop))
-        if dense and not (self.lib.b2a_dft_supported(int(n_fft), int(hop)) and hop <= n_fft):
-            raise NotImplementedError(f"istft: n_fft={n_fft} hop={hop}" + self._large_limit(int(n_fft)))
+        route = self.route(n_fft, hop, 1)
+        if route == _lib.ROUTE_NONE:
+            raise self.route_error(n_fft, hop, 1)
         window = self._prep(window, "window")
         assert window.numel() == n_fft
         start = n_fft // 2 + int(trim)
@@ -130,39 +122,19 @@ class Engine:
         if self._packed_cache[key][1] < 1e-11:
             raise RuntimeError("istft: window overlap add min: 1 (the window envelope vanishes inside the output)")
         out = torch.empty(B, C, int(length), dtype=torch.float32, device=spec.device)
-        if large:  # powers of two 4096 .. 32768: per-frame inverse FFT (csrc/fft_large.cu) + the overlap-add fold of dft.cu
-            nbytes = int(self.lib.b2a_istft_large_workspace_bytes(B * C, N, int(n_fft)))
-            ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=spec.device)
-            rc = self.lib.b2a_istft_large_f32(_dptr(torch.view_as_real(spec)), B * C, N, int(n_fft), int(hop), _dptr(window),
-                                              int(pad_frames), start, int(length), _dptr(out), _dptr(ws), nbytes,
-                                              self._stream(spec))
-            self.lib.check(rc)
-            self.launches += 2
-            return out
-        if dense:  # any other window length (and 32): transposed dense DFT + overlap-add fold (csrc/dft.cu)
-            imat = self.dft_matrix(window, int(n_fft), inverse=True)
-            nbytes = int(self.lib.b2a_istft_dense_workspace_bytes(B * C, N, int(n_fft)))
-            ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=spec.device)
-            rc = self.lib.b2a_istft_dense_f32(_dptr(torch.view_as_real(spec)), B * C, N, int(n_fft), int(hop), _dptr(window),
-                                              _dptr(imat), int(pad_frames), start, int(length), _dptr(out), _dptr(ws),
-                                              nbytes, self._stream(spec))
-            self.lib.check(rc)
-            self.launches += 2
-            return out
+        imat = self.dft_matrix(window, int(n_fft), inverse=1) if route == _lib.ROUTE_DENSE else None
+        nbytes = int(self.lib.b2a_istft_workspace_bytes(B * C, N, int(n_fft), int(hop)))
+        ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=spec.device) if nbytes else None
         rc = self.lib.b2a_istft_f32(_dptr(torch.view_as_real(spec)), B * C, N, int(n_fft), int(hop), _dptr(window),
-                                    int(pad_frames), start, int(length), _dptr(out), self._stream(spec))
+                                    _dptr(imat), int(pad_frames), start, int(length), _dptr(out), _dptr(ws), nbytes,
+                                    self._stream(spec))
         self.lib.check(rc)
-        self.launches += 1
+        self.launches += 1 if route == _lib.ROUTE_FFT else 2  # LARGE / DENSE: frames, then the overlap-add fold
         return out
 
     # ------------------------------------------------------------------ backward passes (csrc/grad.cu)
     def backward_supported(self, n_fft: int, hop: int) -> bool:
-        return bool(self.lib.b2a_stft_backward_supported(int(n_fft), int(hop)))
-
-    def _dense_backward(self, n_fft: int, hop: int) -> bool:
-        """The backward of this geometry runs on the dense DFT (needs a matrix): not a power of two in [64, 32768]."""
-        return not (self.lib.b2a_istft_supported(int(n_fft), int(hop))
-                    or self.lib.b2a_stft_large_supported(int(n_fft), int(hop), 1))
+        return self.route(n_fft, hop, 1) != _lib.ROUTE_NONE
 
     def stft_backward(self, grad_spec: torch.Tensor, T: int, n_fft: int, hop: int, window: torch.Tensor, pad: int = 0,
                       right_pad: int = 0, pad_mode: str = "reflect", drop_edge: int = 0) -> torch.Tensor:
@@ -174,7 +146,8 @@ class Engine:
                                                                 int(right_pad), int(drop_edge)))
         if nbytes == 0:
             raise NotImplementedError(f"stft backward: window_length {n_fft} hop {hop}")
-        amat = self.dft_matrix(window, int(n_fft), inverse=2) if self._dense_backward(n_fft, hop) else None
+        route = self.route(n_fft, hop, 1)
+        amat = self.dft_matrix(window, int(n_fft), inverse=2) if route == _lib.ROUTE_DENSE else None
         ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=grad_spec.device)
         gx = torch.empty(B, C, int(T), dtype=torch.float32, device=grad_spec.device)
         rc = self.lib.b2a_stft_backward_f32(_dptr(torch.view_as_real(grad_spec)), B * C, int(T), int(n_fft), int(hop),
@@ -182,7 +155,7 @@ class Engine:
                                             _lib.PAD_MODES[pad_mode], int(drop_edge), _dptr(gx), _dptr(ws), nbytes,
                                             self._stream(grad_spec))
         self.lib.check(rc)
-        self.launches += 2 if self.lib.b2a_istft_supported(int(n_fft), int(hop)) else 3
+        self.launches += 2 if route == _lib.ROUTE_FFT else 3
         return gx
 
     def istft_backward(self, grad_out: torch.Tensor, n_frames: int, n_fft: int, hop: int, window: torch.Tensor,
@@ -191,7 +164,7 @@ class Engine:
         grad_out = grad_out.to(torch.float32).contiguous()
         B, C, L = grad_out.shape
         window = self._prep(window, "window")
-        mat = self.dft_matrix(window, int(n_fft), inverse=0) if self._dense_backward(n_fft, hop) else None
+        mat = self.dft_matrix(window, int(n_fft), inverse=0) if self.route(n_fft, hop, 1) == _lib.ROUTE_DENSE else None
         nbytes = int(self.lib.b2a_istft_backward_workspace_bytes(B * C, L))
         ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=grad_out.device)
         gs = torch.empty(B, C, n_fft // 2 + 1, int(n_frames), dtype=torch.complex64, device=grad_out.device)
@@ -288,19 +261,30 @@ class Engine:
         self.launches += 2
         return loss, gx, gy
 
-    # ------------------------------------------------------------------ dense DFT (any window length)
+    # ------------------------------------------------------------------ STFT routes, dense DFT (any window length)
+    def route(self, n_fft: int, hop: int, inverse: int) -> int:
+        """``b2a_stft_route``: the kernel family (``_lib.ROUTE_*``) that runs the STFT (inverse 0) or the inverse STFT
+        and both backward passes (inverse 1) of this geometry.  Memoised: ``stft()`` is launch-latency bound at
+        batch=4 x 1 s, where a foreign-function call per call is measurable."""
+        key = (n_fft, hop, inverse)
+        r = self._routes.get(key)
+        if r is None:
+            r = self._routes[key] = int(self.lib.b2a_stft_route(int(n_fft), int(hop), int(inverse)))
+        return r
+
     @staticmethod
-    def fft_window_length(n_fft: int) -> bool:
-        """Window lengths the fused FFT kernel (csrc/spectral.cu) covers: powers of two in [32, 4096]."""
-        return 32 <= n_fft <= 4096 and (n_fft & (n_fft - 1)) == 0
-
-    LARGE_FFT_MAX = 32768  # longest window of csrc/fft_large.cu (one frame per CTA in shared memory)
-
-    def _large_limit(self, n_fft: int) -> str:
-        """The error-message suffix for a power-of-two window beyond the large-window FFT kernels."""
-        if n_fft > self.LARGE_FFT_MAX and (n_fft & (n_fft - 1)) == 0:
-            return f": power-of-two windows run on the FFT kernels up to {self.LARGE_FFT_MAX}"
-        return ""
+    def route_error(n_fft: int, hop: int, inverse: int, backward_of: Optional[str] = None) -> NotImplementedError:
+        """The error for a geometry whose route is ``ROUTE_NONE``: of the STFT (inverse 0), the inverse STFT (inverse 1),
+        or, when ``backward_of`` names the differentiable method, of its backward."""
+        if backward_of is not None:
+            return NotImplementedError(
+                f"{backward_of}: no backward for window_length {n_fft} hop {hop}: gradients through the STFT need "
+                "hop <= window_length and a window of any length up to 8192 or a power of two up to 32768")
+        msg = (f"istft: n_fft={n_fft} hop={hop}" if inverse else
+               f"stft: window_length {n_fft} hop {hop}: the dense DFT path covers 2..8192")
+        if n_fft > 32768 and (n_fft & (n_fft - 1)) == 0:
+            msg += ": power-of-two windows run on the FFT kernels up to 32768"
+        return NotImplementedError(msg)
 
     def dft_matrix(self, window: torch.Tensor, n_fft: int, inverse: int = 0) -> torch.Tensor:
         """The windowed DFT matrix of csrc/dft.cu for (n_fft, window), built on the device once and cached (the cache
@@ -625,8 +609,9 @@ class Engine:
 
     def spectral_kernel_name(self, n_fft: int, hop: int, want_mel: bool = True, want_stft: bool = False) -> str:
         """Name of the kernel ``spectral`` launches for this geometry (bench.py / profiles label their numbers with it)."""
-        if self.lib.b2a_stft_large_supported(int(n_fft), int(hop), 0):
-            name = f"stft_large_kernel<{int(math.log2(n_fft))}>"
+        route = self.route(n_fft, hop, 0)
+        if route in (_lib.ROUTE_LARGE, _lib.ROUTE_DENSE):
+            name = f"stft_large_kernel<{int(math.log2(n_fft))}>" if route == _lib.ROUTE_LARGE else "dft_forward_kernel"
             return name + " + mel_from_stft_kernel" if want_mel else name
         if self.lib.b2a_spectral_uses_tensor_cores(int(n_fft), int(hop), int(want_mel), int(want_stft)):
             return "spectral_tc_kernel"
@@ -666,9 +651,11 @@ class Engine:
             raise _lib.B2AError(f"stft: no frames (T={T}, n_fft={n_fft}, hop={hop})")
         F = n_fft // 2 + 1
         dev = x.device
-        if not self.fft_window_length(int(n_fft)):
-            return self._spectral_dense(x, int(n_fft), int(hop), window, pad, right_pad, pad_mode, drop_edge, gain,
-                                        want_scaled, mel_fb, mel_lo, mel_hi, post, post_eps, post_power, want_stft, N)
+        route = self.route(n_fft, hop, 0)
+        if route != _lib.ROUTE_FFT:
+            return self._spectral_materialised(x, int(n_fft), int(hop), route, window, pad, right_pad, pad_mode,
+                                               drop_edge, gain, want_scaled, mel_fb, mel_lo, mel_hi, post, post_eps,
+                                               post_power, want_stft, N)
         stft = torch.empty(B, C, F, N, dtype=torch.complex64, device=dev) if want_stft else None
         mel = None
         n_mels = 0
@@ -700,24 +687,22 @@ class Engine:
         return {"stft": stft, "mel": mel, "scaled": scaled}
 
 
-    def _spectral_dense(self, x, n_fft, hop, window, pad, right_pad, pad_mode, drop_edge, gain, want_scaled, mel_fb,
-                        mel_lo, mel_hi, post, post_eps, post_power, want_stft, N):
-        """``spectral`` for window lengths outside the fused FFT kernel's set: gain pass (if any) -> the STFT of all
-        frames, materialised -> optional |X| -> banded mel -> post-op from it.  The STFT is a per-frame FFT for the
-        powers of two 8192 .. 32768 (csrc/fft_large.cu) and one dense DFT matrix product otherwise (csrc/dft.cu)."""
+    def _spectral_materialised(self, x, n_fft, hop, route, window, pad, right_pad, pad_mode, drop_edge, gain,
+                               want_scaled, mel_fb, mel_lo, mel_hi, post, post_eps, post_power, want_stft, N):
+        """``spectral`` on the LARGE and DENSE routes: gain pass (if any) -> the STFT of all frames, materialised ->
+        optional |X| -> banded mel -> post-op from it.  The STFT is a per-frame FFT on LARGE (csrc/fft_large.cu) and one
+        dense DFT matrix product on DENSE (csrc/dft.cu)."""
         B, C, T = x.shape
         F = n_fft // 2 + 1
-        large = bool(self.lib.b2a_stft_large_supported(n_fft, hop, 0))
-        if not large and not self.lib.b2a_dft_supported(n_fft, hop):
-            raise NotImplementedError(f"stft: window_length {n_fft} hop {hop}: the dense DFT path covers 2..8192"
-                                      + self._large_limit(n_fft))
+        if route == _lib.ROUTE_NONE:
+            raise self.route_error(n_fft, hop, 0)
         scaled = None
         if gain is not None:
             gain = self._prep(gain.reshape(-1), "gain")
             assert gain.numel() == B
             x = scaled = self.gain(x, gain)
         stft = torch.empty(B, C, F, N, dtype=torch.complex64, device=x.device)
-        if large:
+        if route == _lib.ROUTE_LARGE:
             rc = self.lib.b2a_stft_large_f32(_dptr(x), B * C, T, n_fft, hop, _dptr(window), pad, right_pad,
                                              _lib.PAD_MODES[pad_mode], drop_edge, _dptr(torch.view_as_real(stft)),
                                              self._stream(x))

@@ -53,7 +53,7 @@ const char* b2a_last_error(void);
  *
  *   x        [rows, T]
  *   window   [n_fft]              (AudioSignal.get_window, :1009-1039)
- *   n_fft    power of two in [32, 4096] (any other window length: b2a_stft_dense_f32 below); hop >= 1
+ *   n_fft    power of two in [32, 4096] (b2a_stft_route's B2A_ROUTE_FFT); hop >= 1
  *   pad/right_pad/pad_mode        compute_stft_padding (:1089-1121); 0/0 when !match_stride
  *   drop_edge                     frames dropped at each end (2 when match_stride, else 0)
  *   gain     nullable [rows/rows_per_gain]: x is multiplied by gain[row / rows_per_gain] first
@@ -78,37 +78,49 @@ int b2a_spectral_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop
                      int mel_packed_len, int post, float post_eps, float post_power,
                      float* mel_out, float* stft_out, void* stream);
 
+/* ---- the one route table: which kernel family runs an STFT of (n_fft, hop) -------------------------------------
+ * inverse 0: the forward STFT (b2a_spectral_f32 / b2a_stft_large_f32 / b2a_stft_dense_f32).  inverse 1: b2a_istft_f32
+ * and both backward passes, which route by it themselves.  Everything not in the table is B2A_ROUTE_NONE.
+ *                      FFT                          LARGE                          DENSE
+ *   inverse 0, hop>=1  power of two in [32, 4096]   power of two in [8192, 32768]  any other length in [2, 8192]
+ *   inverse 1, hop in  power of two in [64, 2048]   power of two in [4096, 32768]  any other length in [2, 8192]
+ *   [1, n_fft]                                                                     (incl. 32) */
+#define B2A_ROUTE_NONE 0  /* not supported                                     */
+#define B2A_ROUTE_FFT 1   /* spectral.cu (forward) / istft.cu (inverse)        */
+#define B2A_ROUTE_LARGE 2 /* fft_large.cu                                      */
+#define B2A_ROUTE_DENSE 3 /* dft.cu (needs the b2a_dft_matrix_f32 matrix)      */
+int b2a_stft_route(int n_fft, int hop, int inverse);
+
 /* ---- inverse STFT ---------------------------------------------------------------------------------
  * Replaces AudioSignal.istft (audiotools/core/audio_signal.py:1214-1296 -> torch.istft(center=True, onesided,
  * window of n_fft samples)): inverse real FFT of every frame, window, overlap-add, division by the window
- * envelope, all in one pass.
+ * envelope, on the route b2a_stft_route(n_fft, hop, 1): FFT -> one pass (rows < 2^24); LARGE / DENSE -> the windowed
+ * frames of fft_large.cu / dft.cu into ws, then dft.cu's overlap-add fold (rows <= 65535).
  *   spec   [rows, n_fft/2+1, n_frames] complex64 (re,im), 8-byte aligned (the layout b2a_spectral_f32 writes)
+ *   matrix nullable; on DENSE the kind 1 matrix of b2a_dft_matrix_f32
  *   pad_frames  zero frames put back on either side (match_stride: 2, :1276-1279); they count in the envelope
  *   start  overlap-add coordinate of out[0]: n_fft/2 (+ the match_stride trim `pad`, :1291-1292)
  *   out    [rows, out_len]; samples at or beyond (n_frames + 2*pad_frames - 1)*hop + n_fft are zero, as torch pads
- * The caller checks the envelope (torch raises when its minimum over the kept range is < 1e-11).
- * Supported: power-of-two n_fft in [64, 2048], 1 <= hop <= n_fft (b2a_istft_supported). */
-int b2a_istft_supported(int n_fft, int hop);
+ *   ws     b2a_istft_workspace_bytes(...) bytes, 8-byte aligned; 0 on FFT, where ws may be NULL
+ * The caller checks the envelope (torch raises when its minimum over the kept range is < 1e-11). */
+size_t b2a_istft_workspace_bytes(int64_t rows, int64_t n_frames, int n_fft, int hop);
 int b2a_istft_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,
-                  int pad_frames, int64_t start, int64_t out_len, float* out, void* stream);
+                  const float* matrix, int pad_frames, int64_t start, int64_t out_len, float* out, void* ws,
+                  size_t ws_bytes, void* stream);
 
-/* ---- STFT / inverse STFT for ANY window length (dense DFT, csrc/dft.cu) ---------------------------------------
+/* ---- STFT for ANY window length (dense DFT, csrc/dft.cu) -------------------------------------------------------
  * AudioSignal.stft / istft accept any window_length (audiotools/core/audio_signal.py:1123-1212, 1214-1296 -> torch.stft /
- * torch.istft), e.g. 400 / 480 / 1200-sample speech windows; b2a_spectral_f32 / b2a_istft_f32 cover the powers of two.
- * Everything else is ONE real x complex matrix product over all frames of the batch (FP32 FMA):
+ * torch.istft), e.g. 400 / 480 / 1200-sample speech windows (B2A_ROUTE_DENSE).  Their STFT is ONE real x complex
+ * matrix product over all frames of the batch (FP32 FMA):
  *   b2a_dft_matrix_f32     builds the matrix of (n_fft, window) once: inverse 0 -> M[n][k] = w[n] exp(-2 pi i nk/n_fft)
  *                          for b2a_stft_dense_f32, inverse 1 -> c_k/n_fft . w[n] exp(-2 pi i nk/n_fft) (c = 1 for DC and
- *                          Nyquist, else 2) for b2a_istft_dense_f32, inverse 2 -> the layout of 1 with weight 1 on every
+ *                          Nyquist, else 2) for b2a_istft_f32, inverse 2 -> the layout of 1 with weight 1 on every
  *                          bin for b2a_stft_backward_f32; `matrix`: b2a_dft_matrix_floats(n_fft, inverse)
  *                          floats, 16-byte aligned; angles reduced in integers (nk mod n_fft), evaluated in float64
  *   b2a_stft_dense_f32     the arguments of b2a_spectral_f32 (same framing / padding semantics, bit-exact frame
  *                          indexing) -> stft_out [rows, n_fft/2+1, n_frames] (re,im)
  *   b2a_mel_from_stft_f32  |X| -> banded mel -> post-op from a materialised STFT (AudioSignal.mel_spectrogram :1333-1369
- *                          for these window lengths; the FFT kernel fuses it)
- *   b2a_istft_dense_f32    the arguments of b2a_istft_f32 + the inverse matrix + ws (b2a_istft_dense_workspace_bytes:
- *                          the windowed frames) -> out; also accepts n_fft 32 and 4096, which istft.cu does not
- *                          (the engine routes 4096 to b2a_istft_large_f32 below). */
-int b2a_dft_supported(int n_fft, int hop);
+ *                          for the LARGE and DENSE routes; the FFT kernel fuses it) */
 size_t b2a_dft_matrix_floats(int n_fft, int inverse);
 int b2a_dft_matrix_f32(const float* window, int n_fft, int inverse, float* matrix, void* stream);
 int b2a_stft_dense_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* matrix,
@@ -120,49 +132,33 @@ int b2a_mel_from_stft_f32(const float* stft, int64_t rows, int F, int64_t n_fram
  * out[row][j][n] = sum_m dct[m][j] * logmel[row][m][n];  logmel [rows, n_mels, n_frames], dct [n_mels, n_mfcc] row-major. */
 int b2a_mel_dct_f32(const float* logmel, int64_t rows, int n_mels, int64_t n_frames, const float* dct, int n_mfcc,
                     float* out, void* stream);
-size_t b2a_istft_dense_workspace_bytes(int64_t rows, int64_t n_frames, int n_fft);
-int b2a_istft_dense_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,
-                        const float* imatrix, int pad_frames, int64_t start, int64_t out_len, float* out, void* ws,
-                        size_t ws_bytes, void* stream);
 
-/* ---- STFT / inverse STFT for LARGE power-of-two windows (FFT, one CTA per frame, csrc/fft_large.cu) -----------
- * The window lengths b2a_spectral_f32 / b2a_istft_f32 leave to the dense DFT or do not cover at all: the default
- * window of AudioSignal.stft_params is 2^ceil(log2(0.032 sr)) = 4096 at 88.2 / 96 kHz and 8192 at 176.4 / 192 kHz;
- * 16384 / 32768 serve fine frequency resolution.  FP32; no matrix, no table to build.
- *   b2a_stft_large_supported   (n_fft, hop, inverse): inverse 0 -> n_fft in {8192, 16384, 32768}, hop >= 1;
- *                              inverse 1 -> n_fft in {4096 .. 32768}, 1 <= hop <= n_fft.  65536 and above: 0.
+/* ---- STFT for LARGE power-of-two windows (FFT, one CTA per frame, csrc/fft_large.cu) ---------------------------
+ * B2A_ROUTE_LARGE: the default window of AudioSignal.stft_params is 2^ceil(log2(0.032 sr)) = 4096 at 88.2 / 96 kHz and
+ * 8192 at 176.4 / 192 kHz; 16384 / 32768 serve fine frequency resolution.  FP32; no matrix, no table to build.
  *   b2a_stft_large_f32         the arguments of b2a_stft_dense_f32 with the window instead of the matrix (same framing /
- *                              padding semantics, bit-exact frame indexing) -> stft_out [rows, n_fft/2+1, n_frames]
- *   b2a_istft_large_f32        the arguments of b2a_istft_f32 + ws (b2a_istft_large_workspace_bytes: the windowed
- *                              frames, 8-byte aligned) -> out; the overlap-add / envelope division is the fold of
- *                              b2a_istft_dense_f32. */
-int b2a_stft_large_supported(int n_fft, int hop, int inverse);
+ *                              padding semantics, bit-exact frame indexing) -> stft_out [rows, n_fft/2+1, n_frames] */
 int b2a_stft_large_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window, int pad,
                        int right_pad, int pad_mode, int drop_edge, float* stft_out, void* stream);
-size_t b2a_istft_large_workspace_bytes(int64_t rows, int64_t n_frames, int n_fft);
-int b2a_istft_large_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,
-                        int pad_frames, int64_t start, int64_t out_len, float* out, void* ws, size_t ws_bytes,
-                        void* stream);
 
 /* ---- backward passes of the spectral front end (csrc/grad.cu) ---------------------------------------------------
  * Gradients of AudioSignal.stft / istft / mel_spectrogram / mfcc (audiotools/core/audio_signal.py:1123-1296, 1333-1426;
  * differentiable through torch there, tests/core/test_grad.py).  A complex gradient is G = dL/dRe + i dL/dIm (torch's
- * convention); every pass is deterministic (no atomics, fixed summation order).
- *   b2a_stft_backward_supported  (n_fft, hop): 1 when both backward passes exist: 1 <= hop <= n_fft and n_fft a power of
- *                                two up to 32768 or any length 2 .. 8192.
+ * convention); every pass is deterministic (no atomics, fixed summation order).  Both backward passes exist where
+ * b2a_stft_route(n_fft, hop, 1) is not B2A_ROUTE_NONE, and run on that route.
  *   b2a_stft_backward_f32        grad_spec [rows, n_fft/2+1, n_frames] (re,im) -> grad_x [rows, T], for the STFT that
  *                                b2a_spectral_f32 / b2a_stft_dense_f32 / b2a_stft_large_f32 computed with the same
  *                                (T, n_fft, hop, window, pad, right_pad, pad_mode, drop_edge): per frame
  *                                w[n] sum_k Re(G_k e^{2 pi i kn/n_fft}), overlap-added without envelope division over the
  *                                padded range, folded back through both paddings (each padded position's gradient is
  *                                added to the sample it was read from).  amatrix: the kind 2 matrix of b2a_dft_matrix_f32,
- *                                required for the dense window lengths (not a power of two in [64, 32768]), else unused.
+ *                                required on B2A_ROUTE_DENSE, else unused.
  *                                ws: b2a_stft_backward_workspace_bytes(...) bytes, 8-byte aligned.
  *   b2a_istft_backward_f32       grad_out [rows, out_len] -> grad_spec [rows, n_fft/2+1, n_frames] for the inverse that
- *                                b2a_istft_f32 / _dense_ / _large_ computed with the same arguments: grad_out / envelope
- *                                framed with the window, forward real FFT, bin k scaled by c_k / n_fft (c = 1 at DC and
- *                                Nyquist, else 2), imaginary parts of DC / Nyquist 0.  matrix: the kind 0 (forward) matrix
- *                                of b2a_dft_matrix_f32 for the dense window lengths.  ws: b2a_istft_backward_workspace_bytes.
+ *                                b2a_istft_f32 computed with the same arguments: grad_out / envelope framed with the
+ *                                window, forward real FFT, bin k scaled by c_k / n_fft (c = 1 at DC and Nyquist, else
+ *                                2), imaginary parts of DC / Nyquist 0.  matrix: the kind 0 (forward) matrix
+ *                                of b2a_dft_matrix_f32, required on B2A_ROUTE_DENSE.  ws: b2a_istft_backward_workspace_bytes.
  *   b2a_mel_backward_f32         grad_mel [rows, n_mels, n_frames] -> grad_stft [rows, F, n_frames] (re,im) from the
  *                                complex STFT `stft` the mel came from: recomputes mel from the banded filters, applies the
  *                                post-op's derivative (B2A_POST_LOG10: post_power / (ln10 mel) where mel >= post_eps, else
@@ -170,7 +166,6 @@ int b2a_istft_large_f32(const float* spec, int64_t rows, int64_t n_frames, int n
  *                                X / |X| (0 where |X| = 0).  bin_lo / bin_hi [F] int32: the filters m that may hold bin k
  *                                lie in [bin_lo[k], bin_hi[k]) (mel_lo[m] <= k < mel_hi[m] is checked per filter).
  * The mfcc DCT's backward is b2a_mel_dct_f32 with the transposed basis; the gain's is b2a_gain_f32. */
-int b2a_stft_backward_supported(int n_fft, int hop);
 size_t b2a_stft_backward_workspace_bytes(int64_t rows, int64_t T, int n_fft, int hop, int pad, int right_pad,
                                          int drop_edge);
 int b2a_stft_backward_f32(const float* grad_spec, int64_t rows, int64_t T, int n_fft, int hop, const float* window,

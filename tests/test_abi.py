@@ -63,6 +63,9 @@ def test_bad_arguments_return_codes_not_crashes(lib):
     assert rc == -1 and b"n_fft/2" in lib.b2a_last_error()
     with pytest.raises(_lib.B2AError):
         lib.check(rc)
+    for n_fft, hop in ((65536, 16384), (512, 513)):  # no inverse route: a power of two above 32768; hop > n_fft
+        rc = lib.b2a_istft_f32(p, 1, 4, n_fft, hop, p, None, 0, 0, 1024, p, None, 0, None)
+        assert rc == -2 and f"istft: n_fft={n_fft} hop={hop}".encode() in lib.b2a_last_error()
 
 
 # every forward / backward STFT entry point checks torch's stft(center=True) framing of the padded signal with the

@@ -152,14 +152,17 @@ def test_large_windows_build_no_dft_matrix(eng):
     assert not [k for k in eng._packed_cache if k[0] == "dft" and k[3] >= 4096]
 
 
-def test_window_limits_and_kernel_names(eng):
+def test_window_routes_and_kernel_names(eng):
     lib = eng.lib
-    assert [lib.b2a_stft_large_supported(n, n // 4, 0) for n in (4096, 8192, 16384, 32768, 65536, 12288)] == \
-        [0, 1, 1, 1, 0, 0]
-    assert [lib.b2a_stft_large_supported(n, n // 4, 1) for n in (2048, 4096, 8192, 32768, 65536)] == [0, 1, 1, 1, 0]
-    assert lib.b2a_stft_large_supported(8192, 8193, 1) == 0 and lib.b2a_stft_large_supported(8192, 8193, 0) == 1
+    FFT, LARGE, NONE = _lib.ROUTE_FFT, _lib.ROUTE_LARGE, _lib.ROUTE_NONE
+    assert [lib.b2a_stft_route(n, n // 4, 0) for n in (4096, 8192, 16384, 32768, 65536, 12288)] == \
+        [FFT, LARGE, LARGE, LARGE, NONE, NONE]
+    assert [lib.b2a_stft_route(n, n // 4, 1) for n in (2048, 4096, 8192, 32768, 65536)] == \
+        [FFT, LARGE, LARGE, LARGE, NONE]
+    assert lib.b2a_stft_route(8192, 8193, 1) == NONE and lib.b2a_stft_route(8192, 8193, 0) == LARGE
     assert eng.spectral_kernel_name(8192, 2048, want_mel=False, want_stft=True) == "stft_large_kernel<13>"
     assert eng.spectral_kernel_name(32768, 8192) == "stft_large_kernel<15> + mel_from_stft_kernel"
+    assert eng.spectral_kernel_name(400, 100) == "dft_forward_kernel + mel_from_stft_kernel"
     x = torch.zeros(1, 1, 140000)
     with pytest.raises(NotImplementedError, match="up to 32768"):
         eng.spectral(x, 65536, 16384, torch.ones(65536))
