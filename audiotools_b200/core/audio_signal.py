@@ -306,7 +306,11 @@ class AudioSignal(EffectMixin, LoudnessMixin, ImpulseResponseMixin, DSPMixin):
         """Windowed-sinc polyphase resampling (ref :716-736 -> julius.resample_frac)."""
         if sample_rate == self.sample_rate:
             return self
-        self.audio_data = _engine().resample(self.audio_data, int(self.sample_rate), int(sample_rate))
+        x = self.audio_data
+        if _grad.wants_grad(x):
+            self.audio_data = _grad.Resample.apply(x, int(self.sample_rate), int(sample_rate))
+        else:
+            self.audio_data = _engine().resample(x, int(self.sample_rate), int(sample_rate))
         self.sample_rate = sample_rate
         return self
 

@@ -4,6 +4,7 @@ ref:audiotools/core/effects.py, on the sm_90a engine."""
 import numpy as np
 import torch
 
+from . import grad as _grad
 from . import util
 
 
@@ -26,6 +27,7 @@ class EffectMixin:
 
     def mix(self, other, snr=10, other_eq=None):
         """Add ``other`` at the given signal-to-noise ratio (dB), optionally equalised first (ref :27-64)."""
+        _grad.refuse_param_grad("mix", "snr", snr)
         snr = util.ensure_tensor(snr).to(self.device)
         other.zero_pad(0, max(0, self.signal_length - other.signal_length))
         other.truncate_samples(self.signal_length)
@@ -34,7 +36,10 @@ class EffectMixin:
         other = other.normalize(self.loudness() - snr)
         if _on_engine(self._audio_data):  # the noise's deferred normalisation gain and the add: one pass (csrc/effects.cu)
             g, other._pending_gain = other._pending_gain, None
-            mixed = _engine().mix(self._materialized(), other._audio_data, g)
+            if _grad.wants_grad(self._audio_data) or _grad.wants_grad(other._audio_data):
+                mixed = _grad.Mix.apply(self._materialized(), other._audio_data, g)
+            else:
+                mixed = _engine().mix(self._materialized(), other._audio_data, g)
             if g is not None:
                 other._pending_gain = g  # `other` keeps its own (still deferred) state
             self.audio_data = mixed
@@ -45,8 +50,12 @@ class EffectMixin:
     def convolve(self, other, start_at_max: bool = True, _bypass=None):
         """CIRCULAR convolution with ``other`` (period = signal length), the IR rolled so that its
         peak sits at t=0 and scaled by 1/max|IR| (ref :66-123).  ``_bypass`` [B]: items left untouched."""
-        self.audio_data = _engine().circular_convolve(self._materialized(), other.audio_data,
-                                                      roll_to_peak=start_at_max, bypass=_bypass)
+        x = self._materialized()
+        if _grad.wants_grad(x):
+            _grad.refuse_param_grad("convolve", "the impulse response", other.audio_data)
+            self.audio_data = _grad.CircConv.apply(x, other.audio_data, start_at_max, _bypass)
+            return self
+        self.audio_data = _engine().circular_convolve(x, other.audio_data, roll_to_peak=start_at_max, bypass=_bypass)
         return self
 
     def __matmul__(self, other):
@@ -60,7 +69,9 @@ class EffectMixin:
         if drr is not None:
             ir = ir.alter_drr(drr)
         cuda = _on_engine(self._audio_data)
-        max_spk = _engine().row_absmax(self._materialized()) if cuda else \
+        x0 = self._materialized()
+        # the peaks are values here; with a gradient, PeakScale's backward differentiates through them
+        max_spk = _engine().row_absmax(x0.detach()) if cuda else \
             self.audio_data.abs().max(dim=-1, keepdims=True).values
         phase = self.phase if use_original_phase else None
         self.convolve(ir, _bypass=_bypass)
@@ -68,24 +79,34 @@ class EffectMixin:
             self.stft()
             self.stft_data = self.magnitude * torch.exp(1j * phase)
             self.istft()
-        max_transformed = _engine().row_absmax(self._materialized()) if cuda else \
-            self.audio_data.abs().max(dim=-1, keepdims=True).values
-        scale = max_spk.clamp(1e-8) / max_transformed.clamp(1e-8)
-        if _bypass is not None:
-            byp = torch.as_tensor(_bypass).to(scale.device).bool().reshape(-1, 1, 1)
-            scale = torch.where(byp, torch.ones_like(scale), scale)
-        if cuda:  # per-row scale: the gain kernel with one "item" per (batch, channel) row
-            x = self._materialized()
-            self.audio_data = _engine().gain(x.reshape(-1, 1, x.shape[-1]), scale.reshape(-1)).reshape(x.shape)
+
+        def restore(y):
+            max_transformed = _engine().row_absmax(y.detach()) if cuda else y.abs().max(dim=-1, keepdims=True).values
+            scale = max_spk.clamp(1e-8) / max_transformed.clamp(1e-8)
+            if _bypass is not None:
+                byp = torch.as_tensor(_bypass).to(scale.device).bool().reshape(-1, 1, 1)
+                scale = torch.where(byp, torch.ones_like(scale), scale)
+            if cuda:  # per-row scale: the gain kernel with one "item" per (batch, channel) row
+                return _engine().gain(y.reshape(-1, 1, y.shape[-1]), scale.reshape(-1)).reshape(y.shape)
+            return y * scale
+
+        y = self._materialized() if cuda else self.audio_data
+        if cuda and _grad.wants_grad(y):
+            self.audio_data = _grad.PeakScale.apply(y, x0, 1.0, _bypass, restore)
         else:
-            self.audio_data = self.audio_data * scale
+            self.audio_data = restore(y)
         return self
 
     def ensure_max_of_audio(self, max: float = 1.0):
         """Scale every (item, channel) row whose peak exceeds ``max`` down to it (ref :181-198): a peak pass and a
         scale pass of csrc/effects.cu."""
         if _on_engine(self._audio_data):
-            self.audio_data = _engine().limit_peak(self._materialized(), float(max))
+            x = self._materialized()
+            if _grad.wants_grad(x):
+                self.audio_data = _grad.PeakScale.apply(x, None, float(max), None,
+                                                        lambda y: _engine().limit_peak(y, float(max)))
+            else:
+                self.audio_data = _engine().limit_peak(x, float(max))
             return self
         peak = self.audio_data.abs().max(dim=-1, keepdims=True)[0]
         peak_gain = torch.where(peak > max, max / peak, torch.ones_like(peak))  # no boolean-mask host sync
@@ -156,7 +177,12 @@ class EffectMixin:
                 assert db.shape[0] == self.batch_size
         else:
             db = db.unsqueeze(0)
-        self.audio_data = _engine().equalizer(self._materialized(), self.sample_rate, db.to(self.device), bypass=_bypass)
+        x = self._materialized()
+        if _grad.wants_grad(x):
+            _grad.refuse_param_grad("equalizer", "db", db)
+            self.audio_data = _grad.Equalizer.apply(x, self.sample_rate, db.to(self.device), _bypass)
+            return self
+        self.audio_data = _engine().equalizer(x, self.sample_rate, db.to(self.device), bypass=_bypass)
         return self
 
     def clip_distortion(self, clip_percentile):
@@ -182,7 +208,8 @@ class EffectMixin:
 
     def quantization(self, quantization_channels):
         if _on_engine(self._audio_data):
-            self.audio_data = _engine().quantize(self._materialized(), util.ensure_tensor(quantization_channels, ndim=1))
+            q = util.ensure_tensor(quantization_channels, ndim=1)
+            self.audio_data = self._straight_through(lambda x: _engine().quantize(x, q))
             return self
         q = util.ensure_tensor(quantization_channels, ndim=3).to(self.device)
         x = self.audio_data
@@ -191,10 +218,15 @@ class EffectMixin:
         self.audio_data = 2 * x - 1
         return self
 
+    def _straight_through(self, fwd):
+        """``fwd`` of the samples; with a gradient, the identity backward of the reference's x - (x - q).detach()."""
+        x = self._materialized()
+        return _grad.StraightThrough.apply(x, fwd) if _grad.wants_grad(x) else fwd(x)
+
     def mulaw_quantization(self, quantization_channels):
         if _on_engine(self._audio_data):
-            self.audio_data = _engine().quantize(self._materialized(), util.ensure_tensor(quantization_channels, ndim=1),
-                                                 mulaw=True)
+            q = util.ensure_tensor(quantization_channels, ndim=1)
+            self.audio_data = self._straight_through(lambda x: _engine().quantize(x, q, mulaw=True))
             return self
         mu = util.ensure_tensor(quantization_channels, ndim=3).to(self.device) - 1.0
         x = self.audio_data

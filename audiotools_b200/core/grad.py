@@ -1,6 +1,7 @@
 """``torch.autograd.Function``s over the engine: the differentiable forms of the spectral front end
 (ref:audiotools/core/audio_signal.py:1123-1296, 1333-1426 and effects.py:200-238, differentiable through torch there;
-ref:tests/core/test_grad.py).  ``AudioSignal`` uses them only when grad mode is on and the input requires a gradient;
+ref:tests/core/test_grad.py) and of the time-domain effects (resample, equalizer, convolve, apply_ir,
+ensure_max_of_audio, mix, quantization; gradients with respect to the waveform only).  ``AudioSignal`` uses them only when grad mode is on and the input requires a gradient;
 otherwise it calls the engine directly, with exactly the launches it always made.
 
 Each forward is the engine call of the no-gradient path; each backward is one launch sequence of csrc/grad.cu (or an
@@ -132,6 +133,113 @@ class SpectralLoss(torch.autograd.Function):
             out.append(eng.gain(gw, g.reshape(1).expand(gw.shape[0])))
         ctx.grads = None
         return (out[0], out[1]) + (None,) * 12
+
+
+class Resample(torch.autograd.Function):
+    """x [..., T] -> [..., floor(new T / old)] (``Engine.resample``); backward: ``Engine.resample_backward``."""
+
+    @staticmethod
+    def forward(ctx, x, old_sr, new_sr):
+        ctx.geo = (x.shape[-1], old_sr, new_sr)
+        return _engine().resample(x, old_sr, new_sr)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        T, old_sr, new_sr = ctx.geo
+        return _engine().resample_backward(g, T, old_sr, new_sr), None, None
+
+
+class Equalizer(torch.autograd.Function):
+    """x [B, C, T] -> the mel-band equaliser (``Engine.equalizer``); the band gains are constants."""
+
+    @staticmethod
+    def forward(ctx, x, sample_rate, db, bypass):
+        ctx.save_for_backward(db)  # saved, not kept: an in-place change before backward() is then an error
+        ctx.args = (sample_rate, bypass)
+        return _engine().equalizer(x, sample_rate, db, bypass=bypass)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (db,) = ctx.saved_tensors
+        sample_rate, bypass = ctx.args
+        return _engine().equalizer_backward(g, sample_rate, db, bypass=bypass), None, None, None
+
+
+class CircConv(torch.autograd.Function):
+    """x [B, C, T] -> circular convolution with the rolled, peak-scaled IR (``Engine.circular_convolve``); the IR is a
+    constant."""
+
+    @staticmethod
+    def forward(ctx, x, ir, roll_to_peak, bypass):
+        ctx.save_for_backward(ir)
+        ctx.args = (roll_to_peak, bypass)
+        return _engine().circular_convolve(x, ir, roll_to_peak=roll_to_peak, bypass=bypass)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (ir,) = ctx.saved_tensors
+        roll_to_peak, bypass = ctx.args
+        return _engine().circular_convolve_backward(g, ir, roll_to_peak=roll_to_peak, bypass=bypass), None, None, None
+
+
+class PeakScale(torch.autograd.Function):
+    """A per-row rescale by a factor that depends on the row's peak: ``ensure_max_of_audio`` (``x_ref`` None: y * p,
+    p = max_abs / max|y| where that exceeds max_abs) or apply_ir's restore (y * clamp(max|x_ref|) / clamp(max|y|)).
+    ``fwd(y)`` is the no-gradient path's computation; the backward recomputes the arg-maxes from y and x_ref."""
+
+    @staticmethod
+    def forward(ctx, y, x_ref, max_abs, bypass, fwd):
+        ctx.save_for_backward(y, x_ref)
+        ctx.args = (max_abs, bypass)
+        return fwd(y)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        y, x_ref = ctx.saved_tensors
+        max_abs, bypass = ctx.args
+        gy, gx = _engine().peak_scale_backward(g, y, x_ref, max_abs=max_abs, bypass=bypass)
+        return gy, (gx if ctx.needs_input_grad[1] else None), None, None, None
+
+
+class Mix(torch.autograd.Function):
+    """x + other_gain[item] * other (``Engine.mix``); the gain is a constant (it comes from the loudness)."""
+
+    @staticmethod
+    def forward(ctx, x, other, other_gain):
+        ctx.gain = other_gain
+        return _engine().mix(x, other, other_gain)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        go = None
+        if ctx.needs_input_grad[1]:
+            go = _engine().gain(g, ctx.gain) if ctx.gain is not None else g.clone()
+        return (g if ctx.needs_input_grad[0] else None), go, None
+
+
+class StraightThrough(torch.autograd.Function):
+    """``fwd(x)`` with the identity as its gradient: the reference's quantisers return x - (x - q).detach()."""
+
+    @staticmethod
+    def forward(ctx, x, fwd):
+        return fwd(x)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return g, None
+
+
+def refuse_param_grad(method: str, name: str, t) -> None:
+    """Gradients reach audio_data only: a parameter (IR, db, snr) that requires one raises at forward time."""
+    if torch.is_tensor(t) and wants_grad(t):
+        raise NotImplementedError(f"{method}: {name} requires a gradient; gradients flow to audio_data only "
+                                  f"({name} is a constant of the backward pass)")
 
 
 def wants_grad(t) -> bool:

@@ -377,3 +377,95 @@ extern "C" int b2a_alter_drr_f32(const float* ir, float* out, int64_t rows, int6
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }
+
+/* Backward of the per-row peak rescales (ensure_max_of_audio; apply_ir's peak restore), one CTA per row.
+ * Pass 1 finds the first arg-max of |y| (and of |x_ref|) and dot(g, y) with a fixed-order reduction; pass 2 writes
+ * the scaled gradient, then one thread adds the single-sample corrections (torch's max(dim) backward: the gradient
+ * of the peak goes to the index max returns; the first one here, as for ties torch documents).
+ *   limit   (x_ref == NULL):  y' = y p,  p = max/peak if peak > max else 1
+ *           gy = p g - [peak > max] (max / peak^2) dot(g, y) sign(y_b) e_b
+ *   restore (x_ref != NULL):  y' = y S,  S = clamp(Mx, 1e-8) / clamp(My, 1e-8),  Mx = max|x_ref|, My = max|y|
+ *           gy = S g - [My >= 1e-8] S dot(g, y) / My sign(y_b) e_b
+ *           gx_ref = [Mx >= 1e-8] dot(g, y) / clamp(My, 1e-8) sign(x_a) e_a   (zero elsewhere)
+ *   bypass[row] != 0 (restore only): S = 1, gy = g, gx_ref = 0. */
+namespace b2a {
+namespace effects {
+
+__device__ __forceinline__ void arg_better(float& v, int& i, float ov, int oi) {
+  if (ov > v || (ov == v && oi < i)) { v = ov; i = oi; }
+}
+__device__ __forceinline__ float sgn(float v) { return v > 0.f ? 1.f : (v < 0.f ? -1.f : 0.f); }
+
+__global__ void __launch_bounds__(TPB) peak_scale_bwd_kernel(const float* __restrict__ g, const float* __restrict__ y,
+                                                             const float* __restrict__ xr_, int64_t T, float lim,
+                                                             const int32_t* __restrict__ bypass, float* __restrict__ gy,
+                                                             float* __restrict__ gxr) {
+  __shared__ float sv[TPB], sx[TPB], sd[TPB];
+  __shared__ int si[TPB], sxi[TPB];
+  const int row = blockIdx.x, tid = threadIdx.x;
+  const float* gr = g + (size_t)row * T;
+  const float* yr = y + (size_t)row * T;
+  const float* xr = xr_ ? xr_ + (size_t)row * T : nullptr;
+  float bv = -1.f, bx = -1.f, d = 0.f;
+  int bi = 0, bxi = 0;
+  for (int64_t i = tid; i < T; i += TPB) {
+    const float v = yr[i];
+    if (fabsf(v) > bv) { bv = fabsf(v); bi = (int)i; }
+    d = fmaf(gr[i], v, d);
+    if (xr) {
+      const float a = fabsf(xr[i]);
+      if (a > bx) { bx = a; bxi = (int)i; }
+    }
+  }
+  sv[tid] = bv; si[tid] = bi; sx[tid] = bx; sxi[tid] = bxi; sd[tid] = d;
+  __syncthreads();
+  for (int h = TPB / 2; h > 0; h >>= 1) {
+    if (tid < h) {
+      arg_better(sv[tid], si[tid], sv[tid + h], si[tid + h]);
+      arg_better(sx[tid], sxi[tid], sx[tid + h], sxi[tid + h]);
+      sd[tid] += sd[tid + h];
+    }
+    __syncthreads();
+  }
+  const float My = sv[0], dot = sd[0];
+  const int b = si[0];
+  const bool byp = bypass && bypass[row];
+  float S, cb = 0.f;
+  if (!xr) {
+    S = My > lim ? lim / My : 1.0f;
+    if (My > lim) cb = -(lim / (My * My)) * dot * sgn(yr[b]);
+  } else if (byp) {
+    S = 1.0f;
+  } else {
+    S = fmaxf(sx[0], 1e-8f) / fmaxf(My, 1e-8f);
+    if (My >= 1e-8f) cb = -S * dot / My * sgn(yr[b]);
+  }
+  float* gyr = gy + (size_t)row * T;
+  float* gxo = xr ? gxr + (size_t)row * T : nullptr;
+  for (int64_t i = tid; i < T; i += TPB) {
+    gyr[i] = S * gr[i];
+    if (gxo) gxo[i] = 0.f;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    gyr[b] = S * gr[b] + cb;
+    if (gxo && !byp && sx[0] >= 1e-8f) gxo[sxi[0]] = dot / fmaxf(My, 1e-8f) * sgn(xr[sxi[0]]);
+  }
+}
+
+}  // namespace effects
+}  // namespace b2a
+
+extern "C" int b2a_peak_scale_backward_f32(const float* grad_out, const float* y, const float* x_ref, int64_t rows,
+                                           int64_t T, float max_abs, const int32_t* bypass, float* grad_y,
+                                           float* grad_x_ref, void* stream) {
+  B2A_REQUIRE(grad_out && y && grad_y, B2A_E_INVALID, "peak_scale_backward: null pointer");
+  B2A_REQUIRE(!x_ref || grad_x_ref, B2A_E_INVALID, "peak_scale_backward: x_ref needs grad_x_ref");
+  B2A_REQUIRE(rows >= 1 && rows < ((int64_t)1 << 31) && T >= 1 && T < ((int64_t)1 << 31), B2A_E_INVALID,
+              "peak_scale_backward: bad shape");
+  B2A_REQUIRE(grad_y != grad_out && grad_y != y, B2A_E_INVALID, "peak_scale_backward: grad_y must not alias its inputs");
+  B2A_LAUNCH(peak_scale_bwd_kernel, dim3((unsigned)rows), dim3(TPB), 0, stream, grad_out, y, x_ref, T, max_abs, bypass,
+             grad_y, grad_x_ref);
+  B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
+}

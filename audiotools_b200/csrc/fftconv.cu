@@ -360,3 +360,51 @@ extern "C" int b2a_circconv_f32(const float* x, int64_t rows, int64_t T, const f
               (long long)L, (long long)T);
   return run(x, rows, T, ir, n_ir, Leff, rows_per_ir, pidx, 0, 3, pscale, 0, bypass, out, base, w, stream);
 }
+
+/* Adjoint of b2a_circconv_f32.  The forward is y[n] = s sum_j h[j] x[(n - j + idx) mod T]; its adjoint
+ * gx[m] = s sum_j h[j] g[(m + j - idx) mod T] is the same engine with the taps reversed (h~[k] = h[L-1-k]) and the
+ * per-IR offset L-1-idx; idx and s come from ir_peak_kernel exactly as in the forward.  The reversal is a kernel of its
+ * own (reverse_taps_kernel) so that the shared filter-FFT stage stays caller-agnostic.  Bypassed rows copy g. */
+namespace b2a {
+namespace fftconv {
+
+__global__ void __launch_bounds__(256) reverse_taps_kernel(const float* __restrict__ ir, int L,
+                                                           const int32_t* __restrict__ pidx, float* __restrict__ rev,
+                                                           int32_t* __restrict__ off) {
+  const float* h = ir + (size_t)blockIdx.x * L;
+  float* o = rev + (size_t)blockIdx.x * L;
+  for (int k = threadIdx.x; k < L; k += 256) o[k] = h[L - 1 - k];
+  if (threadIdx.x == 0) off[blockIdx.x] = L - 1 - pidx[blockIdx.x];
+}
+
+}  // namespace fftconv
+}  // namespace b2a
+
+extern "C" size_t b2a_circconv_backward_workspace_bytes(int64_t rows, int64_t T, int64_t n_ir, int64_t L) {
+  if (rows < 1 || T < 1 || n_ir < 1 || L < 1) return 0;
+  const int64_t Leff = L < T ? L : T;
+  return layout(rows, T, n_ir, Leff).total + al((size_t)n_ir * Leff * 4) + al((size_t)n_ir * 4);
+}
+
+extern "C" int b2a_circconv_backward_f32(const float* grad_out, int64_t rows, int64_t T, const float* ir, int64_t n_ir,
+                                         int64_t L, int rows_per_ir, int roll_to_peak, const int32_t* bypass,
+                                         float* grad_x, void* ws, size_t ws_bytes, void* stream) {
+  B2A_REQUIRE(grad_out && ir && grad_x && ws, B2A_E_INVALID, "circconv_backward: null pointer");
+  B2A_REQUIRE(rows >= 1 && T >= 1 && n_ir >= 1 && L >= 1 && rows_per_ir >= 1, B2A_E_INVALID,
+              "circconv_backward: bad shape");
+  B2A_REQUIRE(L <= T, B2A_E_INVALID,
+              "circconv_backward: pass the IR already truncated to the signal length (L=%lld > T=%lld)", (long long)L,
+              (long long)T);
+  B2A_REQUIRE(grad_out != grad_x, B2A_E_INVALID, "circconv_backward: in-place is not supported");
+  const Layout w = layout(rows, T, n_ir, L);
+  B2A_REQUIRE(ws_bytes >= b2a_circconv_backward_workspace_bytes(rows, T, n_ir, L), B2A_E_INVALID,
+              "circconv_backward: workspace too small");
+  char* base = (char*)ws;
+  int32_t* pidx = (int32_t*)(base + w.peak_idx);
+  float* pscale = (float*)(base + w.peak_scale);
+  float* rev = (float*)(base + w.total);
+  int32_t* off = (int32_t*)(base + w.total + al((size_t)n_ir * L * 4));
+  B2A_LAUNCH(ir_peak_kernel, dim3((unsigned)n_ir), dim3(256), 0, stream, ir, (int)L, (int)L, pidx, pscale, roll_to_peak);
+  B2A_LAUNCH(reverse_taps_kernel, dim3((unsigned)n_ir), dim3(256), 0, stream, ir, (int)L, (const int32_t*)pidx, rev, off);
+  return run(grad_out, rows, T, rev, n_ir, L, rows_per_ir, off, 0, 3, pscale, 0, bypass, grad_x, base, w, stream);
+}

@@ -174,3 +174,89 @@ extern "C" int b2a_fir_direct_f32(const float* x, int64_t rows, int64_t T, const
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }
+
+// ---------------------------------------------------------------------------------------------
+// Replicate-padding fold of a stride-1 FIR's adjoint.  For y[m] = sum_k h[k] xv[m + k - left] (xv = x extended by
+// replicate padding), the adjoint is the zero-padded correlation with reversed taps (computed elsewhere) plus what the
+// padded positions carry back to the edge samples:
+//     gx[0]   += sum_{n < left}          P[left - 1 - n] g[n],        P[k] = h[0] + ... + h[k]
+//     gx[T-1] += sum_{n >= T + left - K + 1} S[T + left - n] g[n],    S[k] = h[k] + ... + h[K-1]
+// (P clamped at K-1; holds for any T, also T < K).  P and S per filter come from fir_scan_kernel (one thread per
+// filter and direction, sequential: fixed order); the fold is one warp per row that reads at most 2 K samples.
+// ---------------------------------------------------------------------------------------------
+namespace b2a {
+namespace fir {
+
+__global__ void __launch_bounds__(64) fir_scan_kernel(const float* __restrict__ h, int n_filt, int K,
+                                                      float* __restrict__ ps) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= 2 * n_filt) return;
+  const int f = t >> 1;
+  const float* hr = h + (size_t)f * K;
+  float* o = ps + (size_t)f * 2 * K;
+  float s = 0.f;
+  if ((t & 1) == 0) {
+    for (int k = 0; k < K; ++k) { s += __ldg(hr + k); o[k] = s; }
+  } else {
+    for (int k = K - 1; k >= 0; --k) { s += __ldg(hr + k); o[K + k] = s; }
+  }
+}
+
+__global__ void __launch_bounds__(256) fir_pad_fold_kernel(const float* __restrict__ g, int rows, int T,
+                                                           const float* __restrict__ ps, int K, int rows_per_filt,
+                                                           const int32_t* __restrict__ left, int left0,
+                                                           const int32_t* __restrict__ bypass, float* __restrict__ gx) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  const int f = row / rows_per_filt;
+  if (bypass && __ldg(bypass + f)) return;  // a copied row: its gradient is the plain copy
+  const int lf = left0 + (left ? __ldg(left + f) : 0);
+  const float* P = ps + (size_t)f * 2 * K;
+  const float* S = P + K;
+  const float* gr = g + (size_t)row * T;
+  float sl = 0.f, sr = 0.f;
+  const int nl = lf < T ? lf : T;
+  for (int n = lane; n < nl; n += 32) {
+    const int k = lf - 1 - n;
+    sl = fmaf(P[k < K - 1 ? k : K - 1], __ldg(gr + n), sl);
+  }
+  int n0 = T + lf - K + 1;
+  if (n0 < 0) n0 = 0;
+  for (int n = n0 + lane; n < T; n += 32) sr = fmaf(S[T + lf - n], __ldg(gr + n), sr);
+  sl = warp_sum(sl);
+  sr = warp_sum(sr);
+  if (lane == 0) {
+    float* o = gx + (size_t)row * T;
+    o[0] += sl;
+    o[T - 1] += sr;
+  }
+}
+
+}  // namespace fir
+}  // namespace b2a
+
+extern "C" size_t b2a_fir_pad_fold_workspace_bytes(int64_t n_filt, int K) {
+  if (n_filt < 1 || K < 1) return 0;
+  return (size_t)n_filt * 2 * (size_t)K * sizeof(float);
+}
+
+extern "C" int b2a_fir_pad_fold_f32(const float* grad_out, int64_t rows, int64_t T, const float* taps, int64_t n_filt,
+                                    int K, int rows_per_filt, const int32_t* left, int left0, const int32_t* bypass,
+                                    float* grad_x, void* ws, size_t ws_bytes, void* stream) {
+  using namespace b2a::fir;
+  B2A_REQUIRE(grad_out && taps && grad_x && ws, B2A_E_INVALID, "fir_pad_fold: null pointer");
+  B2A_REQUIRE(rows >= 1 && T >= 1 && T < ((int64_t)1 << 30) && n_filt >= 1 && n_filt < (1 << 24) && K >= 1 &&
+                  rows_per_filt >= 1 && left0 >= 0,
+              B2A_E_INVALID, "fir_pad_fold: bad shape");
+  B2A_REQUIRE((rows + rows_per_filt - 1) / rows_per_filt <= n_filt, B2A_E_INVALID,
+              "fir_pad_fold: %lld rows / %d per filter need more than %lld filters", (long long)rows, rows_per_filt,
+              (long long)n_filt);
+  B2A_REQUIRE(ws_bytes >= b2a_fir_pad_fold_workspace_bytes(n_filt, K), B2A_E_INVALID, "fir_pad_fold: workspace too small");
+  B2A_REQUIRE(rows / 8 < (int64_t)2147483647, B2A_E_UNSUPPORTED, "fir_pad_fold: too many rows");
+  float* ps = reinterpret_cast<float*>(ws);
+  B2A_LAUNCH(fir_scan_kernel, dim3((unsigned)((2 * n_filt + 63) / 64)), dim3(64), 0, stream, taps, (int)n_filt, K, ps);
+  B2A_LAUNCH(fir_pad_fold_kernel, dim3((unsigned)((rows + 7) / 8)), dim3(256), 0, stream, grad_out, (int)rows, (int)T, ps,
+             K, rows_per_filt, left, left0, bypass, grad_x);
+  B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
+}

@@ -33,7 +33,8 @@ class Engine:
 
     # ------------------------------------------------------------------ helpers
     DIFFERENTIABLE = ("AudioSignal.stft", "istft", "mel_spectrogram", "mfcc", "normalize", "volume_change",
-                      "and magnitude / phase / log_magnitude through stft_data")
+                      "and magnitude / phase / log_magnitude through stft_data; resample, equalizer, convolve, apply_ir, "
+                      "ensure_max_of_audio, mix, quantization, mulaw_quantization (gradients to audio_data)")
 
     @classmethod
     def _refuse_grad(cls, t: torch.Tensor, name: str, depth: int = 2):
@@ -525,6 +526,31 @@ class Engine:
         self.launches += 1
         return out
 
+    def peak_scale_backward(self, grad_out: torch.Tensor, y: torch.Tensor, x_ref: Optional[torch.Tensor] = None,
+                            max_abs: float = 1.0, bypass: Optional[torch.Tensor] = None):
+        """Gradients of the per-row peak rescales: :meth:`limit_peak` (``x_ref`` None) -> (dL/dy, None), or apply_ir's
+        restore ``y * clamp(max|x_ref|, 1e-8) / clamp(max|y|, 1e-8)`` -> (dL/dy, dL/dx_ref).  ``bypass`` [B]: items whose
+        scale was 1 (restore only)."""
+        g = self._prep(grad_out, "grad_out")
+        y = self._prep(y, "y")
+        assert g.shape == y.shape
+        T = y.shape[-1]
+        rows = y.numel() // T
+        gx = None
+        if x_ref is not None:
+            x_ref = self._prep(x_ref, "x_ref")
+            assert x_ref.shape == y.shape
+            gx = torch.empty_like(y)
+        if bypass is not None:
+            bypass = torch.as_tensor(bypass).reshape(-1).to(y.device)
+            bypass = self._bypass(bypass.repeat_interleave(rows // bypass.numel()), rows, y.device)
+        gy = torch.empty_like(y)
+        rc = self.lib.b2a_peak_scale_backward_f32(_dptr(g), _dptr(y), _dptr(x_ref), rows, T, float(max_abs),
+                                                  _dptr(bypass), _dptr(gy), _dptr(gx), self._stream(y))
+        self.lib.check(rc)
+        self.launches += 1
+        return gy, gx
+
     def mix(self, x: torch.Tensor, other: torch.Tensor, other_gain: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``x + other_gain[item] * other`` (ref :27-64: the noise's normalize() multiply and the add, one pass)."""
         x = self._prep(x, "x")
@@ -904,25 +930,67 @@ class Engine:
         h = w_last * delta + sum_k (w_k - w_{k+1}) * lowpass_k."""
         x = self._prep(x, "x")
         B, C, T = x.shape
+        h, half = self._equalizer_taps(sample_rate, db, B, x.device, bypass)
+        if half is None:
+            return self.gain(x, h)
+        g = torch.flip(h, dims=[1]).contiguous()
+        return self.fftconv(x, g, rows_per_filt=C, offset0=half, pad_mode="replicate", bypass=bypass)
+
+    def _equalizer_taps(self, sample_rate: int, db: torch.Tensor, B: int, device, bypass=None):
+        """(h [B, 2*half+1] correlation taps, half) of the equaliser's per-item FIR, or (gain [B], None) for one band."""
         db = torch.as_tensor(db)
         if db.ndim == 1:
             db = db.unsqueeze(0)
         n_bands = db.shape[-1]
-        w = (10 ** db).to(x.device).float()
+        w = (10 ** db).to(device).float()
         if w.shape[0] == 1:
             w = w.expand(B, n_bands)
         assert w.shape[0] == B
         if n_bands == 1:
             g1 = w[:, 0].contiguous()
             if bypass is not None:
-                g1 = torch.where(torch.as_tensor(bypass).to(x.device).bool().reshape(-1), torch.ones_like(g1), g1)
-            return self.gain(x, g1)
-        lp, half = self._band_lowpasses(sample_rate, n_bands, x.device)
+                g1 = torch.where(torch.as_tensor(bypass).to(device).bool().reshape(-1), torch.ones_like(g1), g1)
+            return g1, None
+        lp, half = self._band_lowpasses(sample_rate, n_bands, device)
         # [B, n_bands-1] x [n_bands-1, 2*half+1] as a broadcast multiply-add (a few KB: not worth a library GEMM call)
         h = ((w[:, :-1] - w[:, 1:]).unsqueeze(-1) * lp.unsqueeze(0)).sum(dim=1)
         h[:, half] += w[:, -1]
-        g = torch.flip(h, dims=[1]).contiguous()
-        return self.fftconv(x, g, rows_per_filt=C, offset0=half, pad_mode="replicate", bypass=bypass)
+        return h, half
+
+    def equalizer_backward(self, grad_out: torch.Tensor, sample_rate: int, db: torch.Tensor,
+                           bypass: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """dL/dx of :meth:`equalizer`: the zero-padded correlation with the reversed taps (``fftconv`` in constant mode
+        with the correlation taps as convolution taps) plus the replicate edge fold (:meth:`fir_pad_fold`)."""
+        g = self._prep(grad_out, "grad_out")
+        B, C, T = g.shape
+        h, half = self._equalizer_taps(sample_rate, db, B, g.device, bypass)
+        if half is None:
+            return self.gain(g, h)
+        gx = self.fftconv(g, h, rows_per_filt=C, offset0=half, pad_mode="constant", bypass=bypass)
+        return self.fir_pad_fold(g, h, rows_per_filt=C, left0=half, bypass=bypass, grad_x=gx)
+
+    def fir_pad_fold(self, grad_out: torch.Tensor, taps: torch.Tensor, rows_per_filt: int,
+                     left: Optional[torch.Tensor] = None, left0: int = 0, bypass: Optional[torch.Tensor] = None,
+                     grad_x: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Adds to ``grad_x`` (in place) what the replicate padding of the stride-1 correlation
+        ``y[m] = sum_k taps[f, k] xv[m + k - left0 - left[f]]`` carries back to the edge samples of every row."""
+        g = self._prep(grad_out, "grad_out")
+        T = g.shape[-1]
+        rows = g.numel() // T
+        taps = self._prep(taps.to(g.device), "taps")
+        n_filt, K = taps.shape
+        if left is not None:
+            left = self._prep(left.reshape(-1).to(g.device), "left", torch.int32)
+        bypass = self._bypass(bypass, n_filt, g.device)
+        assert grad_x is not None and grad_x.shape == g.shape and grad_x.is_contiguous()
+        ws_bytes = self.lib.b2a_fir_pad_fold_workspace_bytes(n_filt, K)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=g.device)
+        rc = self.lib.b2a_fir_pad_fold_f32(_dptr(g), rows, T, _dptr(taps), n_filt, K, int(rows_per_filt), _dptr(left),
+                                           int(left0), _dptr(bypass), _dptr(grad_x), _dptr(ws), ws_bytes,
+                                           self._stream(g))
+        self.lib.check(rc)
+        self.launches += 2
+        return grad_x
 
     def mel_filterbank(self, x: torch.Tensor, sample_rate: int, n_bands: int) -> torch.Tensor:
         """julius.SplitBands(sample_rate, n_bands)(x).permute(1, 2, 3, 0) -> [B, C, T, n_bands]
@@ -950,6 +1018,20 @@ class Engine:
         items left untouched."""
         x = self._prep(x, "x")
         B, C, T = x.shape
+        ir, n_ir, L, rows_per_ir, bypass = self._circconv_filters(x.shape, ir, bypass, x.device)
+        ws_bytes = self.lib.b2a_circconv_workspace_bytes(B * C, T, n_ir, L)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        out = torch.empty_like(x)
+        rc = self.lib.b2a_circconv_f32(_dptr(x), B * C, T, _dptr(ir), n_ir, L, rows_per_ir, int(bool(roll_to_peak)),
+                                       _dptr(bypass), _dptr(out), _dptr(ws), ws_bytes, self._stream(x))
+        self.lib.check(rc)
+        self.launches += 7
+        return out
+
+    def _circconv_filters(self, shape, ir: torch.Tensor, bypass, device):
+        """The IR bank of :meth:`circular_convolve` for x of ``shape`` [B, C, T]: (ir [n_ir, L] truncated to T, n_ir, L,
+        rows_per_ir, bypass [n_ir] or None)."""
+        B, C, T = shape
         ir = self._prep(ir, "ir")
         assert ir.ndim == 3 and ir.shape[0] in (1, B) and ir.shape[1] in (1, C), ir.shape
         if ir.shape[0] == 1 and B > 1 and (ir.shape[1] != 1 or bypass is not None):
@@ -960,18 +1042,28 @@ class Engine:
         n_ir = ir.shape[0] * ir.shape[1]
         rows_per_ir = (B * C if ir.shape[0] == 1 else C) if ir.shape[1] == 1 else 1
         if bypass is not None:
-            bypass = torch.as_tensor(bypass).reshape(-1).to(x.device)
+            bypass = torch.as_tensor(bypass).reshape(-1).to(device)
             if ir.shape[1] != 1:
                 bypass = bypass.repeat_interleave(C)
-            bypass = self._bypass(bypass, n_ir, x.device)
-        ws_bytes = self.lib.b2a_circconv_workspace_bytes(B * C, T, n_ir, L)
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-        out = torch.empty_like(x)
-        rc = self.lib.b2a_circconv_f32(_dptr(x), B * C, T, _dptr(ir), n_ir, L, rows_per_ir, int(bool(roll_to_peak)),
-                                       _dptr(bypass), _dptr(out), _dptr(ws), ws_bytes, self._stream(x))
+            bypass = self._bypass(bypass, n_ir, device)
+        return ir, n_ir, L, rows_per_ir, bypass
+
+    def circular_convolve_backward(self, grad_out: torch.Tensor, ir: torch.Tensor, roll_to_peak: bool = True,
+                                   bypass: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """dL/dx of :meth:`circular_convolve` (the IR is a constant): circular correlation with the rolled, scaled IR,
+        on the same overlap-save engine (csrc/fftconv.cu)."""
+        g = self._prep(grad_out, "grad_out")
+        B, C, T = g.shape
+        ir, n_ir, L, rows_per_ir, bypass = self._circconv_filters(g.shape, ir, bypass, g.device)
+        ws_bytes = self.lib.b2a_circconv_backward_workspace_bytes(B * C, T, n_ir, L)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=g.device)
+        gx = torch.empty_like(g)
+        rc = self.lib.b2a_circconv_backward_f32(_dptr(g), B * C, T, _dptr(ir), n_ir, L, rows_per_ir,
+                                                int(bool(roll_to_peak)), _dptr(bypass), _dptr(gx), _dptr(ws), ws_bytes,
+                                                self._stream(g))
         self.lib.check(rc)
-        self.launches += 7
-        return out
+        self.launches += 8
+        return gx
 
 
     # ------------------------------------------------------------------ resample
@@ -1011,6 +1103,19 @@ class Engine:
         self.lib.check(rc)
         self.launches += 1
         return out
+
+    def resample_backward(self, grad_out: torch.Tensor, T: int, old_sr: int, new_sr: int) -> torch.Tensor:
+        """dL/dx [..., T] of :meth:`resample` (either route) for dL/dout [..., out_len]."""
+        g = self._prep(grad_out, "grad_out")
+        kt, width, old, new = self._resample_kernel(int(old_sr), int(new_sr), g.device)
+        assert g.shape[-1] == int(self.lib.b2a_resample_out_len(T, old, new)), (g.shape, T)
+        rows = g.numel() // g.shape[-1]
+        gx = torch.empty(*g.shape[:-1], int(T), dtype=torch.float32, device=g.device)
+        rc = self.lib.b2a_resample_backward_f32(_dptr(g), rows, int(T), old, new, width, _dptr(kt), _dptr(gx),
+                                                self._stream(g))
+        self.lib.check(rc)
+        self.launches += 2 if T >= 3 else 1
+        return gx
 
 
     # ------------------------------------------------------------------ pitch shift

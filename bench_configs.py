@@ -3,7 +3,7 @@
 bench.py, which measures configs[1]).  One JSON line per config: device-resident throughput (CUDA events,
 >= 3 warm-ups, inputs larger than L2 or rotated), algorithmic bytes, and the CPU oracle on a bounded sample.
 
-    python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,largewin,grad,loss,gate,masked] [--no-cpu]
+    python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,largewin,grad,loss,gate,masked,effects_grad] [--no-cpu]
 
 Multi-GPU (BASELINE configs[3] = 512 items on 4 GPUs, configs[4] = 2048 items on 8 GPUs): one process per GPU,
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 4 --master-addr 127.0.0.1 --master-port 29511 \
@@ -497,6 +497,74 @@ def main():
         emit({"config": f"masked chain batch={B} mono 10s@44.1k Compose[VolumeNorm, Equalizer, LowPass, HighPass, PitchShift] "
                         "each prob 0.5", "ms_bypass_flags": ms_aware, "ms_gather_scatter": ms_gather,
               "clips_per_s": B / ms_aware * 1e3})
+
+    if "effects_grad" in only:  # backward kernels of the time-domain effects at 64 x 2ch x 10 s@44.1k
+        import subprocess
+
+        from audiotools_b200.engine import get_engine
+        from tests import effects_grad_cases as ec
+
+        try:
+            plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(LOCAL)],
+                                  capture_output=True, text=True, timeout=30).stdout.strip()
+        except Exception:  # noqa: BLE001 (informational field)
+            plim = "unknown"
+        eng = get_engine()
+        B, C, T, sr = 64, 2, 441000, 44100
+        g = torch.Generator().manual_seed(0)
+        x = (0.1 * torch.randn(B, C, T, generator=g)).to(dev)
+        db = ec.db_curve(B, 6, 1).to(dev)
+        ir = ec.synthetic_ir(B, sr, 2).to(dev)
+        fp32_peak = 67e12  # FLOP/s: H100 SXM data sheet, dense FP32, not measured
+        cases = {"resample_44k1_16k": ("resample", dict(new_sr=16000)),
+                 "resample_44k1_22k05": ("resample", dict(new_sr=22050)),
+                 "equalizer_6band": ("equalizer", dict(db=db)), "apply_ir_1s": ("apply_ir", dict(ir=ir))}
+        res = {}
+        for name, (method, kw) in cases.items():
+            fn = ec.ours(method, sr, **kw)
+            y = fn(x)
+            gy = torch.randn(y.shape, generator=g).to(dev)
+
+            def fwd_bwd():
+                xg = x.clone().requires_grad_()
+                (fn(xg) * gy).sum().backward()
+
+            def fwd():
+                with torch.no_grad():
+                    fn(x)
+
+            res[f"{name}_fwd_bwd_ms"] = timed(fwd_bwd, steps=5)
+            res[f"{name}_fwd_ms"] = timed(fwd, steps=5)
+            ref = ec.ref(method, sr, **kw)
+
+            def torch_fwd_bwd():
+                xg = x.clone().requires_grad_()
+                (ref(xg) * gy).sum().backward()
+
+            res[f"{name}_torch_autograd_fp32_ms"] = timed(torch_fwd_bwd, warmup=1, steps=3)
+        # each backward entry point alone, next to its forward launch at the same shape
+        for new_sr, tag in ((16000, "44k1_16k"), (22050, "44k1_22k05")):
+            y = eng.resample(x, sr, new_sr)
+            gy = torch.randn(y.shape, generator=g).to(dev)
+            res[f"resample_{tag}_forward_ms"] = timed(lambda: eng.resample(x, sr, new_sr), steps=10)
+            res[f"resample_{tag}_backward_ms"] = ms_b = timed(lambda: eng.resample_backward(gy, T, sr, new_sr), steps=10)
+            kt, width, old, new = eng._resample_kernel(sr, new_sr, dev)
+            flop = 2.0 * B * C * y.shape[-1] * kt.shape[0]  # one FMA per (output, tap), both directions
+            byts = 4.0 * B * C * (T + y.shape[-1])
+            res[f"resample_{tag}_backward_alg_GFLOP"] = flop / 1e9
+            res[f"resample_{tag}_backward_frac_of_fp32_peak"] = flop / (ms_b * 1e-3) / fp32_peak
+            res[f"resample_{tag}_backward_frac_of_hbm_peak"] = byts / (ms_b * 1e-3) / (peak * 1e9)
+        gx = torch.randn(B, C, T, generator=g).to(dev)
+        res["equalizer_forward_ms"] = timed(lambda: eng.equalizer(x, sr, db), steps=10)
+        res["equalizer_backward_ms"] = timed(lambda: eng.equalizer_backward(gx, sr, db), steps=10)
+        res["circconv_forward_ms"] = timed(lambda: eng.circular_convolve(x, ir), steps=10)
+        res["circconv_backward_ms"] = timed(lambda: eng.circular_convolve_backward(gx, ir), steps=10)
+        res["peak_scale_backward_ms"] = ms_p = timed(lambda: eng.peak_scale_backward(gx, x, x), steps=10)
+        res["peak_scale_backward_frac_of_hbm_peak"] = 4.0 * B * C * T * 5 / (ms_p * 1e-3) / (peak * 1e9)
+        emit({"config": "effects_grad 64x2ch 10s@44.1k: forward+backward, no-grad forward, each backward entry point "
+                        "next to its forward, and torch autograd (fp32, same GPU) over the float64 restatements' code",
+              **res, "gpu": torch.cuda.get_device_name(LOCAL), "power_limit": plim})
+        del x, gx
 
     if "specaug" in only:  # SURVEY 8f.1: SpectralTransform chain stft -> FrequencyMask -> TimeMask -> istft at cfg2's shape
         g = torch.Generator().manual_seed(0)

@@ -290,6 +290,19 @@ int b2a_fir_direct_f32(const float* x, int64_t rows, int64_t T, const float* tap
                        int rows_per_filt, const int32_t* left, int left0, int stride, int64_t out_len,
                        int pad_mode, int subtract_from_input, const int32_t* bypass, float* out, void* stream);
 
+/* Replicate-padding fold of a stride-1 FIR's gradient.  For the correlation form y[m] = sum_k taps[f][k] *
+ * xv[m + k - left0 - left[f]] with replicate padding, the gradient is the zero-padded correlation with the reversed
+ * taps (b2a_fftconv_f32, pad_mode 1) PLUS what the padded positions carry back to the edge samples; this adds that
+ * part to grad_x in place:
+ *   grad_x[0]   += sum_{n < l}           (taps[0] + .. + taps[min(l-1-n, K-1)]) grad_out[n]          (l = left0 + left[f])
+ *   grad_x[T-1] += sum_{n > T + l - K}   (taps[T+l-n] + .. + taps[K-1]) grad_out[n]
+ * valid for any T (also T < K).  Rows of a filter with bypass != 0 are left alone (their gradient is the copy).
+ * ws: b2a_fir_pad_fold_workspace_bytes() bytes (prefix / suffix sums of every filter, computed on the device). */
+size_t b2a_fir_pad_fold_workspace_bytes(int64_t n_filt, int K);
+int b2a_fir_pad_fold_f32(const float* grad_out, int64_t rows, int64_t T, const float* taps, int64_t n_filt, int K,
+                         int rows_per_filt, const int32_t* left, int left0, const int32_t* bypass, float* grad_x,
+                         void* ws, size_t ws_bytes, void* stream);
+
 /* EffectMixin.convolve (audiotools/core/effects.py:66-123): CIRCULAR convolution (period T) of each row with
  * its item's impulse response, the IR rolled so that max|ir| sits at t = 0 (roll_to_peak) and the result
  * scaled by 1 / max(max|ir|, 1e-5).   ir: [n_ir, L] with L <= T (truncate first, as the reference does). */
@@ -297,6 +310,14 @@ size_t b2a_circconv_workspace_bytes(int64_t rows, int64_t T, int64_t n_ir, int64
 int b2a_circconv_f32(const float* x, int64_t rows, int64_t T, const float* ir, int64_t n_ir, int64_t L,
                      int rows_per_ir, int roll_to_peak, const int32_t* bypass, float* out, void* ws, size_t ws_bytes,
                      void* stream);
+/* Gradient of b2a_circconv_f32 with respect to x (same arguments; the IR is a constant): with the forward
+ * y[n] = s sum_j h[j] x[(n - j + idx) mod T], grad_x[m] = s sum_j h[j] grad_out[(m + j - idx) mod T] -- a circular
+ * correlation, run on the same engine with reversed taps.  Bypassed rows: grad_x = grad_out.  grad_x must not alias
+ * grad_out. */
+size_t b2a_circconv_backward_workspace_bytes(int64_t rows, int64_t T, int64_t n_ir, int64_t L);
+int b2a_circconv_backward_f32(const float* grad_out, int64_t rows, int64_t T, const float* ir, int64_t n_ir, int64_t L,
+                              int rows_per_ir, int roll_to_peak, const int32_t* bypass, float* grad_x, void* ws,
+                              size_t ws_bytes, void* stream);
 
 /* ---- windowed-sinc polyphase resampling ------------------------------------------------------
  * AudioSignal.resample (audiotools/core/audio_signal.py:716-736 -> julius.resample_frac): old_r/new_r are
@@ -306,6 +327,13 @@ int b2a_circconv_f32(const float* x, int64_t rows, int64_t T, const float* ir, i
 int64_t b2a_resample_out_len(int64_t T, int old_r, int new_r);
 int b2a_resample_f32(const float* x, int64_t rows, int64_t T, int old_r, int new_r, int width,
                      const float* kernel_t, float* out, void* stream);
+/* Gradient of the resampling with respect to x (either forward route: the polyphase kernel above, or
+ * b2a_fir_direct_f32 when new_r == 1): grad_out [rows, out_len] -> grad_x [rows, T],
+ *   grad_x_ext[u] = sum_{m, i} kernel_t[u + width - m*old_r][i] grad_out[m*new_r + i]   (0 <= u + width - m*old_r < K),
+ * with the replicate padding folded back: grad_x[0] also takes u in [-width, 0), grad_x[T-1] u in [T, T + width + old_r).
+ * Fixed summation order (no atomics): reruns are bit-identical. */
+int b2a_resample_backward_f32(const float* grad_out, int64_t rows, int64_t T, int old_r, int new_r, int width,
+                              const float* kernel_t, float* grad_x, void* stream);
 
 /* ---- pitch shift ---------------------------------------------------------------------------------
  * EffectMixin.pitch_shift (audiotools/core/effects.py:247-277; SoX `pitch -q` + `rate` there): WSOLA
@@ -348,6 +376,16 @@ int b2a_time_stretch_f32(const float* x, int64_t rows, int64_t T, int sr, double
  *   b2a_clamp_items_f32  out = min(max(x, lo[item]), hi[item])                                 (:459) */
 int b2a_row_absmax_f32(const float* x, int64_t rows, int64_t T, float* peak, void* stream);
 int b2a_limit_peak_f32(const float* x, float* out, int64_t rows, int64_t T, const float* peak, float max_abs, void* stream);
+/* Gradient of the per-row peak rescales, one CTA per row (first arg-max and dot(grad_out, y) in a fixed order):
+ *   x_ref == NULL  ensure_max_of_audio, y' = y p with p = max_abs / peak where peak = max|y| > max_abs, else 1:
+ *                  grad_y = p g - [peak > max_abs] (max_abs / peak^2) dot(g, y) sign(y_b) e_b
+ *   x_ref != NULL  apply_ir's peak restore, y' = y S, S = clamp(max|x_ref|, 1e-8) / clamp(max|y|, 1e-8):
+ *                  grad_y = S g - [My >= 1e-8] S dot(g, y) / My sign(y_b) e_b,
+ *                  grad_x_ref = [Mx >= 1e-8] dot(g, y) / clamp(My, 1e-8) sign(x_a) e_a (zero elsewhere, written whole);
+ *                  bypass: nullable [rows] int32, non-zero = S was 1: grad_y = g, grad_x_ref = 0.
+ * e_a, e_b: the first index of the row's maximum.  [rows, T] float32 each. */
+int b2a_peak_scale_backward_f32(const float* grad_out, const float* y, const float* x_ref, int64_t rows, int64_t T,
+                                float max_abs, const int32_t* bypass, float* grad_y, float* grad_x_ref, void* stream);
 int b2a_clamp_items_f32(const float* x, float* out, int64_t B, int64_t per_item, const float* lo, const float* hi,
                         void* stream);
 int b2a_mix_f32(const float* x, const float* other, const float* other_gain, float* out, int64_t B, int64_t per_item,
