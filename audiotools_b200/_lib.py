@@ -115,6 +115,17 @@ SIGNATURES = {
                                           c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "b2a_peak_scale_backward_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float, c_void_p,
                                             c_void_p, c_void_p, c_void_p]),
+    "b2a_spec_band_mask_out_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_int, c_int, c_float, c_float, c_void_p]),
+    "b2a_spec_band_mask_backward_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p,
+                                                c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "b2a_spec_mask_low_out_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_float, c_float, c_float,
+                                          c_void_p, c_void_p]),
+    "b2a_spec_mask_low_backward_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_float, c_float,
+                                               c_float, c_void_p, c_void_p, c_void_p]),
+    "b2a_spec_gate_backward_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int64, c_void_p, c_int64, c_void_p,
+                                           c_int, POINTER(c_float), c_int, POINTER(c_float), c_int, c_void_p,
+                                           c_void_p]),
 }
 
 

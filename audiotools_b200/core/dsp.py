@@ -4,9 +4,11 @@ The reference loops over the batch in Python, building one ``julius.LowPassFilte
 here the per-item tap design and the filtering are one grouped launch each (``csrc/fir.cu``).
 The spectral masks (SURVEY.md §8f.1, ref:audiotools/core/dsp.py:217-370) work on ``stft_data``: the two band
 masks run as one store-only kernel (``csrc/specmask.cu``), the phase operations are container arithmetic on the
-complex tensor.  The chunking helpers (``windows`` / ``collect_windows`` / ``overlap_and_add``) are container reshapes."""
+complex tensor.  When ``stft_data`` requires a gradient the masks run out of place through ``core/grad.py``'s
+Functions (new CUDA backward kernels in specmask.cu); otherwise they make the same in-place launches as always.  The chunking helpers (``windows`` / ``collect_windows`` / ``overlap_and_add``) are container reshapes."""
 import torch
 
+from . import grad as _grad
 from . import util
 
 
@@ -113,7 +115,10 @@ class DSPMixin:
         spec = self.stft_data
         if spec.dtype != torch.complex64 or not spec.is_contiguous():
             spec = spec.to(torch.complex64).contiguous()
-        self.stft_data = _engine().spec_band_mask(spec, axis_vals, lo, hi, axis, val)
+        if _grad.wants_grad(spec):
+            self.stft_data = _grad.SpecBandMask.apply(spec, axis_vals, lo, hi, axis, val)
+        else:
+            self.stft_data = _engine().spec_band_mask(spec, axis_vals, lo, hi, axis, val)
         return self
 
     def mask_frequencies(self, fmin_hz, fmax_hz, val: float = 0.0):
@@ -140,7 +145,13 @@ class DSPMixin:
         if self.stft_data is None:
             self.stft()
         cut = util.ensure_tensor(db_cutoff, ndim=1).float().reshape(-1)
-        self.stft_data = _engine().spec_mask_low(self.stft_data, cut, val)
+        if _grad.wants_grad(self.stft_data):
+            spec = self.stft_data
+            if spec.dtype != torch.complex64 or not spec.is_contiguous():
+                spec = spec.to(torch.complex64).contiguous()
+            self.stft_data = _grad.SpecMaskLow.apply(spec, cut, val)
+        else:
+            self.stft_data = _engine().spec_mask_low(self.stft_data, cut, val)
         return self
 
     def shift_phase(self, shift):

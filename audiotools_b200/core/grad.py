@@ -1,7 +1,8 @@
 """``torch.autograd.Function``s over the engine: the differentiable forms of the spectral front end
 (ref:audiotools/core/audio_signal.py:1123-1296, 1333-1426 and effects.py:200-238, differentiable through torch there;
 ref:tests/core/test_grad.py) and of the time-domain effects (resample, equalizer, convolve, apply_ir,
-ensure_max_of_audio, mix, quantization; gradients with respect to the waveform only).  ``AudioSignal`` uses them only when grad mode is on and the input requires a gradient;
+ensure_max_of_audio, mix, quantization; gradients with respect to the waveform only) and of the spectral masks and the
+spectral gate (ref:audiotools/core/dsp.py:217-334, ml/layers/spectral_gate.py:58-127; gradients to the spectrogram).  ``AudioSignal`` uses them only when grad mode is on and the input requires a gradient;
 otherwise it calls the engine directly, with exactly the launches it always made.
 
 Each forward is the engine call of the no-gradient path; each backward is one launch sequence of csrc/grad.cu (or an
@@ -233,6 +234,60 @@ class StraightThrough(torch.autograd.Function):
     @once_differentiable
     def backward(ctx, g):
         return g, None
+
+
+class SpecBandMask(torch.autograd.Function):
+    """spec [B, C, F, N] complex64 -> a copy with the band lo[item] <= axis_vals < hi[item] filled
+    (``Engine.spec_band_mask_out``); the band is a constant (a comparison in the reference)."""
+
+    @staticmethod
+    def forward(ctx, spec, axis_vals, lo, hi, axis, val):
+        ctx.save_for_backward(spec)
+        ctx.args = (axis_vals, lo, hi, axis)
+        return _engine().spec_band_mask_out(spec, axis_vals, lo, hi, axis, val)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (spec,) = ctx.saved_tensors
+        return _engine().spec_band_mask_backward(g, spec, *ctx.args), None, None, None, None, None
+
+
+class SpecMaskLow(torch.autograd.Function):
+    """``mask_low_magnitudes`` out of place (``Engine.spec_mask_low_out``); the backward reuses the forward's maximum
+    |X|^2 and recomputes the mask from the saved spectrogram."""
+
+    @staticmethod
+    def forward(ctx, spec, db_cutoff, val):
+        out, ws = _engine().spec_mask_low_out(spec, db_cutoff, val)
+        ctx.save_for_backward(spec)
+        ctx.args = (db_cutoff, val, ws)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (spec,) = ctx.saved_tensors
+        db_cutoff, val, ws = ctx.args
+        return _engine().spec_mask_low_backward(g, spec, db_cutoff, val, ws), None, None
+
+
+class SpecGate(torch.autograd.Function):
+    """The spectral gate's ``spec * (1 - amount * mask)`` (``Engine.spec_gate``).  The noise spectrogram and the amount
+    are constants; the backward recomputes the mask from the saved spectrogram and the forward's thresholds."""
+
+    @staticmethod
+    def forward(ctx, spec, nz_spec, n_std, amount, smooth_f, smooth_t):
+        out, thresh = _engine().spec_gate(spec, nz_spec, n_std, amount, smooth_f, smooth_t)
+        ctx.save_for_backward(spec)
+        ctx.args = (thresh, amount, smooth_f, smooth_t)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (spec,) = ctx.saved_tensors
+        return _engine().spec_gate_backward(g, spec, *ctx.args), None, None, None, None, None
 
 
 def refuse_param_grad(method: str, name: str, t) -> None:

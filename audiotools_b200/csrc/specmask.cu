@@ -12,6 +12,13 @@
 //   mask_low_kernel    |X|^2 (one read-only pass, float atomicMax on the bit pattern), then cells whose
 //                      10 log10(max(|X|^2, 1e-10)) (floored at max - 80 dB) is below the item's cut-off get
 //                      magnitude `val` and keep their phase; only those cells are written.
+// The gradient path (a spectrogram that requires a gradient) cannot write in place: autograd may have saved the input
+// for another node.  Its forwards write a new tensor (one read, one write per cell) and its backwards recompute the
+// mask decision from the saved X with the forward's own arithmetic:
+//   band_mask_out_kernel<false> / <true>   out = band ? fill : X  /  gX = band || X == 0 ? 0 : g
+//   mask_low_out_kernel, mask_low_bwd_kernel  unmasked: g (0 at X == 0); masked: val (g - Re(g conj u) u) / |X|,
+//                      u = X / |X| (the phase's derivative, evaluated in float64; 0 at X == 0 and for val == 0)
+//   gate_apply_kernel  reads the booleans from one tensor (X) and multiplies another (X forward, g backward)
 #include "b2a_common.h"
 
 namespace b2a {
@@ -34,6 +41,38 @@ band_mask_kernel(float2* __restrict__ spec, int F, int N, const float* __restric
       const float v = __ldg(axis_vals + n);
       if (l <= v && v < h) p[n] = fill;
     }
+  }
+}
+
+// BWD false: out = in band ? fill : spec.  BWD true: out = in band || spec == 0 ? 0 : g (fill is 0).  The band test is
+// band_mask_kernel's; a line inside a frequency band reads nothing.
+template <bool BWD>
+__global__ void __launch_bounds__(256)
+band_mask_out_kernel(const float2* __restrict__ g, const float2* __restrict__ spec, float2* __restrict__ out, int F,
+                     int N, const float* __restrict__ axis_vals, const float* __restrict__ lo,
+                     const float* __restrict__ hi, int rows_per_item, int axis, float2 fill) {
+  const int line = blockIdx.x;  // row * F + f
+  const int row = line / F, f = line - row * F;
+  const int item = row / rows_per_item;
+  const float l = __ldg(lo + item), h = __ldg(hi + item);
+  const size_t base = (size_t)line * N;
+  bool line_in = false;
+  if (axis == 0) {
+    const float v = __ldg(axis_vals + f);
+    line_in = l <= v && v < h;  // CTA-uniform
+  }
+  for (int n = threadIdx.x; n < N; n += blockDim.x) {
+    bool in = line_in;
+    if (axis != 0) {
+      const float v = __ldg(axis_vals + n);
+      in = l <= v && v < h;
+    }
+    float2 r = fill;
+    if (!in) {
+      r = spec[base + n];
+      if (BWD) r = (r.x == 0.f && r.y == 0.f) ? make_float2(0.f, 0.f) : g[base + n];
+    }
+    out[base + n] = r;
   }
 }
 
@@ -70,21 +109,70 @@ maxpow_kernel(const float2* __restrict__ spec, long long total, unsigned* __rest
   }
 }
 
+// log_magnitude()'s top_db floor from the maximum maxpow_kernel found
+__device__ __forceinline__ float mask_low_floor(const unsigned* max_bits, float amin2, float top_db) {
+  return 10.0f * log10f(fmaxf(__uint_as_float(*max_bits), amin2)) - top_db;
+}
+
+// the mask decision of mask_low_magnitudes, shared by the forwards and the backward
+__device__ __forceinline__ bool mask_low_cell(float2 z, float floor_db, float cut, float amin2) {
+  float db = 10.0f * log10f(fmaxf(power_of(z), amin2));
+  db = fmaxf(db, floor_db);
+  return db < cut;
+}
+
+// magnitude := val, phase kept: val * exp(1j * atan2(im, re))
+__device__ __forceinline__ float2 keep_phase(float2 z, float val) {
+  const float ph = atan2f(z.y, z.x);
+  float sn, cs;
+  sincosf(ph, &sn, &cs);
+  return make_float2(val * cs, val * sn);
+}
+
 __global__ void __launch_bounds__(256)
 mask_low_kernel(float2* __restrict__ spec, long long total, long long cells_per_item, const float* __restrict__ cutoff,
                 const unsigned* __restrict__ max_bits, float amin2, float top_db, float val) {
-  const float floor_db = 10.0f * log10f(fmaxf(__uint_as_float(*max_bits), amin2)) - top_db;
+  const float floor_db = mask_low_floor(max_bits, amin2, top_db);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const float2 z = spec[i];
-    float db = 10.0f * log10f(fmaxf(power_of(z), amin2));
-    db = fmaxf(db, floor_db);
-    if (db < __ldg(cutoff + i / cells_per_item)) {
-      // magnitude := val, phase kept: val * exp(1j * atan2(im, re))
-      const float ph = atan2f(z.y, z.x);
-      float sn, cs;
-      sincosf(ph, &sn, &cs);
-      spec[i] = make_float2(val * cs, val * sn);
+    if (mask_low_cell(z, floor_db, __ldg(cutoff + i / cells_per_item), amin2)) spec[i] = keep_phase(z, val);
+  }
+}
+
+__global__ void __launch_bounds__(256)
+mask_low_out_kernel(const float2* __restrict__ spec, float2* __restrict__ out, long long total, long long cells_per_item,
+                    const float* __restrict__ cutoff, const unsigned* __restrict__ max_bits, float amin2, float top_db,
+                    float val) {
+  const float floor_db = mask_low_floor(max_bits, amin2, top_db);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const float2 z = spec[i];
+    out[i] = mask_low_cell(z, floor_db, __ldg(cutoff + i / cells_per_item), amin2) ? keep_phase(z, val) : z;
+  }
+}
+
+__global__ void __launch_bounds__(256)
+mask_low_bwd_kernel(const float2* __restrict__ g, const float2* __restrict__ spec, float2* __restrict__ gx,
+                    long long total, long long cells_per_item, const float* __restrict__ cutoff,
+                    const unsigned* __restrict__ max_bits, float amin2, float top_db, float val) {
+  const float floor_db = mask_low_floor(max_bits, amin2, top_db);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const float2 z = spec[i];
+    float2 r = make_float2(0.f, 0.f);  // X == 0: |X| and angle(X) both backpropagate 0
+    if (z.x != 0.f || z.y != 0.f) {
+      const float2 gi = g[i];
+      if (!mask_low_cell(z, floor_db, __ldg(cutoff + i / cells_per_item), amin2)) {
+        r = gi;
+      } else if (val != 0.f) {
+        // val * exp(1j angle X): the tangential part of g scaled by val / |X|, i.e. val Im(g conj X) / |X|^3 * (1j X).
+        // In float64: the factor 1 / |X| amplifies every float32 rounding of the small cells, and only masked cells
+        // with a non-zero fill take this branch.
+        const double x = z.x, y = z.y;
+        const double p = x * x + y * y;
+        const double s = (double)val * ((double)gi.y * x - (double)gi.x * y) / (p * sqrt(p));
+        r = make_float2((float)(-s * y), (float)(s * x));
+      }
     }
+    gx[i] = r;
   }
 }
 
@@ -94,10 +182,12 @@ mask_low_kernel(float2* __restrict__ spec, long long total, long long cells_per_
 // -> compare -> conv2d(7 x 11 triangle) -> 1 - amount * mask -> multiply: eight tensor passes + cuDNN).
 //   gate_stats_kernel  per (noise row, bin): thresh = mean_t(db) + n_std * std_t(db) (unbiased, torch.std), with
 //                      db = 20 log10(max(|X|, 1e-4)); one warp per line, frames contiguous.
-//   gate_apply_kernel  out = X * (1 - amount[item] * S),  S = the zero-padded 2-D smoothing of the boolean
-//                      (db < thresh[bin]) with the SEPARABLE kernel rf (x) rt / sum: a CTA stages the booleans of a
+//   gate_apply_kernel  out = Y * (1 - amount[item] * S),  S = the zero-padded 2-D smoothing of the boolean
+//                      (db(X) < thresh[bin]) with the SEPARABLE kernel rf (x) rt / sum: a CTA stages the booleans of a
 //                      (TF + 2 hf) x (TT + 2 ht) tile, smooths along time, then along frequency, and writes the
 //                      product -- one read and one write of the spectrogram (out of place: neighbours read |X|).
+//                      Y = X in the forward; Y = g in the backward (S is a constant of the gradient: the reference
+//                      builds it from a comparison), which reads X again and the saved thresholds.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ float gate_db(float2 z) { return 20.0f * log10f(fmaxf(hypotf(z.x, z.y), 1e-4f)); }
 
@@ -118,7 +208,8 @@ gate_stats_kernel(const float2* __restrict__ nz, int lines, int N, float n_std, 
 constexpr int GT_F = 16, GT_T = 64, G_MAXH = 8;  // tile, largest half-width of either smoothing vector
 
 struct GateParams {
-  const float2* spec;
+  const float2* spec;    // X: the booleans
+  const float2* mul;     // the tensor multiplied (X, or the output gradient)
   float2* out;
   const float* thresh;   // [nz_rows, F]
   const float* amount;   // [rows / rows_per_item]
@@ -158,7 +249,7 @@ __global__ void __launch_bounds__(256) gate_apply_kernel(GateParams p) {
     float acc = 0.f;
     for (int d = 0; d <= 2 * p.hf; ++d) acc = fmaf(p.rf[d], st[a + d][b], acc);
     const float g = 1.0f - acc * amt;
-    const float2 z = sp[(size_t)f * p.N + t];
+    const float2 z = p.mul[((size_t)row * p.F + f) * (size_t)p.N + t];
     op[(size_t)f * p.N + t] = make_float2(z.x * g, z.y * g);
   }
 }
@@ -186,6 +277,45 @@ extern "C" int b2a_spec_band_mask_f32(float* spec, int64_t rows, int F, int N, c
              reinterpret_cast<float2*>(spec), F, N, axis_vals, lo, hi, rows_per_item, axis, make_float2(fill_re, fill_im));
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
+}
+
+// the checks and the launch of both out-of-place band-mask passes
+static int band_mask_out(bool bwd, const float* g, const float* spec, float* out, int64_t rows, int F, int N,
+                         const float* axis_vals, const float* lo, const float* hi, int rows_per_item, int axis,
+                         float2 fill, void* stream) {
+  B2A_REQUIRE(spec && out && axis_vals && lo && hi && (g || !bwd), B2A_E_INVALID, "spec_band_mask: null pointer");
+  B2A_REQUIRE(rows >= 1 && F >= 1 && N >= 1 && rows_per_item >= 1 && (axis == 0 || axis == 1), B2A_E_INVALID,
+              "spec_band_mask: bad argument");
+  B2A_REQUIRE((((uintptr_t)spec | (uintptr_t)out | (uintptr_t)g) & 7) == 0, B2A_E_INVALID,
+              "spec_band_mask: spectra must be 8-byte aligned");
+  B2A_REQUIRE(out != spec && out != g, B2A_E_INVALID, "spec_band_mask: the output must not alias an input");
+  B2A_REQUIRE(rows * F < (int64_t)2147483647, B2A_E_UNSUPPORTED, "spec_band_mask: too many lines");
+  const dim3 grid((unsigned)(rows * F)), block(N >= 256 ? 256 : 64);
+  const float2* gp = reinterpret_cast<const float2*>(g);
+  const float2* sp = reinterpret_cast<const float2*>(spec);
+  float2* op = reinterpret_cast<float2*>(out);
+  if (bwd)
+    B2A_LAUNCH(band_mask_out_kernel<true>, grid, block, 0, stream, gp, sp, op, F, N, axis_vals, lo, hi, rows_per_item,
+               axis, make_float2(0.f, 0.f));
+  else
+    B2A_LAUNCH(band_mask_out_kernel<false>, grid, block, 0, stream, gp, sp, op, F, N, axis_vals, lo, hi, rows_per_item,
+               axis, fill);
+  B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
+}
+
+extern "C" int b2a_spec_band_mask_out_f32(const float* spec, float* out, int64_t rows, int F, int N,
+                                          const float* axis_vals, const float* lo, const float* hi, int rows_per_item,
+                                          int axis, float fill_re, float fill_im, void* stream) {
+  return band_mask_out(false, nullptr, spec, out, rows, F, N, axis_vals, lo, hi, rows_per_item, axis,
+                       make_float2(fill_re, fill_im), stream);
+}
+
+extern "C" int b2a_spec_band_mask_backward_f32(const float* grad_out, const float* spec, int64_t rows, int F, int N,
+                                               const float* axis_vals, const float* lo, const float* hi,
+                                               int rows_per_item, int axis, float* grad_spec, void* stream) {
+  return band_mask_out(true, grad_out, spec, grad_spec, rows, F, N, axis_vals, lo, hi, rows_per_item, axis,
+                       make_float2(0.f, 0.f), stream);
 }
 
 extern "C" int b2a_spec_rotate_f32(float* spec, int64_t items, int64_t cells_per_item, const float* shift,
@@ -219,26 +349,52 @@ extern "C" int b2a_spec_mask_low_f32(float* spec, int64_t items, int64_t cells_p
   return B2A_OK;
 }
 
-extern "C" int b2a_spec_gate_f32(const float* spec, int64_t rows, int F, int64_t N, const float* nz_spec, int64_t nz_rows,
-                                 int64_t nz_N, float n_std, const float* amount, int rows_per_item,
-                                 const float* smooth_f_h, int n_f, const float* smooth_t_h, int n_t, float* out,
-                                 void* ws, void* stream) {
-  B2A_REQUIRE(spec && nz_spec && amount && smooth_f_h && smooth_t_h && out && ws, B2A_E_INVALID, "spec_gate: null pointer");
-  B2A_REQUIRE(rows >= 1 && rows <= 65535 && F >= 1 && N >= 1 && nz_N >= 1 && rows_per_item >= 1, B2A_E_INVALID,
-              "spec_gate: bad shape");
-  B2A_REQUIRE(nz_rows == 1 || nz_rows == rows, B2A_E_INVALID, "spec_gate: noise rows (%lld) must be 1 or %lld",
-              (long long)nz_rows, (long long)rows);
-  B2A_REQUIRE((n_f & 1) && (n_t & 1) && n_f <= 2 * G_MAXH + 1 && n_t <= 2 * G_MAXH + 1, B2A_E_UNSUPPORTED,
-              "spec_gate: smoothing vectors must have odd lengths <= %d (got %d, %d)", 2 * G_MAXH + 1, n_f, n_t);
-  B2A_REQUIRE(out != spec, B2A_E_INVALID, "spec_gate: out must not alias spec");
-  B2A_REQUIRE((((uintptr_t)spec | (uintptr_t)nz_spec | (uintptr_t)out) & 7) == 0, B2A_E_INVALID, "spec_gate: alignment");
-  B2A_REQUIRE(nz_rows * F < (int64_t)2147483647 && (F + GT_F - 1) / GT_F <= 65535, B2A_E_UNSUPPORTED, "spec_gate: too large");
-  float* thresh = reinterpret_cast<float*>(ws);  // [nz_rows, F]
-  B2A_LAUNCH(gate_stats_kernel, dim3((unsigned)((nz_rows * F + 7) / 8)), dim3(256), 0, stream,
-             reinterpret_cast<const float2*>(nz_spec), (int)(nz_rows * F), (int)nz_N, n_std, thresh);
+extern "C" int b2a_spec_mask_low_out_f32(const float* spec, float* out, int64_t items, int64_t cells_per_item,
+                                         const float* db_cutoff, float amin_sq, float top_db, float val,
+                                         void* ws /* >= 4 bytes, kept for the backward */, void* stream) {
+  B2A_REQUIRE(spec && out && db_cutoff && ws, B2A_E_INVALID, "spec_mask_low_out: null pointer");
+  B2A_REQUIRE(items >= 1 && cells_per_item >= 1, B2A_E_INVALID, "spec_mask_low_out: bad argument");
+  B2A_REQUIRE((((uintptr_t)spec | (uintptr_t)out) & 7) == 0 && ((uintptr_t)ws & 3) == 0, B2A_E_INVALID,
+              "spec_mask_low_out: alignment");
+  B2A_REQUIRE(out != spec, B2A_E_INVALID, "spec_mask_low_out: out must not alias spec");
+  const long long total = (long long)items * cells_per_item;
+#ifdef B2A_SIM
+  memset(ws, 0, 4);
+#else
+  B2A_CUDA_OK(cudaMemsetAsync(ws, 0, 4, (cudaStream_t)stream));
+#endif
+  B2A_LAUNCH(maxpow_kernel, dim3(grid_for(total)), dim3(256), 0, stream, reinterpret_cast<const float2*>(spec), total,
+             (unsigned*)ws);
+  B2A_LAUNCH(mask_low_out_kernel, dim3(grid_for(total)), dim3(256), 0, stream, reinterpret_cast<const float2*>(spec),
+             reinterpret_cast<float2*>(out), total, (long long)cells_per_item, db_cutoff, (const unsigned*)ws, amin_sq,
+             top_db, val);
+  B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
+}
+
+extern "C" int b2a_spec_mask_low_backward_f32(const float* grad_out, const float* spec, int64_t items,
+                                              int64_t cells_per_item, const float* db_cutoff, float amin_sq,
+                                              float top_db, float val, const void* ws, float* grad_spec, void* stream) {
+  B2A_REQUIRE(grad_out && spec && db_cutoff && ws && grad_spec, B2A_E_INVALID, "spec_mask_low_backward: null pointer");
+  B2A_REQUIRE(items >= 1 && cells_per_item >= 1, B2A_E_INVALID, "spec_mask_low_backward: bad argument");
+  B2A_REQUIRE((((uintptr_t)grad_out | (uintptr_t)spec | (uintptr_t)grad_spec) & 7) == 0 && ((uintptr_t)ws & 3) == 0,
+              B2A_E_INVALID, "spec_mask_low_backward: alignment");
+  const long long total = (long long)items * cells_per_item;
+  B2A_LAUNCH(mask_low_bwd_kernel, dim3(grid_for(total)), dim3(256), 0, stream,
+             reinterpret_cast<const float2*>(grad_out), reinterpret_cast<const float2*>(spec),
+             reinterpret_cast<float2*>(grad_spec), total, (long long)cells_per_item, db_cutoff,
+             (const unsigned*)ws, amin_sq, top_db, val);
+  B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
+}
+
+// gate_apply_kernel over (spec, mul) -> out with thresholds `thresh` [nz_rows, F]
+static int gate_apply(const float2* spec, const float2* mul, float2* out, int64_t rows, int F, int64_t N,
+                      const float* thresh, int64_t nz_rows, const float* amount, int rows_per_item,
+                      const float* smooth_f_h, int n_f, const float* smooth_t_h, int n_t, void* stream) {
   GateParams p;
   memset(&p, 0, sizeof(p));
-  p.spec = reinterpret_cast<const float2*>(spec); p.out = reinterpret_cast<float2*>(out); p.thresh = thresh;
+  p.spec = spec; p.mul = mul; p.out = out; p.thresh = thresh;
   p.amount = amount; p.F = F; p.N = (int)N; p.rows_per_item = rows_per_item; p.nz_rows = (int)nz_rows;
   p.hf = n_f / 2; p.ht = n_t / 2;
   double sum_f = 0, sum_t = 0;
@@ -251,4 +407,46 @@ extern "C" int b2a_spec_gate_f32(const float* spec, int64_t rows, int F, int64_t
              dim3(256), 0, stream, p);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
+}
+
+// the shape checks both gate entry points share
+#define GATE_REQUIRE_SHAPE(what)                                                                                       \
+  B2A_REQUIRE(rows >= 1 && rows <= 65535 && F >= 1 && N >= 1 && rows_per_item >= 1, B2A_E_INVALID,                     \
+              what ": bad shape");                                                                                     \
+  B2A_REQUIRE(nz_rows == 1 || nz_rows == rows, B2A_E_INVALID, what ": noise rows (%lld) must be 1 or %lld",            \
+              (long long)nz_rows, (long long)rows);                                                                    \
+  B2A_REQUIRE((n_f & 1) && (n_t & 1) && n_f <= 2 * G_MAXH + 1 && n_t <= 2 * G_MAXH + 1, B2A_E_UNSUPPORTED,            \
+              what ": smoothing vectors must have odd lengths <= %d (got %d, %d)", 2 * G_MAXH + 1, n_f, n_t);          \
+  B2A_REQUIRE(nz_rows * F < (int64_t)2147483647 && (F + GT_F - 1) / GT_F <= 65535, B2A_E_UNSUPPORTED, what ": too large")
+
+extern "C" int b2a_spec_gate_f32(const float* spec, int64_t rows, int F, int64_t N, const float* nz_spec, int64_t nz_rows,
+                                 int64_t nz_N, float n_std, const float* amount, int rows_per_item,
+                                 const float* smooth_f_h, int n_f, const float* smooth_t_h, int n_t, float* out,
+                                 void* ws, void* stream) {
+  B2A_REQUIRE(spec && nz_spec && amount && smooth_f_h && smooth_t_h && out && ws, B2A_E_INVALID, "spec_gate: null pointer");
+  B2A_REQUIRE(nz_N >= 1, B2A_E_INVALID, "spec_gate: bad shape");
+  GATE_REQUIRE_SHAPE("spec_gate");
+  B2A_REQUIRE(out != spec, B2A_E_INVALID, "spec_gate: out must not alias spec");
+  B2A_REQUIRE((((uintptr_t)spec | (uintptr_t)nz_spec | (uintptr_t)out) & 7) == 0, B2A_E_INVALID, "spec_gate: alignment");
+  float* thresh = reinterpret_cast<float*>(ws);  // [nz_rows, F]
+  B2A_LAUNCH(gate_stats_kernel, dim3((unsigned)((nz_rows * F + 7) / 8)), dim3(256), 0, stream,
+             reinterpret_cast<const float2*>(nz_spec), (int)(nz_rows * F), (int)nz_N, n_std, thresh);
+  return gate_apply(reinterpret_cast<const float2*>(spec), reinterpret_cast<const float2*>(spec),
+                    reinterpret_cast<float2*>(out), rows, F, N, thresh, nz_rows, amount, rows_per_item, smooth_f_h, n_f,
+                    smooth_t_h, n_t, stream);
+}
+
+extern "C" int b2a_spec_gate_backward_f32(const float* grad_out, const float* spec, int64_t rows, int F, int64_t N,
+                                          const float* thresh, int64_t nz_rows, const float* amount, int rows_per_item,
+                                          const float* smooth_f_h, int n_f, const float* smooth_t_h, int n_t,
+                                          float* grad_spec, void* stream) {
+  B2A_REQUIRE(grad_out && spec && thresh && amount && smooth_f_h && smooth_t_h && grad_spec, B2A_E_INVALID,
+              "spec_gate_backward: null pointer");
+  GATE_REQUIRE_SHAPE("spec_gate_backward");
+  B2A_REQUIRE(grad_spec != spec, B2A_E_INVALID, "spec_gate_backward: grad_spec must not alias spec");
+  B2A_REQUIRE((((uintptr_t)grad_out | (uintptr_t)spec | (uintptr_t)grad_spec) & 7) == 0, B2A_E_INVALID,
+              "spec_gate_backward: alignment");
+  return gate_apply(reinterpret_cast<const float2*>(spec), reinterpret_cast<const float2*>(grad_out),
+                    reinterpret_cast<float2*>(grad_spec), rows, F, N, thresh, nz_rows, amount, rows_per_item,
+                    smooth_f_h, n_f, smooth_t_h, n_t, stream);
 }

@@ -34,7 +34,9 @@ class Engine:
     # ------------------------------------------------------------------ helpers
     DIFFERENTIABLE = ("AudioSignal.stft", "istft", "mel_spectrogram", "mfcc", "normalize", "volume_change",
                       "and magnitude / phase / log_magnitude through stft_data; resample, equalizer, convolve, apply_ir, "
-                      "ensure_max_of_audio, mix, quantization, mulaw_quantization (gradients to audio_data)")
+                      "ensure_max_of_audio, mix, quantization, mulaw_quantization (gradients to audio_data); "
+                      "mask_frequencies, mask_timesteps, mask_low_magnitudes, ml.layers.SpectralGate (gradients to "
+                      "stft_data / the gated signal)")
 
     @classmethod
     def _refuse_grad(cls, t: torch.Tensor, name: str, depth: int = 2):
@@ -311,20 +313,61 @@ class Engine:
         (ref:audiotools/core/dsp.py:217-306).  spec [B, C, F, N] complex64, contiguous; returns it."""
         spec = self._spec_ok(spec, "spec_band_mask")
         B, C, F, N = spec.shape
-        axis_vals = self._prep(axis_vals.to(spec.device), "axis_vals")
-        lo = self._prep(lo.to(spec.device).reshape(-1), "lo")
-        hi = self._prep(hi.to(spec.device).reshape(-1), "hi")
-        if lo.numel() == 1:
-            lo, hi = lo.expand(B).contiguous(), hi.expand(B).contiguous()
-        assert lo.numel() == B and hi.numel() == B and axis_vals.numel() == (F if axis == 0 else N)
-        v = torch.tensor(float(val), dtype=torch.float32)
-        fill = v * torch.exp(1j * v)  # the reference's own arithmetic for a filled cell (complex64)
+        axis_vals, lo, hi = self._band_args(spec, axis_vals, lo, hi, axis)
+        fill = self._band_fill(val)
         rc = self.lib.b2a_spec_band_mask_f32(_dptr(torch.view_as_real(spec)), B * C, F, N, _dptr(axis_vals), _dptr(lo),
                                              _dptr(hi), C, int(axis), float(fill.real), float(fill.imag),
                                              self._stream(spec))
         self.lib.check(rc)
         self.launches += 1
         return spec
+
+    def _band_args(self, spec, axis_vals, lo, hi, axis):
+        B, _, F, N = spec.shape
+        axis_vals = self._prep(axis_vals.to(spec.device), "axis_vals")
+        lo = self._prep(lo.to(spec.device).reshape(-1), "lo")
+        hi = self._prep(hi.to(spec.device).reshape(-1), "hi")
+        if lo.numel() == 1:
+            lo, hi = lo.expand(B).contiguous(), hi.expand(B).contiguous()
+        assert lo.numel() == B and hi.numel() == B and axis_vals.numel() == (F if axis == 0 else N)
+        return axis_vals, lo, hi
+
+    @staticmethod
+    def _band_fill(val):
+        v = torch.tensor(float(val), dtype=torch.float32)
+        return v * torch.exp(1j * v)  # the reference's own arithmetic for a filled cell (complex64)
+
+    def spec_band_mask_out(self, spec: torch.Tensor, axis_vals: torch.Tensor, lo: torch.Tensor, hi: torch.Tensor,
+                           axis: int, val: float = 0.0) -> torch.Tensor:
+        """``spec_band_mask`` into a new tensor (the forward of the gradient path: ``spec`` may be saved by autograd)."""
+        spec = self._spec_ok(spec, "spec_band_mask_out")
+        B, C, F, N = spec.shape
+        axis_vals, lo, hi = self._band_args(spec, axis_vals, lo, hi, axis)
+        fill = self._band_fill(val)
+        out = torch.empty_like(spec)
+        rc = self.lib.b2a_spec_band_mask_out_f32(_dptr(torch.view_as_real(spec)), _dptr(torch.view_as_real(out)), B * C,
+                                                 F, N, _dptr(axis_vals), _dptr(lo), _dptr(hi), C, int(axis),
+                                                 float(fill.real), float(fill.imag), self._stream(spec))
+        self.lib.check(rc)
+        self.launches += 1
+        return out
+
+    def spec_band_mask_backward(self, grad: torch.Tensor, spec: torch.Tensor, axis_vals: torch.Tensor,
+                                lo: torch.Tensor, hi: torch.Tensor, axis: int) -> torch.Tensor:
+        """dL/dspec of ``spec_band_mask``: 0 in the band and where spec == 0, ``grad`` elsewhere (the reference's
+        |X| exp(1j angle X) round trip, differentiated by torch)."""
+        spec = self._spec_ok(spec, "spec_band_mask_backward")
+        grad = self._spec_ok(grad, "spec_band_mask_backward")
+        B, C, F, N = spec.shape
+        assert grad.shape == spec.shape, (grad.shape, spec.shape)
+        axis_vals, lo, hi = self._band_args(spec, axis_vals, lo, hi, axis)
+        gs = torch.empty_like(spec)
+        rc = self.lib.b2a_spec_band_mask_backward_f32(_dptr(torch.view_as_real(grad)), _dptr(torch.view_as_real(spec)),
+                                                      B * C, F, N, _dptr(axis_vals), _dptr(lo), _dptr(hi), C, int(axis),
+                                                      _dptr(torch.view_as_real(gs)), self._stream(spec))
+        self.lib.check(rc)
+        self.launches += 1
+        return gs
 
     def _spec_ok(self, spec: torch.Tensor, what: str) -> torch.Tensor:
         if not torch.is_complex(spec):
@@ -359,16 +402,56 @@ class Engine:
         spec = self._spec_ok(spec, "spec_mask_low")
         B = spec.shape[0]
         cells = spec.numel() // B
-        db_cutoff = self._prep(db_cutoff.to(spec.device), "db_cutoff").reshape(-1)
-        if db_cutoff.numel() == 1:
-            db_cutoff = db_cutoff.expand(B).contiguous()
-        assert db_cutoff.numel() == B
+        db_cutoff = self._cutoff_arg(spec, db_cutoff)
         ws = torch.empty(1, dtype=torch.int32, device=spec.device)
         rc = self.lib.b2a_spec_mask_low_f32(_dptr(torch.view_as_real(spec)), B, cells, _dptr(db_cutoff), float(amin ** 2),
                                             float(top_db), float(val), _dptr(ws), self._stream(spec))
         self.lib.check(rc)
         self.launches += 2
         return spec
+
+    def _cutoff_arg(self, spec, db_cutoff):
+        B = spec.shape[0]
+        db_cutoff = self._prep(db_cutoff.to(spec.device), "db_cutoff").reshape(-1)
+        if db_cutoff.numel() == 1:
+            db_cutoff = db_cutoff.expand(B).contiguous()
+        assert db_cutoff.numel() == B
+        return db_cutoff
+
+    def spec_mask_low_out(self, spec: torch.Tensor, db_cutoff: torch.Tensor, val: float = 0.0, amin: float = 1e-5,
+                          top_db: float = 80.0):
+        """``spec_mask_low`` into a new tensor (the forward of the gradient path) -> (out, ws): ws holds the maximum
+        |X|^2 the top_db floor came from, for ``spec_mask_low_backward``."""
+        spec = self._spec_ok(spec, "spec_mask_low_out")
+        B = spec.shape[0]
+        db_cutoff = self._cutoff_arg(spec, db_cutoff)
+        out = torch.empty_like(spec)
+        ws = torch.empty(1, dtype=torch.int32, device=spec.device)
+        rc = self.lib.b2a_spec_mask_low_out_f32(_dptr(torch.view_as_real(spec)), _dptr(torch.view_as_real(out)), B,
+                                                spec.numel() // B, _dptr(db_cutoff), float(amin ** 2), float(top_db),
+                                                float(val), _dptr(ws), self._stream(spec))
+        self.lib.check(rc)
+        self.launches += 2
+        return out, ws
+
+    def spec_mask_low_backward(self, grad: torch.Tensor, spec: torch.Tensor, db_cutoff: torch.Tensor, val: float,
+                               ws: torch.Tensor, amin: float = 1e-5, top_db: float = 80.0) -> torch.Tensor:
+        """dL/dspec of ``mask_low_magnitudes`` with the mask recomputed from ``spec`` and the forward's ``ws``: unmasked
+        cells pass ``grad``; masked cells (magnitude := val, phase kept) follow the phase, val (g - Re(g conj u) u) / |X|;
+        0 where spec == 0."""
+        spec = self._spec_ok(spec, "spec_mask_low_backward")
+        grad = self._spec_ok(grad, "spec_mask_low_backward")
+        assert grad.shape == spec.shape, (grad.shape, spec.shape)
+        B = spec.shape[0]
+        db_cutoff = self._cutoff_arg(spec, db_cutoff)
+        gs = torch.empty_like(spec)
+        rc = self.lib.b2a_spec_mask_low_backward_f32(_dptr(torch.view_as_real(grad)), _dptr(torch.view_as_real(spec)),
+                                                     B, spec.numel() // B, _dptr(db_cutoff), float(amin ** 2),
+                                                     float(top_db), float(val), _dptr(ws),
+                                                     _dptr(torch.view_as_real(gs)), self._stream(spec))
+        self.lib.check(rc)
+        self.launches += 1
+        return gs
 
     def alter_drr(self, ir: torch.Tensor, sample_rate: int, drr: torch.Tensor) -> torch.Tensor:
         """``ImpulseResponseMixin.alter_drr`` (ref:audiotools/core/effects.py:540-647) for ir [B, C, T] and drr [B]:
@@ -388,11 +471,12 @@ class Engine:
         return out
 
     def spec_gate(self, spec: torch.Tensor, nz_spec: torch.Tensor, n_std: float, amount: torch.Tensor,
-                  smooth_f, smooth_t) -> torch.Tensor:
+                  smooth_f, smooth_t):
         """The spectral noise gate's mask algebra (ref:audiotools/ml/layers/spectral_gate.py:97-124) as two launches:
         per-bin threshold from the noise STFT's dB statistics, then boolean -> separable 2-D smoothing ->
         ``spec * (1 - amount * mask)`` in one pass.  spec [B, C, F, N], nz_spec [1 or B, 1 or C, F, Nz] complex64;
-        amount: scalar or [B]; smooth_f / smooth_t: the two 1-D factors of the smoothing kernel.  Returns a new tensor."""
+        amount: scalar or [B]; smooth_f / smooth_t: the two 1-D factors of the smoothing kernel.  Returns (a new
+        tensor, the thresholds [nz rows, F] that ``spec_gate_backward`` takes)."""
         spec = self._spec_ok(spec, "spec_gate")
         B, C, F, N = spec.shape
         nz_spec = self._spec_ok(nz_spec, "spec_gate")
@@ -400,13 +484,8 @@ class Engine:
             nz_spec = nz_spec.expand(B, C, -1, -1).contiguous()
         assert nz_spec.shape[2] == F, (nz_spec.shape, F)
         nz_rows = nz_spec.shape[0] * nz_spec.shape[1]
-        amount = torch.as_tensor(amount, dtype=torch.float32).reshape(-1).to(spec.device)
-        if amount.numel() == 1:
-            amount = amount.expand(B)
-        amount = self._prep(amount.contiguous(), "amount")
-        assert amount.numel() == B
-        sf = (ctypes.c_float * len(smooth_f))(*[float(v) for v in smooth_f])
-        st = (ctypes.c_float * len(smooth_t))(*[float(v) for v in smooth_t])
+        amount = self._gate_amount(spec, amount)
+        sf, st = self._gate_smoothing(smooth_f, smooth_t)
         out = torch.empty_like(spec)
         ws = torch.empty(nz_rows * F, dtype=torch.float32, device=spec.device)
         rc = self.lib.b2a_spec_gate_f32(_dptr(torch.view_as_real(spec)), B * C, F, N, _dptr(torch.view_as_real(nz_spec)),
@@ -414,7 +493,39 @@ class Engine:
                                         st, len(smooth_t), _dptr(torch.view_as_real(out)), _dptr(ws), self._stream(spec))
         self.lib.check(rc)
         self.launches += 2
-        return out
+        return out, ws.reshape(nz_rows, F)
+
+    def _gate_amount(self, spec, amount):
+        amount = torch.as_tensor(amount, dtype=torch.float32).reshape(-1).to(spec.device)
+        if amount.numel() == 1:
+            amount = amount.expand(spec.shape[0])
+        amount = self._prep(amount.contiguous(), "amount")
+        assert amount.numel() == spec.shape[0]
+        return amount
+
+    @staticmethod
+    def _gate_smoothing(smooth_f, smooth_t):
+        return ((ctypes.c_float * len(smooth_f))(*[float(v) for v in smooth_f]),
+                (ctypes.c_float * len(smooth_t))(*[float(v) for v in smooth_t]))
+
+    def spec_gate_backward(self, grad: torch.Tensor, spec: torch.Tensor, thresh: torch.Tensor, amount: torch.Tensor,
+                           smooth_f, smooth_t) -> torch.Tensor:
+        """dL/dspec of ``spec_gate``: ``grad * (1 - amount * mask)``, the smoothed mask recomputed from ``spec`` and the
+        forward's thresholds (the mask comes from a comparison: a constant of the gradient, as in the reference)."""
+        spec = self._spec_ok(spec, "spec_gate_backward")
+        grad = self._spec_ok(grad, "spec_gate_backward")
+        assert grad.shape == spec.shape, (grad.shape, spec.shape)
+        B, C, F, N = spec.shape
+        amount = self._gate_amount(spec, amount)
+        sf, st = self._gate_smoothing(smooth_f, smooth_t)
+        gs = torch.empty_like(spec)
+        rc = self.lib.b2a_spec_gate_backward_f32(_dptr(torch.view_as_real(grad)), _dptr(torch.view_as_real(spec)), B * C,
+                                                 F, N, _dptr(thresh), thresh.shape[0], _dptr(amount), C, sf,
+                                                 len(smooth_f), st, len(smooth_t), _dptr(torch.view_as_real(gs)),
+                                                 self._stream(spec))
+        self.lib.check(rc)
+        self.launches += 1
+        return gs
 
     # ------------------------------------------------------------------ loudness
     def lufs(self, x: torch.Tensor, sample_rate: float, filter_class: str = "K-weighting",

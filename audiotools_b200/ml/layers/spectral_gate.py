@@ -2,12 +2,15 @@
 reduction): a per-bin threshold from a noise excerpt's STFT statistics, a smoothed binary mask, applied to the
 signal's STFT.  Both STFTs and the inverse run on the engine (``csrc/spectral.cu``, ``csrc/istft.cu``), and so does the
 mask algebra in between (``csrc/specmask.cu``: threshold statistics, then boolean -> separable smoothing -> multiply in
-one pass); ``smoothing_filter`` is kept as a buffer for API compatibility."""
+one pass); ``smoothing_filter`` is kept as a buffer for API compatibility.  When the signal's STFT requires a gradient
+the gate runs through ``core.grad.SpecGate`` (gradient g * (1 - amount * mask)); the noise signal is a constant of it,
+as the reference's comparison makes it, and a ``denoise_amount`` that requires a gradient raises."""
 import torch
 from torch import nn
 
 from ...core import AudioSignal
 from ...core import STFTParams
+from ...core import grad as _grad
 from ...core import util
 
 
@@ -36,10 +39,15 @@ class SpectralGate(nn.Module):
 
         from ...engine import get_engine
 
+        _grad.refuse_param_grad("SpectralGate", "denoise_amount", denoise_amount)
         audio_signal.stft()
-        nz_signal.stft()
+        with torch.no_grad():
+            nz_signal.stft()
         amount = util.ensure_tensor(denoise_amount).reshape(-1)
-        audio_signal.stft_data = get_engine().spec_gate(audio_signal.stft_data, nz_signal.stft_data, float(n_std), amount,
-                                                        self._rf.tolist(), self._rt.tolist())
+        args = (nz_signal.stft_data, float(n_std), amount, self._rf.tolist(), self._rt.tolist())
+        if _grad.wants_grad(audio_signal.stft_data):
+            audio_signal.stft_data = _grad.SpecGate.apply(audio_signal.stft_data, *args)
+        else:
+            audio_signal.stft_data = get_engine().spec_gate(audio_signal.stft_data, *args)[0]
         audio_signal.istft()
         return audio_signal

@@ -3,7 +3,8 @@
 bench.py, which measures configs[1]).  One JSON line per config: device-resident throughput (CUDA events,
 >= 3 warm-ups, inputs larger than L2 or rotated), algorithmic bytes, and the CPU oracle on a bounded sample.
 
-    python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,largewin,grad,loss,gate,masked,effects_grad] [--no-cpu]
+    python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,largewin,grad,loss,gate,masked,effects_grad,
+                                      specaug_grad] [--no-cpu]
 
 Multi-GPU (BASELINE configs[3] = 512 items on 4 GPUs, configs[4] = 2048 items on 8 GPUs): one process per GPU,
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 4 --master-addr 127.0.0.1 --master-port 29511 \
@@ -565,6 +566,110 @@ def main():
                         "next to its forward, and torch autograd (fp32, same GPU) over the float64 restatements' code",
               **res, "gpu": torch.cuda.get_device_name(LOCAL), "power_limit": plim})
         del x, gx
+
+    if "specaug_grad" in only:  # backward kernels of the spectral masks and the gate at 64 x 2ch x 10 s@44.1k, 2048/512
+        import subprocess
+
+        from audiotools_b200.engine import get_engine
+        from audiotools_b200.ml.layers import SpectralGate
+
+        try:
+            plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(LOCAL)],
+                                  capture_output=True, text=True, timeout=30).stdout.strip()
+        except Exception:  # noqa: BLE001 (informational field)
+            plim = "unknown"
+        eng = get_engine()
+        B, C, T, sr = 64, 2, 441000, 44100
+        g = torch.Generator().manual_seed(0)
+        x = (0.1 * torch.randn(B, C, T, generator=g)).to(dev)
+        nz = (0.01 * torch.randn(1, 1, 22050, generator=g)).to(dev)
+        fmin = (torch.rand(B, generator=g) * 8000).to(dev)
+        fmax = fmin + 2000.0
+        tmin = (torch.rand(B, generator=g) * 9.0).to(dev)
+        tmax = tmin + 0.25
+        gy = torch.randn(B, C, T, generator=g).to(dev)
+        gate = SpectralGate().to(dev)
+        amount = torch.full((B,), 0.9, device=dev)
+        res = {}
+
+        def chain(v):
+            s = AudioSignal(v, sr)
+            s.stft(window_length=2048, hop_length=512)
+            s.mask_frequencies(fmin, fmax).mask_timesteps(tmin, tmax)
+            return s.istft(window_length=2048, hop_length=512).audio_data
+
+        def gated(v):
+            return gate(AudioSignal(v, sr), AudioSignal(nz, sr), amount).audio_data
+
+        w = torch.hann_window(2048, periodic=True, device=dev)
+        sw = w.sqrt()
+
+        def torch_chain(v):  # the reference's tensor ops (torch.stft / polar masks / torch.istft) under torch autograd
+            X = torch.stft(v.reshape(-1, T), 2048, 512, window=w, center=True, return_complex=True).reshape(B, C, 1025, -1)
+            for vals, lo, hi, shape in ((torch.linspace(0, sr / 2, 1025, device=dev), fmin, fmax, (1, 1, -1, 1)),
+                                        (torch.linspace(0, T / sr, X.shape[-1], device=dev), tmin, tmax, (1, 1, 1, -1))):
+                m = (lo.reshape(-1, 1, 1, 1) <= vals.reshape(shape)) & (vals.reshape(shape) < hi.reshape(-1, 1, 1, 1))
+                X = torch.abs(X).masked_fill(m, 0.0) * torch.exp(1j * torch.angle(X).masked_fill(m, 0.0))
+            return torch.istft(X.reshape(-1, 1025, X.shape[-1]), 2048, 512, window=w, center=True, length=T).reshape(B, C, T)
+
+        def torch_gate(v):  # ref:audiotools/ml/layers/spectral_gate.py:97-127's tensor ops under torch autograd
+            X = torch.stft(v.reshape(-1, T), 2048, 512, window=sw, center=True, return_complex=True).reshape(B, C, 1025, -1)
+            N = torch.stft(nz.reshape(1, -1), 2048, 512, window=sw, center=True, return_complex=True)
+            nz_db = 20 * N.abs().clamp(1e-4).log10()
+            th = nz_db.mean(-1, keepdim=True) + nz_db.std(-1, keepdim=True) * 3.0
+            m = ((20 * X.abs().clamp(1e-4).log10()) < th).float().reshape(B * C, 1, 1025, -1)
+            k = gate.smoothing_filter
+            m = torch.nn.functional.conv2d(m, k, padding=(k.shape[-2] // 2, k.shape[-1] // 2)).reshape(X.shape)
+            X = X * (1 - m * amount.reshape(-1, 1, 1, 1))
+            return torch.istft(X.reshape(-1, 1025, X.shape[-1]), 2048, 512, window=sw, center=True, length=T).reshape(B, C, T)
+
+        for name, fn, ref in (("mask_chain", chain, torch_chain), ("spectral_gate", gated, torch_gate)):
+            def fwd_bwd(f=fn):
+                xg = x.clone().requires_grad_()
+                (f(xg) * gy).sum().backward()
+
+            def fwd(f=fn):
+                with torch.no_grad():
+                    f(x)
+
+            def torch_fwd_bwd(f=ref):
+                xg = x.clone().requires_grad_()
+                (f(xg) * gy).sum().backward()
+
+            res[f"{name}_fwd_bwd_ms"] = timed(fwd_bwd, steps=5)
+            res[f"{name}_no_grad_fwd_ms"] = timed(fwd, steps=5)
+            res[f"{name}_torch_autograd_fp32_ms"] = timed(torch_fwd_bwd, warmup=1, steps=3)
+        # each backward entry point alone: one read of g and X and one write of gX per cell (24 bytes)
+        with torch.no_grad():
+            X = eng.spectral(x, 2048, 512, w, want_stft=True)["stft"]
+        G = torch.randn(X.shape, dtype=torch.complex64, generator=g).to(dev)
+        cells = X.numel()
+        bins_f = torch.linspace(0, sr / 2, 1025, device=dev)
+        bins_t = torch.linspace(0, T / sr, X.shape[-1], device=dev)
+        cut = torch.full((B,), -20.0, device=dev)
+        _, ws = eng.spec_mask_low_out(X, cut, 0.5)
+        _, thresh = eng.spec_gate(X, eng.spectral(nz, 2048, 512, sw, want_stft=True)["stft"], 3.0, amount,
+                                  gate._rf.tolist(), gate._rt.tolist())
+        kernels = {
+            "band_mask_freq": (lambda: eng.spec_band_mask_out(X, bins_f, fmin, fmax, 0),
+                               lambda: eng.spec_band_mask_backward(G, X, bins_f, fmin, fmax, 0)),
+            "band_mask_time": (lambda: eng.spec_band_mask_out(X, bins_t, tmin, tmax, 1),
+                               lambda: eng.spec_band_mask_backward(G, X, bins_t, tmin, tmax, 1)),
+            "mask_low_val05": (lambda: eng.spec_mask_low_out(X, cut, 0.5),
+                               lambda: eng.spec_mask_low_backward(G, X, cut, 0.5, ws)),
+            "gate_apply": (None, lambda: eng.spec_gate_backward(G, X, thresh, amount, gate._rf.tolist(),
+                                                                 gate._rt.tolist())),
+        }
+        for name, (f_out, f_bwd) in kernels.items():
+            if f_out is not None:
+                res[f"{name}_out_of_place_forward_ms"] = timed(f_out, steps=20)
+            res[f"{name}_backward_ms"] = ms_b = timed(f_bwd, steps=20)
+            res[f"{name}_backward_frac_of_hbm_peak"] = 24.0 * cells / (ms_b * 1e-3) / (peak * 1e9)
+        emit({"config": "specaug_grad 64x2ch 10s@44.1k 2048/512: forward+backward of stft->mask_frequencies->"
+                        "mask_timesteps->istft and of SpectralGate, their no-grad forwards, torch autograd (fp32, same "
+                        "GPU) over the reference's tensor ops, and each mask backward alone",
+              **res, "stft_cells": cells, "gpu": torch.cuda.get_device_name(LOCAL), "power_limit": plim})
+        del x, X, G
 
     if "specaug" in only:  # SURVEY 8f.1: SpectralTransform chain stft -> FrequencyMask -> TimeMask -> istft at cfg2's shape
         g = torch.Generator().manual_seed(0)

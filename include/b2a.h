@@ -230,6 +230,36 @@ int b2a_spec_gate_f32(const float* spec, int64_t rows, int F, int64_t N, const f
                       int64_t nz_N, float n_std, const float* amount, int rows_per_item, const float* smooth_f_h,
                       int n_f, const float* smooth_t_h, int n_t, float* out, void* ws, void* stream);
 
+/* ---- gradients of the spectral masks and the spectral gate (differentiable through torch in the reference) -------
+ * A complex gradient is G = dL/dRe + i dL/dIm (torch's convention).  The forwards of the gradient path write a new
+ * tensor (one read and one write per cell, `out` must not alias `spec`); the backwards recompute each mask decision
+ * from the forward's input `spec` with the forward's arithmetic.  No atomics in any backward.
+ *   b2a_spec_band_mask_out_f32       b2a_spec_band_mask_f32 into `out`: out = fill in the band, spec elsewhere.
+ *   b2a_spec_band_mask_backward_f32  grad_spec = 0 in the band and where spec == 0 (|X| and angle(X) both
+ *                                    backpropagate 0 there), grad_out elsewhere.  Same arguments as the forward.
+ *   b2a_spec_mask_low_out_f32        b2a_spec_mask_low_f32 into `out`; ws (4 bytes) then holds the maximum |X|^2 and is
+ *                                    passed unchanged to the backward.
+ *   b2a_spec_mask_low_backward_f32   unmasked cells: grad_out (0 where spec == 0); masked cells (magnitude := val, phase
+ *                                    kept): val (g - Re(g conj u) u) / |X| with u = X / |X|, 0 where spec == 0.
+ *   b2a_spec_gate_backward_f32       grad_spec = grad_out * (1 - amount[item] * smoothed), the mask recomputed from spec
+ *                                    and the thresholds `thresh` [nz_rows, F] that b2a_spec_gate_f32 left in its ws.
+ *                                    Arguments as b2a_spec_gate_f32; grad_spec must not alias spec. */
+int b2a_spec_band_mask_out_f32(const float* spec, float* out, int64_t rows, int F, int N, const float* axis_vals,
+                               const float* lo, const float* hi, int rows_per_item, int axis, float fill_re,
+                               float fill_im, void* stream);
+int b2a_spec_band_mask_backward_f32(const float* grad_out, const float* spec, int64_t rows, int F, int N,
+                                    const float* axis_vals, const float* lo, const float* hi, int rows_per_item,
+                                    int axis, float* grad_spec, void* stream);
+int b2a_spec_mask_low_out_f32(const float* spec, float* out, int64_t items, int64_t cells_per_item,
+                              const float* db_cutoff, float amin_sq, float top_db, float val, void* ws, void* stream);
+int b2a_spec_mask_low_backward_f32(const float* grad_out, const float* spec, int64_t items, int64_t cells_per_item,
+                                   const float* db_cutoff, float amin_sq, float top_db, float val, const void* ws,
+                                   float* grad_spec, void* stream);
+int b2a_spec_gate_backward_f32(const float* grad_out, const float* spec, int64_t rows, int F, int64_t N,
+                               const float* thresh, int64_t nz_rows, const float* amount, int rows_per_item,
+                               const float* smooth_f_h, int n_f, const float* smooth_t_h, int n_t, float* grad_spec,
+                               void* stream);
+
 /* ---- integrated loudness (ITU-R BS.1770 / LUFS) ----------------------------------------
  * Replaces Meter.integrated_loudness with the IIR semantics of apply_filter_cpu
  * (audiotools/core/loudness.py:102-126, 164-247) and the pad / clamp shell of
