@@ -7,6 +7,7 @@
 //   warp_fft_tables    its role-constant twiddle tables (shared memory, [slot][lane])
 //   load_frame         the windowed frame load in front of warp_fft (spectral.cu, loss.cu)
 //   partner_lane       the lane holding Z[N - k] (the real-FFT untangles of spectral.cu, loss.cu, istft.cu)
+//   untangle           the real-FFT bins of a lane after warp_fft (loss.cu, stoi.cu)
 #pragma once
 #include "b2a_common.h"
 
@@ -263,6 +264,30 @@ __device__ __forceinline__ float2 untangle_twiddle_m(const float2* ut, float2 u0
     case 14: return untangle_twiddle<LOG2N, 14>(ut, u0, l);
     default: return untangle_twiddle<LOG2N, 15>(ut, u0, l);
   }
+}
+
+// The lane's real-FFT bins after warp_fft of a frame whose window was halved (the untangle's 1/2 folded in there):
+// a[m] = X[k], b[m] = X[N - k] for k = l + LPF m (m < 16); h = X[N/2] (valid on l == 0).  src_lane = partner_lane.
+template <int LOG2N>
+__device__ __forceinline__ void untangle(const float2 (&z)[32], const float2* ut, int l, int src_lane, float2 (&a)[16],
+                                         float2 (&b)[16], float2& h) {
+  const float2 u0 = ut[l];
+#pragma unroll
+  for (int m = 0; m < 16; ++m) {
+    const float2 zk = z[m];
+    float2 zn;
+    zn.x = __shfl_sync(0xffffffffu, z[31 - m].x, src_lane);
+    zn.y = __shfl_sync(0xffffffffu, z[31 - m].y, src_lane);
+    if (l == 0) zn = z[(32 - m) & 31];
+    const float2 xe = add2(zk, make_float2(zn.x, -zn.y));
+    const float2 xo = add2(make_float2(zk.y, -zk.x), make_float2(zn.y, zn.x));
+    const float2 w = untangle_twiddle_m<LOG2N>(ut, u0, l, m);
+    const float2 xk = fma2(bcast2(w.x), xo, fma2(make_float2(-w.y, w.y), make_float2(xo.y, xo.x), xe));
+    const float2 d = fma2(bcast2(2.0f), xe, neg2(xk));
+    a[m] = xk;
+    b[m] = make_float2(d.x, -d.y);
+  }
+  h = make_float2(2.0f * z[16].x, -2.0f * z[16].y);
 }
 
 // ---- front end of a warp frame (spectral_warp_kernel and spectral_loss_kernel load it with the same instructions, so

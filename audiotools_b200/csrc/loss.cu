@@ -113,28 +113,7 @@ __device__ __forceinline__ void frame_fft(const float* fs, const float* win, int
   spectral::warp_fft<LOG2N, true>(z, xb, tw, l);
 }
 
-// the lane's real-FFT bins: a[m] = X[k], b[m] = X[N - k] for k = l + LPF m (m < 16); h = X[N/2] (valid on l == 0)
-template <int LOG2N>
-__device__ __forceinline__ void untangle(const float2 (&z)[32], const float2* ut, int l, int src_lane, float2 (&a)[16],
-                                         float2 (&b)[16], float2& h) {
-  const float2 u0 = ut[l];
-#pragma unroll
-  for (int m = 0; m < 16; ++m) {
-    const float2 zk = z[m];
-    float2 zn;
-    zn.x = __shfl_sync(0xffffffffu, z[31 - m].x, src_lane);
-    zn.y = __shfl_sync(0xffffffffu, z[31 - m].y, src_lane);
-    if (l == 0) zn = z[(32 - m) & 31];
-    const float2 xe = add2(zk, make_float2(zn.x, -zn.y));
-    const float2 xo = add2(make_float2(zk.y, -zk.x), make_float2(zn.y, zn.x));
-    const float2 w = spectral::untangle_twiddle_m<LOG2N>(ut, u0, l, m);
-    const float2 xk = fma2(bcast2(w.x), xo, fma2(make_float2(-w.y, w.y), make_float2(xo.y, xo.x), xe));
-    const float2 d = fma2(bcast2(2.0f), xe, neg2(xk));
-    a[m] = xk;
-    b[m] = make_float2(d.x, -d.y);
-  }
-  h = make_float2(2.0f * z[16].x, -2.0f * z[16].y);
-}
+using spectral::untangle;
 
 template <int LOG2N, bool MEL>
 __global__ void __launch_bounds__(256, 2) spectral_loss_kernel(LossParams q) {

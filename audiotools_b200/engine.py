@@ -1304,6 +1304,58 @@ class Engine:
             return out, ws[: rows * jmax * 4].view(torch.int32).reshape(rows, jmax).clone()
         return out
 
+    # ------------------------------------------------------------------ STOI (csrc/stoi.cu)
+    STOI_RATE = 10000
+
+    @staticmethod
+    def stoi_ratio(sample_rate: int):
+        """(up, down): 10000 / sample_rate reduced by the gcd, resample_poly's ratio."""
+        g = math.gcd(Engine.STOI_RATE, int(sample_rate))
+        return Engine.STOI_RATE // g, int(sample_rate) // g
+
+    @staticmethod
+    def stoi_taps(sample_rate: int) -> np.ndarray:
+        """float64 filter of ``resample_poly(x, up, down, window=h / h.sum())`` as pystoi's ``resample_oct`` designs it
+        (Octave's 60 dB Kaiser-windowed sinc, cutoff 1 / (2 max(up, down)), roll-off a tenth of it), times up.  [1] at
+        10 kHz, where pystoi does not resample."""
+        up, down = Engine.stoi_ratio(sample_rate)
+        if up == down == 1:
+            return np.ones(1)
+        fc = 1.0 / (2 * max(up, down))
+        L = np.ceil((60.0 - 8) / (28.714 * fc / 10))
+        t = np.arange(-L, L + 1)
+        h = np.kaiser(2 * L + 1, 0.1102 * (60.0 - 8.7)) * 2 * up * fc * np.sinc(2 * fc * t)
+        return h / h.sum() * up
+
+    def stoi(self, est: torch.Tensor, ref: torch.Tensor, sample_rate: int, extended: bool = False):
+        """STOI (or extended STOI) of the estimates against the clean references, both [B, C, T] (mixed to mono first)
+        -> (score [B] float64, kept [B] int32 frames kept by the silence removal, short [B] bool: fewer than 30 STFT
+        frames were left and the score is 1e-5).  Detached inputs, as the reference's wrapper."""
+        est = self._prep(est.detach(), "estimates")
+        ref = self._prep(ref.detach(), "references")
+        if est.shape != ref.shape or est.ndim != 3:
+            raise ValueError(f"stoi: estimates {tuple(est.shape)} and references {tuple(ref.shape)} must be the same "
+                             "[batch, channels, samples] shape")
+        B, C, T = est.shape
+        up, down = self.stoi_ratio(sample_rate)
+        n10 = -(-T * up // down)
+        if n10 <= 256:
+            raise ValueError(f"stoi: {T} samples at {sample_rate} Hz leave no full 256-sample frame at 10 kHz")
+        key = ("stoi_taps", int(sample_rate), est.device)
+        taps = self._packed_cache.get(key)
+        if taps is None:
+            taps = self._packed_cache[key] = torch.from_numpy(self.stoi_taps(sample_rate)).to(est.device)
+        nbytes = int(self.lib.b2a_stoi_workspace_bytes(B, T, up, down))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=est.device)
+        out = torch.empty(B, dtype=torch.float64, device=est.device)
+        kept = torch.empty(B, dtype=torch.int32, device=est.device)
+        short = torch.empty(B, dtype=torch.int32, device=est.device)
+        rc = self.lib.b2a_stoi_f32(_dptr(est), _dptr(ref), B, C, T, int(bool(extended)), _dptr(taps), taps.numel(), up,
+                                   down, _dptr(out), _dptr(kept), _dptr(short), _dptr(ws), nbytes, self._stream(est))
+        self.lib.check(rc)
+        self.launches += 4 if n10 > 256 + 128 else 3  # one frame at 10 kHz leaves no STFT frame: no band launch
+        return out, kept, short.bool()
+
 
 _ENGINE = None
 

@@ -4,7 +4,7 @@ bench.py, which measures configs[1]).  One JSON line per config: device-resident
 >= 3 warm-ups, inputs larger than L2 or rotated), algorithmic bytes, and the CPU oracle on a bounded sample.
 
     python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,largewin,grad,loss,gate,masked,effects_grad,
-                                      specaug_grad] [--no-cpu]
+                                      specaug_grad,stoi] [--no-cpu]
 
 Multi-GPU (BASELINE configs[3] = 512 items on 4 GPUs, configs[4] = 2048 items on 8 GPUs): one process per GPU,
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 4 --master-addr 127.0.0.1 --master-port 29511 \
@@ -670,6 +670,42 @@ def main():
                         "GPU) over the reference's tensor ops, and each mask backward alone",
               **res, "stft_cells": cells, "gpu": torch.cuda.get_device_name(LOCAL), "power_limit": plim})
         del x, X, G
+
+    if "stoi" in only:  # metrics.quality.stoi on 64 x 10 s validation batches against the per-item float64 CPU loop
+        import subprocess
+
+        from audiotools_b200 import metrics
+        from tests import stoi_oracle as so
+        from tests.golden.make_golden_quality import speech
+
+        try:
+            plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(LOCAL)],
+                                  capture_output=True, text=True, timeout=30).stdout.strip()
+        except Exception:  # noqa: BLE001 (informational field)
+            plim = "unknown"
+        B, n_cpu = 64, 0 if args.no_cpu else 4
+        for sr, C in ((16000, 1), (44100, 1), (44100, 2)):
+            T = 10 * sr
+            # 8 distinct speech-like clips tiled over the batch, the estimate at 5 dB SNR of white noise
+            clips = np.stack([np.stack([speech(sr, T, 8 * i + c) for c in range(C)]) for i in range(8)])
+            ref = torch.from_numpy(np.tile(clips, (B // 8, 1, 1)))
+            est = ref + 0.3 * ref.std() * torch.randn(ref.shape, generator=torch.Generator().manual_seed(sr + C))
+            e, r = AudioSignal(est, sr).to(dev), AudioSignal(ref, sr).to(dev)
+            res = {}
+            for mode, ext in (("std", False), ("ext", True)):
+                res[f"{mode}_ms"] = timed(lambda: metrics.quality.stoi(e, r, ext), warmup=2, steps=10)
+                if n_cpu:
+                    est_np, ref_np = est[:n_cpu].numpy(), ref[:n_cpu].numpy()
+                    want = so.batch_stoi(est_np, ref_np, sr, ext)[0]
+                    res[f"{mode}_max_abs_err_vs_float64"] = float(np.abs(metrics.quality.stoi(e, r, ext)[:n_cpu].numpy()
+                                                                         - want).max())
+                    res[f"{mode}_cpu_float64_per_item_loop_ms"] = cpu_time(
+                        lambda: so.batch_stoi(est_np, ref_np, sr, ext), reps=1) * 1e3 * B / n_cpu
+            emit({"config": f"stoi {B}x{C}ch 10s@{sr}: metrics.quality.stoi (standard / extended, incl. the device->host "
+                            "copy of the scores) vs the float64 restatement of pystoi looped over the items on the CPU "
+                            f"(timed on {n_cpu} items, scaled to {B})", **res,
+                  "gpu": torch.cuda.get_device_name(LOCAL), "power_limit": plim})
+            del e, r, est, ref
 
     if "specaug" in only:  # SURVEY 8f.1: SpectralTransform chain stft -> FrequencyMask -> TimeMask -> istft at cfg2's shape
         g = torch.Generator().manual_seed(0)

@@ -447,6 +447,23 @@ int b2a_spectral_uses_tensor_cores(int n_fft, int hop, int want_mel, int want_st
  * previous setting. */
 int b2a_spectral_tc_enable(int on);
 
+/* ---- STOI / extended STOI (csrc/stoi.cu; metrics.quality.stoi, audiotools/metrics/quality.py:11-57, which calls
+ * pystoi.stoi(references[i, 0], estimates[i, 0], sample_rate, extended) per item after to_mono).
+ *   est, ref   [batch, channels, T] float32; mixed to mono (mean over channels) inside the first launch
+ *   taps       [n_taps] float64, n_taps odd: scipy.signal.resample_poly's filter for up / down (the gcd-reduced
+ *              10000 / sample_rate), already multiplied by up -- pystoi's Octave Kaiser design, normalised to unit sum,
+ *              times up.  At 10 kHz: up = down = 1 and taps = {1}.
+ *   out        [batch] float64 scores; 1e-5 where fewer than 30 STFT frames survive the silence removal
+ *   kept_out   [batch] int32 frames kept by the silence removal (the STFT then has kept_out - 1 frames)
+ *   short_out  [batch] int32, 1 where the score is the 1e-5 of a short item
+ *   ws         b2a_stoi_workspace_bytes(batch, T, up, down) bytes
+ * B2A_E_INVALID when the signal has no full 256-sample frame at 10 kHz.  Four launches, no atomics: bit-identical
+ * reruns.  The extended mode leaves out pystoi's EPS-scale random noise (deterministic). */
+size_t b2a_stoi_workspace_bytes(int64_t batch, int64_t T, int up, int down);
+int b2a_stoi_f32(const float* est, const float* ref, int64_t batch, int channels, int64_t T, int extended,
+                 const double* taps, int n_taps, int up, int down, double* out, int32_t* kept_out, int32_t* short_out,
+                 void* ws, size_t ws_bytes, void* stream);
+
 /* ---- one-sided statistics exchange between the GPUs of a node (NVLink peer memory) --------------------
  * The path shards by batch item with no data-path collective; the one exchange is the per-item loudness vector for
  * whole-batch statistics (the reference has no multi-GPU code of its own: SURVEY.md 8e).  Every rank owns a small
