@@ -10,9 +10,9 @@
 //   consecutive segments (segment = 32 lanes x L2 = 64 samples = 2048 samples); a WARP owns a run and walks it segment
 //   by segment, with no CTA barrier and no inter-warp communication: samples -> warp-private, double-buffered
 //   shared-memory window (cp.async; the next segment lands underneath the arithmetic of the current one), zero-state
-//   end state of every lane chunk (a 66-tap linear map read from the window), affine shuffle scan over the 32 chunks
-//   (state' = A^64 state + e), true lane start states from the state carried in registers, float32 DF-I recursion
-//   (second read of the window), y^2 into "elementary interval" bins:
+//   end state of every lane chunk (a 66-tap linear map read from the window, split table), affine shuffle scan over
+//   the 32 chunks (state' = A^64 state + e), true lane start states from the state carried in registers, float32 DF-I
+//   recursion (second read of the window), y^2 into "elementary interval" bins:
 //   with K = q*stride + r, interval A_j = [j*stride, j*stride+r), B_j = [j*stride+r, (j+1)*stride),
 //   so that block i = sum_{j=i}^{i+q-1}(A_j + B_j) + A_{i+q} -- bit-exact block indexing for any
 //   rate (K is not always 4*stride, e.g. 11025 Hz).  Warp partials are added into float64 bins.
@@ -26,6 +26,16 @@
 //   float32 recursion itself carries (each step rounds at 6e-8 |y| and the feedback amplifies it by ~1/(1 - rho)),
 //   i.e. the results are those of the exact carry to float32 rounding; only a row whose level drops by more than
 //   2^40 across one warm-up can tell the two apart.
+//
+//   State basis.  The high-pass is a (near) double pole at rho ~ 1 - 2 pi 38 Hz / rate.  On the output history
+//   (y[n-1], y[n-2]) its powers A^n have entries up to ~1 / (e (1 - rho)) (74 at 48 kHz, 300 at 192 kHz) that cancel
+//   to an O(1) result, so float32-rounded tables put a systematic error into every lane start state, and bass-heavy
+//   rows came out ~10x less accurate than the sequential float32 cascade.  The scan, the carry and the start states
+//   therefore run on w = (y[n-1] - rho y[n-2], y[n-2]) per stage (rho rounded to float32, so y[n-1] = fma(rho, w1, w0)
+//   converts back with one rounding): there A^n is a Jordan block without cancellation.  The end-state map keeps a
+//   cancelling sum in any basis, so its table is split into float32 high and low halves, summed in two accumulators
+//   (a rounded table is a systematic error; the accumulators' roundings are not).  tests/probes/kweight_state_probe.py
+//   measures each stage.
 // Kernel 2  lufs_gate_kernel             (tiny: one CTA per item)
 //   z -> l -> absolute gate -> relative gate -> LUFS, with the reference's dtypes (float32 z,
 //   float64 logs) and its NaN / inf scrubbing; optionally max(.,-70) and normalize()'s gain.
@@ -46,8 +56,8 @@ constexpr int MAX_STAGES = 2;
 constexpr int TILE = 8192;
 
 template <int NS>
-struct Coef {  // float32-rounded, a0-normalised, stage gain folded into b
-  float b0[NS], b1[NS], b2[NS], a1[NS], a2[NS];
+struct Coef {  // from the float32-rounded, a0-normalised b (stage gain folded in): d0 = b0, d1 = b0 + b1, d2 = b0 + b1 + b2
+  float d0[NS], d1[NS], d2[NS], a1[NS], a2[NS];
 };
 
 __host__ __device__ inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
@@ -66,15 +76,19 @@ __host__ inline WsLayout ws_layout(int64_t rows, int64_t nbins, int64_t nblk) {
   return w;
 }
 
-// one step of the cascade (float32 DF-I, the arithmetic torchaudio.lfilter performs per stage)
+// one step of the cascade: DF-I with the feed-forward sum b0 in0 + b1 in1 + b2 in2 in difference form,
+// d0 (in0 - in1) + d1 (in1 - in2) + d2 in2.  For the high-pass (b = g (1, -2, 1): d1 = -d0, d2 = 0) the differences of
+// slowly varying samples are exact, so the sum carries a rounding of its own size, not of the samples' (the direct form
+// under FMA contraction rounds one product only and leaves u |x|, which the poles near 1 amplify by ~1 / (1 - rho)^2 on
+// DC and bass).  The FMAs are written out so that the simulator rounds as the GPU does.
 template <int NS, class F>
-__host__ __device__ __forceinline__ F cascade_step(const F (&b0)[NS], const F (&b1)[NS], const F (&b2)[NS],
+__host__ __device__ __forceinline__ F cascade_step(const F (&d0)[NS], const F (&d1)[NS], const F (&d2)[NS],
                                                     const F (&a1)[NS], const F (&a2)[NS], F in0, F in1, F in2,
                                                     F (&y1)[NS], F (&y2)[NS]) {
 #pragma unroll
   for (int s = 0; s < NS; ++s) {
-    F f = b0[s] * in0 + (b1[s] * in1 + b2[s] * in2);
-    F y0 = f - a2[s] * y2[s] - a1[s] * y1[s];
+    F f = fma(d0[s], in0 - in1, fma(d1[s], in1 - in2, d2[s] * in2));
+    F y0 = fma(-a1[s], y1[s], fma(-a2[s], y2[s], f));
     in0 = y0; in1 = y1[s]; in2 = y2[s];
     y2[s] = y1[s]; y1[s] = y0;
   }
@@ -98,20 +112,25 @@ static void matmul(const double* a, const double* b, double* c) {
 }
 
 template <int NS>
-struct Tables {
+struct Tables {  // on the state basis w = B (y1, y2): per stage (y1 - rho y2, y2)
   static constexpr int D = 2 * NS;
-  float Wa[L2 + 2][D];        // zero-state end state of a lane chunk as a linear map of its 66 inputs
+  float Wa[L2 + 2][D];        // zero-state end state of a lane chunk as a linear map of its 66 inputs: high half
+  float Wlo[L2 + 2][D];       // and low half (Wa + Wlo = the float64 map to ~2^-48)
   float Mlane[32][D * D];     // A^(L2 l)
   float Mscan[5][D * D];      // A^(L2 2^k)
   float Mseg[D * D];          // A^SEG
+  float rho[NS];              // y1 = rho y2 + w0
 };
+
+template <int NS>
+static double max_pole_radius(const Coef<NS>& cf, int s0 = 0, int s1 = NS);
 
 template <int NS>
 static void build_tables(const Coef<NS>& cf, Tables<NS>* tb) {
   constexpr int D = 2 * NS;
   double b0[NS], b1[NS], b2[NS], a1[NS], a2[NS];
   for (int s = 0; s < NS; ++s) {
-    b0[s] = cf.b0[s]; b1[s] = cf.b1[s]; b2[s] = cf.b2[s]; a1[s] = cf.a1[s]; a2[s] = cf.a2[s];
+    b0[s] = cf.d0[s]; b1[s] = cf.d1[s]; b2[s] = cf.d2[s]; a1[s] = cf.a1[s]; a2[s] = cf.a2[s];
   }
   double A[D * D];
   for (int k = 0; k < D; ++k) {
@@ -120,6 +139,16 @@ static void build_tables(const Coef<NS>& cf, Tables<NS>* tb) {
     cascade_step<NS, double>(b0, b1, b2, a1, a2, 0.0, 0.0, 0.0, y1, y2);
     for (int s = 0; s < NS; ++s) { A[(2 * s) * D + k] = y1[s]; A[(2 * s + 1) * D + k] = y2[s]; }
   }
+  // basis change w = Bm y and its inverse, per stage [[1, -rho], [0, 1]]
+  double Bm[D * D], Bi[D * D];
+  for (int i = 0; i < D * D; ++i) Bm[i] = Bi[i] = (i / D == i % D) ? 1.0 : 0.0;
+  for (int s = 0; s < NS; ++s) {
+    tb->rho[s] = (float)max_pole_radius<NS>(cf, s, s + 1);
+    Bm[(2 * s) * D + 2 * s + 1] = -(double)tb->rho[s];
+    Bi[(2 * s) * D + 2 * s + 1] = (double)tb->rho[s];
+  }
+  matmul<D>(Bm, A, A);
+  matmul<D>(A, Bi, A);  // A on the w basis
   double P[D * D];  // A^L2
   for (int i = 0; i < D * D; ++i) P[i] = A[i];
   for (int l = 1; l < L2; l <<= 1) matmul<D>(P, P, P);
@@ -143,15 +172,21 @@ static void build_tables(const Coef<NS>& cf, Tables<NS>* tb) {
       const double in0 = (i + 2 == j) ? 1.0 : 0.0, in1 = (i + 1 == j) ? 1.0 : 0.0, in2 = (i == j) ? 1.0 : 0.0;
       cascade_step<NS, double>(b0, b1, b2, a1, a2, in0, in1, in2, y1, y2);
     }
-    for (int s = 0; s < NS; ++s) { tb->Wa[j][2 * s] = (float)y1[s]; tb->Wa[j][2 * s + 1] = (float)y2[s]; }
+    for (int s = 0; s < NS; ++s) {
+      const double w[2] = {y1[s] - (double)tb->rho[s] * y2[s], y2[s]};
+      for (int c = 0; c < 2; ++c) {
+        tb->Wa[j][2 * s + c] = (float)w[c];
+        tb->Wlo[j][2 * s + c] = (float)(w[c] - (double)tb->Wa[j][2 * s + c]);
+      }
+    }
   }
 }
 
-// largest pole radius of the cascade (a1, a2 already normalised by a0)
+// largest pole radius of stages [s0, s1) of the cascade (a1, a2 already normalised by a0)
 template <int NS>
-static double max_pole_radius(const Coef<NS>& cf) {
+static double max_pole_radius(const Coef<NS>& cf, int s0, int s1) {
   double rho = 0.0;
-  for (int s = 0; s < NS; ++s) {
+  for (int s = s0; s < s1; ++s) {
     const double a1 = cf.a1[s], a2 = cf.a2[s], disc = a1 * a1 - 4.0 * a2;
     double r;
     if (disc < 0) r = sqrt(a2 > 0 ? a2 : 0.0);
@@ -209,12 +244,10 @@ kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp,
   constexpr int D = 2 * NS;
   B2A_DYN_SMEM(smem);
   float* wins = reinterpret_cast<float*>(smem);  // [WPB][NBUF][BUF]
-  __shared__ __align__(16) float s_wa[L2 + 2][D];
   __shared__ float s_mlane[32][D * D];
   __shared__ float s_mscan[5][D * D];
   __shared__ float s_mseg[D * D];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int i = tid; i < (L2 + 2) * D; i += blockDim.x) (&s_wa[0][0])[i] = (&tbv.Wa[0][0])[i];
   for (int i = tid; i < 32 * D * D; i += blockDim.x) (&s_mlane[0][0])[i] = (&tbv.Mlane[0][0])[i];
   for (int i = tid; i < 5 * D * D; i += blockDim.x) (&s_mscan[0][0])[i] = (&tbv.Mscan[0][0])[i];
   if (tid < D * D) s_mseg[tid] = tbv.Mseg[tid];
@@ -250,19 +283,30 @@ kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp,
         h0 = h.x; h1 = h.y;
       }
       const float4* c4 = reinterpret_cast<const float4*>(&win[CHS * lane]);
-      // ---- zero-state end state of the lane's chunk as a linear map of its 66 inputs
+      // ---- zero-state end state of the lane's chunk as a linear map of its 66 inputs (high and low table halves)
       float g[D];
+      {
+        float gl[D];
 #pragma unroll
-      for (int i = 0; i < D; ++i) g[i] = fmaf(tbv.Wa[0][i], h0, tbv.Wa[1][i] * h1);
-#pragma unroll
-      for (int i4 = 0; i4 < L2 / 4; ++i4) {
-        const float4 q = c4[i4];
-        const float qs[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-#pragma unroll
-          for (int i = 0; i < D; ++i) g[i] = fmaf(tbv.Wa[2 + 4 * i4 + e][i], qs[e], g[i]);  // constant-bank operand
+        for (int i = 0; i < D; ++i) {
+          g[i] = fmaf(tbv.Wa[0][i], h0, tbv.Wa[1][i] * h1);
+          gl[i] = fmaf(tbv.Wlo[0][i], h0, tbv.Wlo[1][i] * h1);
         }
+#pragma unroll
+        for (int i4 = 0; i4 < L2 / 4; ++i4) {
+          const float4 q = c4[i4];
+          const float qs[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+#pragma unroll
+            for (int i = 0; i < D; ++i) {  // constant-bank operands
+              g[i] = fmaf(tbv.Wa[2 + 4 * i4 + e][i], qs[e], g[i]);
+              gl[i] = fmaf(tbv.Wlo[2 + 4 * i4 + e][i], qs[e], gl[i]);
+            }
+          }
+        }
+#pragma unroll
+        for (int i = 0; i < D; ++i) g[i] += gl[i];
       }
 #pragma unroll
       for (int k = 0; k < 5; ++k) {  // inclusive affine scan over the 32 chunks
@@ -289,7 +333,7 @@ kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp,
 #pragma unroll
           for (int i = 0; i < D; ++i) st[i] = ex[i] + row_dot<D>(s_mlane[lane], i, carry);
 #pragma unroll
-          for (int s = 0; s < NS; ++s) { y1[s] = st[2 * s]; y2[s] = st[2 * s + 1]; }
+          for (int s = 0; s < NS; ++s) { y1[s] = fmaf(tbv.rho[s], st[2 * s + 1], st[2 * s]); y2[s] = st[2 * s + 1]; }
         }
         const int n0 = t0 + lane * L2;
         const int nv = min(L2, max(0, Tp - n0));
@@ -320,14 +364,16 @@ kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp,
             const float qs[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-              const float y = cascade_step<NS, float>(cf.b0, cf.b1, cf.b2, cf.a1, cf.a2, qs[e], xm1, xm2, y1, y2);
+              const float y = cascade_step<NS, float>(cf.d0, cf.d1, cf.d2, cf.a1, cf.a2, qs[e], xm1, xm2, y1, y2);
               xm2 = xm1; xm1 = qs[e];
               acc = fmaf(y, y, acc);
             }
           }
           a0 = acc;
         } else {
-          float acc = 0.f, p1 = 0.f, p2 = 0.f;  // running energy and its value at the two interval boundaries
+          // one sum per interval, restarted at each boundary (differences of a running sum would put the rounding
+          // of a loud interval into a quiet neighbour)
+          float acc = 0.f, p1 = 0.f, p2 = 0.f;
 #pragma unroll
           for (int i4 = 0; i4 < L2 / 4; ++i4) {
             const float4 q = c4[i4];
@@ -337,14 +383,15 @@ kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp,
               const int i = 4 * i4 + e;
               p1 = (i == s1) ? acc : p1;
               p2 = (i == s2) ? acc : p2;
-              const float y = cascade_step<NS, float>(cf.b0, cf.b1, cf.b2, cf.a1, cf.a2, qs[e], xm1, xm2, y1, y2);
+              acc = (i == s1 || i == s2) ? 0.f : acc;
+              const float y = cascade_step<NS, float>(cf.d0, cf.d1, cf.d2, cf.a1, cf.a2, qs[e], xm1, xm2, y1, y2);
               xm2 = xm1; xm1 = qs[e];
               acc = (i < nv) ? fmaf(y, y, acc) : acc;
             }
           }
-          if (s1 >= L2) p1 = acc;
-          if (s2 >= L2) p2 = acc;
-          a0 = p1; a1 = p2 - p1; a2 = acc - p2;
+          if (s1 >= L2) { p1 = acc; acc = 0.f; }
+          else if (s2 >= L2) { p2 = acc; acc = 0.f; }
+          a0 = p1; a1 = p2; a2 = acc;
         }
         // one atomic per interval the warp touched (intervals are monotonic in the lane index)
         const int blast = (s2 < L2) ? b2 : ((s1 < L2) ? b1 : b0);  // last interval this lane's chunk reaches
@@ -529,7 +576,10 @@ static int run(const float* x, int64_t B, int C, int64_t T, int64_t Tp, const Ge
     // the reference casts b and a to float32 (:118-119); lfilter then divides by a0 (== 1.0 for pyloudnorm)
     float a0 = (float)c[3];
     float sg = (float)stage_gain_h[s];
-    cf.b0[s] = (float)c[0] / a0 * sg; cf.b1[s] = (float)c[1] / a0 * sg; cf.b2[s] = (float)c[2] / a0 * sg;
+    const float b0 = (float)c[0] / a0 * sg, b1 = (float)c[1] / a0 * sg, b2 = (float)c[2] / a0 * sg;
+    cf.d0[s] = b0;
+    cf.d1[s] = (float)((double)b0 + b1);
+    cf.d2[s] = (float)((double)b0 + b1 + b2);
     cf.a1[s] = (float)c[4] / a0; cf.a2[s] = (float)c[5] / a0;
   }
   char* base = (char*)ws;
