@@ -5,7 +5,9 @@
 // approximation the reference falls back to on CUDA (:69-100) -- followed by the 400 ms / 75 %
 // block energies (:164-174, 214) and the two-pass gating (:208-247).
 //
-// Kernel 1  kweight_energy_warp_kernel   (HBM-bound: 4 B/sample, plus the warm-up reads)
+// Kernel 1  kweight_energy_warp_kernel   (reads 4 B/sample plus the warm-up, but NOT HBM-bound: at 12 warps per SM
+//   each warp walks a segment as a chain of latency-bound phases -- shuffle scan, recursion fused with the next
+//   segment's end-state map, warp sums; tests/probes/kweight_phase_probe.py times the phases)
 //   The cascade of NS biquads is a linear recurrence with a 2*NS-dim state.  A row is cut into RUNS of run_len
 //   consecutive segments (segment = 32 lanes x L2 = 64 samples = 2048 samples); a WARP owns a run and walks it segment
 //   by segment, with no CTA barrier and no inter-warp communication: samples -> warp-private, double-buffered
@@ -48,7 +50,7 @@ constexpr int L2 = 64;              // samples per lane
 constexpr int SEG = 32 * L2;        // samples per warp segment
 constexpr int CHS = L2 + 4;         // shared-memory words per lane chunk: 16 B aligned, conflict-free LDS.128
 constexpr int WPB = 12;             // warps per CTA (one CTA per SM: 12 x 17 KB of windows)
-constexpr int NBUF = 2;             // windows per warp: the next segment lands underneath the arithmetic
+constexpr int NBUF = 2;             // windows per warp: segment seg + 1 is mapped while seg runs its recursion
 constexpr int BUF = 32 * CHS;       // floats per window
 constexpr int MAX_STAGES = 2;
 // Unit of the input range b2a_lufs_f32 accepts: rows shorter than 2^31 - 2 TILE samples (every sample index the
@@ -219,6 +221,17 @@ __device__ __forceinline__ float row_dot(const float* M, int i, const float* v) 
   return a;
 }
 
+// one row of a shared-memory table, N a multiple of 4 floats, 16 B aligned: N / 4 LDS.128 (a broadcast when every lane
+// reads the same row)
+template <int N>
+__device__ __forceinline__ void lds_row(const float* p, float (&w)[N]) {
+#pragma unroll
+  for (int v = 0; v < N / 4; ++v) {
+    const float4 t = reinterpret_cast<const float4*>(p)[v];
+    w[4 * v] = t.x; w[4 * v + 1] = t.y; w[4 * v + 2] = t.z; w[4 * v + 3] = t.w;
+  }
+}
+
 // Stage segment `seg` of row `xr` into a warp window (cp.async when the 8 KB are inside the row and 16 B aligned).
 __device__ __forceinline__ void stage_segment(const float* __restrict__ xr, int seg, int T, float* win, int lane) {
   const int t0 = seg * SEG;
@@ -236,6 +249,119 @@ __device__ __forceinline__ void stage_segment(const float* __restrict__ xr, int 
   }
 }
 
+// Zero-state end state of each lane's chunk of the segment in `win` as a linear map of its 66 inputs: the two samples
+// in front of the chunk (lane 0: `hprev`, the previous segment's last two) and its 64 samples.  The table is split into
+// float32 high and low halves summed in two accumulators (s_map row j: high half, then low half).
+template <int D>
+__device__ __forceinline__ void end_state_map(const float* win, float2 hprev, int lane, const float (*s_map)[2 * D],
+                                              float (&g)[D]) {
+  const float2 h = lane ? *reinterpret_cast<const float2*>(&win[CHS * (lane - 1) + L2 - 2]) : hprev;
+  const float4* c4 = reinterpret_cast<const float4*>(&win[CHS * lane]);
+  float gl[D], w0[2 * D], w1[2 * D];
+  lds_row<2 * D>(s_map[0], w0);
+  lds_row<2 * D>(s_map[1], w1);
+#pragma unroll
+  for (int i = 0; i < D; ++i) {
+    g[i] = fmaf(w0[i], h.x, w1[i] * h.y);
+    gl[i] = fmaf(w0[D + i], h.x, w1[D + i] * h.y);
+  }
+#pragma unroll 4
+  for (int i4 = 0; i4 < L2 / 4; ++i4) {
+    const float4 q = c4[i4];
+    const float qs[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      float w[2 * D];
+      lds_row<2 * D>(s_map[2 + 4 * i4 + e], w);
+#pragma unroll
+      for (int i = 0; i < D; ++i) {
+        g[i] = fmaf(w[i], qs[e], g[i]);
+        gl[i] = fmaf(w[D + i], qs[e], gl[i]);
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < D; ++i) g[i] += gl[i];
+}
+
+// The recursion of one segment (window chunk c4, history h, start state y1 / y2) with its y^2 sums, fused step by
+// step with the end-state map of the next segment (window wn, history hn): two independent dependency chains in one
+// loop body, so that each one's latency is covered by the other's instructions.  Every floating-point operation and
+// its order are those of the two done one after the other.  EDGE: some lane of the warp crosses a gating-interval
+// boundary (at sample s1 or s2) or the row's end (nv samples valid): one sum per interval, restarted at each boundary
+// (differences of a running sum would put the rounding of a loud interval into a quiet neighbour).
+template <int NS, bool EDGE>
+__device__ __forceinline__ void recursion_and_map(const Coef<NS> cf, const float4* c4, float2 h, float (&y1)[NS],
+                                                  float (&y2)[NS], int s1, int s2, int nv, const float* wn, float2 hn,
+                                                  int lane, const float (*s_map)[4 * NS], float& a0, float& a1,
+                                                  float& a2, float (&g)[2 * NS]) {
+  constexpr int D = 2 * NS;
+  const float2 hl = lane ? *reinterpret_cast<const float2*>(&wn[CHS * (lane - 1) + L2 - 2]) : hn;
+  const float4* cn4 = reinterpret_cast<const float4*>(&wn[CHS * lane]);
+  float gl[D];
+  {
+    float w0[2 * D], w1[2 * D];
+    lds_row<2 * D>(s_map[0], w0);
+    lds_row<2 * D>(s_map[1], w1);
+#pragma unroll
+    for (int i = 0; i < D; ++i) {
+      g[i] = fmaf(w0[i], hl.x, w1[i] * hl.y);
+      gl[i] = fmaf(w0[D + i], hl.x, w1[D + i] * hl.y);
+    }
+  }
+  float xm2 = h.x, xm1 = h.y;
+  float acc = 0.f, p1 = 0.f, p2 = 0.f;
+#pragma unroll 4
+  for (int i4 = 0; i4 < L2 / 4; ++i4) {
+    const float4 q = c4[i4], qn = cn4[i4];
+    const float qs[4] = {q.x, q.y, q.z, q.w}, qns[4] = {qn.x, qn.y, qn.z, qn.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int i = 4 * i4 + e;
+      if (EDGE) {
+        p1 = (i == s1) ? acc : p1;
+        p2 = (i == s2) ? acc : p2;
+        acc = (i == s1 || i == s2) ? 0.f : acc;
+      }
+      const float y = cascade_step<NS, float>(cf.d0, cf.d1, cf.d2, cf.a1, cf.a2, qs[e], xm1, xm2, y1, y2);
+      xm2 = xm1; xm1 = qs[e];
+      acc = (!EDGE || i < nv) ? fmaf(y, y, acc) : acc;
+      float w[2 * D];
+      lds_row<2 * D>(s_map[2 + i], w);
+#pragma unroll
+      for (int k = 0; k < D; ++k) {
+        g[k] = fmaf(w[k], qns[e], g[k]);
+        gl[k] = fmaf(w[D + k], qns[e], gl[k]);
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < D; ++i) g[i] += gl[i];
+  if (EDGE) {
+    if (s1 >= L2) { p1 = acc; acc = 0.f; }
+    else if (s2 >= L2) { p2 = acc; acc = 0.f; }
+    a0 = p1; a1 = p2; a2 = acc;
+  } else {
+    a0 = acc;
+  }
+}
+
+// B2A_K2_PROBE (tests/probes/kweight_phase_probe.py only): lane 0 of every warp stamps clock64() at the K2_STAMPS phase
+// boundaries of the first K2_PROBE_SEGS energy segments of its run.  Without the macro the stamps compile to nothing.
+#ifdef B2A_K2_PROBE
+__device__ unsigned long long* g_k2_probe;  // [grid][WPB][K2_PROBE_SEGS][K2_STAMPS] clock64 stamps of lane 0
+int g_k2_last[3];                           // occupancy (CTAs per SM), grid, dynamic shared memory of the last launch
+#define K2_PROBE_SEGS 16
+#define K2_STAMPS 7
+#define K2_STAMP(k)                                                                                              \
+  do {                                                                                                           \
+    if (g_k2_probe && lane == 0 && seg >= seg0 && seg - seg0 < K2_PROBE_SEGS)                                    \
+      g_k2_probe[(((size_t)blockIdx.x * WPB + warp) * K2_PROBE_SEGS + (seg - seg0)) * K2_STAMPS + (k)] = clock64();     \
+  } while (0)
+#else
+#define K2_STAMP(k) do { } while (0)
+#endif
+
 template <int NS>
 __global__ void __launch_bounds__(32 * WPB, 1)
 kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp, int nseg, int run_len, int n_runs,
@@ -244,10 +370,19 @@ kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp,
   constexpr int D = 2 * NS;
   B2A_DYN_SMEM(smem);
   float* wins = reinterpret_cast<float*>(smem);  // [WPB][NBUF][BUF]
-  __shared__ float s_mlane[32][D * D];
-  __shared__ float s_mscan[5][D * D];
-  __shared__ float s_mseg[D * D];
+  // The tables every lane reads at the same address are copied to shared memory: a broadcast LDS.128 fetches four
+  // weights into ordinary registers, where the compiler can load them ahead of the FMAs.  Read from the parameter's
+  // constant bank they become ULDC.64 + uniform-register operands, one ULDC in front of every two FMAs, and the few
+  // uniform registers serialise each ULDC's latency (DESIGN.md, K2: the phase clock).
+  __shared__ __align__(16) float s_map[L2 + 2][2 * D];  // row j: Wa[j][0..D), Wlo[j][0..D)
+  __shared__ __align__(16) float s_mlane[32][D * D];
+  __shared__ __align__(16) float s_mscan[5][D * D];
+  __shared__ __align__(16) float s_mseg[D * D];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int i = tid; i < (L2 + 2) * 2 * D; i += blockDim.x) {
+    const int j = i / (2 * D), c = i - j * (2 * D);
+    s_map[j][c] = c < D ? tbv.Wa[j][c] : tbv.Wlo[j][c - D];
+  }
   for (int i = tid; i < 32 * D * D; i += blockDim.x) (&s_mlane[0][0])[i] = (&tbv.Mlane[0][0])[i];
   for (int i = tid; i < 5 * D * D; i += blockDim.x) (&s_mscan[0][0])[i] = (&tbv.Mscan[0][0])[i];
   if (tid < D * D) s_mseg[tid] = tbv.Mseg[tid];
@@ -266,57 +401,39 @@ kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp,
 #pragma unroll
     for (int j = 0; j < D; ++j) carry[j] = 0.f;
     stage_segment(xr, segw, T, win0, lane);
+    // the two samples in front of the segment (lane 0's history); later segments take them from the window before
+    // it is refilled
+    float2 hseg = make_float2(0.f, 0.f);
+    if (lane == 0) {
+      const int t0 = segw * SEG;
+      hseg.x = (t0 >= 2 && t0 - 2 < T) ? __ldg(xr + t0 - 2) : 0.f;
+      hseg.y = (t0 >= 1 && t0 - 1 < T) ? __ldg(xr + t0 - 1) : 0.f;
+    }
+    cp_async_wait_all();
+    __syncwarp();
+    if (segw + 1 < seg1) stage_segment(xr, segw + 1, T, win0 + BUF, lane);
+    float g[D];  // zero-state end state of the lane's chunk of the current segment
+    end_state_map<D>(win0, hseg, lane, s_map, g);
     int par = 0;
+    // Software pipeline: the end-state map of segment seg + 1 sits in the same basic block as the recursion of
+    // segment seg (both read their window; neither depends on the other), so the compiler interleaves two independent
+    // chains instead of running each one's latency alone.  Segment seg + 2 is staged once seg's window is released.
 #pragma unroll 1
-    for (int seg = segw; seg < seg1; ++seg, par ^= (NBUF - 1)) {
-      cp_async_wait_all();
-      __syncwarp();
+    for (int seg = segw; seg < seg1; ++seg, par ^= 1) {
+      K2_STAMP(0);
       const float* win = win0 + par * BUF;
-      if (NBUF == 2 && seg + 1 < seg1) stage_segment(xr, seg + 1, T, win0 + (par ^ 1) * BUF, lane);
+      const float* wnext = win0 + (par ^ 1) * BUF;  // segment seg + 1 (stale after the run's last segment: unused)
       const int t0 = seg * SEG;
-      float h0, h1;  // the two samples in front of this lane's chunk
-      if (lane == 0) {
-        h0 = (t0 >= 2 && t0 - 2 < T) ? __ldg(xr + t0 - 2) : 0.f;
-        h1 = (t0 >= 1 && t0 - 1 < T) ? __ldg(xr + t0 - 1) : 0.f;
-      } else {
-        const float2 h = *reinterpret_cast<const float2*>(&win[CHS * (lane - 1) + L2 - 2]);
-        h0 = h.x; h1 = h.y;
-      }
-      const float4* c4 = reinterpret_cast<const float4*>(&win[CHS * lane]);
-      // ---- zero-state end state of the lane's chunk as a linear map of its 66 inputs (high and low table halves)
-      float g[D];
-      {
-        float gl[D];
-#pragma unroll
-        for (int i = 0; i < D; ++i) {
-          g[i] = fmaf(tbv.Wa[0][i], h0, tbv.Wa[1][i] * h1);
-          gl[i] = fmaf(tbv.Wlo[0][i], h0, tbv.Wlo[1][i] * h1);
-        }
-#pragma unroll
-        for (int i4 = 0; i4 < L2 / 4; ++i4) {
-          const float4 q = c4[i4];
-          const float qs[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-#pragma unroll
-            for (int i = 0; i < D; ++i) {  // constant-bank operands
-              g[i] = fmaf(tbv.Wa[2 + 4 * i4 + e][i], qs[e], g[i]);
-              gl[i] = fmaf(tbv.Wlo[2 + 4 * i4 + e][i], qs[e], gl[i]);
-            }
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < D; ++i) g[i] += gl[i];
-      }
 #pragma unroll
       for (int k = 0; k < 5; ++k) {  // inclusive affine scan over the 32 chunks
         float o[D];
 #pragma unroll
         for (int j = 0; j < D; ++j) o[j] = __shfl_up_sync(0xffffffffu, g[j], 1u << k);
-        if (lane >= (1 << k)) {
+        float t[D];  // every lane computes the step and keeps it where it applies: no divergent branch
 #pragma unroll
-          for (int i = 0; i < D; ++i) g[i] += row_dot<D>(tbv.Mscan[k], i, o);  // (k is unrolled: constant-bank operands)
-        }
+        for (int i = 0; i < D; ++i) t[i] = g[i] + row_dot<D>(s_mscan[k], i, o);
+#pragma unroll
+        for (int i = 0; i < D; ++i) g[i] = lane >= (1 << k) ? t[i] : g[i];
       }
       float ex[D], agg[D];
 #pragma unroll
@@ -325,92 +442,81 @@ kweight_energy_warp_kernel(const float* __restrict__ x, int rows, int T, int Tp,
         if (lane == 0) ex[j] = 0.f;
         agg[j] = __shfl_sync(0xffffffffu, g[j], 31);
       }
-      if (seg >= seg0) {
-        // ---- true start state, recursion, energies into the interval bins
-        float y1[NS], y2[NS];
-        {
-          float st[D];
+      K2_STAMP(1);
+      // ---- true start state and the lane's interval boundaries (energy segments only)
+      const bool energy = seg >= seg0;
+      float y1[NS], y2[NS];
+      {
+        float st[D];
 #pragma unroll
-          for (int i = 0; i < D; ++i) st[i] = ex[i] + row_dot<D>(s_mlane[lane], i, carry);
+        for (int i = 0; i < D; ++i) st[i] = ex[i] + row_dot<D>(s_mlane[lane], i, carry);
 #pragma unroll
-          for (int s = 0; s < NS; ++s) { y1[s] = fmaf(tbv.rho[s], st[2 * s + 1], st[2 * s]); y2[s] = st[2 * s + 1]; }
+        for (int s = 0; s < NS; ++s) { y1[s] = fmaf(tbv.rho[s], st[2 * s + 1], st[2 * s]); y2[s] = st[2 * s + 1]; }
+      }
+      const int n0 = t0 + lane * L2;
+      const int nv = min(L2, max(0, Tp - n0));
+      int j0 = n0 / stride, rem0 = n0 - j0 * stride;
+      int b0 = 2 * j0 + (rem0 >= r ? 1 : 0);
+      int end0 = (b0 & 1) ? (j0 + 1) * stride : j0 * stride + r;
+      const int s1 = min(end0 - n0, L2);
+      int s2 = L2, b1 = b0, b2 = b0;
+      if (s1 < L2) {
+        const int n1 = n0 + s1, j1 = n1 / stride, rem1 = n1 - j1 * stride;
+        b1 = 2 * j1 + (rem1 >= r ? 1 : 0);
+        const int end1 = (b1 & 1) ? (j1 + 1) * stride : j1 * stride + r;
+        s2 = min(end1 - n0, L2);
+        if (s2 < L2) {
+          const int n2 = n0 + s2, j2 = n2 / stride, rem2 = n2 - j2 * stride;
+          b2 = 2 * j2 + (rem2 >= r ? 1 : 0);
         }
-        const int n0 = t0 + lane * L2;
-        const int nv = min(L2, max(0, Tp - n0));
-        int j0 = n0 / stride, rem0 = n0 - j0 * stride;
-        int b0 = 2 * j0 + (rem0 >= r ? 1 : 0);
-        int end0 = (b0 & 1) ? (j0 + 1) * stride : j0 * stride + r;
-        const int s1 = min(end0 - n0, L2);
-        int s2 = L2, b1 = b0, b2 = b0;
-        if (s1 < L2) {
-          const int n1 = n0 + s1, j1 = n1 / stride, rem1 = n1 - j1 * stride;
-          b1 = 2 * j1 + (rem1 >= r ? 1 : 0);
-          const int end1 = (b1 & 1) ? (j1 + 1) * stride : j1 * stride + r;
-          s2 = min(end1 - n0, L2);
-          if (s2 < L2) {
-            const int n2 = n0 + s2, j2 = n2 / stride, rem2 = n2 - j2 * stride;
-            b2 = 2 * j2 + (rem2 >= r ? 1 : 0);
-          }
-        }
-        const bool simple = (s1 >= L2) && (nv == L2);
-        const bool clean = __all_sync(0xffffffffu, simple);  // warp-uniform: no lane straddles an interval boundary
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-        float xm2 = h0, xm1 = h1;
-        if (clean) {
-          float acc = 0.f;
+      }
+      const bool simple = (s1 >= L2) && (nv == L2);
+      const bool clean = __all_sync(0xffffffffu, simple);  // warp-uniform: no lane straddles an interval boundary
+      // ---- carry into the next segment: A^SEG carry + (zero-state end state of this segment)
+      {
+        float cn[D];
 #pragma unroll
-          for (int i4 = 0; i4 < L2 / 4; ++i4) {
-            const float4 q = c4[i4];
-            const float qs[4] = {q.x, q.y, q.z, q.w};
+        for (int i = 0; i < D; ++i) cn[i] = agg[i] + row_dot<D>(s_mseg, i, carry);
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float y = cascade_step<NS, float>(cf.d0, cf.d1, cf.d2, cf.a1, cf.a2, qs[e], xm1, xm2, y1, y2);
-              xm2 = xm1; xm1 = qs[e];
-              acc = fmaf(y, y, acc);
-            }
-          }
-          a0 = acc;
-        } else {
-          // one sum per interval, restarted at each boundary (differences of a running sum would put the rounding
-          // of a loud interval into a quiet neighbour)
-          float acc = 0.f, p1 = 0.f, p2 = 0.f;
-#pragma unroll
-          for (int i4 = 0; i4 < L2 / 4; ++i4) {
-            const float4 q = c4[i4];
-            const float qs[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int i = 4 * i4 + e;
-              p1 = (i == s1) ? acc : p1;
-              p2 = (i == s2) ? acc : p2;
-              acc = (i == s1 || i == s2) ? 0.f : acc;
-              const float y = cascade_step<NS, float>(cf.d0, cf.d1, cf.d2, cf.a1, cf.a2, qs[e], xm1, xm2, y1, y2);
-              xm2 = xm1; xm1 = qs[e];
-              acc = (i < nv) ? fmaf(y, y, acc) : acc;
-            }
-          }
-          if (s1 >= L2) { p1 = acc; acc = 0.f; }
-          else if (s2 >= L2) { p2 = acc; acc = 0.f; }
-          a0 = p1; a1 = p2; a2 = acc;
-        }
+        for (int i = 0; i < D; ++i) carry[i] = cn[i];
+      }
+      K2_STAMP(2);
+      cp_async_wait_all();  // segment seg + 1
+      __syncwarp();
+      K2_STAMP(3);
+      const float2 h = lane ? *reinterpret_cast<const float2*>(&win[CHS * (lane - 1) + L2 - 2]) : hseg;
+      const float2 hnext = *reinterpret_cast<const float2*>(&win[CHS * 31 + L2 - 2]);  // the next segment's history
+      const float4* c4 = reinterpret_cast<const float4*>(&win[CHS * lane]);
+      float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+      float gn[D];
+      if (energy && clean)
+        recursion_and_map<NS, false>(cf, c4, h, y1, y2, s1, s2, nv, wnext, hnext, lane, s_map, a0, a1, a2, gn);
+      else if (energy)
+        recursion_and_map<NS, true>(cf, c4, h, y1, y2, s1, s2, nv, wnext, hnext, lane, s_map, a0, a1, a2, gn);
+      else
+        end_state_map<D>(wnext, hnext, lane, s_map, gn);  // warm-up: carry only
+      K2_STAMP(4);
+      if (energy) {
         // one atomic per interval the warp touched (intervals are monotonic in the lane index)
         const int blast = (s2 < L2) ? b2 : ((s1 < L2) ? b1 : b0);  // last interval this lane's chunk reaches
         const int bf = __shfl_sync(0xffffffffu, b0, 0), bl = __shfl_sync(0xffffffffu, blast, 31);
         for (int id = bf; id <= bl; ++id) {
+          // an interval no lane reaches (an empty one: r == 0 at 44.1 kHz) would add +0.0, which leaves a bin as it is
+          const bool has = (b0 == id) || (!clean && ((s1 < L2 && b1 == id) || (s2 < L2 && b2 == id)));
+          if (!__any_sync(0xffffffffu, has)) continue;
           float v = (b0 == id) ? a0 : 0.f;
           if (!clean) v += ((s1 < L2 && b1 == id) ? a1 : 0.f) + ((s2 < L2 && b2 == id) ? a2 : 0.f);
           v = warp_sum(v);
           if (lane == 0 && id < nbins) atomicAdd(rb + id, (double)v);
         }
       }
-      // ---- carry into the next segment: A^SEG carry + (zero-state end state of this segment)
-      float cn[D];
+      K2_STAMP(5);
 #pragma unroll
-      for (int i = 0; i < D; ++i) cn[i] = agg[i] + row_dot<D>(tbv.Mseg, i, carry);
-#pragma unroll
-      for (int i = 0; i < D; ++i) carry[i] = cn[i];
+      for (int i = 0; i < D; ++i) g[i] = gn[i];
+      hseg = hnext;
       __syncwarp();  // every lane is done with this window before it is refilled
-      if (NBUF == 1 && seg + 1 < seg1) stage_segment(xr, seg + 1, T, win0, lane);
+      if (seg + 2 < seg1) stage_segment(xr, seg + 2, T, win0 + par * BUF, lane);
+      K2_STAMP(6);
     }
   }
   cp_async_wait_all();
@@ -614,6 +720,12 @@ static int run(const float* x, int64_t B, int C, int64_t T, int64_t Tp, const Ge
   B2A_CUDA_OK(cudaFuncSetAttribute(kweight_energy_warp_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   B2A_LAUNCH(kweight_energy_warp_kernel<NS>, dim3(grid), dim3(32 * WPB), smem, stream, x, (int)rows, (int)T, (int)Tp,
              g.nseg, run_len, n_runs, n_warm, cf, tb, (double*)(base + w.bins), g.stride, g.r, g.nbins);
+#ifdef B2A_K2_PROBE
+  B2A_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&g_k2_last[0], kweight_energy_warp_kernel<NS>, 32 * WPB,
+                                                            smem));
+  g_k2_last[1] = (int)grid;
+  g_k2_last[2] = (int)smem;
+#endif
   GateParams gp;
   for (int c = 0; c < 8; ++c) gp.G[c] = c < C ? chan_gain_h[c] : 0.0;
   gp.scale = (float)(1.0 / (block_s * rate));
@@ -666,6 +778,22 @@ extern "C" int b2a_lufs_f32(const float* x, int64_t B, int C, int64_t T, int64_t
   return run<2>(x, B, C, T, T_padded, g, sos_h, stage_gain_h, rate, block_s, chan_gain_h, z_blocks, lufs_out,
                 loud_out, target_db, n_target, gain_out, ws, ws_bytes, stream);
 }
+
+#ifdef B2A_K2_PROBE
+// Phase-clock probe of kweight_energy_warp_kernel (tests/probes/kweight_phase_probe.py): not part of include/b2a.h and
+// compiled only with -DB2A_K2_PROBE.  `buf` (device, or null to stop recording): [grid][WPB][K2_PROBE_SEGS][K2_STAMPS] u64.
+extern "C" int b2a_k2_probe_set(void* buf) {
+  B2A_CUDA_OK(cudaMemcpyToSymbol(b2a::lufs::g_k2_probe, &buf, sizeof(buf)));
+  return B2A_OK;
+}
+extern "C" int b2a_k2_probe_segs() { return K2_PROBE_SEGS; }
+extern "C" int b2a_k2_probe_wpb() { return WPB; }
+extern "C" int b2a_k2_probe_stamps() { return K2_STAMPS; }
+// (occupancy in CTAs per SM, grid, dynamic shared memory bytes) of the last K-weighting launch
+extern "C" void b2a_k2_probe_last(int* out) {
+  for (int i = 0; i < 3; ++i) out[i] = b2a::lufs::g_k2_last[i];
+}
+#endif
 
 extern "C" int b2a_gain_f32(const float* x, float* out, int64_t B, int64_t per_item, const float* gain,
                             void* stream) {
