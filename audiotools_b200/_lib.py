@@ -51,7 +51,6 @@ SIGNATURES = {
     "b2a_mix_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p]),
     "b2a_quantize_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int, c_void_p]),
     "b2a_order_stats_f32": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p]),
-    "b2a_spectral_uses_tensor_cores": (c_int, [c_int, c_int, c_int, c_int]),
     "b2a_spectral_tc_enable": (c_int, [c_int]),
     "b2a_peer_buffer_bytes": (c_size_t, [c_int, c_int]),
     "b2a_peer_buffer_create": (c_int, [c_int, c_int, c_void_p, c_void_p]),

@@ -801,7 +801,6 @@ extern "C" int b2a_spectral_f32(const float* x, int64_t rows, int64_t T, int n_f
   p.mel_packed_len = (mel_out && mel_packed_len > 0) ? mel_packed_len : 0;
   p.center = 1; p.origin = -(n_fft / 2) - pad; p.row_origin = nullptr;
   p.rows_per_gain = gain ? rows_per_gain : 1; p.post = post; p.post_eps = post_eps; p.post_power = post_power;
-  if (tc_supported(p)) return launch_tc(p, stream);  // tensor-core path (spectral_tc.cu): n_fft 2048 log-mel / mel
   switch (n_fft) {
     case 32: return launch<4>(p, stream);
     case 64: return launch_warp<5>(p, stream);
@@ -813,6 +812,12 @@ extern "C" int b2a_spectral_f32(const float* x, int64_t rows, int64_t T, int n_f
     case 4096: return launch<11>(p, stream);  // 64 lanes per frame: CTA-cooperative kernel
   }
   return b2a::fail(B2A_E_UNSUPPORTED, "spectral: n_fft %d", n_fft);
+}
+
+extern "C" int b2a_spectral_tc_enable(int on) {
+  if (on == 0) return 0;
+  return b2a::fail(B2A_E_UNSUPPORTED,
+                   "spectral_tc_enable: the tensor-core spectral kernel was removed; the FP32 kernel runs every launch");
 }
 
 #ifdef B2A_K1_PROBE

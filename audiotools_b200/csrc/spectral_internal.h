@@ -94,11 +94,6 @@ __device__ __forceinline__ float mel_band(const float* fb, const int32_t* mel_lo
 int check_framing(const char* who, int64_t T, int n_fft, int hop, int pad, int right_pad, int pad_mode, int drop_edge,
                   int64_t* n_frames);
 
-// Tensor-core (wgmma) variant of the fused kernel for n_fft = 2048 mel / log-mel launches (spectral_tc.cu).
-// tc_supported: the launch can take that path (geometry, shared memory, switched on by b2a_spectral_tc_enable).
-bool tc_supported(const Params& p);
-int launch_tc(Params& p, void* stream);
-
 // Forward real FFT of raw (un-centred) blocks: block n of row r covers x-coordinates
 // [n*hop + origin + row_origin[r], +n_fft), out of range samples resolved by pad_mode
 // (B2A_PAD_CONSTANT zero / B2A_PAD_REPLICATE / 3 = circular).  out: [rows, n_fft/2+1, n_frames] (re,im).

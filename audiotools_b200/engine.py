@@ -750,8 +750,6 @@ class Engine:
         if route in (_lib.ROUTE_LARGE, _lib.ROUTE_DENSE):
             name = f"stft_large_kernel<{int(math.log2(n_fft))}>" if route == _lib.ROUTE_LARGE else "dft_forward_kernel"
             return name + " + mel_from_stft_kernel" if want_mel else name
-        if self.lib.b2a_spectral_uses_tensor_cores(int(n_fft), int(hop), int(want_mel), int(want_stft)):
-            return "spectral_tc_kernel"
         if n_fft in (32, 4096):
             return f"spectral_kernel<{int(math.log2(n_fft)) - 1}>"
         mode = 2 if (want_stft and want_mel) else (1 if want_stft else 0)

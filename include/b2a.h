@@ -438,13 +438,9 @@ int b2a_alter_drr_f32(const float* ir, float* out, int64_t rows, int64_t T, int 
 int b2a_pack_rows_f32(const float* const* src_ptrs, const int64_t* src_len, const int64_t* src_stride,
                       const int64_t* src_off, int64_t n_items, int C, int64_t T_out, float* out, void* stream);
 
-/* 1 when b2a_spectral_f32 runs a launch of this geometry on the tensor-core kernel (csrc/spectral_tc.cu: wgmma,
- * accumulators in registers): window_length 2048, hop <= 512, mel / log-mel output without the complex STFT, and
- * the path switched on with b2a_spectral_tc_enable(1).  It is opt-in: the FP32 warp kernel of
- * spectral.cu is the default; every other launch uses the FP32 kernels. */
-int b2a_spectral_uses_tensor_cores(int n_fft, int hop, int want_mel, int want_stft);
-/* Switch the tensor-core path on / off for this process (A/B measurements, parity tests of both kernels); returns the
- * previous setting. */
+/* Stub left from the removed tensor-core spectral kernel, which was slower and less accurate than the FP32 kernel.
+ * bench.py --tc still calls it.  Returns 0 for on == 0 and B2A_E_UNSUPPORTED for any other value; b2a_spectral_f32
+ * runs the FP32 kernels either way. */
 int b2a_spectral_tc_enable(int on);
 
 /* ---- STOI / extended STOI (csrc/stoi.cu; metrics.quality.stoi, audiotools/metrics/quality.py:11-57, which calls

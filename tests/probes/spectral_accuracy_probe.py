@@ -102,26 +102,20 @@ def main():
 
     # mel, one-bin and empty bands
     for n, nm, sr in [(2048, 320, 44100), (32, 5, 44100), (8192, 128, 44100), (400, 40, 44100), (512, 160, 44100)]:
-        for tc in ([False, True] if (n == 2048 and not SIM) else [False]):
-            hop = n // 4
-            T = 30 * hop + n
-            xn = torch.randn(2, 1, T, generator=g)
-            w = AudioSignal.get_window("hann", n, "cpu")
-            fb, lo, hi = AudioSignal._mel_tables(sr, n, nm, 0.0, None, dev)
-            prev = eng.lib.b2a_spectral_tc_enable(1 if tc else 0)
-            try:
-                m = eng.spectral(xn.to(dev), n, hop, w.to(dev), mel_fb=fb, mel_lo=lo, mel_hi=hi, want_stft=False)["mel"]
-            finally:
-                eng.lib.b2a_spectral_tc_enable(prev)
-            ref = gc.stft64(xn.double().to(dev), n, hop).cpu()
-            rt = s64.route(n, tc)
-            bound0, mel = s64.mel_bound(fb, ref, s64.budget(n, rt), 0.0)
-            err = (m.cpu().double() - mel).abs()
-            need = ((err - bound0).clamp_min(0) / mel.clamp_min(1e-300)).max().item()
-            widths = (hi - lo).cpu()
-            emit(kind="mel", n_fft=n, n_mels=nm, tc=tc, empty_bands=int((widths <= 0).sum()),
-                 one_bin_bands=int((widths == 1).sum()), max_err_over_fbdelta=(err / bound0.clamp_min(1e-300)).max().item(),
-                 rtol_needed_u=need / s64.U)
+        hop = n // 4
+        T = 30 * hop + n
+        xn = torch.randn(2, 1, T, generator=g)
+        w = AudioSignal.get_window("hann", n, "cpu")
+        fb, lo, hi = AudioSignal._mel_tables(sr, n, nm, 0.0, None, dev)
+        m = eng.spectral(xn.to(dev), n, hop, w.to(dev), mel_fb=fb, mel_lo=lo, mel_hi=hi, want_stft=False)["mel"]
+        ref = gc.stft64(xn.double().to(dev), n, hop).cpu()
+        bound0, mel = s64.mel_bound(fb, ref, s64.budget(n), 0.0)
+        err = (m.cpu().double() - mel).abs()
+        need = ((err - bound0).clamp_min(0) / mel.clamp_min(1e-300)).max().item()
+        widths = (hi - lo).cpu()
+        emit(kind="mel", n_fft=n, n_mels=nm, empty_bands=int((widths <= 0).sum()),
+             one_bin_bands=int((widths == 1).sum()), max_err_over_fbdelta=(err / bound0.clamp_min(1e-300)).max().item(),
+             rtol_needed_u=need / s64.U)
 
     seven_scale(eng, dev, AudioSignal, gc, s64)
 

@@ -29,14 +29,11 @@ BUDGET_C = {
     "cta4096": 2.0,    # spectral_kernel<11>, n_fft 4096
     "large": 2.0,      # stft_large_kernel, n_fft 8192 .. 32768
     "dense": 6.0,      # dft_forward_kernel, any other n_fft <= 8192 (g = sqrt n)
-    "tc": 8.0,         # spectral_tc_kernel (TF32 split products), n_fft 2048, mel only
 }
 
 
-def route(n_fft: int, tc: bool = False) -> str:
+def route(n_fft: int) -> str:
     """The forward kernel ``Engine.spectral`` launches for a window length (hop <= n_fft)."""
-    if tc:
-        return "tc"
     if n_fft & (n_fft - 1) == 0 and 32 <= n_fft <= 32768:
         return {32: "cta32", 2048: "warp_lean", 4096: "cta4096"}.get(n_fft, "warp" if n_fft < 4096 else "large")
     return "dense"
@@ -46,9 +43,9 @@ def growth(n_fft: int, rt: str) -> float:
     return math.sqrt(n_fft) if rt == "dense" else math.log2(n_fft)
 
 
-def budget(n_fft: int, rt: str = None) -> float:
+def budget(n_fft: int) -> float:
     """The bound on ``bin_err`` of a route at a window length (in units of the frame's RMS bin magnitude)."""
-    rt = rt or route(n_fft)
+    rt = route(n_fft)
     return BUDGET_C[rt] * U * growth(n_fft, rt)
 
 

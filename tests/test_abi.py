@@ -68,6 +68,13 @@ def test_bad_arguments_return_codes_not_crashes(lib):
         assert rc == -2 and f"istft: n_fft={n_fft} hop={hop}".encode() in lib.b2a_last_error()
 
 
+def test_spectral_tc_enable_is_a_stub(lib):
+    # the tensor-core spectral kernel is gone: switching it off is a no-op, switching it on is unsupported
+    assert lib.b2a_spectral_tc_enable(0) == 0
+    assert lib.b2a_spectral_tc_enable(1) == -2 and b"tensor-core spectral kernel was removed" in lib.b2a_last_error()
+    assert lib.b2a_spectral_tc_enable(0) == 0
+
+
 # every forward / backward STFT entry point checks torch's stft(center=True) framing of the padded signal with the
 # same codes and messages, before any CUDA call
 FRAMING_ENTRY_POINTS = {  # prefix of the message, n_fft, hop

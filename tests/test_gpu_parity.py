@@ -647,12 +647,12 @@ def test_host_mirror_follows_in_place_writes(at):
 
 
 # ------------------------------------------------------------------------------------------
-# tensor-core spectral kernel (csrc/spectral_tc.cu): same launches on the tensor cores (wgmma) and on the FP32 warp kernel, both
-# against the oracle, per cell (elementwise_ok) and globally; then BASELINE cfg2 at its full size
+# 2048-point mel / log-mel kernel (spectral_warp_kernel<10,0>) against the oracle, per cell (elementwise_ok) and
+# globally; then BASELINE cfg2 at its full size
 # ------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("hop,T,n_mels,wtype", [(512, 60000, 128, "hann"), (256, 20000, 80, "hann"),
                                                 (300, 17000, 64, "sqrt_hann"), (512, 441000, 128, "hann")])
-def test_spectral_tc_vs_fp32_kernel_vs_oracle(at, sp, hop, T, n_mels, wtype):
+def test_spectral_2048_mel_vs_oracle(at, sp, hop, T, n_mels, wtype):
     from audiotools_b200 import _lib
     from audiotools_b200.engine import get_engine
 
@@ -667,57 +667,37 @@ def test_spectral_tc_vs_fp32_kernel_vs_oracle(at, sp, hop, T, n_mels, wtype):
     w = at.AudioSignal.get_window(wtype, 2048, DEV)
     gain = torch.tensor([0.7, -3.0, 1.5], device=DEV)
     xd = x.to(DEV)
-    kw = dict(gain=gain, want_scaled=True, mel_fb=fb, mel_lo=lo, mel_hi=hi, want_stft=False)
-    prev = eng.lib.b2a_spectral_tc_enable(1)  # the tensor-core path is opt-in
-    try:
-        assert eng.spectral_kernel_name(2048, hop) == "spectral_tc_kernel"
-        tc = eng.spectral(xd, 2048, hop, w, **kw)
-        lg = eng.spectral(xd, 2048, hop, w, mel_fb=fb, mel_lo=lo, mel_hi=hi, post=_lib.POST_LOG10, post_eps=1e-5,
-                          post_power=2.0, want_stft=False)["mel"].cpu()
-        eng.lib.b2a_spectral_tc_enable(0)
-        assert eng.spectral_kernel_name(2048, hop) == "spectral_warp_kernel<10,0>"
-        fp = eng.spectral(xd, 2048, hop, w, **kw)
-    finally:
-        eng.lib.b2a_spectral_tc_enable(prev)
+    assert eng.spectral_kernel_name(2048, hop) == "spectral_warp_kernel<10,0>"
+    out = eng.spectral(xd, 2048, hop, w, gain=gain, want_scaled=True, mel_fb=fb, mel_lo=lo, mel_hi=hi, want_stft=False)
+    lg = eng.spectral(xd, 2048, hop, w, mel_fb=fb, mel_lo=lo, mel_hi=hi, post=_lib.POST_LOG10, post_eps=1e-5,
+                      post_power=2.0, want_stft=False)["mel"].cpu()
     torch.cuda.synchronize()
-    assert torch.equal(tc["scaled"], fp["scaled"])
+    assert torch.equal(out["scaled"].cpu(), x * gain.cpu()[:, None, None])
     ref = sp.mel_spectrogram(x * gain.cpu()[:, None, None], sr, n_mels, window_length=2048, hop_length=hop,
                              window_type=wtype)
-    assert tc["mel"].shape == ref.shape  # frame indexing bit-exact
+    assert out["mel"].shape == ref.shape  # frame indexing bit-exact
     for b in range(3):
-        for name, got in (("tensor-core", tc["mel"]), ("fp32", fp["mel"])):
-            assert rel_err(got[b].cpu(), ref[b]) < 2e-5, (name, b)
-            assert elementwise_ok(got[b].cpu(), ref[b]), (name, b)
+        assert rel_err(out["mel"][b].cpu(), ref[b]) < 2e-5, b
+        assert elementwise_ok(out["mel"][b].cpu(), ref[b]), b
     ref_log = sp.log_mel(sp.mel_spectrogram(x, sr, n_mels, window_length=2048, hop_length=hop, window_type=wtype))
     assert (lg[:2] - ref_log[:2]).abs().max() < 2e-4  # log10 units (item 2: see tests/test_sim_kernels.py)
 
 
-def test_cfg2_full_size_tc_strided_oracle(at, sp):
-    """BASELINE configs[1] at its stated size (64 x 2ch x 10 s @ 44.1 kHz) through the public API on the tensor-core
-    kernel; the oracle checks a strided subset of the items (it needs ~0.3 s per clip), the FP32 kernel all of them."""
+def test_cfg2_full_size_strided_oracle(at, sp):
+    """BASELINE configs[1] at its stated size (64 x 2ch x 10 s @ 44.1 kHz) through the public API; the oracle checks a
+    strided subset of the items (it needs ~0.3 s per clip)."""
     from audiotools_b200.engine import get_engine
 
     import bench
 
     eng = get_engine()
     x = bench.make_batch(64, 4242)
-    prev = eng.lib.b2a_spectral_tc_enable(1)
-    try:
-        sig = at.AudioSignal(x.clone(), 44100).to(DEV)
-        sig.normalize(-24.0)
-        logmel = sig.mel_spectrogram(n_mels=128, window_length=2048, hop_length=512, window_type="hann", log=True)
-        y = sig.audio_data
-        assert eng.spectral_kernel_name(2048, 512) == "spectral_tc_kernel"
-        assert logmel.shape == (64, 2, 128, 862) and y.shape == x.shape
-        eng.lib.b2a_spectral_tc_enable(0)
-        sig2 = at.AudioSignal(x.clone(), 44100).to(DEV)
-        sig2.normalize(-24.0)
-        logmel_fp = sig2.mel_spectrogram(n_mels=128, window_length=2048, hop_length=512, window_type="hann", log=True)
-        y_fp = sig2.audio_data
-    finally:
-        eng.lib.b2a_spectral_tc_enable(prev)
-    assert torch.equal(y, y_fp)
-    assert (logmel - logmel_fp).abs().max().item() < 2e-4  # log10 units, all 64 items
+    sig = at.AudioSignal(x.clone(), 44100).to(DEV)
+    sig.normalize(-24.0)
+    logmel = sig.mel_spectrogram(n_mels=128, window_length=2048, hop_length=512, window_type="hann", log=True)
+    y = sig.audio_data
+    assert eng.spectral_kernel_name(2048, 512) == "spectral_warp_kernel<10,0>"
+    assert logmel.shape == (64, 2, 128, 862) and y.shape == x.shape
     for i in range(0, 64, 13):
         y_ref, _ = sp.normalize(x[i:i + 1], 44100, -24.0)
         ref = sp.log_mel(sp.mel_spectrogram(y_ref, 44100, 128, window_length=2048, hop_length=512, window_type="hann"))

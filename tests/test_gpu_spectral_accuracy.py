@@ -1,6 +1,6 @@
 """Every spectral route on the H100 (``-m gpu``) against float64, bin by bin and frame by frame (tests/spectral64.py):
 the DFT matrix itself through impulses, noise under three windows and three levels, high dynamic range, DC and
-Nyquist, every padding mode, mel with empty and one-bin bands (and the tensor-core kernel), the inverse STFT, the
+Nyquist, every padding mode, mel with empty and one-bin bands, the inverse STFT, the
 backward passes, and exact invariances (power-of-two scaling, row independence, frame shift, kernel modes).  Each
 error is held to its route's budget (tests/spectral64.py, measured on an H100 80GB HBM3 at a 700 W power limit) and to
 a stated factor of cuFFT's error (torch.stft / torch.istft in float32 on the same GPU and input).
@@ -139,7 +139,7 @@ MEL_CASES = [(2048, 320, 44100), (32, 5, 44100), (8192, 128, 44100), (400, 40, 4
              (4096, 128, 16000)]
 
 
-def _mel_check(eng, n_fft, n_mels, sr, tc=False):
+def _mel_check(eng, n_fft, n_mels, sr):
     from audiotools_b200 import AudioSignal, _lib
 
     hop = n_fft // 4
@@ -147,29 +147,22 @@ def _mel_check(eng, n_fft, n_mels, sr, tc=False):
     fb, lo, hi = AudioSignal._mel_tables(sr, n_fft, n_mels, 0.0, None, DEV)
     widths = (hi - lo).cpu()
     w = s64.windows(n_fft, DEV)["hann"]
-    rt = s64.route(n_fft, tc)
-    prev = eng.lib.b2a_spectral_tc_enable(1 if tc else 0)
-    try:
-        if tc:
-            assert eng.spectral_kernel_name(n_fft, hop) == "spectral_tc_kernel"
-        for name in ("noise", "tones_120dB", "dc"):
-            xs = x[name].to(DEV)
-            with _NoTorchSpectral():
-                mel = eng.spectral(xs, n_fft, hop, w, mel_fb=fb, mel_lo=lo, mel_hi=hi, want_stft=False)["mel"]
-                lg = eng.spectral(xs, n_fft, hop, w, mel_fb=fb, mel_lo=lo, mel_hi=hi, post=_lib.POST_LOG10,
-                                  post_eps=1e-5, post_power=2.0, want_stft=False)["mel"]
-            ref = s64.stft_ref(xs, n_fft, hop, w)
-            bound, mel64 = s64.mel_bound(fb, ref, s64.budget(n_fft, rt), s64.MEL_RTOL)
-            err = (mel.cpu().double() - mel64).abs()
-            assert bool((err <= bound).all()), (n_fft, n_mels, tc, name, (err / bound).max().item())
-            # log-mel: for cells above post_eps, error <= power (relative mel bound) / ln 10 + lg2.approx's error
-            above = mel64 > 1e-5
-            rel = bound / mel64.clamp_min(1e-300)
-            lbound = 2.0 * (rel / math.log(10) + s64.LG2_APPROX * math.log10(2)) + 4 * s64.U * (2 * mel64.clamp_min(1e-5).log10().abs())
-            lerr = (lg.cpu().double() - 2.0 * mel64.clamp_min(1e-5).log10()).abs()
-            assert bool((lerr <= lbound)[above].all()), (n_fft, n_mels, tc, name, (lerr / lbound)[above].max().item())
-    finally:
-        eng.lib.b2a_spectral_tc_enable(prev)
+    for name in ("noise", "tones_120dB", "dc"):
+        xs = x[name].to(DEV)
+        with _NoTorchSpectral():
+            mel = eng.spectral(xs, n_fft, hop, w, mel_fb=fb, mel_lo=lo, mel_hi=hi, want_stft=False)["mel"]
+            lg = eng.spectral(xs, n_fft, hop, w, mel_fb=fb, mel_lo=lo, mel_hi=hi, post=_lib.POST_LOG10,
+                              post_eps=1e-5, post_power=2.0, want_stft=False)["mel"]
+        ref = s64.stft_ref(xs, n_fft, hop, w)
+        bound, mel64 = s64.mel_bound(fb, ref, s64.budget(n_fft), s64.MEL_RTOL)
+        err = (mel.cpu().double() - mel64).abs()
+        assert bool((err <= bound).all()), (n_fft, n_mels, name, (err / bound).max().item())
+        # log-mel: for cells above post_eps, error <= power (relative mel bound) / ln 10 + lg2.approx's error
+        above = mel64 > 1e-5
+        rel = bound / mel64.clamp_min(1e-300)
+        lbound = 2.0 * (rel / math.log(10) + s64.LG2_APPROX * math.log10(2)) + 4 * s64.U * (2 * mel64.clamp_min(1e-5).log10().abs())
+        lerr = (lg.cpu().double() - 2.0 * mel64.clamp_min(1e-5).log10()).abs()
+        assert bool((lerr <= lbound)[above].all()), (n_fft, n_mels, name, (lerr / lbound)[above].max().item())
     return int((widths <= 0).sum()), int((widths == 1).sum())
 
 
@@ -181,12 +174,6 @@ def test_mel_and_log_mel_per_band(eng, n_fft, n_mels, sr):
     empty, one = _mel_check(eng, n_fft, n_mels, sr)
     if (n_fft, n_mels) in ((2048, 320), (512, 160)):
         assert one > 0  # the shapes where a band reads a single bin
-
-
-def test_tensor_core_mel_per_band(eng):
-    """The opt-in tensor-core kernel (n_fft 2048, mel only) under its own budget (TF32 split products)."""
-    _mel_check(eng, 2048, 320, 44100, tc=True)
-    _mel_check(eng, 2048, 128, 44100, tc=True)
 
 
 @pytest.mark.parametrize("n_fft", FFT_LENGTHS + [400, 1001, 4095, 8191])
