@@ -58,13 +58,46 @@ class LoudnessMixin:
         """Integrated gated loudness [B] in LUFS, clamped to >= -70; cached until ``audio_data`` is reassigned."""
         if self._loudness is not None:
             return self._loudness.to(self.device)
-        T = self.signal_length
-        padded = T
-        if self.signal_duration < 0.5:  # zero-extend to 0.5 s (ref :302-305); no copy: the kernel reads zeros
-            padded = T + int((0.5 - self.signal_duration) * self.sample_rate)
         kweighting.design(float(self.sample_rate), filter_class)
         # detached: the loudness is not differentiable (nor is the reference's, ref:tests/core/test_grad.py:70)
         out = _engine().lufs(self._materialized().detach(), self.sample_rate, filter_class, block_size,
-                             padded_length=padded)
+                             padded_length=self._padded_length())
         self._loudness = out["loud"]
         return self._loudness.to(self.device)
+
+    def _padded_length(self) -> int:
+        if self.signal_duration < 0.5:  # zero-extend to 0.5 s (ref :302-305); no copy: the kernel reads zeros
+            return self.signal_length + int((0.5 - self.signal_duration) * self.sample_rate)
+        return self.signal_length
+
+    def loudness_stats(self, filter_class: str = "K-weighting", series: bool = False):
+        """EBU R128 loudness statistics of every item, the numbers of the reference's ``r128stats``
+        (ref:audiotools/core/ffmpeg.py:13-62) computed on the GPU: a dict of [B] float32 tensors
+
+        * ``"I"``: integrated loudness, bit-identical to the engine's unclamped BS.1770 loudness (``-inf`` for silence;
+          ``loudness()`` clamps it to -70);
+        * ``"I Threshold"``: the relative gate of that measurement, ``-inf`` when no 400 ms block passes -70 LUFS;
+        * ``"LRA"``, ``"LRA Threshold"``, ``"LRA Low"``, ``"LRA High"``: the loudness range of EBU Tech 3342.
+
+        With ``series=True`` also ``"momentary"`` [B, n_400ms] (the loudness of every 400 ms gating block, 100 ms
+        apart) and ``"short_term"`` [B, n_3s] (3 s blocks, 100 ms apart), in LUFS.
+
+        Definitions, with s = int(0.1 * rate) samples (the gating stride), G_c the BS.1770 channel gains and the
+        K-weighted energies of the strides summed in float64:
+
+        * short-term block i covers strides i .. i + 29, S_i = -0.691 + 10 log10(sum_c G_c E_c,i / (30 s)), rounded to
+          float32; there are (T - 30 s) // s + 1 of them (none below 30 s samples).  30 s is 3 s of audio at every
+          common rate, but 33060 samples (2.9986 s) at 11025 Hz;
+        * LRA Threshold = -0.691 + 10 log10(mean of 10^((S + 0.691) / 10) over S > -70) - 20;
+        * the kept S are those > -70 and > LRA Threshold; sorted ascending (n of them), LRA Low = v[floor(0.10 (n - 1)
+          + 0.5)], LRA High = v[floor(0.95 (n - 1) + 0.5)] (nearest rank, as libebur128), LRA = High - Low;
+        * no S above -70 (including signals shorter than 3 s): LRA = 0 and the other three are -inf.
+
+        These are not ffmpeg's numbers: ffmpeg's ebur128 filter quantises its gating histogram, this uses the BS.1770
+        arithmetic of ``loudness()``.  The two have not been compared.  Items shorter than 0.5 s are zero-extended to
+        0.5 s as in ``loudness()``.  The values are detached, and no cache (``loudness()``'s, ``stft_data``) is read or
+        written.  Only ``filter_class="K-weighting"`` is implemented; R128 fixes the block at 0.4 s."""
+        kweighting.design(float(self.sample_rate), filter_class)  # raises for classes that are not implemented
+        out = _engine().loudness_stats(self._materialized().detach(), self.sample_rate,
+                                       padded_length=self._padded_length(), want_series=series)
+        return {k: v.to(self.device) for k, v in out.items()}

@@ -147,13 +147,6 @@ __global__ void __launch_bounds__(TPB) quantize_kernel(const float* __restrict__
 }
 
 // ---- exact k-th smallest by 4-pass (8 bits each) radix selection: one CTA per requested order statistic
-__device__ __forceinline__ unsigned ord_key(float v) {
-  const unsigned b = __float_as_uint(v);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float ord_val(unsigned k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
 constexpr int ST = 1024;
 __global__ void __launch_bounds__(ST) order_stat_kernel(const float* __restrict__ row, int64_t T,
                                                         const int64_t* __restrict__ ks, float* __restrict__ out) {

@@ -40,7 +40,11 @@
 //   measures each stage.
 // Kernel 2  lufs_gate_kernel             (tiny: one CTA per item)
 //   z -> l -> absolute gate -> relative gate -> LUFS, with the reference's dtypes (float32 z,
-//   float64 logs) and its NaN / inf scrubbing; optionally max(.,-70) and normalize()'s gain.
+//   float64 logs) and its NaN / inf scrubbing; optionally max(.,-70) and normalize()'s gain.  For loudness statistics
+//   it also writes the relative gate and the momentary loudness of every block.
+// Kernel 3  loudness_stats_kernel        (one CTA per item; b2a_loudness_stats_f32 only)
+//   EBU R128 loudness range from the same interval bins: 3 s short-term loudness (30 strides), both gates, and the
+//   10 % / 95 % nearest-rank percentiles by radix selection -- no host synchronisation, no sort.
 #include "b2a_common.h"
 
 namespace b2a {
@@ -545,10 +549,13 @@ struct GateParams {
   int C, nblk, nbins, q;
 };
 
+// gr_out (nullable) [B]: the relative gate Gamma_r, -inf when no block passes the absolute gate; mom_out (nullable)
+// [B, nblk]: the momentary loudness l of every block (loudness_stats)
 __global__ void __launch_bounds__(GT)
 lufs_gate_kernel(const double* __restrict__ bins, GateParams gp, float* __restrict__ zws,
                  float* __restrict__ z_out, float* __restrict__ lufs_out, float* __restrict__ loud_out,
-                 const float* __restrict__ target_db, int n_target, float* __restrict__ gain_out) {
+                 const float* __restrict__ target_db, int n_target, float* __restrict__ gain_out,
+                 float* __restrict__ gr_out, float* __restrict__ mom_out) {
   __shared__ double sd[GT];
   __shared__ int si[GT];
   const int b = blockIdx.x, C = gp.C, nblk = gp.nblk, q = gp.q;
@@ -575,6 +582,7 @@ lufs_gate_kernel(const double* __restrict__ bins, GateParams gp, float* __restri
     double acc = 0.0;
     for (int c = 0; c < C; ++c) acc += gp.G[c] * (double)z[c * nblk + i];
     double l = -0.691 + 10.0 * log10(acc);
+    if (mom_out) mom_out[(size_t)b * nblk + i] = (float)l;
     // z[l <= Ga] = 0 (a NaN l is NOT zeroed), masked = l > Ga (a NaN l is NOT counted)
     if (!(l <= Gamma_a))
       for (int c = 0; c < C; ++c) sum1[c] += (double)z[c * nblk + i];
@@ -588,6 +596,7 @@ lufs_gate_kernel(const double* __restrict__ bins, GateParams gp, float* __restri
     gr_acc += (double)zavg * gp.G[c];
   }
   const double Gamma_r = -0.691 + 10.0 * log10(gr_acc) - 10.0;
+  if (gr_out && tid == 0) gr_out[b] = n1t > 0 ? (float)Gamma_r : -INFINITY;  // 0 / 0 gives NaN above
   // pass 2: absolute + relative gate (comparisons with NaN are false, as in torch)
   double sum2[8];
   for (int c = 0; c < C; ++c) sum2[c] = 0.0;
@@ -621,6 +630,139 @@ lufs_gate_kernel(const double* __restrict__ bins, GateParams gp, float* __restri
       float db = target_db[n_target == 1 ? 0 : b];
       float gdb = db - loud;
       gain_out[b] = expf(gdb * 0.11512925464970229f);  // GAIN_FACTOR = ln(10)/20 (effects.py:12)
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// loudness range (EBU Tech 3342) from the same interval bins: one CTA per item
+//   S_i = float32(-0.691 + 10 log10(sum_c G_c E_c,i / (30 stride))), E_c,i = sum_{j=i}^{i+29} (A_j + B_j) in float64,
+//   in that order (a 3 s window is 30 strides at every rate whose stride is exact; 33060 samples at 11025 Hz);
+//   absolute gate S > -70, LRA Threshold = -0.691 + 10 log10(mean 10^((S + 0.691) / 10)) - 20 over the abs-gated S,
+//   relative gate S > LRA Threshold (applied to the abs-gated S), nearest-rank 10 % / 95 % percentiles of the n kept
+//   values v (ascending): v[floor(0.10 (n - 1) + 0.5)], v[floor(0.95 (n - 1) + 0.5)], evaluated as the equal integer
+//   expressions (n + 4) / 10 and (19 n - 9) / 20.
+// The two percentiles come from a 4-pass (8 bits each) radix selection over order-preserving keys of the kept S
+// (unkept: key 0, which no float below NaN maps to), both ranks per pass.  The keys of a row live in shared memory
+// when it has at most ST_SMEM_KEYS short-term blocks, else in the workspace: the selection is exact for any row length.
+// ---------------------------------------------------------------------------------------------
+constexpr int ST_STRIDES = 30;  // 3 s short-term block / 0.1 s gating stride
+constexpr int MAX_C = 5;        // channels with BS.1770 gains
+#ifdef B2A_SIM
+constexpr int ST_SMEM_KEYS = 64;  // the simulator's rows spill to the workspace at a few seconds of audio
+#else
+constexpr int ST_SMEM_KEYS = 8192;  // 32 KB: 13.7 minutes of audio
+#endif
+
+struct StatsParams {
+  double G[8];
+  double len;  // samples per short-term block: 30 stride
+  int C, nbins, n_st;
+};
+
+__global__ void __launch_bounds__(GT)
+loudness_stats_kernel(const double* __restrict__ bins, StatsParams sp, const float* __restrict__ lufs,
+                      const float* __restrict__ gate_r, unsigned* __restrict__ keys_ws, float* __restrict__ st_out,
+                      float* __restrict__ stats_out) {
+  __shared__ double s_e[MAX_C][GT + ST_STRIDES - 1];  // stride energies A_j + B_j of a tile of GT short-term blocks
+  __shared__ unsigned s_keys[ST_SMEM_KEYS];
+  __shared__ unsigned s_hist[2][256];
+  __shared__ unsigned s_sel[2][2];  // per rank: key prefix, rank within it
+  __shared__ double sd[GT];
+  __shared__ int si[GT];
+  const int b = blockIdx.x, tid = threadIdx.x, C = sp.C, n = sp.n_st;
+  unsigned* keys = n <= ST_SMEM_KEYS ? s_keys : keys_ws + (size_t)b * n;
+  // 1. short-term loudness; power sum over the absolute gate
+  double pw = 0.0;
+  int n1 = 0;
+  for (int i0 = 0; i0 < n; i0 += GT) {
+    const int m = min(GT, n - i0) + ST_STRIDES - 1;
+    __syncthreads();  // the previous tile's reads of s_e are done
+    for (int idx = tid; idx < C * m; idx += GT) {
+      const int c = idx / m, j = idx - c * m;
+      const double* e = bins + ((size_t)b * C + c) * sp.nbins + 2 * (size_t)(i0 + j);
+      s_e[c][j] = e[0] + e[1];
+    }
+    __syncthreads();
+    const int i = i0 + tid;
+    if (i < n) {
+      double acc = 0.0;
+      for (int c = 0; c < C; ++c) {
+        double e = 0.0;
+        for (int k = 0; k < ST_STRIDES; ++k) e += s_e[c][tid + k];
+        acc += sp.G[c] * e;
+      }
+      const float s = (float)(-0.691 + 10.0 * log10(acc / sp.len));
+      if (st_out) st_out[(size_t)b * n + i] = s;
+      keys[i] = __float_as_uint(s);
+      if (s > -70.f) {
+        pw += pow(10.0, ((double)s + 0.691) / 10.0);
+        n1++;
+      }
+    }
+  }
+  const int n1t = block_sum<int>(n1, si);
+  const double thr = -0.691 + 10.0 * log10(block_sum<double>(pw, sd) / n1t) - 20.0;  // NaN when n1t == 0: unused
+  // 2. both gates: kept S -> order-preserving key, the rest -> 0
+  int n2 = 0;
+  for (int i = tid; i < n; i += GT) {
+    const float s = __uint_as_float(keys[i]);
+    const bool keep = s > -70.f && (double)s > thr;
+    keys[i] = keep ? ord_key(s) : 0u;
+    n2 += keep;
+  }
+  const int n2t = block_sum<int>(n2, si);  // its barrier also publishes the keys
+  // 3. the keys at ranks lo and hi among the kept ones (n2t is CTA-uniform)
+  unsigned pre[2] = {0u, 0u};
+  unsigned rank[2] = {(unsigned)((n2t + 4) / 10), (unsigned)(((int64_t)19 * n2t - 9) / 20)};
+  for (int shift = 24; n2t > 0 && shift >= 0; shift -= 8) {
+    for (int i = tid; i < 2 * 256; i += GT) (&s_hist[0][0])[i] = 0u;
+    __syncthreads();
+    const unsigned hmask = shift == 24 ? 0u : ~0u << (shift + 8);  // the digits selected so far
+    // runs of equal digits are counted in registers first: the S of one row share their leading digits, and an
+    // atomic per key would serialise on one bin
+    unsigned cd[2] = {0u, 0u}, cn[2] = {0u, 0u};
+    for (int i = tid; i < n; i += GT) {
+      const unsigned k = keys[i];
+      if (k == 0u) continue;
+      const unsigned d = (k >> shift) & 255u;
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        if ((k & hmask) != pre[r]) continue;
+        if (cn[r] && d != cd[r]) {
+          atomicAdd(&s_hist[r][cd[r]], cn[r]);
+          cn[r] = 0u;
+        }
+        cd[r] = d;
+        ++cn[r];
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+      if (cn[r]) atomicAdd(&s_hist[r][cd[r]], cn[r]);
+    __syncthreads();
+    if (tid < 2) {  // thread r: the digit where the running count passes rank r
+      const unsigned p = tid ? pre[1] : pre[0], k = tid ? rank[1] : rank[0];
+      unsigned c = 0u, d = 0u;
+      for (; d < 255u; ++d) {
+        if (c + s_hist[tid][d] > k) break;
+        c += s_hist[tid][d];
+      }
+      s_sel[tid][0] = p | (d << shift);
+      s_sel[tid][1] = k - c;
+    }
+    __syncthreads();
+    for (int r = 0; r < 2; ++r) { pre[r] = s_sel[r][0]; rank[r] = s_sel[r][1]; }
+  }
+  if (tid == 0) {
+    float* o = stats_out + (size_t)b * 6;  // I, I Threshold, LRA, LRA Threshold, LRA Low, LRA High
+    o[0] = lufs[b];
+    o[1] = gate_r[b];
+    if (n2t > 0) {
+      const float lo = ord_val(pre[0]), hi = ord_val(pre[1]);
+      o[2] = hi - lo; o[3] = (float)thr; o[4] = lo; o[5] = hi;
+    } else {
+      o[2] = 0.f; o[3] = -INFINITY; o[4] = -INFINITY; o[5] = -INFINITY;
     }
   }
 }
@@ -667,14 +809,11 @@ static int geometry(int64_t Tp, double rate, double block_s, Geometry* g) {
   return 0;
 }
 
+// Kernel 1 into the interval bins at the start of `ws` (zeroed first): the one K-weighting pass of b2a_lufs_f32 and
+// b2a_loudness_stats_f32
 template <int NS>
-static int run(const float* x, int64_t B, int C, int64_t T, int64_t Tp, const Geometry& g, const double* sos_h,
-               const double* stage_gain_h, double rate, double block_s, const double* chan_gain_h,
-               float* z_blocks, float* lufs_out, float* loud_out, const float* target_db, int n_target,
-               float* gain_out, void* ws, size_t ws_bytes, void* stream) {
-  const int64_t rows = B * C;
-  WsLayout w = ws_layout(rows, g.nbins, g.nblk);
-  B2A_REQUIRE(ws_bytes >= w.total, B2A_E_INVALID, "lufs: workspace too small (%zu < %zu)", ws_bytes, w.total);
+static int energy(const float* x, int64_t rows, int64_t T, int64_t Tp, const Geometry& g, const double* sos_h,
+                  const double* stage_gain_h, const WsLayout& w, void* ws, void* stream) {
   Coef<NS> cf;
   for (int s = 0; s < NS; ++s) {
     const double* c = sos_h + 6 * s;
@@ -726,14 +865,69 @@ static int run(const float* x, int64_t B, int C, int64_t T, int64_t Tp, const Ge
   g_k2_last[1] = (int)grid;
   g_k2_last[2] = (int)smem;
 #endif
+  return B2A_OK;
+}
+
+static int energy_pass(const float* x, int64_t rows, int64_t T, int64_t Tp, const Geometry& g, const double* sos_h,
+                       const double* stage_gain_h, int n_stage, const WsLayout& w, void* ws, void* stream) {
+  if (n_stage == 1) return energy<1>(x, rows, T, Tp, g, sos_h, stage_gain_h, w, ws, stream);
+  return energy<2>(x, rows, T, Tp, g, sos_h, stage_gain_h, w, ws, stream);
+}
+
+// Kernel 2 on the bins of energy_pass
+static int gate(int64_t B, int C, const Geometry& g, double rate, double block_s, const double* chan_gain_h,
+                const WsLayout& w, void* ws, float* z_blocks, float* lufs_out, float* loud_out, const float* target_db,
+                int n_target, float* gain_out, float* gr_out, float* mom_out, void* stream) {
+  char* base = (char*)ws;
   GateParams gp;
   for (int c = 0; c < 8; ++c) gp.G[c] = c < C ? chan_gain_h[c] : 0.0;
   gp.scale = (float)(1.0 / (block_s * rate));
   gp.C = C; gp.nblk = g.nblk; gp.nbins = g.nbins; gp.q = g.q;
   B2A_LAUNCH(lufs_gate_kernel, dim3((unsigned)B), dim3(GT), 0, stream, (const double*)(base + w.bins), gp,
-             (float*)(base + w.zws), z_blocks, lufs_out, loud_out, target_db, n_target, gain_out);
+             (float*)(base + w.zws), z_blocks, lufs_out, loud_out, target_db, n_target, gain_out, gr_out, mom_out);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
+}
+
+// the argument checks both entry points share, in this order around their own
+static int check_input(int64_t B, int C, int64_t T, int64_t T_padded, int n_stage) {
+  B2A_REQUIRE(B >= 1 && C >= 1 && T >= 1, B2A_E_INVALID, "lufs: empty input (B=%lld C=%d T=%lld)", (long long)B, C,
+              (long long)T);
+  B2A_REQUIRE(C <= MAX_C, B2A_E_INVALID, "lufs: at most 5 channels have BS.1770 gains (got %d)", C);
+  B2A_REQUIRE(T_padded >= T, B2A_E_INVALID, "lufs: T_padded < T");
+  B2A_REQUIRE(T_padded < (int64_t)2147483647 - 2 * TILE, B2A_E_UNSUPPORTED, "lufs: rows longer than 2^31 samples");
+  B2A_REQUIRE(B * C * ((T_padded + TILE - 1) / TILE) < (int64_t)2147483647, B2A_E_UNSUPPORTED, "lufs: too many tiles");
+  B2A_REQUIRE(n_stage >= 1 && n_stage <= MAX_STAGES, B2A_E_UNSUPPORTED,
+              "lufs: %d biquad stages (1..%d supported: K-weighting has 2)", n_stage, MAX_STAGES);
+  return B2A_OK;
+}
+static int check_geometry(int64_t T_padded, double rate, double block_s, Geometry* g) {
+  B2A_REQUIRE(geometry(T_padded, rate, block_s, g) == 0, B2A_E_UNSUPPORTED,
+              "lufs: gating stride int(block_s*rate/4) must be >= 64 samples (rate=%g block_s=%g)", rate, block_s);
+  return B2A_OK;
+}
+
+// ---- loudness statistics: the loudness workspace, then I and Gamma_r of the gate kernel [B] each, the keys [B, n_st]
+constexpr double R128_BLOCK_S = 0.4;
+
+static int64_t num_short_term(int64_t Tp, const Geometry& g) {
+  const int64_t len = (int64_t)ST_STRIDES * g.stride;
+  return Tp >= len ? (Tp - len) / g.stride + 1 : 0;
+}
+
+struct StatsWs {
+  WsLayout k;
+  size_t lufs, gate_r, keys, total;
+};
+static StatsWs stats_ws_layout(int64_t B, int C, const Geometry& g, int64_t n_st) {
+  StatsWs s;
+  s.k = ws_layout(B * C, g.nbins, g.nblk);
+  size_t o = s.k.total;
+  s.lufs = o; o = align256(o + sizeof(float) * B);
+  s.gate_r = o; o = align256(o + sizeof(float) * B);
+  s.keys = o; o = align256(o + sizeof(unsigned) * B * n_st);
+  s.total = o;
+  return s;
 }
 
 }  // namespace lufs
@@ -759,24 +953,64 @@ extern "C" int b2a_lufs_f32(const float* x, int64_t B, int C, int64_t T, int64_t
                             const float* target_db, int n_target, float* gain_out, void* ws, size_t ws_bytes,
                             void* stream) {
   B2A_REQUIRE(x && lufs_out && ws && sos_h && stage_gain_h && chan_gain_h, B2A_E_INVALID, "lufs: null pointer");
-  B2A_REQUIRE(B >= 1 && C >= 1 && T >= 1, B2A_E_INVALID, "lufs: empty input (B=%lld C=%d T=%lld)", (long long)B, C,
-              (long long)T);
-  B2A_REQUIRE(C <= 5, B2A_E_INVALID, "lufs: at most 5 channels have BS.1770 gains (got %d)", C);
-  B2A_REQUIRE(T_padded >= T, B2A_E_INVALID, "lufs: T_padded < T");
-  B2A_REQUIRE(T_padded < (int64_t)2147483647 - 2 * TILE, B2A_E_UNSUPPORTED, "lufs: rows longer than 2^31 samples");
-  B2A_REQUIRE(B * C * ((T_padded + TILE - 1) / TILE) < (int64_t)2147483647, B2A_E_UNSUPPORTED, "lufs: too many tiles");
-  B2A_REQUIRE(n_stage >= 1 && n_stage <= MAX_STAGES, B2A_E_UNSUPPORTED,
-              "lufs: %d biquad stages (1..%d supported: K-weighting has 2)", n_stage, MAX_STAGES);
+  int rc = check_input(B, C, T, T_padded, n_stage);
+  if (rc != B2A_OK) return rc;
   B2A_REQUIRE(!gain_out || (target_db && (n_target == 1 || n_target == B)), B2A_E_INVALID,
               "lufs: gain_out needs target_db with 1 or B entries");
   Geometry g;
-  B2A_REQUIRE(geometry(T_padded, rate, block_s, &g) == 0, B2A_E_UNSUPPORTED,
-              "lufs: gating stride int(block_s*rate/4) must be >= 64 samples (rate=%g block_s=%g)", rate, block_s);
-  if (n_stage == 1)
-    return run<1>(x, B, C, T, T_padded, g, sos_h, stage_gain_h, rate, block_s, chan_gain_h, z_blocks, lufs_out,
-                  loud_out, target_db, n_target, gain_out, ws, ws_bytes, stream);
-  return run<2>(x, B, C, T, T_padded, g, sos_h, stage_gain_h, rate, block_s, chan_gain_h, z_blocks, lufs_out,
-                loud_out, target_db, n_target, gain_out, ws, ws_bytes, stream);
+  rc = check_geometry(T_padded, rate, block_s, &g);
+  if (rc != B2A_OK) return rc;
+  const WsLayout w = ws_layout(B * C, g.nbins, g.nblk);
+  B2A_REQUIRE(ws_bytes >= w.total, B2A_E_INVALID, "lufs: workspace too small (%zu < %zu)", ws_bytes, w.total);
+  const int re = energy_pass(x, B * C, T, T_padded, g, sos_h, stage_gain_h, n_stage, w, ws, stream);
+  if (re != B2A_OK) return re;
+  return gate(B, C, g, rate, block_s, chan_gain_h, w, ws, z_blocks, lufs_out, loud_out, target_db, n_target, gain_out,
+              nullptr, nullptr, stream);
+}
+
+extern "C" int64_t b2a_loudness_stats_num_short_term(int64_t T_padded, double rate) {
+  Geometry g;
+  if (T_padded < 1 || geometry(T_padded, rate, R128_BLOCK_S, &g) != 0) return -1;
+  return num_short_term(T_padded, g);
+}
+
+extern "C" size_t b2a_loudness_stats_workspace_bytes(int64_t B, int C, int64_t T_padded, double rate) {
+  Geometry g;
+  if (B < 1 || C < 1 || T_padded < 1 || geometry(T_padded, rate, R128_BLOCK_S, &g) != 0) return 0;
+  return stats_ws_layout(B, C, g, num_short_term(T_padded, g)).total;
+}
+
+extern "C" int b2a_loudness_stats_f32(const float* x, int64_t B, int C, int64_t T, int64_t T_padded, double rate,
+                                      const double* sos_h, const double* stage_gain_h, int n_stage,
+                                      const double* chan_gain_h, float* stats_out, float* momentary_out,
+                                      float* short_term_out, void* ws, size_t ws_bytes, void* stream) {
+  B2A_REQUIRE(x && stats_out && ws && sos_h && stage_gain_h && chan_gain_h, B2A_E_INVALID,
+              "loudness_stats: null pointer");
+  int rc = check_input(B, C, T, T_padded, n_stage);
+  if (rc != B2A_OK) return rc;
+  Geometry g;
+  rc = check_geometry(T_padded, rate, R128_BLOCK_S, &g);
+  if (rc != B2A_OK) return rc;
+  const int64_t n_st = num_short_term(T_padded, g);
+  const StatsWs w = stats_ws_layout(B, C, g, n_st);
+  B2A_REQUIRE(ws_bytes >= w.total, B2A_E_INVALID, "loudness_stats: workspace too small (%zu < %zu)", ws_bytes,
+              w.total);
+  const int re = energy_pass(x, B * C, T, T_padded, g, sos_h, stage_gain_h, n_stage, w.k, ws, stream);
+  if (re != B2A_OK) return re;
+  char* base = (char*)ws;
+  float* lufs = (float*)(base + w.lufs);
+  float* gate_r = (float*)(base + w.gate_r);
+  const int rg = gate(B, C, g, rate, R128_BLOCK_S, chan_gain_h, w.k, ws, nullptr, lufs, nullptr, nullptr, 0, nullptr,
+                      gate_r, momentary_out, stream);
+  if (rg != B2A_OK) return rg;
+  StatsParams sp;
+  for (int c = 0; c < 8; ++c) sp.G[c] = c < C ? chan_gain_h[c] : 0.0;
+  sp.len = (double)ST_STRIDES * g.stride;
+  sp.C = C; sp.nbins = g.nbins; sp.n_st = (int)n_st;
+  B2A_LAUNCH(loudness_stats_kernel, dim3((unsigned)B), dim3(GT), 0, stream, (const double*)(base + w.k.bins), sp,
+             (const float*)lufs, (const float*)gate_r, (unsigned*)(base + w.keys), short_term_out, stats_out);
+  B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
 }
 
 #ifdef B2A_K2_PROBE

@@ -572,6 +572,44 @@ class Engine:
         self.launches += 2  # kweight_energy, lufs_gate (+ one memset node)
         return {"lufs": lufs, "loud": loud, "gain": gain, "blocks": blocks}
 
+    LOUDNESS_STATS = ("I", "I Threshold", "LRA", "LRA Threshold", "LRA Low", "LRA High")
+
+    def loudness_stats(self, x: torch.Tensor, sample_rate: float, padded_length: Optional[int] = None,
+                       want_series: bool = False):
+        """EBU R128 statistics of ``x`` [B, C, T] with the K-weighting and 0.4 s blocks of ``lufs``
+        (``b2a_loudness_stats_f32``): a dict of [B] float32 tensors under the keys of ``LOUDNESS_STATS``, plus
+        ``momentary`` [B, nblk] and ``short_term`` [B, n_st] (LUFS) when ``want_series``."""
+        x = self._prep(x, "x")
+        assert x.ndim == 3, "x must be [B, C, T]"
+        B, C, T = x.shape
+        Tp = T if padded_length is None else int(padded_length)
+        if C > len(kweighting.CHANNEL_GAINS):
+            raise ValueError(f"loudness supports at most 5 channels, got {C}")
+        sos, sgain = kweighting.design(float(sample_rate))
+        G = np.ascontiguousarray(kweighting.CHANNEL_GAINS[:C], dtype=np.float64)
+        L = self.lib
+        nblk = L.b2a_lufs_num_blocks(Tp, float(sample_rate), 0.4)
+        n_st = L.b2a_loudness_stats_num_short_term(Tp, float(sample_rate))
+        ws_bytes = L.b2a_loudness_stats_workspace_bytes(B, C, Tp, float(sample_rate))
+        if nblk < 1 or n_st < 0 or ws_bytes == 0:
+            raise _lib.B2AError(f"loudness_stats: unsupported geometry (T={Tp}, rate={sample_rate})")
+        dev = x.device
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        stats = torch.empty(B, 6, dtype=torch.float32, device=dev)
+        mom = torch.empty(B, nblk, dtype=torch.float32, device=dev) if want_series else None
+        st = torch.empty(B, n_st, dtype=torch.float32, device=dev) if want_series else None
+        dp = ctypes.POINTER(ctypes.c_double)
+        rc = L.b2a_loudness_stats_f32(_dptr(x), B, C, T, Tp, float(sample_rate),
+                                      sos.ctypes.data_as(dp), sgain.ctypes.data_as(dp), sos.shape[0],
+                                      G.ctypes.data_as(dp), _dptr(stats), _dptr(mom), _dptr(st), _dptr(ws), ws_bytes,
+                                      self._stream(x))
+        L.check(rc)
+        self.launches += 3  # kweight_energy, lufs_gate, loudness_stats (+ one memset node)
+        out = dict(zip(self.LOUDNESS_STATS, stats.unbind(1)))
+        if want_series:
+            out["momentary"], out["short_term"] = mom, st
+        return out
+
     def gain(self, x: torch.Tensor, gain: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``x[b] * gain[b]`` (ref:audiotools/core/effects.py:219,237)."""
         x = self._prep(x, "x")

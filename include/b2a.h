@@ -287,6 +287,27 @@ int b2a_lufs_f32(const float* x, int64_t B, int C, int64_t T, int64_t T_padded, 
                  const float* target_db, int n_target, float* gain_out,
                  void* ws, size_t ws_bytes, void* stream);
 
+/* ---- EBU R128 loudness statistics ------------------------------------------------------
+ * The six numbers of audiotools/core/ffmpeg.py:13-62 (r128stats) for every item, in one
+ * K-weighting pass of the GPU instead of one ffmpeg process per item.  BS.1770 arithmetic of
+ * b2a_lufs_f32 (block 0.4 s), not ffmpeg's quantised gating histogram.  Arguments as b2a_lufs_f32.
+ *   stats_out [B, 6] float32: I (== b2a_lufs_f32's lufs_out, -inf for silence), I Threshold (the
+ *            relative gate, -inf when no block passes -70), LRA, LRA Threshold, LRA Low, LRA High
+ *   momentary_out nullable [B, nblk]: -0.691 + 10 log10(sum_c G_c z_c) per 400 ms block
+ *   short_term_out nullable [B, n_st]: 3 s short-term loudness S_i over strides i .. i+29,
+ *            n_st = (T_padded - 30 stride) / stride + 1 (0 when T_padded < 30 stride)
+ *   LRA fields from S: absolute gate S > -70, LRA Threshold = power mean of those - 20 LU,
+ *   relative gate S > LRA Threshold, nearest-rank 10 % / 95 % percentiles (Low / High) of the
+ *   kept S, LRA = High - Low; LRA = 0 and the other three -inf when no S passes -70.
+ *   ws: b2a_loudness_stats_workspace_bytes(...) bytes of scratch, contents irrelevant on entry.
+ */
+int64_t b2a_loudness_stats_num_short_term(int64_t T_padded, double rate);
+size_t b2a_loudness_stats_workspace_bytes(int64_t B, int C, int64_t T_padded, double rate);
+int b2a_loudness_stats_f32(const float* x, int64_t B, int C, int64_t T, int64_t T_padded, double rate,
+                           const double* sos_h, const double* stage_gain_h, int n_stage,
+                           const double* chan_gain_h, float* stats_out, float* momentary_out,
+                           float* short_term_out, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- per-item gain ---------------------------------------------------------------------
  * x[b, :, :] * gain[b]  (EffectMixin.normalize / volume_change, effects.py:219,237).
  * out may alias x.  per_item = C*T. */
