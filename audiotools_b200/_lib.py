@@ -21,12 +21,13 @@ SIGNATURES = {
     "b2a_version": (c_int, []),
     "b2a_last_error": (c_char_p, []),
     "b2a_stft_num_frames": (c_int64, [c_int64, c_int, c_int, c_int, c_int, c_int]),
-    "b2a_spectral_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p,
+    "b2a_spectral_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
+    "b2a_spectral_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p,
                                  c_int, c_int, c_int, c_int,
                                  c_void_p, c_int, c_void_p,
                                  c_void_p, c_void_p, c_void_p, c_int, c_int,
                                  c_int, c_float, c_float,
-                                 c_void_p, c_void_p, c_void_p]),
+                                 c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "b2a_lufs_num_blocks": (c_int64, [c_int64, c_double, c_double]),
     "b2a_lufs_workspace_bytes": (c_size_t, [c_int64, c_int, c_int64, c_double, c_double]),
     "b2a_lufs_f32": (c_int, [c_void_p, c_int64, c_int, c_int64, c_int64, c_double,
@@ -79,17 +80,11 @@ SIGNATURES = {
     "b2a_alter_drr_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_float, c_void_p]),
     "b2a_dft_matrix_floats": (c_size_t, [c_int, c_int]),
     "b2a_dft_matrix_f32": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
-    "b2a_stft_dense_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int,
-                                   c_void_p, c_void_p]),
-    "b2a_mel_from_stft_f32": (c_int, [c_void_p, c_int64, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                      c_float, c_float, c_void_p, c_void_p]),
     "b2a_mel_dct_f32": (c_int, [c_void_p, c_int64, c_int, c_int64, c_void_p, c_int, c_void_p, c_void_p]),
     "b2a_stft_route": (c_int, [c_int, c_int, c_int]),
     "b2a_istft_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_int]),
     "b2a_istft_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_int, c_int64, c_int64,
                               c_void_p, c_void_p, c_size_t, c_void_p]),
-    "b2a_stft_large_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int,
-                                   c_void_p, c_void_p]),
     "b2a_stft_backward_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_int, c_int, c_int, c_int]),
     "b2a_stft_backward_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                       c_int, c_void_p, c_void_p, c_size_t, c_void_p]),

@@ -367,8 +367,8 @@ extern "C" int b2a_dft_matrix_f32(const float* window, int n_fft, int inverse, f
 
 static int launch_forward(FwdParams& p, int64_t rows, void* stream);
 
-extern "C" int b2a_stft_dense_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* matrix,
-                                  int pad, int right_pad, int pad_mode, int drop_edge, float* stft_out, void* stream) {
+int b2a::dft::stft(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* matrix, int pad,
+                   int right_pad, int pad_mode, int drop_edge, float* stft_out, void* stream) {
   B2A_REQUIRE(x && matrix && stft_out, B2A_E_INVALID, "stft_dense: null pointer");
   B2A_REQUIRE(rows >= 1 && T >= 1, B2A_E_INVALID, "stft_dense: empty input");
   B2A_REQUIRE(T < (int64_t)1 << 30, B2A_E_UNSUPPORTED, "stft_dense: rows longer than 2^30 samples");
@@ -407,9 +407,9 @@ int b2a::dft::forward_raw(const float* x, int64_t rows, int64_t T, int n_fft, in
   return launch_forward(p, rows, stream);
 }
 
-extern "C" int b2a_mel_from_stft_f32(const float* stft, int64_t rows, int F, int64_t n_frames, const float* mel_fb,
-                                     const int32_t* mel_lo, const int32_t* mel_hi, int n_mels, int post, float post_eps,
-                                     float post_power, float* mel_out, void* stream) {
+int b2a::dft::mel_from_stft(const float* stft, int64_t rows, int F, int64_t n_frames, const float* mel_fb,
+                            const int32_t* mel_lo, const int32_t* mel_hi, int n_mels, int post, float post_eps,
+                            float post_power, float* mel_out, void* stream) {
   B2A_REQUIRE(stft && mel_fb && mel_lo && mel_hi && mel_out, B2A_E_INVALID, "mel_from_stft: null pointer");
   B2A_REQUIRE(rows >= 1 && rows <= 65535 && F >= 1 && n_frames >= 1 && n_mels >= 1, B2A_E_INVALID,
               "mel_from_stft: bad shape");

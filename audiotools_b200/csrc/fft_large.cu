@@ -244,8 +244,8 @@ static bool supported(int n_fft, int hop, int inverse) {
 
 static int launch_fwd_any(const FwdParams& p, int64_t rows, int n_fft, void* stream);
 
-extern "C" int b2a_stft_large_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window,
-                                  int pad, int right_pad, int pad_mode, int drop_edge, float* stft_out, void* stream) {
+int b2a::large::stft(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window, int pad,
+                     int right_pad, int pad_mode, int drop_edge, float* stft_out, void* stream) {
   B2A_REQUIRE(x && window && stft_out, B2A_E_INVALID, "stft_large: null pointer");
   B2A_REQUIRE(rows >= 1 && T >= 1, B2A_E_INVALID, "stft_large: empty input");
   B2A_REQUIRE(T < (int64_t)1 << 30, B2A_E_UNSUPPORTED, "stft_large: rows longer than 2^30 samples");

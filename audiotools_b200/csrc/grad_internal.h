@@ -1,5 +1,6 @@
-// grad_internal.h -- the pieces of the STFT / inverse STFT kernels that other translation units reuse: the inverse
-// routes of b2a_istft_f32 (istft.cu) and the backward passes (grad.cu).
+// grad_internal.h -- the pieces of the STFT / inverse STFT kernels that other translation units reuse: the forward
+// routes of b2a_spectral_f32 (spectral.cu), the inverse routes of b2a_istft_f32 (istft.cu) and the backward passes
+// (grad.cu).
 #pragma once
 #include "b2a_common.h"
 
@@ -12,6 +13,9 @@ int run(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, c
 }  // namespace istft
 
 namespace large {
+// The STFT of b2a_spectral_f32 on B2A_ROUTE_LARGE (its framing arguments) -> stft_out [rows, n_fft/2+1, n_frames].
+int stft(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window, int pad, int right_pad,
+         int pad_mode, int drop_edge, float* stft_out, void* stream);
 // b2a_istft_f32 on B2A_ROUTE_LARGE: inverse_frames into ws (rows * n_frames * n_fft floats), then dft.cu's fold.
 int istft(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window, int pad_frames,
           int64_t start, int64_t out_len, float* out, void* ws, size_t ws_bytes, void* stream);
@@ -24,6 +28,13 @@ int forward_raw(const float* x, int64_t rows, int64_t T, int n_fft, int hop, con
 }  // namespace large
 
 namespace dft {
+// The STFT of b2a_spectral_f32 on B2A_ROUTE_DENSE, with the kind 0 matrix instead of the window.
+int stft(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* matrix, int pad, int right_pad,
+         int pad_mode, int drop_edge, float* stft_out, void* stream);
+// |X| -> banded mel -> post-op of a materialised STFT [rows, F, n_frames] (b2a_spectral_f32's mel arguments).
+int mel_from_stft(const float* stft, int64_t rows, int F, int64_t n_frames, const float* mel_fb, const int32_t* mel_lo,
+                  const int32_t* mel_hi, int n_mels, int post, float post_eps, float post_power, float* mel_out,
+                  void* stream);
 // b2a_istft_f32 on B2A_ROUTE_DENSE (also runs n_fft 32 and 4096): inverse_frames with the kind 1 matrix into ws, then
 // the fold.
 int istft(const float* spec, int64_t rows, int64_t n_frames, int n_fft, int hop, const float* window,

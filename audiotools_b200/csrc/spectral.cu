@@ -26,6 +26,7 @@
 //      memory -> coalesced store along the frame axis.
 #include "b2a_common.h"
 #include "fft_warp.cuh"
+#include "grad_internal.h"
 #include "spectral_internal.h"
 
 namespace b2a {
@@ -770,11 +771,12 @@ extern "C" int b2a_stft_route(int n_fft, int hop, int inverse) {
   return n_fft <= 8192 ? B2A_ROUTE_DENSE : B2A_ROUTE_NONE;
 }
 
-extern "C" int b2a_spectral_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window,
-                                int pad, int right_pad, int pad_mode, int drop_edge, const float* gain,
-                                int rows_per_gain, float* y_out, const float* mel_fb, const int32_t* mel_lo,
-                                const int32_t* mel_hi, int n_mels, int mel_packed_len, int post, float post_eps,
-                                float post_power, float* mel_out, float* stft_out, void* stream) {
+// b2a_spectral_f32 on B2A_ROUTE_FFT: everything in one launch of the fused kernel.
+static int spectral_fft(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window, int pad,
+                        int right_pad, int pad_mode, int drop_edge, const float* gain, int rows_per_gain, float* y_out,
+                        const float* mel_fb, const int32_t* mel_lo, const int32_t* mel_hi, int n_mels,
+                        int mel_packed_len, int post, float post_eps, float post_power, float* mel_out,
+                        float* stft_out, void* stream) {
   using namespace b2a::spectral;
   B2A_REQUIRE(x && window, B2A_E_INVALID, "spectral: null x/window");
   B2A_REQUIRE(mel_out || stft_out, B2A_E_INVALID, "spectral: neither mel_out nor stft_out requested");
@@ -812,6 +814,77 @@ extern "C" int b2a_spectral_f32(const float* x, int64_t rows, int64_t T, int n_f
     case 4096: return launch<11>(p, stream);  // 64 lanes per frame: CTA-cooperative kernel
   }
   return b2a::fail(B2A_E_UNSUPPORTED, "spectral: n_fft %d", n_fft);
+}
+
+extern "C" size_t b2a_spectral_workspace_bytes(int64_t rows, int64_t T, int n_fft, int hop, int pad, int right_pad,
+                                                int drop_edge, int stft_scratch, int scaled_scratch) {
+  const int r = b2a_stft_route(n_fft, hop, 0);
+  const int64_t nfr = b2a_stft_num_frames(T, n_fft, hop, pad, right_pad, drop_edge);
+  if (rows < 1 || nfr < 1 || r == B2A_ROUTE_NONE || r == B2A_ROUTE_FFT) return 0;
+  size_t bytes = 0;
+  if (stft_scratch) bytes += (size_t)rows * (size_t)(n_fft / 2 + 1) * (size_t)nfr * 2 * sizeof(float);
+  if (scaled_scratch) bytes += (size_t)rows * (size_t)T * sizeof(float);
+  return bytes;
+}
+
+// b2a_spectral_f32 on B2A_ROUTE_LARGE / DENSE: the gain pass, the STFT of all frames, then the mel from that STFT.
+// The outputs the caller did not ask for go to ws: the STFT at its start, the scaled signal after it.
+static int spectral_materialised(int route, const float* x, int64_t rows, int64_t T, int n_fft, int hop,
+                                 const float* window, const float* matrix, int pad, int right_pad, int pad_mode,
+                                 int drop_edge, const float* gain, int rows_per_gain, float* y_out,
+                                 const float* mel_fb, const int32_t* mel_lo, const int32_t* mel_hi, int n_mels,
+                                 int post, float post_eps, float post_power, float* mel_out, float* stft_out,
+                                 void* ws, size_t ws_bytes, void* stream) {
+  B2A_REQUIRE(mel_out || stft_out, B2A_E_INVALID, "spectral: neither mel_out nor stft_out requested");
+  // the framing is checked before the gain pass, with the message the STFT's own check gives
+  int64_t nfr;
+  int rc = b2a::spectral::check_framing(route == B2A_ROUTE_LARGE ? "stft_large" : "stft_dense", T, n_fft, hop, pad,
+                                        right_pad, pad_mode, drop_edge, &nfr);
+  if (rc != B2A_OK) return rc;
+  const size_t need = b2a_spectral_workspace_bytes(rows, T, n_fft, hop, pad, right_pad, drop_edge, !stft_out,
+                                                   gain && !y_out);
+  B2A_REQUIRE(ws_bytes >= need && (ws || need == 0), B2A_E_INVALID, "spectral: workspace too small");
+  B2A_REQUIRE(((uintptr_t)ws & 7) == 0, B2A_E_INVALID, "spectral: workspace must be 8-byte aligned");
+  const int F = n_fft / 2 + 1;
+  char* scratch = static_cast<char*>(ws);
+  float* stft = stft_out;
+  if (!stft) {
+    stft = reinterpret_cast<float*>(scratch);
+    scratch += (size_t)rows * F * (size_t)nfr * 2 * sizeof(float);
+  }
+  if (gain) {
+    B2A_REQUIRE(rows_per_gain >= 1 && rows % rows_per_gain == 0, B2A_E_INVALID, "spectral: rows_per_gain");
+    float* scaled = y_out ? y_out : reinterpret_cast<float*>(scratch);
+    rc = b2a_gain_f32(x, scaled, rows / rows_per_gain, rows_per_gain * T, gain, stream);
+    if (rc != B2A_OK) return rc;
+    x = scaled;
+  }
+  rc = route == B2A_ROUTE_LARGE
+           ? b2a::large::stft(x, rows, T, n_fft, hop, window, pad, right_pad, pad_mode, drop_edge, stft, stream)
+           : b2a::dft::stft(x, rows, T, n_fft, hop, matrix, pad, right_pad, pad_mode, drop_edge, stft, stream);
+  if (rc != B2A_OK || !mel_out) return rc;
+  return b2a::dft::mel_from_stft(stft, rows, F, nfr, mel_fb, mel_lo, mel_hi, n_mels, post, post_eps, post_power,
+                                 mel_out, stream);
+}
+
+extern "C" int b2a_spectral_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window,
+                                const float* matrix, int pad, int right_pad, int pad_mode, int drop_edge,
+                                const float* gain, int rows_per_gain, float* y_out, const float* mel_fb,
+                                const int32_t* mel_lo, const int32_t* mel_hi, int n_mels, int mel_packed_len, int post,
+                                float post_eps, float post_power, float* mel_out, float* stft_out, void* ws,
+                                size_t ws_bytes, void* stream) {
+  const int route = b2a_stft_route(n_fft, hop, 0);
+  if (route == B2A_ROUTE_FFT)
+    return spectral_fft(x, rows, T, n_fft, hop, window, pad, right_pad, pad_mode, drop_edge, gain, rows_per_gain, y_out,
+                        mel_fb, mel_lo, mel_hi, n_mels, mel_packed_len, post, post_eps, post_power, mel_out, stft_out,
+                        stream);
+  if (route == B2A_ROUTE_LARGE || route == B2A_ROUTE_DENSE)
+    return spectral_materialised(route, x, rows, T, n_fft, hop, window, matrix, pad, right_pad, pad_mode, drop_edge,
+                                 gain, rows_per_gain, y_out, mel_fb, mel_lo, mel_hi, n_mels, post, post_eps, post_power,
+                                 mel_out, stft_out, ws, ws_bytes, stream);
+  return b2a::fail(B2A_E_UNSUPPORTED,
+                   "spectral: n_fft=%d hop=%d (hop >= 1; powers of two up to 32768, any other length up to 8192)",
+                   n_fft, hop);
 }
 
 extern "C" int b2a_spectral_tc_enable(int on) {

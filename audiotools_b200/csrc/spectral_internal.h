@@ -90,7 +90,7 @@ __device__ __forceinline__ float mel_band(const float* fb, const int32_t* mel_lo
 
 // torch's stft(center=True) framing of the explicitly padded signal (F.pad(pad, pad + right_pad, pad_mode), then the
 // centre reflect), shared by every STFT entry point: B2A_OK and the frame count, or the error code with the message
-// prefixed by `who`.  Which entry point runs a window length is b2a_stft_route (include/b2a.h), defined beside it.
+// prefixed by `who`.  Which kernel family runs a window length is b2a_stft_route (include/b2a.h), defined beside it.
 int check_framing(const char* who, int64_t T, int n_fft, int hop, int pad, int right_pad, int pad_mode, int drop_edge,
                   int64_t* n_frames);
 

@@ -807,7 +807,8 @@ class Engine:
                  mel_fb: Optional[torch.Tensor] = None, mel_lo: Optional[torch.Tensor] = None,
                  mel_hi: Optional[torch.Tensor] = None, post: int = _lib.POST_NONE, post_eps: float = 0.0,
                  post_power: float = 1.0, want_stft: bool = True):
-        """Fused framing -> window -> rFFT -> (|.| -> banded mel -> post) over ``x`` [B, C, T].
+        """Framing -> window -> rFFT -> (|.| -> banded mel -> post) over ``x`` [B, C, T], one ``b2a_spectral_f32`` call:
+        one fused launch on the FFT route, gain pass + STFT + mel launches on the LARGE / DENSE routes.
 
         Returns dict(stft=[B,C,F,N] complex64 | None, mel=[B,C,n_mels,N] | None, scaled=[B,C,T] | None).
         """
@@ -825,10 +826,9 @@ class Engine:
         F = n_fft // 2 + 1
         dev = x.device
         route = self.route(n_fft, hop, 0)
-        if route != _lib.ROUTE_FFT:
-            return self._spectral_materialised(x, int(n_fft), int(hop), route, window, pad, right_pad, pad_mode,
-                                               drop_edge, gain, want_scaled, mel_fb, mel_lo, mel_hi, post, post_eps,
-                                               post_power, want_stft, N)
+        if route == _lib.ROUTE_NONE:
+            raise self.route_error(n_fft, hop, 0)
+        fft = route == _lib.ROUTE_FFT
         stft = torch.empty(B, C, F, N, dtype=torch.complex64, device=dev) if want_stft else None
         mel = None
         n_mels = 0
@@ -840,7 +840,8 @@ class Engine:
             mel_lo = self._prep(mel_lo, "mel_lo", torch.int32)
             mel_hi = self._prep(mel_hi, "mel_hi", torch.int32)
             mel = torch.empty(B, C, n_mels, N, dtype=torch.float32, device=dev)
-            packed_len = self._packed_len(mel_lo, mel_hi, n_fft)
+            if fft:
+                packed_len = self._packed_len(mel_lo, mel_hi, n_fft)
         scaled = None
         rows_per_gain = 1
         if gain is not None:
@@ -849,57 +850,21 @@ class Engine:
             rows_per_gain = C
             if want_scaled:
                 scaled = torch.empty_like(x)
+        mat = self.dft_matrix(window, int(n_fft), inverse=0) if route == _lib.ROUTE_DENSE else None
+        # LARGE / DENSE: the STFT and the scaled signal go to a workspace when the caller does not keep them
+        nbytes = 0 if fft else int(self.lib.b2a_spectral_workspace_bytes(
+            rows, T, n_fft, hop, pad, right_pad, drop_edge, stft is None, gain is not None and scaled is None))
+        ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=dev) if nbytes else None
         rc = self.lib.b2a_spectral_f32(
-            _dptr(x), rows, T, n_fft, hop, _dptr(window), pad, right_pad, _lib.PAD_MODES[pad_mode], drop_edge,
-            _dptr(gain), rows_per_gain, _dptr(scaled),
+            _dptr(x), rows, T, n_fft, hop, _dptr(window), _dptr(mat), pad, right_pad, _lib.PAD_MODES[pad_mode],
+            drop_edge, _dptr(gain), rows_per_gain, _dptr(scaled),
             _dptr(mel_fb), _dptr(mel_lo), _dptr(mel_hi), n_mels, packed_len, post, float(post_eps),
             float(post_power),
-            _dptr(mel), _dptr(torch.view_as_real(stft)) if stft is not None else None, self._stream(x))
+            _dptr(mel), _dptr(torch.view_as_real(stft)) if stft is not None else None, _dptr(ws), nbytes,
+            self._stream(x))
         self.lib.check(rc)
-        self.launches += 1
+        self.launches += 1 if fft else 1 + (gain is not None) + (mel is not None)  # LARGE / DENSE: gain, STFT, mel
         return {"stft": stft, "mel": mel, "scaled": scaled}
-
-
-    def _spectral_materialised(self, x, n_fft, hop, route, window, pad, right_pad, pad_mode, drop_edge, gain,
-                               want_scaled, mel_fb, mel_lo, mel_hi, post, post_eps, post_power, want_stft, N):
-        """``spectral`` on the LARGE and DENSE routes: gain pass (if any) -> the STFT of all frames, materialised ->
-        optional |X| -> banded mel -> post-op from it.  The STFT is a per-frame FFT on LARGE (csrc/fft_large.cu) and one
-        dense DFT matrix product on DENSE (csrc/dft.cu)."""
-        B, C, T = x.shape
-        F = n_fft // 2 + 1
-        if route == _lib.ROUTE_NONE:
-            raise self.route_error(n_fft, hop, 0)
-        scaled = None
-        if gain is not None:
-            gain = self._prep(gain.reshape(-1), "gain")
-            assert gain.numel() == B
-            x = scaled = self.gain(x, gain)
-        stft = torch.empty(B, C, F, N, dtype=torch.complex64, device=x.device)
-        if route == _lib.ROUTE_LARGE:
-            rc = self.lib.b2a_stft_large_f32(_dptr(x), B * C, T, n_fft, hop, _dptr(window), pad, right_pad,
-                                             _lib.PAD_MODES[pad_mode], drop_edge, _dptr(torch.view_as_real(stft)),
-                                             self._stream(x))
-        else:
-            mat = self.dft_matrix(window, n_fft, inverse=False)
-            rc = self.lib.b2a_stft_dense_f32(_dptr(x), B * C, T, n_fft, hop, _dptr(mat), pad, right_pad,
-                                             _lib.PAD_MODES[pad_mode], drop_edge, _dptr(torch.view_as_real(stft)),
-                                             self._stream(x))
-        self.lib.check(rc)
-        self.launches += 1
-        mel = None
-        if mel_fb is not None:
-            mel_fb = self._prep(mel_fb, "mel_fb")
-            assert mel_fb.shape[1] == F, (mel_fb.shape, F)
-            n_mels = mel_fb.shape[0]
-            mel_lo = self._prep(mel_lo, "mel_lo", torch.int32)
-            mel_hi = self._prep(mel_hi, "mel_hi", torch.int32)
-            mel = torch.empty(B, C, n_mels, N, dtype=torch.float32, device=x.device)
-            rc = self.lib.b2a_mel_from_stft_f32(_dptr(torch.view_as_real(stft)), B * C, F, N, _dptr(mel_fb), _dptr(mel_lo),
-                                                _dptr(mel_hi), n_mels, post, float(post_eps), float(post_power), _dptr(mel),
-                                                self._stream(x))
-            self.lib.check(rc)
-            self.launches += 1
-        return {"stft": stft if want_stft else None, "mel": mel, "scaled": scaled if want_scaled else None}
 
     def mel_dct(self, logmel: torch.Tensor, dct: torch.Tensor) -> torch.Tensor:
         """``(logmel.transpose(-1, -2) @ dct).transpose(-1, -2)`` for logmel [B, C, n_mels, N], dct [n_mels, n_mfcc]

@@ -229,7 +229,6 @@ def main():
               "frac_of_fp32_peak": 4 * macs / ms_stft / 1e6 / 67000.0})
 
     if "largewin" in only:  # large power-of-two windows (csrc/fft_large.cu): the default 8192 window at 192 kHz
-        import ctypes
         import subprocess
 
         from audiotools_b200.engine import get_engine
@@ -248,23 +247,7 @@ def main():
         X = sig.stft_data
         ms_istft = timed(lambda: sig.istft(), steps=5)
         ms_32k = timed(lambda: AudioSignal(x, sr).stft(window_length=32768, hop_length=8192), steps=3)
-        # the dense route these sizes took before (csrc/dft.cu): the engine's matrix + product, called directly
-        w = sig.get_window("hann", 8192, x.device)
-        mat = eng.dft_matrix(w, 8192)
-        dense_out = torch.empty_like(X)
         xs = x.reshape(B * C, T)
-
-        def dense():
-            eng.lib.check(eng.lib.b2a_stft_dense_f32(ctypes.c_void_p(xs.data_ptr()), B * C, T, 8192, 2048,
-                                                     ctypes.c_void_p(mat.data_ptr()), 0, 0, 0, 0,
-                                                     ctypes.c_void_p(torch.view_as_real(dense_out).data_ptr()),
-                                                     ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
-
-        ms_dense = timed(dense, warmup=1, steps=2)
-        dense_rel = float((dense_out - X).abs().max() / X.abs().max())
-        del dense_out, mat
-        for k in [k for k in eng._packed_cache if k[0] == "dft"]:  # release the 270 MB matrix
-            del eng._packed_cache[k]
         wt = torch.hann_window(8192, periodic=True, device=dev)
         ms_torch = timed(lambda: torch.stft(xs, 8192, 2048, window=wt, center=True, return_complex=True), steps=5)
         Xr = X.reshape(B * C, 4097, -1)
@@ -278,7 +261,6 @@ def main():
         emit({"config": "largewin 64x2ch 10s@192k default window 8192 hop 2048 (stft, log-mel, istft; stft 32768)",
               "kernel": eng.spectral_kernel_name(8192, 2048, want_mel=False, want_stft=True),
               "ms_stft": ms_stft, "ms_logmel": ms_logmel, "ms_istft": ms_istft, "ms_stft_32768": ms_32k,
-              "ms_dense_dft_stft_8192": ms_dense, "dense_vs_fft_rel_err": dense_rel,
               "ms_torch_stft_cufft": ms_torch, "ms_torch_istft_cufft": ms_torch_inv,
               "clips_per_s_stft": B / ms_stft * 1e3, "alg_bytes_stft": alg, "achieved_GBps": alg / ms_stft / 1e6,
               "frac_of_hbm_peak": alg / ms_stft / 1e6 / peak, "gpu": torch.cuda.get_device_name(LOCAL),

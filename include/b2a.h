@@ -49,16 +49,23 @@ const char* b2a_last_error(void);
  * Replaces the device work of AudioSignal.stft (audiotools/core/audio_signal.py:1123-1212:
  * F.pad(pad, pad+right_pad, padding_type) -> torch.stft(center=True, reflect) -> optional
  * drop of 2+2 edge frames) and AudioSignal.mel_spectrogram (:1333-1369: |X| @ mel_basis.T),
- * fused: framing -> window -> real FFT -> |.| -> banded mel -> post-op, one pass over x.
+ * on the route b2a_stft_route(n_fft, hop, 0), with the same framing and bit-exact frame indexing on every route:
+ *   FFT           one fused pass over x: framing -> window -> real FFT -> |.| -> banded mel -> post-op.
+ *   LARGE / DENSE the gain pass (b2a_gain_f32) if gain != NULL, the STFT of all frames (fft_large.cu's per-frame FFT /
+ *                 dft.cu's dense DFT), then |X| -> banded mel -> post-op from that STFT if mel_out != NULL: up to
+ *                 3 launches (the gain pass takes rows / rows_per_gain <= 65535, the mel pass rows <= 65535).
+ *                 The STFT and the scaled signal go to ws when the caller does not ask for them.
  *
  *   x        [rows, T]
  *   window   [n_fft]              (AudioSignal.get_window, :1009-1039)
- *   n_fft    power of two in [32, 4096] (b2a_stft_route's B2A_ROUTE_FFT); hop >= 1
+ *   matrix   nullable; on DENSE the kind 0 matrix of b2a_dft_matrix_f32
+ *   n_fft/hop                     any pair whose forward route is not B2A_ROUTE_NONE
  *   pad/right_pad/pad_mode        compute_stft_padding (:1089-1121); 0/0 when !match_stride
  *   drop_edge                     frames dropped at each end (2 when match_stride, else 0)
  *   gain     nullable [rows/rows_per_gain]: x is multiplied by gain[row / rows_per_gain] first
  *            (EffectMixin.normalize's x*gain, effects.py:219) and, if y_out != NULL, the scaled
- *            waveform is written there ([rows, T]) by the same pass.
+ *            waveform is written there ([rows, T]); on FFT by the same pass, which needs pad == right_pad ==
+ *            drop_edge == 0 for y_out.  On LARGE / DENSE rows_per_gain divides rows.
  *   mel_fb   nullable [n_mels, F] row-major dense filterbank (get_mel_filters, :1298-1331);
  *   mel_lo/mel_hi  [n_mels] int32: mel_fb[m, k] == 0 outside mel_lo[m] <= k < mel_hi[m]
  *            (the caller derives them from the actual non-zeros, so the banded sum equals the
@@ -67,24 +74,32 @@ const char* b2a_last_error(void);
  *            with n4[m] = (ceil4(mel_hi[m]) - floor4(mel_lo[m]))/4, 4 * sum over filters m of
  *            even(max(n4[m'] : m' in {4g .. 4g + 3})) where g = m / 4, even(v) = (v+1) & ~1
  *            (the 4 consecutive filters one warp projects in one step share a trip count; the loop is unrolled by two).
- *   mel_out  nullable [rows, n_mels, n_frames]    stft_out  nullable [rows, F, n_frames] (re,im)
+ *            Used on FFT only.
+ *   mel_out  nullable [rows, n_mels, n_frames]    stft_out  nullable [rows, F, n_frames] (re,im); at least one of them
  *   n_frames = 1 + (T + 2*pad + right_pad)/hop - 2*drop_edge,  F = n_fft/2 + 1
+ *   ws       b2a_spectral_workspace_bytes(..., stft_out == NULL, gain != NULL && y_out == NULL) bytes, 8-byte aligned:
+ *            the STFT when stft_out is NULL, then the scaled signal when y_out is NULL.  0 on FFT, where ws may be NULL.
  */
 int64_t b2a_stft_num_frames(int64_t T, int n_fft, int hop, int pad, int right_pad, int drop_edge);
+size_t b2a_spectral_workspace_bytes(int64_t rows, int64_t T, int n_fft, int hop, int pad, int right_pad, int drop_edge,
+                                    int stft_scratch, int scaled_scratch);
 int b2a_spectral_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window,
-                     int pad, int right_pad, int pad_mode, int drop_edge,
+                     const float* matrix, int pad, int right_pad, int pad_mode, int drop_edge,
                      const float* gain, int rows_per_gain, float* y_out,
                      const float* mel_fb, const int32_t* mel_lo, const int32_t* mel_hi, int n_mels,
                      int mel_packed_len, int post, float post_eps, float post_power,
-                     float* mel_out, float* stft_out, void* stream);
+                     float* mel_out, float* stft_out, void* ws, size_t ws_bytes, void* stream);
 
 /* ---- the one route table: which kernel family runs an STFT of (n_fft, hop) -------------------------------------
- * inverse 0: the forward STFT (b2a_spectral_f32 / b2a_stft_large_f32 / b2a_stft_dense_f32).  inverse 1: b2a_istft_f32
- * and both backward passes, which route by it themselves.  Everything not in the table is B2A_ROUTE_NONE.
+ * inverse 0: the forward STFT, b2a_spectral_f32.  inverse 1: b2a_istft_f32 and both backward passes.  Each of these
+ * routes by the table itself.  Everything not in the table is B2A_ROUTE_NONE.
  *                      FFT                          LARGE                          DENSE
  *   inverse 0, hop>=1  power of two in [32, 4096]   power of two in [8192, 32768]  any other length in [2, 8192]
  *   inverse 1, hop in  power of two in [64, 2048]   power of two in [4096, 32768]  any other length in [2, 8192]
- *   [1, n_fft]                                                                     (incl. 32) */
+ *   [1, n_fft]                                                                     (incl. 32)
+ * LARGE serves the default window of AudioSignal.stft_params, 2^ceil(log2(0.032 sr)), at high rates: 8192 at 176.4 /
+ * 192 kHz (and the inverse of 4096 at 88.2 / 96 kHz); 16384 / 32768 serve fine frequency resolution.  It needs no
+ * matrix and no table. */
 #define B2A_ROUTE_NONE 0  /* not supported                                     */
 #define B2A_ROUTE_FFT 1   /* spectral.cu (forward) / istft.cu (inverse)        */
 #define B2A_ROUTE_LARGE 2 /* fft_large.cu                                      */
@@ -113,33 +128,16 @@ int b2a_istft_f32(const float* spec, int64_t rows, int64_t n_frames, int n_fft, 
  * torch.istft), e.g. 400 / 480 / 1200-sample speech windows (B2A_ROUTE_DENSE).  Their STFT is ONE real x complex
  * matrix product over all frames of the batch (FP32 FMA):
  *   b2a_dft_matrix_f32     builds the matrix of (n_fft, window) once: inverse 0 -> M[n][k] = w[n] exp(-2 pi i nk/n_fft)
- *                          for b2a_stft_dense_f32, inverse 1 -> c_k/n_fft . w[n] exp(-2 pi i nk/n_fft) (c = 1 for DC and
+ *                          for b2a_spectral_f32, inverse 1 -> c_k/n_fft . w[n] exp(-2 pi i nk/n_fft) (c = 1 for DC and
  *                          Nyquist, else 2) for b2a_istft_f32, inverse 2 -> the layout of 1 with weight 1 on every
  *                          bin for b2a_stft_backward_f32; `matrix`: b2a_dft_matrix_floats(n_fft, inverse)
- *                          floats, 16-byte aligned; angles reduced in integers (nk mod n_fft), evaluated in float64
- *   b2a_stft_dense_f32     the arguments of b2a_spectral_f32 (same framing / padding semantics, bit-exact frame
- *                          indexing) -> stft_out [rows, n_fft/2+1, n_frames] (re,im)
- *   b2a_mel_from_stft_f32  |X| -> banded mel -> post-op from a materialised STFT (AudioSignal.mel_spectrogram :1333-1369
- *                          for the LARGE and DENSE routes; the FFT kernel fuses it) */
+ *                          floats, 16-byte aligned; angles reduced in integers (nk mod n_fft), evaluated in float64 */
 size_t b2a_dft_matrix_floats(int n_fft, int inverse);
 int b2a_dft_matrix_f32(const float* window, int n_fft, int inverse, float* matrix, void* stream);
-int b2a_stft_dense_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* matrix,
-                       int pad, int right_pad, int pad_mode, int drop_edge, float* stft_out, void* stream);
-int b2a_mel_from_stft_f32(const float* stft, int64_t rows, int F, int64_t n_frames, const float* mel_fb,
-                          const int32_t* mel_lo, const int32_t* mel_hi, int n_mels, int post, float post_eps,
-                          float post_power, float* mel_out, void* stream);
 /* AudioSignal.mfcc's `log-mel^T @ create_dct(n_mfcc, n_mels, "ortho")` (audio_signal.py:1420-1426):
  * out[row][j][n] = sum_m dct[m][j] * logmel[row][m][n];  logmel [rows, n_mels, n_frames], dct [n_mels, n_mfcc] row-major. */
 int b2a_mel_dct_f32(const float* logmel, int64_t rows, int n_mels, int64_t n_frames, const float* dct, int n_mfcc,
                     float* out, void* stream);
-
-/* ---- STFT for LARGE power-of-two windows (FFT, one CTA per frame, csrc/fft_large.cu) ---------------------------
- * B2A_ROUTE_LARGE: the default window of AudioSignal.stft_params is 2^ceil(log2(0.032 sr)) = 4096 at 88.2 / 96 kHz and
- * 8192 at 176.4 / 192 kHz; 16384 / 32768 serve fine frequency resolution.  FP32; no matrix, no table to build.
- *   b2a_stft_large_f32         the arguments of b2a_stft_dense_f32 with the window instead of the matrix (same framing /
- *                              padding semantics, bit-exact frame indexing) -> stft_out [rows, n_fft/2+1, n_frames] */
-int b2a_stft_large_f32(const float* x, int64_t rows, int64_t T, int n_fft, int hop, const float* window, int pad,
-                       int right_pad, int pad_mode, int drop_edge, float* stft_out, void* stream);
 
 /* ---- backward passes of the spectral front end (csrc/grad.cu) ---------------------------------------------------
  * Gradients of AudioSignal.stft / istft / mel_spectrogram / mfcc (audiotools/core/audio_signal.py:1123-1296, 1333-1426;
@@ -147,8 +145,8 @@ int b2a_stft_large_f32(const float* x, int64_t rows, int64_t T, int n_fft, int h
  * convention); every pass is deterministic (no atomics, fixed summation order).  Both backward passes exist where
  * b2a_stft_route(n_fft, hop, 1) is not B2A_ROUTE_NONE, and run on that route.
  *   b2a_stft_backward_f32        grad_spec [rows, n_fft/2+1, n_frames] (re,im) -> grad_x [rows, T], for the STFT that
- *                                b2a_spectral_f32 / b2a_stft_dense_f32 / b2a_stft_large_f32 computed with the same
- *                                (T, n_fft, hop, window, pad, right_pad, pad_mode, drop_edge): per frame
+ *                                b2a_spectral_f32 computed with the same (T, n_fft, hop, window, pad, right_pad,
+ *                                pad_mode, drop_edge) and no gain: per frame
  *                                w[n] sum_k Re(G_k e^{2 pi i kn/n_fft}), overlap-added without envelope division over the
  *                                padded range, folded back through both paddings (each padded position's gradient is
  *                                added to the sample it was read from).  amatrix: the kind 2 matrix of b2a_dft_matrix_f32,

@@ -50,22 +50,51 @@ def test_version_and_pure_host_queries(lib):
 
 def test_bad_arguments_return_codes_not_crashes(lib):
     # null pointers / unsupported sizes are rejected before any CUDA call is made
-    rc = lib.b2a_spectral_f32(None, 1, 100, 512, 128, None, 0, 0, 0, 0, None, 1, None, None, None, None, 0, 0, 0, 0.0,
-                              1.0, None, None, None)
+    rc = lib.b2a_spectral_f32(None, 1, 100, 512, 128, None, None, 0, 0, 0, 0, None, 1, None, None, None, None, 0, 0, 0,
+                              0.0, 1.0, None, None, None, 0, None)
     assert rc == -1 and b"null" in lib.b2a_last_error()
     buf = (ctypes.c_float * 1024)()
     p = ctypes.cast(buf, ctypes.c_void_p)
-    rc = lib.b2a_spectral_f32(p, 1, 1024, 500, 128, p, 0, 0, 0, 0, None, 1, None, None, None, None, 0, 0, 0, 0.0, 1.0,
-                              None, p, None)
-    assert rc == -2 and b"power of two" in lib.b2a_last_error()
-    rc = lib.b2a_spectral_f32(p, 1, 100, 512, 128, p, 0, 0, 0, 0, None, 1, None, None, None, None, 0, 0, 0, 0.0, 1.0,
-                              None, p, None)
+    for n_fft, hop in ((65536, 128), (512, 0)):  # no forward route: a power of two above 32768; hop < 1
+        rc = lib.b2a_spectral_f32(p, 1, 1024, n_fft, hop, p, None, 0, 0, 0, 0, None, 1, None, None, None, None, 0, 0, 0,
+                                  0.0, 1.0, None, p, None, 0, None)
+        assert rc == -2 and f"spectral: n_fft={n_fft} hop={hop}".encode() in lib.b2a_last_error()
+    rc = lib.b2a_spectral_f32(p, 1, 100, 512, 128, p, None, 0, 0, 0, 0, None, 1, None, None, None, None, 0, 0, 0, 0.0,
+                              1.0, None, p, None, 0, None)
     assert rc == -1 and b"n_fft/2" in lib.b2a_last_error()
     with pytest.raises(_lib.B2AError):
         lib.check(rc)
+    # LARGE / DENSE: the checks of the gain + STFT + mel sequence come before its first launch
+    for n_fft, hop in ((8192, 2048), (500, 125)):
+        rc = lib.b2a_spectral_f32(p, 1, 20000, n_fft, hop, p, p, 0, 0, 0, 0, None, 1, None, None, None, None, 0, 0, 0,
+                                  0.0, 1.0, None, None, None, 0, None)
+        assert rc == -1 and lib.b2a_last_error() == b"spectral: neither mel_out nor stft_out requested"
+        need = lib.b2a_spectral_workspace_bytes(1, 20000, n_fft, hop, 0, 0, 0, 1, 0)
+        for ws, ws_bytes in ((None, 0), (p, need - 1)):  # the STFT under a mel-only call needs scratch
+            rc = lib.b2a_spectral_f32(p, 1, 20000, n_fft, hop, p, p, 0, 0, 0, 0, None, 1, None, p, p, p, 4, 0, 0, 0.0,
+                                      1.0, p, None, ws, ws_bytes, None)
+            assert rc == -1 and lib.b2a_last_error() == b"spectral: workspace too small"
+        rc = lib.b2a_spectral_f32(p, 3, 20000, n_fft, hop, p, p, 0, 0, 0, 0, p, 2, p, None, None, None, 0, 0, 0, 0.0,
+                                  1.0, None, p, None, 0, None)  # the gain pass scales whole items of rows_per_gain rows
+        assert rc == -1 and lib.b2a_last_error() == b"spectral: rows_per_gain"
     for n_fft, hop in ((65536, 16384), (512, 513)):  # no inverse route: a power of two above 32768; hop > n_fft
         rc = lib.b2a_istft_f32(p, 1, 4, n_fft, hop, p, None, 0, 0, 1024, p, None, 0, None)
         assert rc == -2 and f"istft: n_fft={n_fft} hop={hop}".encode() in lib.b2a_last_error()
+
+
+def test_spectral_workspace_bytes(lib):
+    # 0 where b2a_spectral_f32 needs no scratch: the FFT route, no route, no frames
+    for n_fft, hop, T in ((512, 128, 20000), (4096, 1024, 20000), (65536, 128, 20000), (512, 0, 20000), (500, 125, 0)):
+        assert [lib.b2a_spectral_workspace_bytes(3, T, n_fft, hop, 0, 0, 0, s, g) for s in (0, 1) for g in (0, 1)] == \
+            [0, 0, 0, 0], (n_fft, hop, T)
+    # LARGE / DENSE: the STFT [rows, F, n_frames] complex64 and / or the scaled signal [rows, T] float32, nothing more
+    for n_fft, hop in ((8192, 2048), (32768, 8192), (500, 125), (8191, 2047)):
+        T, pad, right_pad, drop_edge = 40000, (n_fft - hop) // 2, 37, 2
+        N = lib.b2a_stft_num_frames(T, n_fft, hop, pad, right_pad, drop_edge)
+        stft, scaled = 3 * (n_fft // 2 + 1) * N * 8, 3 * T * 4
+        got = [lib.b2a_spectral_workspace_bytes(3, T, n_fft, hop, pad, right_pad, drop_edge, s, g)
+               for s in (0, 1) for g in (0, 1)]
+        assert got == [0, scaled, stft, stft + scaled], (n_fft, hop)
 
 
 def test_spectral_tc_enable_is_a_stub(lib):
@@ -86,10 +115,16 @@ FRAMING_ENTRY_POINTS = {  # prefix of the message, n_fft, hop
 }
 FRAMING_FAILURES = {  # (T, pad, right_pad, pad_mode, drop_edge) as functions of n_fft -> (code, message)
     "negative_padding": (lambda n: (n, -1, 0, 0, 0), lambda n: (-1, "negative padding")),
+    "negative_right_pad": (lambda n: (n, 0, -1, 0, 0), lambda n: (-1, "negative padding")),
+    "negative_drop_edge": (lambda n: (n, 0, 0, 0, -1), lambda n: (-1, "negative padding")),
     "pad_mode": (lambda n: (n, 0, 0, 5, 0), lambda n: (-2, "pad mode 5")),
+    "pad_mode_3": (lambda n: (n, 0, 0, 3, 0), lambda n: (-2, "pad mode 3")),  # circular: FIR padding only
+    "pad_mode_negative": (lambda n: (n, 0, 0, -1, 0), lambda n: (-2, "pad mode -1")),
     "short_signal": (lambda n: (n // 4, 0, 0, 0, 0),
                      lambda n: (-1, f"n_fft/2 ({n // 2}) must be < padded length ({n // 4})")),
     "reflect_padding": (lambda n: (n, n, 0, 0, 0), lambda n: (-1, f"reflect padding ({n}) must be < signal length ({n})")),
+    "reflect_right_padding": (lambda n: (n, 0, n, 0, 0),
+                              lambda n: (-1, f"reflect padding ({n}) must be < signal length ({n})")),
     "no_frames": (lambda n: (n, 0, 0, 0, 100), lambda n: (-1, "no frames")),
 }
 
@@ -97,13 +132,9 @@ FRAMING_FAILURES = {  # (T, pad, right_pad, pad_mode, drop_edge) as functions of
 def _call_framed(lib, who, T, n_fft, hop, pad, right_pad, pad_mode, drop_edge):
     buf = (ctypes.c_float * 1024)()
     p = ctypes.cast(buf, ctypes.c_void_p)
-    if who == "spectral":
-        return lib.b2a_spectral_f32(p, 1, T, n_fft, hop, p, pad, right_pad, pad_mode, drop_edge, None, 1, None, None,
-                                    None, None, 0, 0, 0, 0.0, 1.0, None, p, None)
-    if who == "stft_large":
-        return lib.b2a_stft_large_f32(p, 1, T, n_fft, hop, p, pad, right_pad, pad_mode, drop_edge, p, None)
-    if who == "stft_dense":
-        return lib.b2a_stft_dense_f32(p, 1, T, n_fft, hop, p, pad, right_pad, pad_mode, drop_edge, p, None)
+    if who in ("spectral", "stft_large", "stft_dense"):  # the one forward entry point, on its three routes
+        return lib.b2a_spectral_f32(p, 1, T, n_fft, hop, p, p, pad, right_pad, pad_mode, drop_edge, None, 1, None, None,
+                                    None, None, 0, 0, 0, 0.0, 1.0, None, p, None, 0, None)
     if who == "stft_backward":
         return lib.b2a_stft_backward_f32(p, 1, T, n_fft, hop, p, None, pad, right_pad, pad_mode, drop_edge, p, p, 4096,
                                          None)

@@ -1,6 +1,7 @@
 """Large power-of-two windows (csrc/fft_large.cu: forward 8192 .. 32768, inverse 4096 .. 32768) on the CPU-simulated
 build of the kernels (tests/cusim): against the REAL reference's outputs (tests/golden/make_golden_largewindow.py) and
 against torch.stft / torch.istft semantics (oracle/signal_path.py), frame counts exactly."""
+import ctypes
 import os
 import subprocess
 import sys
@@ -170,8 +171,11 @@ def test_window_routes_and_kernel_names(eng):
         eng.istft(torch.zeros(1, 1, 32769, 4, dtype=torch.complex64), 65536, 16384, torch.ones(65536), 40000)
     with pytest.raises(NotImplementedError, match="dense DFT path"):  # not a power of two: the dense path's limit
         eng.spectral(torch.zeros(1, 1, 40000), 10000, 2500, torch.ones(10000))
-    with pytest.raises(_lib.B2AError, match="stft_large"):  # the C ABI checks its arguments itself
-        lib.check(lib.b2a_stft_large_f32(None, 1, 40000, 8192, 2048, None, 0, 0, 0, 0, None, None))
+    buf = (ctypes.c_float * 2)()  # stft_out, never written: x is null
+    out = ctypes.cast(buf, ctypes.c_void_p)
+    with pytest.raises(_lib.B2AError, match="stft_large: null pointer"):  # the C ABI checks its arguments itself
+        lib.check(lib.b2a_spectral_f32(None, 1, 40000, 8192, 2048, None, None, 0, 0, 0, 0, None, 1, None, None, None,
+                                       None, 0, 0, 0, 0.0, 1.0, None, out, None, 0, None))
 
 
 _SHUFFLED = r"""
