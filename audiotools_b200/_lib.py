@@ -128,6 +128,9 @@ SIGNATURES = {
     "b2a_stoi_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_int]),
     "b2a_stoi_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int64, c_int, c_void_p, c_int, c_int, c_int,
                              c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "b2a_stoi_backward_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_int]),
+    "b2a_stoi_backward_f32": (c_int, [c_void_p, c_void_p, c_size_t, c_int64, c_int, c_int64, c_int, c_void_p, c_int,
+                                      c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
 
 

@@ -2,7 +2,8 @@
 (ref:audiotools/core/audio_signal.py:1123-1296, 1333-1426 and effects.py:200-238, differentiable through torch there;
 ref:tests/core/test_grad.py) and of the time-domain effects (resample, equalizer, convolve, apply_ir,
 ensure_max_of_audio, mix, quantization; gradients with respect to the waveform only) and of the spectral masks and the
-spectral gate (ref:audiotools/core/dsp.py:217-334, ml/layers/spectral_gate.py:58-127; gradients to the spectrogram).  ``AudioSignal`` uses them only when grad mode is on and the input requires a gradient;
+spectral gate (ref:audiotools/core/dsp.py:217-334, ml/layers/spectral_gate.py:58-127; gradients to the spectrogram)
+and of STOI (``metrics.quality.STOILoss``; gradients to the estimates).  ``AudioSignal`` uses them only when grad mode is on and the input requires a gradient;
 otherwise it calls the engine directly, with exactly the launches it always made.
 
 Each forward is the engine call of the no-gradient path; each backward is one launch sequence of csrc/grad.cu (or an
@@ -288,6 +289,26 @@ class SpecGate(torch.autograd.Function):
     def backward(ctx, g):
         (spec,) = ctx.saved_tensors
         return _engine().spec_gate_backward(g, spec, *ctx.args), None, None, None, None, None
+
+
+class STOI(torch.autograd.Function):
+    """(estimates, references) [B, C, T] -> STOI scores [B] float64 on the device (``Engine.stoi``).  The forward keeps
+    its workspace (10 kHz signals, kept frames, band envelopes); the backward (``Engine.stoi_backward``) recomputes
+    only the estimate's frame spectra from it.  The silence mask depends on the references alone, and the references
+    are constants: no gradient flows to them."""
+
+    @staticmethod
+    def forward(ctx, est, ref, sample_rate, extended):
+        score, _, _, ws = _engine().stoi(est, ref, sample_rate, extended, return_workspace=True)
+        ctx.ws = ws
+        ctx.args = (tuple(est.shape), sample_rate, extended)
+        return score
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        shape, sample_rate, extended = ctx.args
+        return _engine().stoi_backward(g, ctx.ws, shape, sample_rate, extended), None, None, None
 
 
 def refuse_param_grad(method: str, name: str, t) -> None:

@@ -1328,10 +1328,20 @@ class Engine:
         h = np.kaiser(2 * L + 1, 0.1102 * (60.0 - 8.7)) * 2 * up * fc * np.sinc(2 * fc * t)
         return h / h.sum() * up
 
-    def stoi(self, est: torch.Tensor, ref: torch.Tensor, sample_rate: int, extended: bool = False):
+    def _stoi_taps(self, sample_rate: int, device) -> torch.Tensor:
+        key = ("stoi_taps", int(sample_rate), device)
+        taps = self._packed_cache.get(key)
+        if taps is None:
+            taps = self._packed_cache[key] = torch.from_numpy(self.stoi_taps(sample_rate)).to(device)
+        return taps
+
+    def stoi(self, est: torch.Tensor, ref: torch.Tensor, sample_rate: int, extended: bool = False,
+             return_workspace: bool = False):
         """STOI (or extended STOI) of the estimates against the clean references, both [B, C, T] (mixed to mono first)
         -> (score [B] float64, kept [B] int32 frames kept by the silence removal, short [B] bool: fewer than 30 STFT
-        frames were left and the score is 1e-5).  Detached inputs, as the reference's wrapper."""
+        frames were left and the score is 1e-5).  Detached inputs, as the reference's wrapper.  ``return_workspace``:
+        also return the forward's workspace (uint8; the 10 kHz signals, kept-frame lists, counts and band envelopes)
+        as a fourth value, the input of :meth:`stoi_backward`."""
         est = self._prep(est.detach(), "estimates")
         ref = self._prep(ref.detach(), "references")
         if est.shape != ref.shape or est.ndim != 3:
@@ -1342,10 +1352,7 @@ class Engine:
         n10 = -(-T * up // down)
         if n10 <= 256:
             raise ValueError(f"stoi: {T} samples at {sample_rate} Hz leave no full 256-sample frame at 10 kHz")
-        key = ("stoi_taps", int(sample_rate), est.device)
-        taps = self._packed_cache.get(key)
-        if taps is None:
-            taps = self._packed_cache[key] = torch.from_numpy(self.stoi_taps(sample_rate)).to(est.device)
+        taps = self._stoi_taps(sample_rate, est.device)
         nbytes = int(self.lib.b2a_stoi_workspace_bytes(B, T, up, down))
         ws = torch.empty(nbytes, dtype=torch.uint8, device=est.device)
         out = torch.empty(B, dtype=torch.float64, device=est.device)
@@ -1355,7 +1362,28 @@ class Engine:
                                    down, _dptr(out), _dptr(kept), _dptr(short), _dptr(ws), nbytes, self._stream(est))
         self.lib.check(rc)
         self.launches += 4 if n10 > 256 + 128 else 3  # one frame at 10 kHz leaves no STFT frame: no band launch
+        if return_workspace:
+            return out, kept, short.bool(), ws
         return out, kept, short.bool()
+
+    def stoi_backward(self, grad_score: torch.Tensor, ws: torch.Tensor, shape, sample_rate: int,
+                      extended: bool = False) -> torch.Tensor:
+        """dL/d estimates [B, C, T] float32 of :meth:`stoi` for dL/dscore [B] (float64), from the forward workspace
+        ``ws`` that ``stoi(..., return_workspace=True)`` returned for estimates of ``shape``.  Items scored 1e-5 get
+        a zero gradient."""
+        B, C, T = (int(v) for v in shape)
+        g = self._prep(grad_score, "grad_score", dtype=torch.float64)
+        assert g.shape == (B,), (tuple(g.shape), B)
+        up, down = self.stoi_ratio(sample_rate)
+        taps = self._stoi_taps(sample_rate, ws.device)
+        nbytes = int(self.lib.b2a_stoi_backward_workspace_bytes(B, T, up, down))
+        bws = torch.empty(nbytes, dtype=torch.uint8, device=ws.device)
+        gx = torch.empty(B, C, T, dtype=torch.float32, device=ws.device)
+        rc = self.lib.b2a_stoi_backward_f32(_dptr(g), _dptr(ws), ws.numel(), B, C, T, int(bool(extended)), _dptr(taps),
+                                            taps.numel(), up, down, _dptr(gx), _dptr(bws), nbytes, self._stream(ws))
+        self.lib.check(rc)
+        self.launches += 4 if -(-T * up // down) > 256 + 128 else 3
+        return gx
 
 
 _ENGINE = None

@@ -6,6 +6,7 @@ from . import quality
 from . import spectral
 from .distance import L1Loss
 from .distance import SISDRLoss
+from .quality import STOILoss
 from .spectral import MelSpectrogramLoss
 from .spectral import MultiScaleSTFTLoss
 from .spectral import PhaseLoss

@@ -1,7 +1,10 @@
 """The reference's quality metrics (ref:audiotools/metrics/quality.py).  ``stoi`` runs on ``csrc/stoi.cu`` for the
-whole batch at once; ``pesq`` and ``visqol`` call an external C library / binary in the reference and are not ported.
+whole batch at once, and ``STOILoss`` is the same score as a differentiable training loss; ``pesq`` and ``visqol``
+call an external C library / binary in the reference and are not ported.
 """
 import warnings
+
+from torch import nn
 
 from ..core import AudioSignal
 
@@ -56,6 +59,62 @@ def stoi(estimates: AudioSignal, references: AudioSignal, extended: int = False)
                       f"frames (items {short.nonzero().flatten().tolist()}). Returning 1e-5 for them. Please check "
                       "your audio", RuntimeWarning)
     return score
+
+
+class STOILoss(nn.Module):
+    """Negative STOI (or extended STOI) as a differentiable training loss: ``-score`` per item, where ``score`` is
+    exactly what ``stoi(estimates, references, extended)`` returns (same kernels, same value), so a model trains on
+    the number that is later reported.
+
+    The arguments are in ``stoi``'s order: the estimates FIRST, then the clean references.  (``SISDRLoss`` takes the
+    reference first, as in the reference.)
+
+    Gradients reach ``estimates.audio_data`` only, through any deferred gain (``normalize`` / ``volume_change``);
+    the references are constants, and references that require a gradient raise ``NotImplementedError``.  The silence
+    removal depends on the references alone, so it is a constant of the backward pass; every other stage is
+    differentiated exactly (CUDA backward kernels, no host synchronisation).  An item with fewer than 30 STFT frames
+    left scores 1e-5, as in ``stoi``, and gets a zero gradient; unlike ``stoi`` it raises no warning.  Without a
+    gradient (no-grad mode, or estimates that do not require one) the loss makes exactly ``stoi``'s launches.
+
+    Parameters
+    ----------
+    extended : bool, optional
+        Extended STOI [3] instead of STOI, by default False
+    reduction : str, optional
+        'mean', 'sum' or anything else for none, by default 'mean'
+    weight : float, optional
+        Weight of this loss, defaults to 1.0 (stored, not applied).
+
+    Returns (``forward``)
+    ---------------------
+    Tensor
+        float32 on the estimates' device: the loss per item [batch] (no reduction) or its mean / sum, reduced in
+        float64 before the cast.
+    """
+
+    def __init__(self, extended: bool = False, reduction: str = "mean", weight: float = 1.0):
+        self.extended = extended
+        self.reduction = reduction
+        self.weight = weight
+        super().__init__()
+
+    def forward(self, estimates: AudioSignal, references: AudioSignal):
+        from ..core import grad as _grad
+        from ..engine import get_engine
+
+        est, ref = estimates._materialized(), references._materialized()
+        _grad.refuse_param_grad("STOILoss", "references", ref)
+        sr, ext = references.sample_rate, bool(self.extended)
+        if _grad.wants_grad(est):
+            score = _grad.STOI.apply(est, ref, sr, ext)
+        else:
+            score = get_engine().stoi(est, ref, sr, ext)[0]
+        loss = -score
+        if self.reduction == "mean":
+            loss = loss.mean()
+        elif self.reduction == "sum":
+            loss = loss.sum()
+        return loss.float()
 
 
 def pesq(estimates: AudioSignal, references: AudioSignal, mode: str = "wb", target_sr: float = 16000):

@@ -4,7 +4,7 @@ bench.py, which measures configs[1]).  One JSON line per config: device-resident
 >= 3 warm-ups, inputs larger than L2 or rotated), algorithmic bytes, and the CPU oracle on a bounded sample.
 
     python bench_configs.py [--only cfg1,cfg3,cfg4,cfg5,istft,specaug,dense,largewin,grad,loss,gate,masked,effects_grad,
-                                      specaug_grad,stoi] [--no-cpu]
+                                      specaug_grad,stoi,stoi_grad] [--no-cpu]
 
 Multi-GPU (BASELINE configs[3] = 512 items on 4 GPUs, configs[4] = 2048 items on 8 GPUs): one process per GPU,
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 4 --master-addr 127.0.0.1 --master-port 29511 \
@@ -688,6 +688,71 @@ def main():
                             f"(timed on {n_cpu} items, scaled to {B})", **res,
                   "gpu": torch.cuda.get_device_name(LOCAL), "power_limit": plim})
             del e, r, est, ref
+
+    if "stoi_grad" in only:  # metrics.STOILoss: forward, forward + backward, backward alone, against its floors
+        import subprocess
+
+        from audiotools_b200 import metrics
+        from audiotools_b200.engine import Engine, get_engine
+        from tests import stoi_grad_cases as sg
+        from tests.golden.make_golden_quality import speech
+
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(LOCAL)],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+        eng = get_engine()
+        fp64_peak = 34.0e12  # FLOP/s: H100 SXM data sheet, FP64 (non-tensor), not measured
+        B, n_t = 64, 8
+        for sr, C, sec in ((16000, 1, 4), (44100, 2, 10)):
+            T = sec * sr
+            clips = np.stack([np.stack([speech(sr, T, 8 * i + c) for c in range(C)]) for i in range(8)])
+            ref = torch.from_numpy(np.tile(clips, (B // 8, 1, 1))).to(dev)
+            est = (ref + 0.3 * ref.std() * torch.randn(ref.shape, generator=torch.Generator().manual_seed(sr + C))
+                   .to(dev)).contiguous()
+            r = AudioSignal(ref, sr)
+            up, down = Engine.stoi_ratio(sr)
+            n_taps = Engine.stoi_taps(sr).size
+            n10 = -(-T * up // down)
+            n_fr = max(-(-(n10 - 256) // 128), 0)
+            # backward floors from shapes: the transposed FIR's FP64 FMAs, and the bytes the four kernels must move
+            fma = B * T * -(-n_taps // down) if up * down > 1 else 0
+            nbytes = B * (4 * n10 + 2 * 4 * 15 * n_fr + 2 * 1800 * n_fr + 2 * 120 * n_fr + 2 * 1024 * n_fr
+                          + 2 * 4 * n10 + 4 * C * T)
+            res = {}
+            for mode, ext in (("std", False), ("ext", True)):
+                x = est.clone().requires_grad_()
+                loss_fn = metrics.STOILoss(ext)
+
+                def fwd():
+                    with torch.no_grad():
+                        return loss_fn(AudioSignal(x, sr), r)
+
+                def fwd_bwd():
+                    return torch.autograd.grad(loss_fn(AudioSignal(x, sr), r), x)
+
+                _, _, _, ws = eng.stoi(est, ref, sr, ext, return_workspace=True)
+                gs = torch.full((B,), -1.0 / B, dtype=torch.float64, device=dev)
+                res[f"{mode}_fwd_ms"] = timed(fwd, warmup=3, steps=10)
+                res[f"{mode}_fwd_bwd_ms"] = timed(fwd_bwd, warmup=3, steps=10)
+                res[f"{mode}_bwd_ms"] = timed(lambda: eng.stoi_backward(gs, ws, est.shape, sr, ext), warmup=3, steps=10)
+                # torch autograd over the float32 restatement (gather resampler, rfft, envelopes; a per-item loop, so
+                # timed on the first n_t items), same GPU
+                try:
+                    xt = est[:n_t].clone().requires_grad_()
+
+                    def torch_fb():
+                        return torch.autograd.grad(-sg.batch_stoi(xt, ref[:n_t], sr, ext).mean(), xt)
+
+                    res[f"{mode}_torch_autograd_fp32_{n_t}_items_ms"] = timed(torch_fb, warmup=1, steps=1)
+                except torch.cuda.OutOfMemoryError:
+                    res[f"{mode}_torch_autograd_fp32_{n_t}_items_ms"] = "does not fit in memory"
+                del ws
+                torch.cuda.empty_cache()
+            emit({"config": f"stoi_grad {B}x{C}ch {sec}s@{sr}: STOILoss (standard / extended) no-grad forward, "
+                            "forward + backward, backward alone (Engine.stoi_backward: 4 launches), and torch autograd "
+                            f"over the float32 restatement on {n_t} of the items ({n_t}x{C}x{T})", **res,
+                  "bwd_fp64_fma": fma, "bwd_fp64_floor_ms": 2 * fma / fp64_peak * 1e3, "bwd_bytes": nbytes,
+                  "bwd_hbm_floor_ms": nbytes / (peak * 1e9) * 1e3, "gpu_and_power_limit": q})
+            del est, ref, r
 
     if "specaug" in only:  # SURVEY 8f.1: SpectralTransform chain stft -> FrequencyMask -> TimeMask -> istft at cfg2's shape
         g = torch.Generator().manual_seed(0)

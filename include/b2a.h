@@ -479,6 +479,28 @@ int b2a_stoi_f32(const float* est, const float* ref, int64_t batch, int channels
                  const double* taps, int n_taps, int up, int down, double* out, int32_t* kept_out, int32_t* short_out,
                  void* ws, size_t ws_bytes, void* stream);
 
+/* ---- backward of b2a_stoi_f32 with respect to the estimates (metrics.quality.STOILoss; the references are constants)
+ *   grad_score  [batch] float64 dL/dscore
+ *   fwd_ws      the workspace b2a_stoi_f32 filled for the same est, ref, batch, channels, T, taps, up, down and left
+ *               untouched since (its 10 kHz signals, kept-frame lists and counts and band envelopes are read);
+ *               fwd_ws_bytes >= b2a_stoi_workspace_bytes(batch, T, up, down)
+ *   grad_est    [batch, channels, T] float32 dL/dest; exactly 0 for an item scored 1e-5 (fewer than 30 STFT frames)
+ *               and for samples that only dropped (silent) frames cover
+ *   ws          b2a_stoi_backward_workspace_bytes(batch, T, up, down) bytes.  With n10 = ceil(T up / down) and
+ *               n_fr = ceil((n10 - 256) / 128) (0 when n10 <= 256), each part rounded up to 256 bytes:
+ *                 1800 batch n_fr   (per-cell derivatives, float [n_fr][15][30])
+ *               +  120 batch n_fr   (dL/d band envelope, float64 [15][n_fr])
+ *               +    4 batch n_fr   (frame -> kept position, int32)
+ *               + 1024 batch n_fr   (dL/d STOI frame, float [n_fr][256])
+ *               +    4 batch n10    (dL/d 10 kHz estimate, float)
+ * Arguments are checked as b2a_stoi_f32 checks them (messages prefixed "stoi_backward:"), plus the forward workspace's
+ * size; B2A_E_UNSUPPORTED when the transposed FIR's tile (1024 inputs) needs more than 200 KB of shared memory.  Four
+ * launches (three when n10 <= 384), no atomics: bit-identical reruns. */
+size_t b2a_stoi_backward_workspace_bytes(int64_t batch, int64_t T, int up, int down);
+int b2a_stoi_backward_f32(const double* grad_score, const void* fwd_ws, size_t fwd_ws_bytes, int64_t batch,
+                          int channels, int64_t T, int extended, const double* taps, int n_taps, int up, int down,
+                          float* grad_est, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- one-sided statistics exchange between the GPUs of a node (NVLink peer memory) --------------------
  * The path shards by batch item with no data-path collective; the one exchange is the per-item loudness vector for
  * whole-batch statistics (the reference has no multi-GPU code of its own: SURVEY.md 8e).  Every rank owns a small
