@@ -45,8 +45,6 @@ SIGNATURES = {
                                 c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "b2a_resample_out_len": (c_int64, [c_int64, c_int, c_int]),
     "b2a_resample_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
-    "b2a_pitch_shift_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_float]),
-    "b2a_pitch_shift_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
     "b2a_pitch_shift_multi_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_void_p, c_int]),
     "b2a_pitch_shift_multi_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                           c_size_t, c_void_p]),
@@ -155,11 +153,20 @@ class B2ALibrary:
             fn.restype = res
             fn.argtypes = args
             setattr(self, name, fn)
+        # b2a_kernel_launches: ``kernel_launches.value`` reads the library's launch count with no foreign-function call
+        self.kernel_launches = c_int64.in_dll(self.cdll, "b2a_kernel_launches")
 
     def check(self, rc: int):
         if rc != B2A_OK:
             msg = self.b2a_last_error()
             raise B2AError(f"libb2a error {rc}: {msg.decode() if msg else '?'}")
+
+    def call(self, fn, *args) -> int:
+        """Call ``fn``, an entry point that launches kernels, raise on its error code, and return the number of kernels
+        it launched (read from ``b2a_kernel_launches`` around the call)."""
+        n0 = self.kernel_launches.value
+        self.check(fn(*args))
+        return self.kernel_launches.value - n0
 
 
 _LIB = None

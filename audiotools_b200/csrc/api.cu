@@ -1,5 +1,5 @@
-// api.cu -- version + thread-local error message of libb2a.so (include/b2a.h), and the SM count the persistent grids
-// are sized by.
+// api.cu -- version, thread-local error message and kernel launch count of libb2a.so (include/b2a.h), and the SM
+// count the persistent grids are sized by.
 #include <atomic>
 
 #include "b2a_common.h"
@@ -29,6 +29,8 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 }  // namespace b2a
+
+int64_t b2a_kernel_launches = 0;  // C linkage from its declaration in b2a.h
 
 extern "C" int b2a_version(void) { return B2A_VERSION; }
 extern "C" const char* b2a_last_error(void) { return b2a::err_buf(); }

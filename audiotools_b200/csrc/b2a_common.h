@@ -41,6 +41,8 @@ int fail(int code, const char* fmt, ...);
 
 // ---------------------------------------------------------------------------------------
 // launch + dynamic shared memory, CUDA vs sim
+// B2A_LAUNCH is the only place a kernel is launched; each launch adds one to b2a_kernel_launches (b2a.h) in both
+// builds, so the simulator counts exactly what the GPU build launches.
 // ---------------------------------------------------------------------------------------
 #ifdef B2A_SIM
 #define B2A_GRID_CONSTANT
@@ -48,14 +50,22 @@ int fail(int code, const char* fmt, ...);
 #define B2A_GRID_CONSTANT __grid_constant__
 #endif
 
+#define B2A_COUNT_LAUNCH() __atomic_fetch_add(&b2a_kernel_launches, 1, __ATOMIC_RELAXED)
+
 #ifdef B2A_SIM
-#define B2A_LAUNCH(kernel, grid, block, smem, stream, ...) \
-  cusim::launch((grid), (block), (smem), [&] { kernel(__VA_ARGS__); })
+#define B2A_LAUNCH(kernel, grid, block, smem, stream, ...)                 \
+  do {                                                                     \
+    B2A_COUNT_LAUNCH();                                                    \
+    cusim::launch((grid), (block), (smem), [&] { kernel(__VA_ARGS__); }); \
+  } while (0)
 #define B2A_DYN_SMEM(name) unsigned char* name = cusim::ctx()->dyn_smem
 #define B2A_BAR_SYNC(id, nthreads) cusim::named_bar((id), (nthreads))
 #else
-#define B2A_LAUNCH(kernel, grid, block, smem, stream, ...) \
-  kernel<<<(grid), (block), (smem), (cudaStream_t)(stream)>>>(__VA_ARGS__)
+#define B2A_LAUNCH(kernel, grid, block, smem, stream, ...)                           \
+  do {                                                                               \
+    B2A_COUNT_LAUNCH();                                                              \
+    kernel<<<(grid), (block), (smem), (cudaStream_t)(stream)>>>(__VA_ARGS__);        \
+  } while (0)
 #define B2A_DYN_SMEM(name) extern __shared__ __align__(1024) unsigned char name[]
 // named barrier over a sub-set of the CTA's warps (ids 1..15; 0 is __syncthreads)
 #define B2A_BAR_SYNC(id, nthreads) asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory")

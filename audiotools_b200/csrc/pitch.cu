@@ -472,15 +472,6 @@ extern "C" int b2a_pitch_shift_multi_f32(const float* x, int64_t rows, int64_t T
   return B2A_OK;
 }
 
-extern "C" size_t b2a_pitch_shift_workspace_bytes(int64_t rows, int64_t T, int sr, float semitones) {
-  return b2a_pitch_shift_multi_workspace_bytes(rows, T, sr, &semitones, 1);
-}
-
-extern "C" int b2a_pitch_shift_f32(const float* x, int64_t rows, int64_t T, int sr, float semitones, float* out,
-                                   void* ws, size_t ws_bytes, void* stream) {
-  return b2a_pitch_shift_multi_f32(x, rows, T, sr, &semitones, 1, nullptr, out, ws, ws_bytes, stream);
-}
-
 extern "C" int b2a_pitch_shift_num_frames(int64_t T, int sr, float semitones) {
   if (T < 1 || sr < 1 || !(fabsf(semitones) <= 24.f)) return -1;
   Geo g;

@@ -39,14 +39,19 @@ class Engine:
                       "stft_data / the gated signal)")
 
     @classmethod
-    def _refuse_grad(cls, t: torch.Tensor, name: str, depth: int = 2):
+    def _refuse_grad(cls, t: torch.Tensor, name: str):
         """A tensor that requires a gradient while grad mode is on reaches a kernel without a backward: raise instead
-        of returning a silently detached result.  The message names the engine method that was called."""
+        of returning a silently detached result.  The message names the engine method that was called: the innermost
+        caller whose name does not start with an underscore, so private helpers (``_prep``, ``_per_item``,
+        ``_band_args``, ...) and dunder callers (a transform's ``__call__``) are skipped."""
         if t.requires_grad and torch.is_grad_enabled():
-            method = sys._getframe(depth).f_code.co_name
+            frame = sys._getframe(1)
+            while frame.f_code.co_name.startswith("_") and frame.f_back is not None:
+                frame = frame.f_back
             raise NotImplementedError(
-                f"{method}: {name} requires a gradient, and this method has no backward.  Differentiable: "
-                f"{', '.join(cls.DIFFERENTIABLE)}.  Call it under torch.no_grad() or on a detached signal.")
+                f"{frame.f_code.co_name}: {name} requires a gradient, and this method has no backward.  "
+                f"Differentiable: {', '.join(cls.DIFFERENTIABLE)}.  Call it under torch.no_grad() or on a detached "
+                "signal.")
 
     def _prep(self, t: torch.Tensor, name: str, dtype=torch.float32) -> torch.Tensor:
         if not torch.is_tensor(t):
@@ -59,6 +64,14 @@ class Engine:
             t = t.to(dtype)
         return t.contiguous()
 
+    def _per_item(self, v, n: int, name: str, device) -> torch.Tensor:
+        """``v`` (a tensor, number or sequence of 1 or ``n`` values) as a contiguous float32 [n] tensor on ``device``:
+        one value is broadcast to all ``n`` items."""
+        v = torch.as_tensor(v).reshape(-1).to(device=device, dtype=torch.float32)
+        assert v.numel() in (1, n), f"{name} must have 1 or {n} entries, got {v.numel()}"
+        self._refuse_grad(v, name)
+        return v.expand(n).contiguous()
+
     def _stream(self, t: torch.Tensor):
         """The stream the call is issued on.  Every entry point of the library launches on the CURRENT device, so a
         tensor that lives on another GPU of the process (``AudioSignal(..., device="cuda:1")``) makes its device
@@ -68,6 +81,11 @@ class Engine:
                 torch.cuda.set_device(t.device)
             return ctypes.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
         return None
+
+    def _call(self, fn, *args):
+        """Every call of an entry point that launches kernels goes through here: raise on its error code, and count
+        the kernels it launched in ``launches``."""
+        self.launches += self.lib.call(fn, *args)
 
     # ------------------------------------------------------------------ inverse STFT
     @staticmethod
@@ -128,11 +146,8 @@ class Engine:
         imat = self.dft_matrix(window, int(n_fft), inverse=1) if route == _lib.ROUTE_DENSE else None
         nbytes = int(self.lib.b2a_istft_workspace_bytes(B * C, N, int(n_fft), int(hop)))
         ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=spec.device) if nbytes else None
-        rc = self.lib.b2a_istft_f32(_dptr(torch.view_as_real(spec)), B * C, N, int(n_fft), int(hop), _dptr(window),
-                                    _dptr(imat), int(pad_frames), start, int(length), _dptr(out), _dptr(ws), nbytes,
-                                    self._stream(spec))
-        self.lib.check(rc)
-        self.launches += 1 if route == _lib.ROUTE_FFT else 2  # LARGE / DENSE: frames, then the overlap-add fold
+        self._call(self.lib.b2a_istft_f32, _dptr(spec), B * C, N, int(n_fft), int(hop), _dptr(window), _dptr(imat),
+                   int(pad_frames), start, int(length), _dptr(out), _dptr(ws), nbytes, self._stream(spec))
         return out
 
     # ------------------------------------------------------------------ backward passes (csrc/grad.cu)
@@ -142,7 +157,7 @@ class Engine:
     def stft_backward(self, grad_spec: torch.Tensor, T: int, n_fft: int, hop: int, window: torch.Tensor, pad: int = 0,
                       right_pad: int = 0, pad_mode: str = "reflect", drop_edge: int = 0) -> torch.Tensor:
         """Gradient wrt x [B, C, T] of ``spectral``'s STFT from grad_spec [B, C, F, N] (complex, torch's convention)."""
-        grad_spec = grad_spec.to(torch.complex64).contiguous()
+        grad_spec = self._complex64(grad_spec)
         B, C, F, N = grad_spec.shape
         window = self._prep(window, "window")
         nbytes = int(self.lib.b2a_stft_backward_workspace_bytes(B * C, int(T), int(n_fft), int(hop), int(pad),
@@ -153,12 +168,9 @@ class Engine:
         amat = self.dft_matrix(window, int(n_fft), inverse=2) if route == _lib.ROUTE_DENSE else None
         ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=grad_spec.device)
         gx = torch.empty(B, C, int(T), dtype=torch.float32, device=grad_spec.device)
-        rc = self.lib.b2a_stft_backward_f32(_dptr(torch.view_as_real(grad_spec)), B * C, int(T), int(n_fft), int(hop),
-                                            _dptr(window), _dptr(amat), int(pad), int(right_pad),
-                                            _lib.PAD_MODES[pad_mode], int(drop_edge), _dptr(gx), _dptr(ws), nbytes,
-                                            self._stream(grad_spec))
-        self.lib.check(rc)
-        self.launches += 2 if route == _lib.ROUTE_FFT else 3
+        self._call(self.lib.b2a_stft_backward_f32, _dptr(grad_spec), B * C, int(T), int(n_fft), int(hop), _dptr(window),
+                   _dptr(amat), int(pad), int(right_pad), _lib.PAD_MODES[pad_mode], int(drop_edge), _dptr(gx), _dptr(ws),
+                   nbytes, self._stream(grad_spec))
         return gx
 
     def istft_backward(self, grad_out: torch.Tensor, n_frames: int, n_fft: int, hop: int, window: torch.Tensor,
@@ -171,11 +183,9 @@ class Engine:
         nbytes = int(self.lib.b2a_istft_backward_workspace_bytes(B * C, L))
         ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=grad_out.device)
         gs = torch.empty(B, C, n_fft // 2 + 1, int(n_frames), dtype=torch.complex64, device=grad_out.device)
-        rc = self.lib.b2a_istft_backward_f32(_dptr(grad_out), B * C, int(n_frames), int(n_fft), int(hop), _dptr(window),
-                                             _dptr(mat), int(pad_frames), n_fft // 2 + int(trim), L,
-                                             _dptr(torch.view_as_real(gs)), _dptr(ws), nbytes, self._stream(grad_out))
-        self.lib.check(rc)
-        self.launches += 3
+        self._call(self.lib.b2a_istft_backward_f32, _dptr(grad_out), B * C, int(n_frames), int(n_fft), int(hop),
+                   _dptr(window), _dptr(mat), int(pad_frames), n_fft // 2 + int(trim), L, _dptr(gs), _dptr(ws), nbytes,
+                   self._stream(grad_out))
         return gs
 
     def _bin_table(self, mel_lo: torch.Tensor, mel_hi: torch.Tensor, F: int):
@@ -199,7 +209,7 @@ class Engine:
                      mel_hi: torch.Tensor, post: int = _lib.POST_NONE, post_eps: float = 0.0,
                      post_power: float = 1.0) -> torch.Tensor:
         """Gradient wrt the complex STFT [B, C, F, N] of ``spectral``'s mel output from grad_mel [B, C, n_mels, N]."""
-        stft = stft.to(torch.complex64).contiguous()
+        stft = self._complex64(stft)
         B, C, F, N = stft.shape
         grad_mel = grad_mel.to(torch.float32).contiguous()
         mel_fb = self._prep(mel_fb, "mel_fb")
@@ -207,12 +217,9 @@ class Engine:
         mel_hi = self._prep(mel_hi, "mel_hi", torch.int32)
         bin_lo, bin_hi = self._bin_table(mel_lo, mel_hi, F)
         out = torch.empty_like(stft)
-        rc = self.lib.b2a_mel_backward_f32(_dptr(torch.view_as_real(stft)), B * C, F, N, _dptr(mel_fb), _dptr(mel_lo),
-                                           _dptr(mel_hi), mel_fb.shape[0], _dptr(bin_lo), _dptr(bin_hi), int(post),
-                                           float(post_eps), float(post_power), _dptr(grad_mel),
-                                           _dptr(torch.view_as_real(out)), self._stream(stft))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_mel_backward_f32, _dptr(stft), B * C, F, N, _dptr(mel_fb), _dptr(mel_lo), _dptr(mel_hi),
+                   mel_fb.shape[0], _dptr(bin_lo), _dptr(bin_hi), int(post), float(post_eps), float(post_power),
+                   _dptr(grad_mel), _dptr(out), self._stream(stft))
         return out
 
     # ------------------------------------------------------------------ spectral L1 losses (csrc/loss.cu)
@@ -254,14 +261,10 @@ class Engine:
         loss = torch.empty((), dtype=torch.float32, device=dev)
         gx = torch.empty(B, C, F, max(N, 1), dtype=torch.complex64, device=dev) if want_grad_x else None
         gy = torch.empty(B, C, F, max(N, 1), dtype=torch.complex64, device=dev) if want_grad_y else None
-        rc = self.lib.b2a_spectral_loss_f32(
-            _dptr(x), _dptr(y), B * C, T, int(n_fft), int(hop), _dptr(window), int(pad), int(right_pad),
-            _lib.PAD_MODES[pad_mode], int(drop_edge), _dptr(fb), _dptr(lo), _dptr(hi), _dptr(blo), _dptr(bhi), n_mels,
-            float(clamp_eps), float(pow), float(log_weight), float(mag_weight), _dptr(loss),
-            _dptr(torch.view_as_real(gx)) if gx is not None else None,
-            _dptr(torch.view_as_real(gy)) if gy is not None else None, _dptr(ws), nbytes, self._stream(x))
-        self.lib.check(rc)
-        self.launches += 2
+        self._call(self.lib.b2a_spectral_loss_f32, _dptr(x), _dptr(y), B * C, T, int(n_fft), int(hop), _dptr(window),
+                   int(pad), int(right_pad), _lib.PAD_MODES[pad_mode], int(drop_edge), _dptr(fb), _dptr(lo), _dptr(hi),
+                   _dptr(blo), _dptr(bhi), n_mels, float(clamp_eps), float(pow), float(log_weight), float(mag_weight),
+                   _dptr(loss), _dptr(gx), _dptr(gy), _dptr(ws), nbytes, self._stream(x))
         return loss, gx, gy
 
     # ------------------------------------------------------------------ STFT routes, dense DFT (any window length)
@@ -300,9 +303,8 @@ class Engine:
             if n == 0:
                 raise NotImplementedError(f"window_length {n_fft}: the dense DFT path covers 2..8192")
             mat = torch.empty(n, dtype=torch.float32, device=window.device)
-            self.lib.check(self.lib.b2a_dft_matrix_f32(_dptr(window), int(n_fft), int(inverse), _dptr(mat),
-                                                       self._stream(window)))
-            self.launches += 1
+            self._call(self.lib.b2a_dft_matrix_f32, _dptr(window), int(n_fft), int(inverse), _dptr(mat),
+                       self._stream(window))
             hit = self._packed_cache[key] = (mat, window)
         return hit[0]
 
@@ -315,22 +317,15 @@ class Engine:
         B, C, F, N = spec.shape
         axis_vals, lo, hi = self._band_args(spec, axis_vals, lo, hi, axis)
         fill = self._band_fill(val)
-        rc = self.lib.b2a_spec_band_mask_f32(_dptr(torch.view_as_real(spec)), B * C, F, N, _dptr(axis_vals), _dptr(lo),
-                                             _dptr(hi), C, int(axis), float(fill.real), float(fill.imag),
-                                             self._stream(spec))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_spec_band_mask_f32, _dptr(spec), B * C, F, N, _dptr(axis_vals), _dptr(lo), _dptr(hi), C,
+                   int(axis), float(fill.real), float(fill.imag), self._stream(spec))
         return spec
 
     def _band_args(self, spec, axis_vals, lo, hi, axis):
         B, _, F, N = spec.shape
         axis_vals = self._prep(axis_vals.to(spec.device), "axis_vals")
-        lo = self._prep(lo.to(spec.device).reshape(-1), "lo")
-        hi = self._prep(hi.to(spec.device).reshape(-1), "hi")
-        if lo.numel() == 1:
-            lo, hi = lo.expand(B).contiguous(), hi.expand(B).contiguous()
-        assert lo.numel() == B and hi.numel() == B and axis_vals.numel() == (F if axis == 0 else N)
-        return axis_vals, lo, hi
+        assert axis_vals.numel() == (F if axis == 0 else N)
+        return axis_vals, self._per_item(lo, B, "lo", spec.device), self._per_item(hi, B, "hi", spec.device)
 
     @staticmethod
     def _band_fill(val):
@@ -345,11 +340,8 @@ class Engine:
         axis_vals, lo, hi = self._band_args(spec, axis_vals, lo, hi, axis)
         fill = self._band_fill(val)
         out = torch.empty_like(spec)
-        rc = self.lib.b2a_spec_band_mask_out_f32(_dptr(torch.view_as_real(spec)), _dptr(torch.view_as_real(out)), B * C,
-                                                 F, N, _dptr(axis_vals), _dptr(lo), _dptr(hi), C, int(axis),
-                                                 float(fill.real), float(fill.imag), self._stream(spec))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_spec_band_mask_out_f32, _dptr(spec), _dptr(out), B * C, F, N, _dptr(axis_vals),
+                   _dptr(lo), _dptr(hi), C, int(axis), float(fill.real), float(fill.imag), self._stream(spec))
         return out
 
     def spec_band_mask_backward(self, grad: torch.Tensor, spec: torch.Tensor, axis_vals: torch.Tensor,
@@ -362,11 +354,8 @@ class Engine:
         assert grad.shape == spec.shape, (grad.shape, spec.shape)
         axis_vals, lo, hi = self._band_args(spec, axis_vals, lo, hi, axis)
         gs = torch.empty_like(spec)
-        rc = self.lib.b2a_spec_band_mask_backward_f32(_dptr(torch.view_as_real(grad)), _dptr(torch.view_as_real(spec)),
-                                                      B * C, F, N, _dptr(axis_vals), _dptr(lo), _dptr(hi), C, int(axis),
-                                                      _dptr(torch.view_as_real(gs)), self._stream(spec))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_spec_band_mask_backward_f32, _dptr(grad), _dptr(spec), B * C, F, N, _dptr(axis_vals),
+                   _dptr(lo), _dptr(hi), C, int(axis), _dptr(gs), self._stream(spec))
         return gs
 
     def _spec_ok(self, spec: torch.Tensor, what: str) -> torch.Tensor:
@@ -376,9 +365,14 @@ class Engine:
         if self.require_cuda and not spec.is_cuda:
             raise RuntimeError(f"stft_data is on {spec.device}: audiotools_b200 runs on CUDA (sm_90a) only and has "
                                "no CPU fallback")
-        if spec.dtype != torch.complex64 or not spec.is_contiguous():
-            spec = spec.to(torch.complex64).contiguous()
-        return spec
+        return self._complex64(spec)
+
+    @staticmethod
+    def _complex64(t: torch.Tensor) -> torch.Tensor:
+        """``t`` as a contiguous complex64 tensor whose memory holds its values.  A lazy conjugate or negative view
+        (``X.conj()``, which autograd hands to a backward when the loss used it) shares its buffer with ``X``, and the
+        kernels read the buffer as it lies: such a view is resolved into a copy first."""
+        return t.resolve_conj().resolve_neg().to(torch.complex64).contiguous()
 
     def spec_rotate(self, spec: torch.Tensor, shift: torch.Tensor) -> torch.Tensor:
         """``spec * exp(1j * shift)`` in place on a contiguous complex64 [B, ...] tensor (a copy otherwise);
@@ -387,13 +381,10 @@ class Engine:
         B = spec.shape[0]
         cells = spec.numel() // B
         shift = self._prep(shift.to(spec.device), "shift").reshape(-1)
-        if shift.numel() == 1:
-            shift = shift.expand(B).contiguous()
-        assert shift.numel() in (B, spec.numel()), (shift.shape, spec.shape)
-        rc = self.lib.b2a_spec_rotate_f32(_dptr(torch.view_as_real(spec)), B, cells, _dptr(shift),
-                                          int(shift.numel() == spec.numel() and cells > 1), self._stream(spec))
-        self.lib.check(rc)
-        self.launches += 1
+        per_cell = shift.numel() == spec.numel() and cells > 1
+        if not per_cell:
+            shift = self._per_item(shift, B, "shift", spec.device)
+        self._call(self.lib.b2a_spec_rotate_f32, _dptr(spec), B, cells, _dptr(shift), int(per_cell), self._stream(spec))
         return spec
 
     def spec_mask_low(self, spec: torch.Tensor, db_cutoff: torch.Tensor, val: float = 0.0, amin: float = 1e-5,
@@ -402,21 +393,11 @@ class Engine:
         spec = self._spec_ok(spec, "spec_mask_low")
         B = spec.shape[0]
         cells = spec.numel() // B
-        db_cutoff = self._cutoff_arg(spec, db_cutoff)
+        db_cutoff = self._per_item(db_cutoff, B, "db_cutoff", spec.device)
         ws = torch.empty(1, dtype=torch.int32, device=spec.device)
-        rc = self.lib.b2a_spec_mask_low_f32(_dptr(torch.view_as_real(spec)), B, cells, _dptr(db_cutoff), float(amin ** 2),
-                                            float(top_db), float(val), _dptr(ws), self._stream(spec))
-        self.lib.check(rc)
-        self.launches += 2
+        self._call(self.lib.b2a_spec_mask_low_f32, _dptr(spec), B, cells, _dptr(db_cutoff), float(amin ** 2),
+                   float(top_db), float(val), _dptr(ws), self._stream(spec))
         return spec
-
-    def _cutoff_arg(self, spec, db_cutoff):
-        B = spec.shape[0]
-        db_cutoff = self._prep(db_cutoff.to(spec.device), "db_cutoff").reshape(-1)
-        if db_cutoff.numel() == 1:
-            db_cutoff = db_cutoff.expand(B).contiguous()
-        assert db_cutoff.numel() == B
-        return db_cutoff
 
     def spec_mask_low_out(self, spec: torch.Tensor, db_cutoff: torch.Tensor, val: float = 0.0, amin: float = 1e-5,
                           top_db: float = 80.0):
@@ -424,14 +405,11 @@ class Engine:
         |X|^2 the top_db floor came from, for ``spec_mask_low_backward``."""
         spec = self._spec_ok(spec, "spec_mask_low_out")
         B = spec.shape[0]
-        db_cutoff = self._cutoff_arg(spec, db_cutoff)
+        db_cutoff = self._per_item(db_cutoff, B, "db_cutoff", spec.device)
         out = torch.empty_like(spec)
         ws = torch.empty(1, dtype=torch.int32, device=spec.device)
-        rc = self.lib.b2a_spec_mask_low_out_f32(_dptr(torch.view_as_real(spec)), _dptr(torch.view_as_real(out)), B,
-                                                spec.numel() // B, _dptr(db_cutoff), float(amin ** 2), float(top_db),
-                                                float(val), _dptr(ws), self._stream(spec))
-        self.lib.check(rc)
-        self.launches += 2
+        self._call(self.lib.b2a_spec_mask_low_out_f32, _dptr(spec), _dptr(out), B, spec.numel() // B, _dptr(db_cutoff),
+                   float(amin ** 2), float(top_db), float(val), _dptr(ws), self._stream(spec))
         return out, ws
 
     def spec_mask_low_backward(self, grad: torch.Tensor, spec: torch.Tensor, db_cutoff: torch.Tensor, val: float,
@@ -443,14 +421,11 @@ class Engine:
         grad = self._spec_ok(grad, "spec_mask_low_backward")
         assert grad.shape == spec.shape, (grad.shape, spec.shape)
         B = spec.shape[0]
-        db_cutoff = self._cutoff_arg(spec, db_cutoff)
+        db_cutoff = self._per_item(db_cutoff, B, "db_cutoff", spec.device)
         gs = torch.empty_like(spec)
-        rc = self.lib.b2a_spec_mask_low_backward_f32(_dptr(torch.view_as_real(grad)), _dptr(torch.view_as_real(spec)),
-                                                     B, spec.numel() // B, _dptr(db_cutoff), float(amin ** 2),
-                                                     float(top_db), float(val), _dptr(ws),
-                                                     _dptr(torch.view_as_real(gs)), self._stream(spec))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_spec_mask_low_backward_f32, _dptr(grad), _dptr(spec), B, spec.numel() // B,
+                   _dptr(db_cutoff), float(amin ** 2), float(top_db), float(val), _dptr(ws), _dptr(gs),
+                   self._stream(spec))
         return gs
 
     def alter_drr(self, ir: torch.Tensor, sample_rate: int, drr: torch.Tensor) -> torch.Tensor:
@@ -459,15 +434,10 @@ class Engine:
         launch (csrc/effects.cu)."""
         ir = self._prep(ir, "ir")
         B, C, T = ir.shape
-        drr = self._prep(drr.to(ir.device).float().reshape(-1), "drr")
-        if drr.numel() == 1:
-            drr = drr.expand(B).contiguous()
-        assert drr.numel() == B
+        drr = self._per_item(drr, B, "drr", ir.device)
         out = torch.empty_like(ir)
-        rc = self.lib.b2a_alter_drr_f32(_dptr(ir), _dptr(out), B * C, T, C, int(sample_rate * 0.0025), _dptr(drr), 1.0,
-                                        self._stream(ir))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_alter_drr_f32, _dptr(ir), _dptr(out), B * C, T, C, int(sample_rate * 0.0025), _dptr(drr),
+                   1.0, self._stream(ir))
         return out
 
     def spec_gate(self, spec: torch.Tensor, nz_spec: torch.Tensor, n_std: float, amount: torch.Tensor,
@@ -484,24 +454,14 @@ class Engine:
             nz_spec = nz_spec.expand(B, C, -1, -1).contiguous()
         assert nz_spec.shape[2] == F, (nz_spec.shape, F)
         nz_rows = nz_spec.shape[0] * nz_spec.shape[1]
-        amount = self._gate_amount(spec, amount)
+        amount = self._per_item(amount, B, "amount", spec.device)
         sf, st = self._gate_smoothing(smooth_f, smooth_t)
         out = torch.empty_like(spec)
         ws = torch.empty(nz_rows * F, dtype=torch.float32, device=spec.device)
-        rc = self.lib.b2a_spec_gate_f32(_dptr(torch.view_as_real(spec)), B * C, F, N, _dptr(torch.view_as_real(nz_spec)),
-                                        nz_rows, nz_spec.shape[-1], float(n_std), _dptr(amount), C, sf, len(smooth_f),
-                                        st, len(smooth_t), _dptr(torch.view_as_real(out)), _dptr(ws), self._stream(spec))
-        self.lib.check(rc)
-        self.launches += 2
+        self._call(self.lib.b2a_spec_gate_f32, _dptr(spec), B * C, F, N, _dptr(nz_spec), nz_rows, nz_spec.shape[-1],
+                   float(n_std), _dptr(amount), C, sf, len(smooth_f), st, len(smooth_t), _dptr(out), _dptr(ws),
+                   self._stream(spec))
         return out, ws.reshape(nz_rows, F)
-
-    def _gate_amount(self, spec, amount):
-        amount = torch.as_tensor(amount, dtype=torch.float32).reshape(-1).to(spec.device)
-        if amount.numel() == 1:
-            amount = amount.expand(spec.shape[0])
-        amount = self._prep(amount.contiguous(), "amount")
-        assert amount.numel() == spec.shape[0]
-        return amount
 
     @staticmethod
     def _gate_smoothing(smooth_f, smooth_t):
@@ -516,15 +476,12 @@ class Engine:
         grad = self._spec_ok(grad, "spec_gate_backward")
         assert grad.shape == spec.shape, (grad.shape, spec.shape)
         B, C, F, N = spec.shape
-        amount = self._gate_amount(spec, amount)
+        amount = self._per_item(amount, B, "amount", spec.device)
         sf, st = self._gate_smoothing(smooth_f, smooth_t)
         gs = torch.empty_like(spec)
-        rc = self.lib.b2a_spec_gate_backward_f32(_dptr(torch.view_as_real(grad)), _dptr(torch.view_as_real(spec)), B * C,
-                                                 F, N, _dptr(thresh), thresh.shape[0], _dptr(amount), C, sf,
-                                                 len(smooth_f), st, len(smooth_t), _dptr(torch.view_as_real(gs)),
-                                                 self._stream(spec))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_spec_gate_backward_f32, _dptr(grad), _dptr(spec), B * C, F, N, _dptr(thresh),
+                   thresh.shape[0], _dptr(amount), C, sf, len(smooth_f), st, len(smooth_t), _dptr(gs),
+                   self._stream(spec))
         return gs
 
     # ------------------------------------------------------------------ loudness
@@ -564,12 +521,10 @@ class Engine:
                 raise ValueError(f"target_db must have 1 or {B} entries, got {n_target}")
             gain = torch.empty(B, dtype=torch.float32, device=dev)
         dp = ctypes.POINTER(ctypes.c_double)
-        rc = L.b2a_lufs_f32(_dptr(x), B, C, T, Tp, float(sample_rate),
-                            sos.ctypes.data_as(dp), sgain.ctypes.data_as(dp), sos.shape[0], float(block_size),
-                            G.ctypes.data_as(dp), _dptr(blocks), _dptr(lufs), _dptr(loud),
-                            _dptr(target_db), n_target, _dptr(gain), _dptr(ws), ws_bytes, self._stream(x))
-        L.check(rc)
-        self.launches += 2  # kweight_energy, lufs_gate (+ one memset node)
+        self._call(L.b2a_lufs_f32, _dptr(x), B, C, T, Tp, float(sample_rate), sos.ctypes.data_as(dp),
+                   sgain.ctypes.data_as(dp), sos.shape[0], float(block_size), G.ctypes.data_as(dp), _dptr(blocks),
+                   _dptr(lufs), _dptr(loud), _dptr(target_db), n_target, _dptr(gain), _dptr(ws), ws_bytes,
+                   self._stream(x))
         return {"lufs": lufs, "loud": loud, "gain": gain, "blocks": blocks}
 
     LOUDNESS_STATS = ("I", "I Threshold", "LRA", "LRA Threshold", "LRA Low", "LRA High")
@@ -599,12 +554,9 @@ class Engine:
         mom = torch.empty(B, nblk, dtype=torch.float32, device=dev) if want_series else None
         st = torch.empty(B, n_st, dtype=torch.float32, device=dev) if want_series else None
         dp = ctypes.POINTER(ctypes.c_double)
-        rc = L.b2a_loudness_stats_f32(_dptr(x), B, C, T, Tp, float(sample_rate),
-                                      sos.ctypes.data_as(dp), sgain.ctypes.data_as(dp), sos.shape[0],
-                                      G.ctypes.data_as(dp), _dptr(stats), _dptr(mom), _dptr(st), _dptr(ws), ws_bytes,
-                                      self._stream(x))
-        L.check(rc)
-        self.launches += 3  # kweight_energy, lufs_gate, loudness_stats (+ one memset node)
+        self._call(L.b2a_loudness_stats_f32, _dptr(x), B, C, T, Tp, float(sample_rate), sos.ctypes.data_as(dp),
+                   sgain.ctypes.data_as(dp), sos.shape[0], G.ctypes.data_as(dp), _dptr(stats), _dptr(mom), _dptr(st),
+                   _dptr(ws), ws_bytes, self._stream(x))
         out = dict(zip(self.LOUDNESS_STATS, stats.unbind(1)))
         if want_series:
             out["momentary"], out["short_term"] = mom, st
@@ -618,9 +570,7 @@ class Engine:
         assert gain.numel() == B
         if out is None:
             out = torch.empty_like(x)
-        per_item = x.numel() // B
-        self.lib.check(self.lib.b2a_gain_f32(_dptr(x), _dptr(out), B, per_item, _dptr(gain), self._stream(x)))
-        self.launches += 1
+        self._call(self.lib.b2a_gain_f32, _dptr(x), _dptr(out), B, x.numel() // B, _dptr(gain), self._stream(x))
         return out
 
     # ------------------------------------------------------------------ collate (csrc/collate.cu)
@@ -644,10 +594,8 @@ class Engine:
                               for v, o in views], dtype=torch.int64).t().contiguous()
         table = table.to(dev, non_blocking=True)  # [4, n]: pointers, lengths, row strides, offsets
         out = torch.empty(n, C, int(T_out), dtype=torch.float32, device=dev)
-        rc = self.lib.b2a_pack_rows_f32(_dptr(table[0]), _dptr(table[1]), _dptr(table[2]), _dptr(table[3]), n, int(C),
-                                        int(T_out), _dptr(out), self._stream(out))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_pack_rows_f32, _dptr(table[0]), _dptr(table[1]), _dptr(table[2]), _dptr(table[3]), n,
+                   int(C), int(T_out), _dptr(out), self._stream(out))
         out._b2a_keepalive = [v for v, _ in views]  # the sources must outlive the (asynchronous) gather
         return out
 
@@ -658,8 +606,7 @@ class Engine:
         T = x.shape[-1]
         rows = x.numel() // T
         peak = torch.empty(*x.shape[:-1], 1, dtype=torch.float32, device=x.device)
-        self.lib.check(self.lib.b2a_row_absmax_f32(_dptr(x), rows, T, _dptr(peak), self._stream(x)))
-        self.launches += 1
+        self._call(self.lib.b2a_row_absmax_f32, _dptr(x), rows, T, _dptr(peak), self._stream(x))
         return peak
 
     def limit_peak(self, x: torch.Tensor, max_abs: float = 1.0, peak: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -670,9 +617,8 @@ class Engine:
         if peak is None:
             peak = self.row_absmax(x)
         out = torch.empty_like(x)
-        self.lib.check(self.lib.b2a_limit_peak_f32(_dptr(x), _dptr(out), rows, T, _dptr(peak), float(max_abs),
-                                                   self._stream(x)))
-        self.launches += 1
+        self._call(self.lib.b2a_limit_peak_f32, _dptr(x), _dptr(out), rows, T, _dptr(peak), float(max_abs),
+                   self._stream(x))
         return out
 
     def peak_scale_backward(self, grad_out: torch.Tensor, y: torch.Tensor, x_ref: Optional[torch.Tensor] = None,
@@ -694,10 +640,8 @@ class Engine:
             bypass = torch.as_tensor(bypass).reshape(-1).to(y.device)
             bypass = self._bypass(bypass.repeat_interleave(rows // bypass.numel()), rows, y.device)
         gy = torch.empty_like(y)
-        rc = self.lib.b2a_peak_scale_backward_f32(_dptr(g), _dptr(y), _dptr(x_ref), rows, T, float(max_abs),
-                                                  _dptr(bypass), _dptr(gy), _dptr(gx), self._stream(y))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_peak_scale_backward_f32, _dptr(g), _dptr(y), _dptr(x_ref), rows, T, float(max_abs),
+                   _dptr(bypass), _dptr(gy), _dptr(gx), self._stream(y))
         return gy, gx
 
     def mix(self, x: torch.Tensor, other: torch.Tensor, other_gain: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -710,23 +654,18 @@ class Engine:
             other_gain = self._prep(other_gain.reshape(-1), "other_gain")
             assert other_gain.numel() == B
         out = torch.empty_like(x)
-        self.lib.check(self.lib.b2a_mix_f32(_dptr(x), _dptr(other), _dptr(other_gain), _dptr(out), B, x.numel() // B,
-                                            self._stream(x)))
-        self.launches += 1
+        self._call(self.lib.b2a_mix_f32, _dptr(x), _dptr(other), _dptr(other_gain), _dptr(out), B, x.numel() // B,
+                   self._stream(x))
         return out
 
     def quantize(self, x: torch.Tensor, channels: torch.Tensor, mulaw: bool = False) -> torch.Tensor:
         """Linear (ref :463-491) or mu-law (ref :493-523) quantisation to ``channels`` (1 or B values) levels."""
         x = self._prep(x, "x")
         B = x.shape[0]
-        channels = self._prep(torch.as_tensor(channels).to(x.device).reshape(-1).float(), "channels")
-        if channels.numel() == 1:
-            channels = channels.expand(B).contiguous()
-        assert channels.numel() == B
+        channels = self._per_item(channels, B, "channels", x.device)
         out = torch.empty_like(x)
-        self.lib.check(self.lib.b2a_quantize_f32(_dptr(x), _dptr(out), B, x.numel() // B, _dptr(channels), int(mulaw),
-                                                 self._stream(x)))
-        self.launches += 1
+        self._call(self.lib.b2a_quantize_f32, _dptr(x), _dptr(out), B, x.numel() // B, _dptr(channels), int(mulaw),
+                   self._stream(x))
         return out
 
     def order_stats(self, row: torch.Tensor, k: torch.Tensor) -> torch.Tensor:
@@ -734,9 +673,8 @@ class Engine:
         row = self._prep(row.reshape(-1), "row")
         k = k.to(row.device).reshape(-1).to(torch.int64).contiguous()
         out = torch.empty(k.numel(), dtype=torch.float32, device=row.device)
-        self.lib.check(self.lib.b2a_order_stats_f32(_dptr(row), row.numel(), _dptr(k), k.numel(), _dptr(out),
-                                                    self._stream(row)))
-        self.launches += 1
+        self._call(self.lib.b2a_order_stats_f32, _dptr(row), row.numel(), _dptr(k), k.numel(), _dptr(out),
+                   self._stream(row))
         return out
 
     def quantile(self, row: torch.Tensor, q: torch.Tensor) -> torch.Tensor:
@@ -755,13 +693,11 @@ class Engine:
         """``x.clamp(lo[item], hi[item])`` (ref :459)."""
         x = self._prep(x, "x")
         B = x.shape[0]
-        lo = self._prep(lo.to(x.device).reshape(-1), "lo")
-        hi = self._prep(hi.to(x.device).reshape(-1), "hi")
-        assert lo.numel() == B and hi.numel() == B
+        lo = self._per_item(lo, B, "lo", x.device)
+        hi = self._per_item(hi, B, "hi", x.device)
         out = torch.empty_like(x)
-        self.lib.check(self.lib.b2a_clamp_items_f32(_dptr(x), _dptr(out), B, x.numel() // B, _dptr(lo), _dptr(hi),
-                                                    self._stream(x)))
-        self.launches += 1
+        self._call(self.lib.b2a_clamp_items_f32, _dptr(x), _dptr(out), B, x.numel() // B, _dptr(lo), _dptr(hi),
+                   self._stream(x))
         return out
 
     # ------------------------------------------------------------------ STFT / mel
@@ -855,15 +791,10 @@ class Engine:
         nbytes = 0 if fft else int(self.lib.b2a_spectral_workspace_bytes(
             rows, T, n_fft, hop, pad, right_pad, drop_edge, stft is None, gain is not None and scaled is None))
         ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=dev) if nbytes else None
-        rc = self.lib.b2a_spectral_f32(
-            _dptr(x), rows, T, n_fft, hop, _dptr(window), _dptr(mat), pad, right_pad, _lib.PAD_MODES[pad_mode],
-            drop_edge, _dptr(gain), rows_per_gain, _dptr(scaled),
-            _dptr(mel_fb), _dptr(mel_lo), _dptr(mel_hi), n_mels, packed_len, post, float(post_eps),
-            float(post_power),
-            _dptr(mel), _dptr(torch.view_as_real(stft)) if stft is not None else None, _dptr(ws), nbytes,
-            self._stream(x))
-        self.lib.check(rc)
-        self.launches += 1 if fft else 1 + (gain is not None) + (mel is not None)  # LARGE / DENSE: gain, STFT, mel
+        self._call(self.lib.b2a_spectral_f32, _dptr(x), rows, T, n_fft, hop, _dptr(window), _dptr(mat), pad, right_pad,
+                   _lib.PAD_MODES[pad_mode], drop_edge, _dptr(gain), rows_per_gain, _dptr(scaled), _dptr(mel_fb),
+                   _dptr(mel_lo), _dptr(mel_hi), n_mels, packed_len, post, float(post_eps), float(post_power),
+                   _dptr(mel), _dptr(stft), _dptr(ws), nbytes, self._stream(x))
         return {"stft": stft, "mel": mel, "scaled": scaled}
 
     def mel_dct(self, logmel: torch.Tensor, dct: torch.Tensor) -> torch.Tensor:
@@ -875,9 +806,8 @@ class Engine:
         assert dct.shape[0] == n_mels, (dct.shape, n_mels)
         n_mfcc = dct.shape[1]
         out = torch.empty(B, C, n_mfcc, N, dtype=torch.float32, device=logmel.device)
-        rc = self.lib.b2a_mel_dct_f32(_dptr(logmel), B * C, n_mels, N, _dptr(dct), n_mfcc, _dptr(out), self._stream(logmel))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_mel_dct_f32, _dptr(logmel), B * C, n_mels, N, _dptr(dct), n_mfcc, _dptr(out),
+                   self._stream(logmel))
         return out
 
     # ------------------------------------------------------------------ FIR / convolution
@@ -916,12 +846,9 @@ class Engine:
             raise _lib.B2AError("fftconv: bad shape")
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
         out = torch.empty_like(x)
-        rc = self.lib.b2a_fftconv_f32(_dptr(x), rows, T, _dptr(taps), n_filt, L, int(rows_per_filt), _dptr(offset),
-                                      int(offset0), mode, _dptr(post_scale), int(bool(subtract_from_input)),
-                                      _dptr(bypass), _dptr(out), _dptr(ws), ws_bytes, self._stream(x))
-        self.lib.check(rc)
-        nchunk = 1  # kernels: fill, filter FFT, then per row-chunk: origins, block FFT, bin FIR, inverse FFT
-        self.launches += 2 + 4 * nchunk
+        self._call(self.lib.b2a_fftconv_f32, _dptr(x), rows, T, _dptr(taps), n_filt, L, int(rows_per_filt),
+                   _dptr(offset), int(offset0), mode, _dptr(post_scale), int(bool(subtract_from_input)), _dptr(bypass),
+                   _dptr(out), _dptr(ws), ws_bytes, self._stream(x))
         return out
 
     DIRECT_FIR_MAX_TAPS = 320  # longer filters are cheaper through the FFT engine
@@ -941,11 +868,9 @@ class Engine:
         out_len = T if out_len is None else int(out_len)
         bypass = self._bypass(bypass, n_filt, x.device)
         out = torch.empty(*x.shape[:-1], out_len, dtype=torch.float32, device=x.device)
-        rc = self.lib.b2a_fir_direct_f32(_dptr(x), rows, T, _dptr(taps), n_filt, K, int(rows_per_filt), _dptr(left),
-                                         int(left0), int(stride), out_len, {"constant": 1, "replicate": 2}[pad_mode],
-                                         int(bool(subtract_from_input)), _dptr(bypass), _dptr(out), self._stream(x))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_fir_direct_f32, _dptr(x), rows, T, _dptr(taps), n_filt, K, int(rows_per_filt),
+                   _dptr(left), int(left0), int(stride), out_len, {"constant": 1, "replicate": 2}[pad_mode],
+                   int(bool(subtract_from_input)), _dptr(bypass), _dptr(out), self._stream(x))
         return out
 
     @staticmethod
@@ -1097,11 +1022,8 @@ class Engine:
         assert grad_x is not None and grad_x.shape == g.shape and grad_x.is_contiguous()
         ws_bytes = self.lib.b2a_fir_pad_fold_workspace_bytes(n_filt, K)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=g.device)
-        rc = self.lib.b2a_fir_pad_fold_f32(_dptr(g), rows, T, _dptr(taps), n_filt, K, int(rows_per_filt), _dptr(left),
-                                           int(left0), _dptr(bypass), _dptr(grad_x), _dptr(ws), ws_bytes,
-                                           self._stream(g))
-        self.lib.check(rc)
-        self.launches += 2
+        self._call(self.lib.b2a_fir_pad_fold_f32, _dptr(g), rows, T, _dptr(taps), n_filt, K, int(rows_per_filt),
+                   _dptr(left), int(left0), _dptr(bypass), _dptr(grad_x), _dptr(ws), ws_bytes, self._stream(g))
         return grad_x
 
     def mel_filterbank(self, x: torch.Tensor, sample_rate: int, n_bands: int) -> torch.Tensor:
@@ -1134,10 +1056,8 @@ class Engine:
         ws_bytes = self.lib.b2a_circconv_workspace_bytes(B * C, T, n_ir, L)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
         out = torch.empty_like(x)
-        rc = self.lib.b2a_circconv_f32(_dptr(x), B * C, T, _dptr(ir), n_ir, L, rows_per_ir, int(bool(roll_to_peak)),
-                                       _dptr(bypass), _dptr(out), _dptr(ws), ws_bytes, self._stream(x))
-        self.lib.check(rc)
-        self.launches += 7
+        self._call(self.lib.b2a_circconv_f32, _dptr(x), B * C, T, _dptr(ir), n_ir, L, rows_per_ir,
+                   int(bool(roll_to_peak)), _dptr(bypass), _dptr(out), _dptr(ws), ws_bytes, self._stream(x))
         return out
 
     def _circconv_filters(self, shape, ir: torch.Tensor, bypass, device):
@@ -1170,11 +1090,8 @@ class Engine:
         ws_bytes = self.lib.b2a_circconv_backward_workspace_bytes(B * C, T, n_ir, L)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=g.device)
         gx = torch.empty_like(g)
-        rc = self.lib.b2a_circconv_backward_f32(_dptr(g), B * C, T, _dptr(ir), n_ir, L, rows_per_ir,
-                                                int(bool(roll_to_peak)), _dptr(bypass), _dptr(gx), _dptr(ws), ws_bytes,
-                                                self._stream(g))
-        self.lib.check(rc)
-        self.launches += 8
+        self._call(self.lib.b2a_circconv_backward_f32, _dptr(g), B * C, T, _dptr(ir), n_ir, L, rows_per_ir,
+                   int(bool(roll_to_peak)), _dptr(bypass), _dptr(gx), _dptr(ws), ws_bytes, self._stream(g))
         return gx
 
 
@@ -1211,9 +1128,7 @@ class Engine:
             return self.fir_direct(x, kt.reshape(1, -1), rows_per_filt=rows, left0=width, stride=old, out_len=out_len,
                                    pad_mode="replicate")
         out = torch.empty(*x.shape[:-1], out_len, dtype=torch.float32, device=x.device)
-        rc = self.lib.b2a_resample_f32(_dptr(x), rows, T, old, new, width, _dptr(kt), _dptr(out), self._stream(x))
-        self.lib.check(rc)
-        self.launches += 1
+        self._call(self.lib.b2a_resample_f32, _dptr(x), rows, T, old, new, width, _dptr(kt), _dptr(out), self._stream(x))
         return out
 
     def resample_backward(self, grad_out: torch.Tensor, T: int, old_sr: int, new_sr: int) -> torch.Tensor:
@@ -1223,10 +1138,8 @@ class Engine:
         assert g.shape[-1] == int(self.lib.b2a_resample_out_len(T, old, new)), (g.shape, T)
         rows = g.numel() // g.shape[-1]
         gx = torch.empty(*g.shape[:-1], int(T), dtype=torch.float32, device=g.device)
-        rc = self.lib.b2a_resample_backward_f32(_dptr(g), rows, int(T), old, new, width, _dptr(kt), _dptr(gx),
-                                                self._stream(g))
-        self.lib.check(rc)
-        self.launches += 2 if T >= 3 else 1
+        self._call(self.lib.b2a_resample_backward_f32, _dptr(g), rows, int(T), old, new, width, _dptr(kt), _dptr(gx),
+                   self._stream(g))
         return gx
 
 
@@ -1270,10 +1183,8 @@ class Engine:
             raise NotImplementedError(f"pitch_shift: unsupported shifts {sem.tolist()} (|semitones| <= 24)")
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
         out = torch.empty_like(x)
-        rc = self.lib.b2a_pitch_shift_multi_f32(_dptr(x), rows, T, int(sample_rate), sem_p, int(sem.size),
-                                                _dptr(row_group), _dptr(out), _dptr(ws), ws_bytes, self._stream(x))
-        self.lib.check(rc)
-        self.launches += 4
+        self._call(self.lib.b2a_pitch_shift_multi_f32, _dptr(x), rows, T, int(sample_rate), sem_p, int(sem.size),
+                   _dptr(row_group), _dptr(out), _dptr(ws), ws_bytes, self._stream(x))
         if return_positions:
             assert row_group is None, "return_positions: one shift for the whole batch"
             jmax = self.lib.b2a_pitch_shift_num_frames(T, int(sample_rate), float(sem[0]))
@@ -1295,10 +1206,8 @@ class Engine:
             raise NotImplementedError(f"time_stretch: factor {factor} (supported: 0.25 ... 4)")
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
         out = torch.empty(*x.shape[:-1], out_len, dtype=torch.float32, device=x.device)
-        rc = self.lib.b2a_time_stretch_f32(_dptr(x), rows, T, int(sample_rate), factor, _dptr(out), _dptr(ws), ws_bytes,
-                                           self._stream(x))
-        self.lib.check(rc)
-        self.launches += 4 if factor != 1.0 else 1
+        self._call(self.lib.b2a_time_stretch_f32, _dptr(x), rows, T, int(sample_rate), factor, _dptr(out), _dptr(ws),
+                   ws_bytes, self._stream(x))
         if return_positions and factor != 1.0:
             st = float(np.float32(12.0 * math.log2(1.0 / factor)))
             jmax = self.lib.b2a_pitch_shift_num_frames(T, int(sample_rate), st)
@@ -1358,10 +1267,8 @@ class Engine:
         out = torch.empty(B, dtype=torch.float64, device=est.device)
         kept = torch.empty(B, dtype=torch.int32, device=est.device)
         short = torch.empty(B, dtype=torch.int32, device=est.device)
-        rc = self.lib.b2a_stoi_f32(_dptr(est), _dptr(ref), B, C, T, int(bool(extended)), _dptr(taps), taps.numel(), up,
-                                   down, _dptr(out), _dptr(kept), _dptr(short), _dptr(ws), nbytes, self._stream(est))
-        self.lib.check(rc)
-        self.launches += 4 if n10 > 256 + 128 else 3  # one frame at 10 kHz leaves no STFT frame: no band launch
+        self._call(self.lib.b2a_stoi_f32, _dptr(est), _dptr(ref), B, C, T, int(bool(extended)), _dptr(taps),
+                   taps.numel(), up, down, _dptr(out), _dptr(kept), _dptr(short), _dptr(ws), nbytes, self._stream(est))
         if return_workspace:
             return out, kept, short.bool(), ws
         return out, kept, short.bool()
@@ -1379,10 +1286,8 @@ class Engine:
         nbytes = int(self.lib.b2a_stoi_backward_workspace_bytes(B, T, up, down))
         bws = torch.empty(nbytes, dtype=torch.uint8, device=ws.device)
         gx = torch.empty(B, C, T, dtype=torch.float32, device=ws.device)
-        rc = self.lib.b2a_stoi_backward_f32(_dptr(g), _dptr(ws), ws.numel(), B, C, T, int(bool(extended)), _dptr(taps),
-                                            taps.numel(), up, down, _dptr(gx), _dptr(bws), nbytes, self._stream(ws))
-        self.lib.check(rc)
-        self.launches += 4 if -(-T * up // down) > 256 + 128 else 3
+        self._call(self.lib.b2a_stoi_backward_f32, _dptr(g), _dptr(ws), ws.numel(), B, C, T, int(bool(extended)),
+                   _dptr(taps), taps.numel(), up, down, _dptr(gx), _dptr(bws), nbytes, self._stream(ws))
         return gx
 
 

@@ -170,11 +170,10 @@ class PeerLoudnessExchange:
         while len(self._n) > 8:
             self._n.pop(min(self._n))
         with self._on_side():
-            self.lib.check(self.lib.b2a_peer_put_f32(self._ct.c_void_p(loud_local.data_ptr()), n, self.peers, self.world,
-                                                     self.rank, self.n_max, self.seq, self._stream_ptr()))
+            self.launches += self.lib.call(self.lib.b2a_peer_put_f32, self._ct.c_void_p(loud_local.data_ptr()), n,
+                                           self.peers, self.world, self.rank, self.n_max, self.seq, self._stream_ptr())
         if self.side is not None:
             loud_local.record_stream(self.side)
-        self.launches += 1
         return self.seq
 
     def latest(self, n: Optional[int] = None):
@@ -186,10 +185,9 @@ class PeerLoudnessExchange:
         out = torch.empty(self.world, n, dtype=torch.float32, device=self.device)
         seqs = torch.zeros(self.world, dtype=torch.int32, device=self.device)
         with self._on_side():
-            self.lib.check(self.lib.b2a_peer_latest_f32(self._ct.c_void_p(self.local), self.world, n, self.n_max,
-                                                        self._ct.c_void_p(out.data_ptr()),
-                                                        self._ct.c_void_p(seqs.data_ptr()), self._stream_ptr()))
-        self.launches += 1
+            self.launches += self.lib.call(self.lib.b2a_peer_latest_f32, self._ct.c_void_p(self.local), self.world, n,
+                                           self.n_max, self._ct.c_void_p(out.data_ptr()),
+                                           self._ct.c_void_p(seqs.data_ptr()), self._stream_ptr())
         return out, seqs
 
     def collect(self, seq: int, return_seqs: bool = False):
@@ -200,10 +198,9 @@ class PeerLoudnessExchange:
         out = torch.empty(self.world * n, dtype=torch.float32, device=self.device)
         seqs = torch.zeros(self.world, dtype=torch.int32, device=self.device)
         with self._on_side():
-            self.lib.check(self.lib.b2a_peer_collect_f32(self._ct.c_void_p(self.local), self.world, n, self.n_max, seq,
-                                                         self._ct.c_void_p(out.data_ptr()),
-                                                         self._ct.c_void_p(seqs.data_ptr()), self._stream_ptr()))
-        self.launches += 1
+            self.launches += self.lib.call(self.lib.b2a_peer_collect_f32, self._ct.c_void_p(self.local), self.world, n,
+                                           self.n_max, seq, self._ct.c_void_p(out.data_ptr()),
+                                           self._ct.c_void_p(seqs.data_ptr()), self._stream_ptr())
         return (out, seqs) if return_seqs else out
 
     def status(self) -> int:

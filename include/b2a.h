@@ -45,6 +45,12 @@ extern "C" {
 int b2a_version(void);
 const char* b2a_last_error(void);
 
+/* Kernels the library has launched in this process, over all entry points, devices, streams and threads.  Every
+ * kernel launch adds one (a relaxed atomic add on the host); memsets and copies are not counted.  A caller that reads
+ * it before and after an entry point gets the kernels that call launched, provided no other thread launched in
+ * between.  It is a variable rather than a function so that reading it costs no foreign-function call. */
+extern int64_t b2a_kernel_launches;
+
 /* ---- STFT / mel ---------------------------------------------------------------------
  * Replaces the device work of AudioSignal.stft (audiotools/core/audio_signal.py:1123-1212:
  * F.pad(pad, pad+right_pad, padding_type) -> torch.stft(center=True, reflect) -> optional
@@ -388,14 +394,11 @@ int b2a_resample_backward_f32(const float* grad_out, int64_t rows, int64_t T, in
  * EffectMixin.pitch_shift (audiotools/core/effects.py:247-277; SoX `pitch -q` + `rate` there): WSOLA
  * time-scale modification by r = 2^(semitones/12) (search -> overlap-add into the workspace) + band-limited
  * rate change by 1/r (windowed sinc, cutoff 0.95*min(1,1/r), 8 zero crossings), output length == T.
- * ws: 16-byte aligned, b2a_pitch_shift_workspace_bytes() bytes (frame positions + the stretched rows). */
-size_t b2a_pitch_shift_workspace_bytes(int64_t rows, int64_t T, int sr, float semitones);
-int b2a_pitch_shift_f32(const float* x, int64_t rows, int64_t T, int sr, float semitones, float* out, void* ws,
-                        size_t ws_bytes, void* stream);
-/* Several shifts in one launch (a batch whose items drew different shifts, e.g. a PitchShift transform):
+ * One call takes one shift or several (a batch whose items drew different shifts, e.g. a PitchShift transform):
  * semitones_h HOST [n_groups] (n_groups <= 8 distinct values, 0 = copy the row), row_group DEVICE [rows] int32
  * in [0, n_groups) (nullable when n_groups == 1).  Rows of all groups share every launch, so the one-CTA-per-row
- * search fills the GPU with the whole batch instead of one group at a time. */
+ * search fills the GPU with the whole batch instead of one group at a time.  Four launches.
+ * ws: 16-byte aligned, b2a_pitch_shift_multi_workspace_bytes() bytes (frame positions + the stretched rows). */
 size_t b2a_pitch_shift_multi_workspace_bytes(int64_t rows, int64_t T, int sr, const float* semitones_h, int n_groups);
 int b2a_pitch_shift_multi_f32(const float* x, int64_t rows, int64_t T, int sr, const float* semitones_h, int n_groups,
                               const int32_t* row_group, float* out, void* ws, size_t ws_bytes, void* stream);

@@ -76,6 +76,34 @@ def test_adjoint_identity(sim_signals, wl, hop, ms, pt, T):
     assert abs(lhs - rhs) <= 1e-5 * (abs(lhs) + (y.double().abs() * gy.double().abs()).sum().item())
 
 
+def test_conjugate_views_reach_the_kernels_resolved(sim_signals):
+    """``X.conj()`` is a lazy view on X's buffer.  The engine hands the kernels its values: istft, stft_backward,
+    mel_backward and a band mask give what they give for the resolved tensor, and a loss through stft_data.conj()
+    (autograd passes STFT.backward a conjugate view) gets autograd's gradient."""
+    eng = sim_signals
+    wl, hop, T = 512, 128, 4096
+    x = _x((1, 2, T), 11)
+    w = AudioSignal.get_window("hann", wl, "cpu")
+    X = eng.spectral(x, wl, hop, w)["stft"]
+    Xc, Xr = X.conj(), X.conj().resolve_conj()
+    assert Xc.is_conj() and Xc.data_ptr() == X.data_ptr()
+    assert torch.equal(eng.istft(Xc, wl, hop, w, T), eng.istft(Xr, wl, hop, w, T))
+    assert torch.equal(eng.stft_backward(Xc, T, wl, hop, w), eng.stft_backward(Xr, T, wl, hop, w))
+    fb, lo, hi = AudioSignal._mel_tables(44100, wl, 40, 0.0, None, "cpu")
+    gm = torch.randn(1, 2, 40, X.shape[-1], generator=torch.Generator().manual_seed(6))
+    assert torch.equal(eng.mel_backward(Xc, gm, fb, lo, hi), eng.mel_backward(Xr, gm, fb, lo, hi))
+    vals, band = torch.linspace(0, 22050, X.shape[2]), (torch.tensor([1000.0]), torch.tensor([5000.0]))
+    assert torch.equal(eng.spec_band_mask_out(Xc, vals, *band, 0), eng.spec_band_mask_out(Xr, vals, *band, 0))
+
+    xg = x.clone().requires_grad_()
+    Xg = AudioSignal(xg, 44100).stft(window_length=wl, hop_length=hop)
+    G = torch.randn(Xg.shape, dtype=torch.complex64, generator=torch.Generator().manual_seed(7))
+    (gx,) = torch.autograd.grad((Xg.conj() * G).real.sum(), xg)
+    xd = x.double().requires_grad_()
+    (want,) = torch.autograd.grad((gc.stft64(xd, wl, hop).conj() * G.to(torch.complex128)).real.sum(), xd)
+    assert rel_err(gx, want) < TOL
+
+
 @pytest.mark.parametrize("wl,n_mels,log", [(2048, 150, False), (512, 80, False), (512, 80, True), (400, 40, False),
                                            (8192, 128, False)])
 def test_mel_spectrogram_grad_matches_autograd(sim_signals, wl, n_mels, log):
