@@ -297,6 +297,10 @@ __global__ void __launch_bounds__(32) loss_finalize_kernel(const double* __restr
 }
 
 constexpr int MAX_CTAS_PER_SM = 8;  // 256-thread CTAs: the partials buffer holds this many per SM
+// The 227 KB a CTA may opt in to hold the kernel's static shared memory too: s_bar and s_red, which the 1024-byte
+// alignment of the dynamic buffer (B2A_DYN_SMEM) rounds up to 1024 bytes (ptxas -v: "1024 bytes smem").
+constexpr int STATIC_SMEM = 1024;
+constexpr int MAX_DYN_SMEM = 227 * 1024 - STATIC_SMEM;
 
 // shared-memory layout of one launch; returns the bytes
 template <int LOG2N>
@@ -335,9 +339,9 @@ static int launch(LossParams& q, int64_t numel, double log_weight, double mag_we
   q.py.span = p.span;
   q.py.n_tiles = p.n_tiles;
   const int o = layout<LOG2N>(q, p.hop, q.mel_fb ? q.n_mels : 0);
-  B2A_REQUIRE(o <= 227 * 1024, B2A_E_UNSUPPORTED,
-              "spectral_loss: n_fft=%d hop=%d n_mels=%d needs %d bytes of shared memory (> 227 KB)", p.n_fft, p.hop,
-              q.n_mels, o);
+  B2A_REQUIRE(o <= MAX_DYN_SMEM, B2A_E_UNSUPPORTED,
+              "spectral_loss: n_fft=%d hop=%d n_mels=%d needs %d bytes of shared memory (> %d)", p.n_fft, p.hop,
+              q.n_mels, o, MAX_DYN_SMEM);
   const int64_t total = (int64_t)p.rows * p.n_tiles;
   B2A_REQUIRE(total < (int64_t)2147483647, B2A_E_UNSUPPORTED, "spectral_loss: too many tiles");
   auto kern = q.mel_fb ? spectral_loss_kernel<LOG2N, true> : spectral_loss_kernel<LOG2N, false>;
@@ -362,7 +366,7 @@ using namespace b2a::loss;
 
 extern "C" int b2a_spectral_loss_supported(int n_fft, int hop, int n_mels) {
   if (!pow2_window(n_fft) || hop < 1 || hop > n_fft || n_mels < 0) return 0;
-  return smem_bytes(n_fft, hop, n_mels) <= 227 * 1024;
+  return smem_bytes(n_fft, hop, n_mels) <= MAX_DYN_SMEM;
 }
 
 extern "C" size_t b2a_spectral_loss_workspace_bytes(int n_fft, int hop, int n_mels) {

@@ -95,6 +95,26 @@ def mel_loss(x_mel, y_mel, n_mels, window_lengths, log_weight, mag_weight, pow, 
     return loss
 
 
+def undecided(vx, vy, clamp_eps, tol_log, tol_clamp_x, tol_clamp_y=None, tol_mag=None):
+    """The L1 cells whose derivative is decided below FP32 resolution, from the float64 magnitudes (or mels) vx, vy of
+    the two signals: boolean masks (sign, clamp_x, clamp_y, mag).  Each tolerance is a scalar or a per-cell tensor:
+      - sign:  |log10 max(vx, eps) - log10 max(vy, eps)| <= tol_log, unless both are clamped (no log gradient either
+               way, and both sides' log terms are the same number);
+      - clamp: |log10 v - log10 eps| <= tol_clamp on that side (the clamp's step); clamp_y only with tol_clamp_y;
+      - mag:   |vx - vy| <= tol_mag (the magnitude term's sign), only with tol_mag; a cell whose tensor tolerance is 0
+               (two silent frames: both spectra exactly 0) is decided."""
+    lx, ly = vx.clamp(clamp_eps).log10(), vy.clamp(clamp_eps).log10()
+    both_clamped = (vx < clamp_eps) & (vy < clamp_eps)
+    sign = ((lx - ly).abs() <= tol_log) & ~both_clamped
+    clamp_x = (vx.log10() - math.log10(clamp_eps)).abs() <= tol_clamp_x
+    clamp_y = (vy.log10() - math.log10(clamp_eps)).abs() <= tol_clamp_y if tol_clamp_y is not None else None
+    mag = None
+    if tol_mag is not None:
+        d = (vx - vy).abs()
+        mag = (d <= tol_mag) & (tol_mag > 0) if torch.is_tensor(tol_mag) else (d <= tol_mag)
+    return sign, clamp_x, clamp_y, mag
+
+
 def fp32_resolution_keep(x, y, sr, n_mels, window_lengths, pow=2.0, tol=1e-4, clamp_eps=1e-5, **_):
     """The mel cells of MelSpectrogramLoss whose log-term gradient FP32 arithmetic can resolve, from the float64 mels
     of x and y: one boolean mask per scale, and the number of cells dropped for each reason.  A cell is dropped when
@@ -114,10 +134,7 @@ def fp32_resolution_keep(x, y, sr, n_mels, window_lengths, pow=2.0, tol=1e-4, cl
         X = stft64(x.double(), wl, hop).abs()
         xm = (X.transpose(2, -1) @ fb.T).transpose(-1, 2)
         ym = mel64(y.double(), sr, nm, wl, hop)
-        xl, yl = xm.clamp(clamp_eps).log10(), ym.clamp(clamp_eps).log10()
-        both_clamped = (xm < clamp_eps) & (ym < clamp_eps)  # no gradient either way
-        sign = ((xl - yl).abs() <= tau) & ~both_clamped
-        clamp = (xm.log10() - math.log10(clamp_eps)).abs() <= tau
+        sign, clamp, _, _ = undecided(xm, ym, clamp_eps, tau, tau)
         rms = X.pow(2).mean(-2, keepdim=True).sqrt()
         small = X < (2.0 * 2.0 ** -24 * math.log2(wl) / tol) * rms  # [B, C, F, N]
         share = ((X * small).transpose(2, -1) @ fb.T).transpose(-1, 2)  # the mel of the small bins

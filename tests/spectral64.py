@@ -223,10 +223,11 @@ def windows(n_fft: int, dev, seed: int = 0):
 
 
 def stft_ref(x: torch.Tensor, n_fft: int, hop: int, window: torch.Tensor, pad=0, right_pad=0, pad_mode="reflect",
-             drop_edge=0) -> torch.Tensor:
-    """The engine's STFT geometry in float64 through torch.stft (complex128, on x's device)."""
-    y = torch.nn.functional.pad(x.double(), (pad, pad + right_pad), mode=pad_mode) if (pad or right_pad) else x.double()
-    X = torch.stft(y.reshape(-1, y.shape[-1]), n_fft, hop, window=window.double().to(x.device), center=True,
+             drop_edge=0, dtype=torch.float64) -> torch.Tensor:
+    """The engine's STFT geometry through torch.stft, on x's device: float64 (complex128) by default; float32 gives
+    torch's own FP32 arithmetic (cuFFT on the GPU) for comparison."""
+    y = torch.nn.functional.pad(x.to(dtype), (pad, pad + right_pad), mode=pad_mode) if (pad or right_pad) else x.to(dtype)
+    X = torch.stft(y.reshape(-1, y.shape[-1]), n_fft, hop, window=window.to(x.device, dtype), center=True,
                    return_complex=True, pad_mode="reflect")
     X = X.reshape(*x.shape[:-1], *X.shape[-2:])
     return X[..., drop_edge:X.shape[-1] - drop_edge] if drop_edge else X

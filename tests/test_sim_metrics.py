@@ -52,13 +52,18 @@ def test_default_losses_match_reference_golden(sim):
     assert ours <= max(1e-4, 1.25 * ref_err), (ours, ref_err)
 
 
-@pytest.mark.parametrize("wl,hop,mel,ms,pt,wt,kw", [
+# (window, hop, mel = (sr, n_mels, fmin, fmax), match_stride, padding, window type, loss options): both MEL modes, every
+# padding mode, match_stride, an odd hop and non-default weights (also per cell in tests/test_sim_loss_accuracy.py)
+ENGINE_GEOMETRIES = [
     (256, 64, None, False, "reflect", "hann", {}),
     (128, 32, (SR, 20, 0.0, None), True, "constant", "hann", {}),
     (64, 13, None, False, "replicate", "hann", dict(pow=1.0, clamp_eps=1e-4)),          # odd hop
     (512, 128, (SR, 40, 100.0, 6000.0), False, "reflect", "sqrt_hann", dict(log_weight=0.5, mag_weight=2.0)),
     (2048, 512, (SR, 80, 0.0, None), True, "replicate", "hann", dict(mag_weight=0.0)),
-])
+]
+
+
+@pytest.mark.parametrize("wl,hop,mel,ms,pt,wt,kw", ENGINE_GEOMETRIES)
 def test_engine_loss_and_both_gradients_match_float64(sim, wl, hop, mel, ms, pt, wt, kw):
     """Engine.spectral_loss + the STFT adjoint against torch.autograd in float64, for x and y, both MEL modes, every
     padding mode, match_stride, an odd hop and non-default weights."""
