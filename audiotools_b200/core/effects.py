@@ -113,10 +113,15 @@ class EffectMixin:
         self.audio_data = self.audio_data * peak_gain
         return self
 
-    def normalize(self, db=-24.0, _bypass=None):
+    def normalize(self, db=-24.0, _bypass=None, *, true_peak_limit=None):
         """Scale every item to ``db`` LUFS (scalar or [B]) (ref :200-220).  The per-item gain comes
         out of the loudness kernel; the multiply is deferred and fused into the next kernel that
-        reads the samples (``stft`` / ``mel_spectrogram``) or materialised on first access."""
+        reads the samples (``stft`` / ``mel_spectrogram``) or materialised on first access.
+
+        ``true_peak_limit`` (dBTP, scalar or [B]; an extension): an item whose true peak (``true_peak()``, measured
+        before the gain) would exceed the limit after normalisation gets the smaller gain that puts it at the limit,
+        ``min(gain, 10^((limit - true_peak) / 20))``, so it ends below ``db`` LUFS.  Other items keep the gain they
+        get without a limit, bit for bit.  The gain stays a constant of the backward pass."""
         db = util.ensure_tensor(db).to(self.device).float().reshape(-1)
         if self._loudness is None and self._pending_gain is None:
             T = self.signal_length
@@ -130,6 +135,14 @@ class EffectMixin:
         else:
             measured = self.loudness()
             gain = torch.exp((db - measured) * float(np.float32(self.GAIN_FACTOR)))
+        if true_peak_limit is not None:
+            limit = float(true_peak_limit) if isinstance(true_peak_limit, (int, float)) else \
+                util.ensure_tensor(true_peak_limit).to(gain.device).float().reshape(-1)  # a number needs no copy
+            peak = _engine().true_peak(self._audio_data.detach(), self.sample_rate)["db"]
+            cap = torch.exp((limit - peak) * float(np.float32(self.GAIN_FACTOR)))
+            if self._pending_gain is not None:  # still deferred (a cached loudness was used): it scales the peak too
+                cap = cap / self._pending_gain
+            gain = torch.minimum(gain, cap)
         if _bypass is not None:  # items the transform's mask does not select keep their samples (gain exactly 1)
             gain = torch.where(torch.as_tensor(_bypass).to(gain.device).bool().reshape(-1), torch.ones_like(gain), gain)
         self._defer_gain(gain)

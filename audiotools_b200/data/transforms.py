@@ -280,17 +280,19 @@ class VolumeChange(BaseTransform):
 
 
 class VolumeNorm(BaseTransform):
-    """``signal.normalize(db)`` -- LUFS normalisation (ref :973-1003)."""
+    """``signal.normalize(db)`` -- LUFS normalisation (ref :973-1003).  ``true_peak_limit`` (dBTP, an extension):
+    passed to ``normalize``, which lowers the gain of items whose true peak would exceed it.  It is not drawn."""
 
-    def __init__(self, db: tuple = ("const", -24), name: str = None, prob: float = 1.0):
+    def __init__(self, db: tuple = ("const", -24), name: str = None, prob: float = 1.0, true_peak_limit: float = None):
         super().__init__(name=name, prob=prob)
         self.db = db
+        self.true_peak_limit = true_peak_limit
 
     def _instantiate(self, state: RandomState):
         return {"db": util.sample_from_dist(self.db, state)}
 
     def _transform(self, signal, db, _bypass=None):
-        return signal.normalize(db, _bypass=_bypass)
+        return signal.normalize(db, _bypass=_bypass, true_peak_limit=self.true_peak_limit)
 
 
 class GlobalVolumeNorm(BaseTransform):

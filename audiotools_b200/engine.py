@@ -562,6 +562,29 @@ class Engine:
             out["momentary"], out["short_term"] = mom, st
         return out
 
+    def true_peak_taps(self, sample_rate: float) -> np.ndarray:
+        """The float32 taps ``true_peak`` interpolates with at this rate: [L - 1, 12] (phase p = 1 .. L-1, tap
+        d = -6 .. 5), empty for L = 1 (``b2a_true_peak_taps``)."""
+        L = self.lib.b2a_true_peak_factor(float(sample_rate))
+        self.lib.check(min(L, 0))
+        taps = np.zeros((L - 1, 12), dtype=np.float32)
+        self.lib.check(self.lib.b2a_true_peak_taps(L, taps.ctypes.data_as(ctypes.c_void_p)))
+        return taps
+
+    def true_peak(self, x: torch.Tensor, sample_rate: float):
+        """True-peak level of ``x`` [B, C, T] (``b2a_true_peak_f32``): ``rows`` [B, C], the linear peak of every row
+        oversampled by 4 (below 96 kHz), 2 (below 192 kHz) or 1, and ``db`` [B], 20 log10 of each item's channel
+        maximum in dBTP (-inf for silence).  float32 on x's device."""
+        x = self._prep(x, "x")
+        assert x.ndim == 3, "x must be [B, C, T]"
+        B, C, T = x.shape
+        L = self.lib.b2a_true_peak_factor(float(sample_rate))
+        self.lib.check(min(L, 0))
+        rows = torch.empty(B, C, dtype=torch.float32, device=x.device)
+        db = torch.empty(B, dtype=torch.float32, device=x.device)
+        self._call(self.lib.b2a_true_peak_f32, _dptr(x), B, C, T, L, _dptr(rows), _dptr(db), self._stream(x))
+        return {"rows": rows, "db": db}
+
     def gain(self, x: torch.Tensor, gain: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``x[b] * gain[b]`` (ref:audiotools/core/effects.py:219,237)."""
         x = self._prep(x, "x")

@@ -312,6 +312,25 @@ int b2a_loudness_stats_f32(const float* x, int64_t B, int C, int64_t T, int64_t 
                            const double* chan_gain_h, float* stats_out, float* momentary_out,
                            float* short_term_out, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- true-peak level (ITU-R BS.1770 Annex 2 structure, this package's interpolator; csrc/truepeak.cu) -----------
+ * The largest |value| of each row oversampled by L with a 12-tap Hann-windowed-sinc polyphase FIR:
+ *   b2a_true_peak_factor   L for a sample rate: 4 below 96 kHz, 2 below 192 kHz, else 1 (host only; B2A_E_INVALID for
+ *                          a rate that is not positive and finite)
+ *   b2a_true_peak_taps     the float taps the kernel uses (host only): taps_h [(factor - 1) * 12], phase p = 1 .. L-1
+ *                          at [(p - 1) * 12], tap d = -6 .. 5 at [+ d + 6]; h_p[d] = float(sinc(u) (1 + cos(pi u / 6)) / 2)
+ *                          with u = d + p / L, designed in double.  No per-phase renormalisation.
+ *   b2a_true_peak_f32      x [B, C, T]; the instants are every (n, p) with n < T - 1 plus (T - 1, 0), where phase 0 is
+ *                          x[n] itself and phase p >= 1 is sum_{d=-6..5} h_p[d] x[n - d] (x = 0 outside [0, T)).
+ *                          row_peak [B * C] linear max |y| over those instants (>= max |x|, bit for bit; NaN or +inf
+ *                          for a row with a non-finite sample); item_db nullable [B]: 20 log10 of the channel maximum
+ *                          (-inf for silence).  factor 1, 2 or 4.  Two launches (one without item_db) and a memset; the
+ *                          maximum is exact and order-independent: reruns are bit-identical.  Not the Annex's coefficient table:
+ *                          values are not those of ffmpeg / libebur128. */
+int b2a_true_peak_factor(double rate);
+int b2a_true_peak_taps(int factor, float* taps_h);
+int b2a_true_peak_f32(const float* x, int64_t B, int C, int64_t T, int factor, float* row_peak, float* item_db,
+                      void* stream);
+
 /* ---- per-item gain ---------------------------------------------------------------------
  * x[b, :, :] * gain[b]  (EffectMixin.normalize / volume_change, effects.py:219,237).
  * out may alias x.  per_item = C*T. */
