@@ -42,6 +42,9 @@ SIGNATURES = {
     "b2a_true_peak_factor": (c_int, [c_double]),
     "b2a_true_peak_taps": (c_int, [c_int, c_void_p]),
     "b2a_true_peak_f32": (c_int, [c_void_p, c_int64, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
+    "b2a_limiter_workspace_bytes": (c_size_t, [c_int64, c_int, c_int64]),
+    "b2a_limiter_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int64, c_int, c_void_p, c_int, c_float, c_void_p,
+                                c_void_p, c_void_p, c_void_p]),
     "b2a_gain_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
     "b2a_fftconv_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64, c_int64]),
     "b2a_fftconv_f32": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int,

@@ -121,7 +121,8 @@ class EffectMixin:
         ``true_peak_limit`` (dBTP, scalar or [B]; an extension): an item whose true peak (``true_peak()``, measured
         before the gain) would exceed the limit after normalisation gets the smaller gain that puts it at the limit,
         ``min(gain, 10^((limit - true_peak) / 20))``, so it ends below ``db`` LUFS.  Other items keep the gain they
-        get without a limit, bit for bit.  The gain stays a constant of the backward pass."""
+        get without a limit, bit for bit.  The gain stays a constant of the backward pass.  To keep the loudness and
+        still meet a ceiling, follow ``normalize(db)`` with :meth:`limit`, which reshapes the waveform around the overs."""
         db = util.ensure_tensor(db).to(self.device).float().reshape(-1)
         if self._loudness is None and self._pending_gain is None:
             T = self.signal_length
@@ -147,6 +148,23 @@ class EffectMixin:
             gain = torch.where(torch.as_tensor(_bypass).to(gain.device).bool().reshape(-1), torch.ones_like(gain), gain)
         self._defer_gain(gain)
         self._measured_loudness = measured  # extension: the LUFS the gain was derived from (logging / statistics)
+        return self
+
+    def limit(self, ceiling_db=-1.0, lookahead: float = 0.0015, release: float = 0.05):
+        """Look-ahead true-peak limiter (an extension; DESIGN.md K18): every item is multiplied by one gain series,
+        shared by its channels, that dips around each instant where the true-peak envelope (``true_peak()``'s
+        interpolator) passes ``ceiling_db`` (dBTP, scalar or [B]) and is exactly 1 elsewhere, so
+        ``normalize(-16).limit(-1)`` keeps the loudness that a whole-item cap would give up.  ``lookahead`` (s) is the
+        hold before an over and the length of the box attack, ``release`` (s) the time constant of the recovery; the
+        windows are centred, so nothing is delayed.  Samples away from every over, and items that never pass the
+        ceiling, come back bit for bit.  A gain deferred by ``normalize`` / ``volume_change`` is applied inside the
+        limiter's own passes.  No backward: a signal that requires a gradient raises ``NotImplementedError``."""
+        if not isinstance(ceiling_db, (int, float)):  # a number needs no copy to the device
+            ceiling_db = util.ensure_tensor(ceiling_db).to(self.device).float().reshape(-1)
+        # the setter drops the consumed gain and the loudness cache
+        self.audio_data = _engine().limit(self._audio_data, self.sample_rate, ceiling_db, lookahead, release,
+                                          gain=self._pending_gain)
+        self.stft_data = None
         return self
 
     def volume_change(self, db, _bypass=None):

@@ -295,6 +295,24 @@ class VolumeNorm(BaseTransform):
         return signal.normalize(db, _bypass=_bypass, true_peak_limit=self.true_peak_limit)
 
 
+class Limiter(BaseTransform):
+    """``signal.limit(ceiling)`` -- look-ahead true-peak limiter (an extension; the reference has none).  ``ceiling``
+    (dBTP) is drawn per item; ``lookahead`` and ``release`` (seconds) are not drawn."""
+
+    def __init__(self, ceiling: tuple = ("const", -1.0), lookahead: float = 0.0015, release: float = 0.05,
+                 name: str = None, prob: float = 1.0):
+        super().__init__(name=name, prob=prob)
+        self.ceiling = ceiling
+        self.lookahead = lookahead
+        self.release = release
+
+    def _instantiate(self, state: RandomState):
+        return {"ceiling": util.sample_from_dist(self.ceiling, state)}
+
+    def _transform(self, signal, ceiling):
+        return signal.limit(ceiling, lookahead=self.lookahead, release=self.release)
+
+
 class GlobalVolumeNorm(BaseTransform):
     """Normalise using the loudness of the whole source file, read from
     ``signal.metadata["loudness"]`` (ref :1006-1050)."""

@@ -585,6 +585,57 @@ class Engine:
         self._call(self.lib.b2a_true_peak_f32, _dptr(x), B, C, T, L, _dptr(rows), _dptr(db), self._stream(x))
         return {"rows": rows, "db": db}
 
+    LIMITER_MAX_LOOKAHEAD = 1024  # samples (csrc/limiter.cu)
+
+    def limiter_params(self, sample_rate: float, ceiling_db, lookahead: float, release: float, B: int, device):
+        """What ``limit`` hands to ``b2a_limiter_f32``: the oversampling factor, the linear ceiling [B] (float32 on
+        ``device``; a Python number is filled in without a host copy), the look-ahead in samples and the float32
+        release coefficient exp(-1 / (release * rate))."""
+        L = self.lib.b2a_true_peak_factor(float(sample_rate))
+        self.lib.check(min(L, 0))
+        A = int(round(float(lookahead) * float(sample_rate)))
+        if not 0 <= A <= self.LIMITER_MAX_LOOKAHEAD:
+            raise ValueError(f"limit: a lookahead of {lookahead} s is {A} samples at {sample_rate} Hz; "
+                             f"0 .. {self.LIMITER_MAX_LOOKAHEAD} are supported")
+        if not float(release) > 0:
+            raise ValueError(f"limit: release must be positive, got {release}")
+        a = float(np.float32(np.exp(-1.0 / (float(release) * float(sample_rate)))))
+        if isinstance(ceiling_db, (int, float)):
+            ceiling = torch.full((B,), float(np.float32(10.0 ** (float(ceiling_db) / 20.0))), dtype=torch.float32,
+                                 device=device)
+        else:
+            db = self._per_item(ceiling_db, B, "ceiling_db", device)
+            ceiling = torch.exp(db * float(np.float32(np.log(10) / 20)))
+        return L, ceiling, A, a
+
+    def limit(self, x: torch.Tensor, sample_rate: float, ceiling_db, lookahead: float = 0.0015, release: float = 0.05,
+              gain: Optional[torch.Tensor] = None, want_reduction: bool = False, out: Optional[torch.Tensor] = None):
+        """Look-ahead true-peak limiter of ``x`` [B, C, T] (``b2a_limiter_f32``, DESIGN.md K18): every item is
+        multiplied by one gain series ``1 - r[n]`` that keeps the true-peak envelope of ``true_peak``'s interpolator
+        at or under ``ceiling_db`` (dBTP, a number or 1 / B values) and is exactly 1 away from the overs.
+        ``lookahead`` (s) is both the hold and the length of the box attack, ``release`` (s) the time constant of the
+        exponential release.  ``gain`` [B]: the item is ``float32(gain * x)`` (a deferred normalisation gain needs no
+        pass of its own).  ``out`` may be ``x``.  Returns the limited signal, or ``(signal, r [B, T])`` with
+        ``want_reduction``."""
+        x = self._prep(x, "x")
+        assert x.ndim == 3, "x must be [B, C, T]"
+        B, C, T = x.shape
+        L, ceiling, A, a = self.limiter_params(sample_rate, ceiling_db, lookahead, release, B, x.device)
+        if gain is not None:
+            gain = self._prep(gain.reshape(-1), "gain")
+            assert gain.numel() == B
+        if out is None:
+            out = torch.empty_like(x)
+        assert out.shape == x.shape and out.dtype == torch.float32 and out.is_contiguous() and out.device == x.device
+        ws_bytes = int(self.lib.b2a_limiter_workspace_bytes(B, C, T))
+        if ws_bytes == 0:
+            raise _lib.B2AError(f"limit: unsupported shape {tuple(x.shape)}")
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        red = torch.empty(B, T, dtype=torch.float32, device=x.device) if want_reduction else None
+        self._call(self.lib.b2a_limiter_f32, _dptr(x), _dptr(gain), B, C, T, L, _dptr(ceiling), A, a, _dptr(out),
+                   _dptr(red), _dptr(ws), self._stream(x))
+        return (out, red) if want_reduction else out
+
     def gain(self, x: torch.Tensor, gain: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``x[b] * gain[b]`` (ref:audiotools/core/effects.py:219,237)."""
         x = self._prep(x, "x")

@@ -331,6 +331,23 @@ int b2a_true_peak_taps(int factor, float* taps_h);
 int b2a_true_peak_f32(const float* x, int64_t B, int C, int64_t T, int factor, float* row_peak, float* item_db,
                       void* stream);
 
+/* ---- look-ahead true-peak limiter (csrc/limiter.cu) ----------------------------------------------------------------
+ * One gain series per item that keeps the true-peak envelope of b2a_true_peak_f32's interpolator under a ceiling and is
+ * exactly 1 away from the overs.  x [B, C, T]; gain nullable [B] (x means float(gain[b] x) below); ceiling [B] linear;
+ * lookahead = A samples, 0 .. 1024; release_a = exp(-1 / (release seconds * rate)) in [0, 1); factor 1, 2 or 4.
+ *   e[n]  = max over the channels of max(|x[n]|, max_p |y[n, p]|, max_p |y[n - 1, p]|), y and its instants as in
+ *           b2a_true_peak_f32
+ *   q[n]  = 0 where e[n] <= ceiling, else 1 - ceiling / e[n] (NaN where e[n] is not finite)
+ *   h[n]  = max q[j], |j - n| <= A;  d[n] = max(h[n], a d[n - 1]), then d < 2^-26 counts as 0
+ *   r[n]  = mean d[j], |j - n| <= A, over the j inside [0, T);  out[b, c, n] = x[b, c, n] (1 - r[n])
+ * out [B, C, T] may alias x; reduction nullable [B, T] receives r.  Where r = 0 out equals x bit for bit.  A NaN or inf
+ * sample makes r NaN from at most 2 A + 6 samples before it to the end of that item; other items are unaffected.
+ * ws: b2a_limiter_workspace_bytes(B, C, T) bytes of scratch (0 for a bad shape), contents irrelevant on entry.  Three
+ * launches, no host sync; reruns and batch-versus-single calls are bit-identical. */
+size_t b2a_limiter_workspace_bytes(int64_t B, int C, int64_t T);
+int b2a_limiter_f32(const float* x, const float* gain, int64_t B, int C, int64_t T, int factor, const float* ceiling,
+                    int lookahead, float release_a, float* out, float* reduction, void* ws, void* stream);
+
 /* ---- per-item gain ---------------------------------------------------------------------
  * x[b, :, :] * gain[b]  (EffectMixin.normalize / volume_change, effects.py:219,237).
  * out may alias x.  per_item = C*T. */
