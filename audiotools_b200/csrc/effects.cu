@@ -10,6 +10,7 @@
 //   b2a_order_stats_f32  k-th smallest values of one row           ref :452-453 (torch.quantile's sorted gather), by
 //                        (exact: 4-pass radix select)               radix selection instead of a full sort
 //   b2a_clamp_items_f32  y = min(max(x, lo[item]), hi[item])       ref :459
+//   b2a_gain_f32         y = g[item] * x                          ref :219, :237 (normalize / volume_change)
 #include "b2a_common.h"
 
 namespace b2a {
@@ -17,25 +18,42 @@ namespace effects {
 
 constexpr int TPB = 256;
 
-__device__ __forceinline__ int64_t grid_threads() { return (int64_t)gridDim.x * blockDim.x; }
+// The walk of every element-wise kernel over its row (grid.y) of n floats, grid-stride: vec4(i) for the float4 at each
+// i = 0, 4, 8, ... when vec_ok (n % 4 == 0 and the row's pointers 16-byte aligned), else one(i) for every element.
+template <class V4, class V1>
+__device__ __forceinline__ void walk(int64_t n, int vec_ok, V4 vec4, V1 one) {
+  const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nt = (int64_t)gridDim.x * blockDim.x;
+  if (vec_ok) {
+    for (int64_t i = gid; i < n >> 2; i += nt) vec4(4 * i);
+  } else {
+    for (int64_t i = gid; i < n; i += nt) one(i);
+  }
+}
+
+// y = f(x) over one row, streamed
+template <class F>
+__device__ __forceinline__ void map_row(const float* __restrict__ x, float* __restrict__ y, int64_t n, int vec_ok, F f) {
+  walk(n, vec_ok,
+       [&](int64_t i) {
+         float4 v = ld_stream4(x + i);
+         v.x = f(v.x); v.y = f(v.y); v.z = f(v.z); v.w = f(v.w);
+         st_stream4(y + i, v);
+       },
+       [&](int64_t i) { y[i] = f(x[i]); });
+}
 
 // peak must be zeroed by the caller (memset inside the entry point); |x| >= 0, so float bits order like ints
 __global__ void __launch_bounds__(TPB) absmax_kernel(const float* __restrict__ x, int64_t T, int vec_ok,
                                                      float* __restrict__ peak) {
   const int row = blockIdx.y;
   const float* xr = x + (size_t)row * (size_t)T;
-  const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nt = grid_threads();
   float m = 0.f;
-  if (vec_ok) {
-    const int64_t n4 = T >> 2;
-    for (int64_t i = gid; i < n4; i += nt) {
-      const float4 v = ld_stream4(xr + 4 * i);
-      m = fmaxf(fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
-    }
-    for (int64_t i = (n4 << 2) + gid; i < T; i += nt) m = fmaxf(m, fabsf(xr[i]));
-  } else {
-    for (int64_t i = gid; i < T; i += nt) m = fmaxf(m, fabsf(xr[i]));
-  }
+  walk(T, vec_ok,
+       [&](int64_t i) {
+         const float4 v = ld_stream4(xr + i);
+         m = fmaxf(fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
+       },
+       [&](int64_t i) { m = fmaxf(m, fabsf(xr[i])); });
   m = warp_max(m);
   __shared__ float s[TPB / 32];
   if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = m;
@@ -62,19 +80,14 @@ __global__ void __launch_bounds__(TPB) rows_kernel(const float* __restrict__ x, 
   } else {
     p0 = __ldg(a + row); p1 = __ldg(b + row);
   }
-  auto f = [&](float v) { return MODE == 0 ? v * p0 : fminf(fmaxf(v, p0), p1); };
-  const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nt = grid_threads();
-  if (vec_ok) {
-    const int64_t n4 = T >> 2;
-    for (int64_t i = gid; i < n4; i += nt) {
-      float4 v = ld_stream4(xr + 4 * i);
-      v.x = f(v.x); v.y = f(v.y); v.z = f(v.z); v.w = f(v.w);
-      st_stream4(yr + 4 * i, v);
-    }
-    for (int64_t i = (n4 << 2) + gid; i < T; i += nt) yr[i] = f(xr[i]);
-  } else {
-    for (int64_t i = gid; i < T; i += nt) yr[i] = f(xr[i]);
-  }
+  map_row(xr, yr, T, vec_ok, [&](float v) { return MODE == 0 ? v * p0 : fminf(fmaxf(v, p0), p1); });
+}
+
+__global__ void __launch_bounds__(TPB) gain_kernel(const float* __restrict__ x, float* __restrict__ out,
+                                                   int64_t per_item, int vec_ok, const float* __restrict__ gain) {
+  const int b = blockIdx.y;
+  const float g = __ldg(gain + b);
+  map_row(x + (size_t)b * per_item, out + (size_t)b * per_item, per_item, vec_ok, [&](float v) { return v * g; });
 }
 
 __global__ void __launch_bounds__(TPB) mix_kernel(const float* __restrict__ x, const float* __restrict__ other,
@@ -85,21 +98,14 @@ __global__ void __launch_bounds__(TPB) mix_kernel(const float* __restrict__ x, c
   const float* xr = x + (size_t)b * per_item;
   const float* orow = other + (size_t)b * per_item;
   float* yr = out + (size_t)b * per_item;
-  const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nt = grid_threads();
   // the reference multiplies first (normalize) and adds afterwards: two roundings, not one fused multiply-add
-  if (vec_ok) {
-    const int64_t n4 = per_item >> 2;
-    for (int64_t i = gid; i < n4; i += nt) {
-      const float4 a = ld_stream4(xr + 4 * i), o = ld_stream4(orow + 4 * i);
-      float4 v;
-      v.x = __fadd_rn(a.x, __fmul_rn(o.x, g)); v.y = __fadd_rn(a.y, __fmul_rn(o.y, g));
-      v.z = __fadd_rn(a.z, __fmul_rn(o.z, g)); v.w = __fadd_rn(a.w, __fmul_rn(o.w, g));
-      st_stream4(yr + 4 * i, v);
-    }
-    for (int64_t i = (n4 << 2) + gid; i < per_item; i += nt) yr[i] = __fadd_rn(xr[i], __fmul_rn(orow[i], g));
-  } else {
-    for (int64_t i = gid; i < per_item; i += nt) yr[i] = __fadd_rn(xr[i], __fmul_rn(orow[i], g));
-  }
+  auto f = [&](float a, float o) { return __fadd_rn(a, __fmul_rn(o, g)); };
+  walk(per_item, vec_ok,
+       [&](int64_t i) {
+         const float4 a = ld_stream4(xr + i), o = ld_stream4(orow + i);
+         st_stream4(yr + i, make_float4(f(a.x, o.x), f(a.y, o.y), f(a.z, o.z), f(a.w, o.w)));
+       },
+       [&](int64_t i) { yr[i] = f(xr[i], orow[i]); });
 }
 
 // ref:audiotools/core/effects.py:481-491 (linear) and :509-523 (mu-law), operation by operation in float32
@@ -131,19 +137,7 @@ __global__ void __launch_bounds__(TPB) quantize_kernel(const float* __restrict__
   const float mu = __fadd_rn(q, -1.0f), l1p = log1pf(mu);
   const float* xr = x + (size_t)b * per_item;
   float* yr = out + (size_t)b * per_item;
-  auto f = [&](float v) { return mulaw ? quant_mulaw(v, mu, l1p) : quant_linear(v, q); };
-  const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nt = grid_threads();
-  if (vec_ok) {
-    const int64_t n4 = per_item >> 2;
-    for (int64_t i = gid; i < n4; i += nt) {
-      float4 v = ld_stream4(xr + 4 * i);
-      v.x = f(v.x); v.y = f(v.y); v.z = f(v.z); v.w = f(v.w);
-      st_stream4(yr + 4 * i, v);
-    }
-    for (int64_t i = (n4 << 2) + gid; i < per_item; i += nt) yr[i] = f(xr[i]);
-  } else {
-    for (int64_t i = gid; i < per_item; i += nt) yr[i] = f(xr[i]);
-  }
+  map_row(xr, yr, per_item, vec_ok, [&](float v) { return mulaw ? quant_mulaw(v, mu, l1p) : quant_linear(v, q); });
 }
 
 // ---- exact k-th smallest by 4-pass (8 bits each) radix selection: one CTA per requested order statistic
@@ -185,10 +179,20 @@ __global__ void __launch_bounds__(ST) order_stat_kernel(const float* __restrict_
   if (tid == 0) out[blockIdx.x] = ord_val(prefix);
 }
 
-static unsigned grid_x(int64_t work, int64_t rows) {
-  const int64_t want = (work + TPB - 1) / TPB;
-  int64_t cap = (int64_t)B2A_NUM_SMS * 8 / (rows > 0 ? rows : 1) + 1;  // ~8 resident CTAs per SM across the rows
-  return (unsigned)(want < cap ? (want < 1 ? 1 : want) : cap);
+// The checks and the launch of an element-wise kernel over `rows` rows of n floats: grid.y = row (so at most 65535
+// rows), grid.x ~8 resident CTAs per SM across the rows, grid-stride inside.  vec_ok: n % 4 == 0 and `ptrs`, the OR of
+// the row pointers, 16-byte aligned.
+struct RowsLaunch {
+  dim3 grid;
+  int vec_ok;
+};
+static int rows_launch(const char* op, bool non_null, int64_t rows, int64_t n, uintptr_t ptrs, RowsLaunch* l) {
+  B2A_REQUIRE(non_null, B2A_E_INVALID, "%s: null pointer", op);
+  B2A_REQUIRE(rows >= 1 && rows <= 65535 && n >= 1, B2A_E_INVALID, "%s: bad shape", op);
+  l->vec_ok = ptrs % 16 == 0 && n % 4 == 0;
+  const int64_t want = ((l->vec_ok ? n / 4 : n) + TPB - 1) / TPB, cap = (int64_t)B2A_NUM_SMS * 8 / rows + 1;
+  l->grid = dim3((unsigned)(want < cap ? want : cap), (unsigned)rows);
+  return B2A_OK;
 }
 
 }  // namespace effects
@@ -299,55 +303,60 @@ alter_drr_kernel(const float* __restrict__ x, float* __restrict__ out, int T, in
 using namespace b2a::effects;
 
 extern "C" int b2a_row_absmax_f32(const float* x, int64_t rows, int64_t T, float* peak, void* stream) {
-  B2A_REQUIRE(x && peak, B2A_E_INVALID, "row_absmax: null pointer");
-  B2A_REQUIRE(rows >= 1 && rows <= 65535 && T >= 1, B2A_E_INVALID, "row_absmax: bad shape");
+  RowsLaunch l;
+  const int rc = rows_launch("row_absmax", x && peak, rows, T, (uintptr_t)x, &l);
+  if (rc != B2A_OK) return rc;
   B2A_CUDA_OK(cudaMemsetAsync(peak, 0, (size_t)rows * sizeof(float), (cudaStream_t)stream));
-  const int vec_ok = (((uintptr_t)x) % 16 == 0) && (T % 4 == 0);
-  B2A_LAUNCH(absmax_kernel, dim3(grid_x(vec_ok ? T / 4 : T, rows), (unsigned)rows), dim3(TPB), 0, stream, x, T, vec_ok, peak);
+  B2A_LAUNCH(absmax_kernel, l.grid, dim3(TPB), 0, stream, x, T, l.vec_ok, peak);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }
 
 extern "C" int b2a_limit_peak_f32(const float* x, float* out, int64_t rows, int64_t T, const float* peak, float max_abs,
                                   void* stream) {
-  B2A_REQUIRE(x && out && peak, B2A_E_INVALID, "limit_peak: null pointer");
-  B2A_REQUIRE(rows >= 1 && rows <= 65535 && T >= 1, B2A_E_INVALID, "limit_peak: bad shape");
-  const int vec_ok = (((uintptr_t)x | (uintptr_t)out) % 16 == 0) && (T % 4 == 0);
-  B2A_LAUNCH(rows_kernel<0>, dim3(grid_x(vec_ok ? T / 4 : T, rows), (unsigned)rows), dim3(TPB), 0, stream, x, out, T, vec_ok,
-             peak, (const float*)nullptr, max_abs);
+  RowsLaunch l;
+  const int rc = rows_launch("limit_peak", x && out && peak, rows, T, (uintptr_t)x | (uintptr_t)out, &l);
+  if (rc != B2A_OK) return rc;
+  B2A_LAUNCH(rows_kernel<0>, l.grid, dim3(TPB), 0, stream, x, out, T, l.vec_ok, peak, (const float*)nullptr, max_abs);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }
 
 extern "C" int b2a_clamp_items_f32(const float* x, float* out, int64_t B, int64_t per_item, const float* lo,
                                    const float* hi, void* stream) {
-  B2A_REQUIRE(x && out && lo && hi, B2A_E_INVALID, "clamp_items: null pointer");
-  B2A_REQUIRE(B >= 1 && B <= 65535 && per_item >= 1, B2A_E_INVALID, "clamp_items: bad shape");
-  const int vec_ok = (((uintptr_t)x | (uintptr_t)out) % 16 == 0) && (per_item % 4 == 0);
-  B2A_LAUNCH(rows_kernel<1>, dim3(grid_x(vec_ok ? per_item / 4 : per_item, B), (unsigned)B), dim3(TPB), 0, stream, x, out,
-             per_item, vec_ok, lo, hi, 0.f);
+  RowsLaunch l;
+  const int rc = rows_launch("clamp_items", x && out && lo && hi, B, per_item, (uintptr_t)x | (uintptr_t)out, &l);
+  if (rc != B2A_OK) return rc;
+  B2A_LAUNCH(rows_kernel<1>, l.grid, dim3(TPB), 0, stream, x, out, per_item, l.vec_ok, lo, hi, 0.f);
+  B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
+}
+
+extern "C" int b2a_gain_f32(const float* x, float* out, int64_t B, int64_t per_item, const float* gain, void* stream) {
+  RowsLaunch l;
+  const int rc = rows_launch("gain", x && out && gain, B, per_item, (uintptr_t)x | (uintptr_t)out, &l);
+  if (rc != B2A_OK) return rc;
+  B2A_LAUNCH(gain_kernel, l.grid, dim3(TPB), 0, stream, x, out, per_item, l.vec_ok, gain);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }
 
 extern "C" int b2a_mix_f32(const float* x, const float* other, const float* other_gain, float* out, int64_t B,
                            int64_t per_item, void* stream) {
-  B2A_REQUIRE(x && other && out, B2A_E_INVALID, "mix: null pointer");
-  B2A_REQUIRE(B >= 1 && B <= 65535 && per_item >= 1, B2A_E_INVALID, "mix: bad shape");
-  const int vec_ok = (((uintptr_t)x | (uintptr_t)other | (uintptr_t)out) % 16 == 0) && (per_item % 4 == 0);
-  B2A_LAUNCH(mix_kernel, dim3(grid_x(vec_ok ? per_item / 4 : per_item, B), (unsigned)B), dim3(TPB), 0, stream, x, other,
-             other_gain, out, per_item, vec_ok);
+  RowsLaunch l;
+  const int rc = rows_launch("mix", x && other && out, B, per_item, (uintptr_t)x | (uintptr_t)other | (uintptr_t)out, &l);
+  if (rc != B2A_OK) return rc;
+  B2A_LAUNCH(mix_kernel, l.grid, dim3(TPB), 0, stream, x, other, other_gain, out, per_item, l.vec_ok);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }
 
 extern "C" int b2a_quantize_f32(const float* x, float* out, int64_t B, int64_t per_item, const float* channels, int mulaw,
                                 void* stream) {
-  B2A_REQUIRE(x && out && channels, B2A_E_INVALID, "quantize: null pointer");
-  B2A_REQUIRE(B >= 1 && B <= 65535 && per_item >= 1, B2A_E_INVALID, "quantize: bad shape");
-  const int vec_ok = (((uintptr_t)x | (uintptr_t)out) % 16 == 0) && (per_item % 4 == 0);
-  B2A_LAUNCH(quantize_kernel, dim3(grid_x(vec_ok ? per_item / 4 : per_item, B), (unsigned)B), dim3(TPB), 0, stream, x, out,
-             per_item, vec_ok, channels, mulaw ? 1 : 0);
+  RowsLaunch l;
+  const int rc = rows_launch("quantize", x && out && channels, B, per_item, (uintptr_t)x | (uintptr_t)out, &l);
+  if (rc != B2A_OK) return rc;
+  B2A_LAUNCH(quantize_kernel, l.grid, dim3(TPB), 0, stream, x, out, per_item, l.vec_ok, channels, mulaw ? 1 : 0);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }

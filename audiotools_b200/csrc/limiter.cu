@@ -27,23 +27,19 @@
 //                          below 2^-26 skips all of that: it copies, or in place without a gain does nothing.
 // Every maximum is taken on the bits of non-negative floats, so NaN propagates without a branch; sums are per item and
 // in a fixed order: reruns and batch-versus-single calls are bit-identical.
-#include "b2a_common.h"
+#include "truepeak_internal.h"
 
 namespace b2a {
 namespace limiter {
 
-constexpr int TPB = 256;             // threads per CTA of the envelope kernel
-constexpr int RUN = 16;              // consecutive samples per thread
-constexpr int CHUNK = TPB * RUN;     // samples of an item per CTA work item (tests cover T = CHUNK +- 1)
-constexpr int HALO = 8;              // reach of the taps, as in truepeak.cu
-constexpr int NTAP = 12;
+// truepeak_internal.h: TPB threads per CTA of the envelope kernel, runs of RUN samples per thread, chunks of CHUNK
+// samples of an item per CTA work item (tests cover T = CHUNK +- 1), the taps' reach HALO, Taps, design, stage_run, phase
+using namespace truepeak;
+
 constexpr int AMAX = 1024;           // largest look-ahead in samples
 constexpr int TPB3 = 384;            // release kernel: one thread per run of the chunk plus both halos
 constexpr float TINY = 1.4901161193847656e-08f;  // 2^-26
 
-struct Taps {
-  float h[3][NTAP];  // b2a_true_peak_taps: phase p at h[p - 1], tap d (-6 .. 5) at [d + 6]
-};
 struct Decay {
   float p1[RUN + 1];       // a^k
   float p16[33];           // a^(16 m)
@@ -68,12 +64,7 @@ __device__ __forceinline__ void run_envelope(const float (&v)[RUN + 2 * HALO], c
   for (int k = -1; k < RUN; ++k) {
     unsigned m = 0;
 #pragma unroll
-    for (int p = 0; p < NP; ++p) {
-      float y = taps.h[p][0] * v[k + HALO + 6];
-#pragma unroll
-      for (int d = -5; d <= 5; ++d) y = fmaf(taps.h[p][d + 6], v[k + HALO - d], y);
-      m = max(m, __float_as_uint(fabsf(y)));
-    }
+    for (int p = 0; p < NP; ++p) m = max(m, __float_as_uint(fabsf(phase(taps, p, v, k))));
     if (EDGE && !(n0 + k >= 0 && n0 + k < T - 1)) m = 0;
     if (k >= 0) e[k] = max(__float_as_uint(fabsf(v[k + HALO])), max(m, prev));  // x is 0 outside the row
     prev = m;
@@ -128,12 +119,7 @@ __global__ void __launch_bounds__(TPB) envelope_hold_kernel(const float* __restr
           for (int k = 0; k < RUN; ++k) e[k] = 0;
         } else {
           float v[RUN + 2 * HALO];
-          const float4* s4 = reinterpret_cast<const float4*>(sx + r * RUN);
-#pragma unroll
-          for (int j = 0; j < (RUN + 2 * HALO) / 4; ++j) {
-            const float4 q = s4[j];
-            v[4 * j] = q.x, v[4 * j + 1] = q.y, v[4 * j + 2] = q.z, v[4 * j + 3] = q.w;
-          }
+          stage_run(sx + r * RUN, v);
           if (n0 >= 1 && n0 + RUN < T)
             run_envelope<NP, false>(v, taps, n0, T, e);
           else
@@ -348,8 +334,7 @@ extern "C" int b2a_limiter_f32(const float* x, const float* gain, int64_t B, int
               "limiter: release coefficient %g is not in [0, 1): the release must be positive and at most about 1e7 samples",
               (double)release_a);
   Taps taps;
-  memset(&taps, 0, sizeof(taps));
-  const int rc = b2a_true_peak_taps(factor, factor > 1 ? &taps.h[0][0] : nullptr);  // B2A_E_INVALID for a bad factor
+  const int rc = design(factor, &taps);
   if (rc != B2A_OK) return rc;
   const double a = (double)release_a;
   Decay dec;

@@ -767,31 +767,6 @@ loudness_stats_kernel(const double* __restrict__ bins, StatsParams sp, const flo
   }
 }
 
-// ---------------------------------------------------------------------------------------------
-// per-item gain
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-gain_kernel(const float* __restrict__ x, float* __restrict__ out, int64_t per_item, const float* __restrict__ gain,
-            int vec_ok) {
-  const int b = blockIdx.y;
-  const float g = __ldg(gain + b);
-  const float* xi = x + (size_t)b * per_item;
-  float* oi = out + (size_t)b * per_item;
-  const int64_t nthreads = (int64_t)gridDim.x * blockDim.x;
-  const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (vec_ok) {
-    const int64_t n4 = per_item >> 2;
-    for (int64_t i = gid; i < n4; i += nthreads) {
-      float4 v = ld_stream4(xi + 4 * i);
-      v.x *= g; v.y *= g; v.z *= g; v.w *= g;
-      st_stream4(oi + 4 * i, v);
-    }
-    for (int64_t i = (n4 << 2) + gid; i < per_item; i += nthreads) oi[i] = xi[i] * g;
-  } else {
-    for (int64_t i = gid; i < per_item; i += nthreads) oi[i] = xi[i] * g;
-  }
-}
-
 struct Geometry {
   int K, stride, q, r, nblk, nbins, nseg;
 };
@@ -1028,18 +1003,3 @@ extern "C" void b2a_k2_probe_last(int* out) {
   for (int i = 0; i < 3; ++i) out[i] = b2a::lufs::g_k2_last[i];
 }
 #endif
-
-extern "C" int b2a_gain_f32(const float* x, float* out, int64_t B, int64_t per_item, const float* gain,
-                            void* stream) {
-  B2A_REQUIRE(x && out && gain, B2A_E_INVALID, "gain: null pointer");
-  B2A_REQUIRE(B >= 1 && per_item >= 1 && B <= 65535, B2A_E_INVALID, "gain: bad shape");
-  int vec_ok = (((uintptr_t)x | (uintptr_t)out) % 16 == 0) && (per_item % 4 == 0);
-  int64_t work = vec_ok ? per_item / 4 : per_item;
-  int64_t want = (work + 255) / 256;
-  // ~8 resident CTAs per SM in total across the batch; grid-stride inside
-  int64_t cap = (int64_t)B2A_NUM_SMS * 8 / B + 1;
-  unsigned gx = (unsigned)(want < cap ? want : cap);
-  B2A_LAUNCH(gain_kernel, dim3(gx, (unsigned)B), dim3(256), 0, stream, x, out, per_item, gain, vec_ok);
-  B2A_CUDA_OK(cudaGetLastError());
-  return B2A_OK;
-}

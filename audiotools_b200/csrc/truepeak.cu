@@ -15,33 +15,13 @@
 // exact, so the per-warp atomicMax into the zeroed row buffer gives the same bits in any order.  NaN: fmaxf would drop
 // it, so phase 0 is compared as uint bits of |x| (every NaN sorts above inf); a NaN among the interpolated values needs
 // a non-finite sample, which phase 0 already reports.  item_db_kernel: the channel maximum and 20 log10.
-#include "b2a_common.h"
+// The constants, the taps, the run staging and the phase evaluation are in truepeak_internal.h.
+#include "truepeak_internal.h"
 
 namespace b2a {
 namespace truepeak {
 
-constexpr int TPB = 256;             // threads per CTA
-constexpr int RUN = 16;              // consecutive instants n per thread
-constexpr int CHUNK = TPB * RUN;     // samples of a row per CTA work item (tests cover T = CHUNK +- 1)
-constexpr int HALO = 8;              // taps reach 6 samples ahead and 5 behind; 8 keeps the float4 reads aligned
 constexpr int TILE = CHUNK + 2 * HALO;
-constexpr int NTAP = 12;
-
-struct Taps {
-  float h[3][NTAP];  // phase p (1 .. L-1) at h[p - 1], tap d (-6 .. 5) at [d + 6]
-};
-
-// Taps of factor L (1, 2 or 4), designed in double and rounded to float; B2A_E_INVALID for any other L.
-int design(int L, Taps* t) {
-  B2A_REQUIRE(L == 1 || L == 2 || L == 4, B2A_E_INVALID, "true_peak: factor must be 1, 2 or 4, got %d", L);
-  memset(t, 0, sizeof(*t));
-  for (int p = 1; p < L; ++p)
-    for (int d = -6; d <= 5; ++d) {
-      const double u = d + (double)p / L, a = M_PI * u;  // |u| < 6 and u != 0
-      t->h[p - 1][d + 6] = (float)(sin(a) / a * 0.5 * (1.0 + cos(a / 6.0)));
-    }
-  return B2A_OK;
-}
 
 // v[k + HALO] = x[n0 + k].  Folds |x[n0 + k]| into m0 (as bits) and |y[n0 + k, p]| into mi.  EDGE: the run reaches the
 // row's last sample, so only the instants inside the row count.
@@ -53,9 +33,7 @@ __device__ __forceinline__ void run_max(const float (&v)[RUN + 2 * HALO], const 
     if (!EDGE || n0 + k < T) m0 = max(m0, __float_as_uint(v[k + HALO]) & 0x7fffffffu);
 #pragma unroll
     for (int p = 0; p < NP; ++p) {
-      float y = taps.h[p][0] * v[k + HALO + 6];
-#pragma unroll
-      for (int d = -5; d <= 5; ++d) y = fmaf(taps.h[p][d + 6], v[k + HALO - d], y);
+      const float y = phase(taps, p, v, k);
       if (!EDGE || n0 + k < T - 1) mi = fmaxf(mi, fabsf(y));
     }
   }
@@ -79,12 +57,7 @@ __global__ void __launch_bounds__(TPB) true_peak_kernel(const float* __restrict_
     float mi = 0.f;
     if (n0 < T) {
       float v[RUN + 2 * HALO];
-      const float4* s4 = reinterpret_cast<const float4*>(s + threadIdx.x * RUN);
-#pragma unroll
-      for (int j = 0; j < (RUN + 2 * HALO) / 4; ++j) {
-        const float4 q = s4[j];
-        v[4 * j] = q.x, v[4 * j + 1] = q.y, v[4 * j + 2] = q.z, v[4 * j + 3] = q.w;
-      }
+      stage_run(s + threadIdx.x * RUN, v);
       if (n0 + RUN < T)
         run_max<NP, false>(v, taps, n0, T, m0, mi);
       else

@@ -562,11 +562,16 @@ class Engine:
             out["momentary"], out["short_term"] = mom, st
         return out
 
+    def _true_peak_factor(self, sample_rate: float) -> int:
+        """The oversampling factor of ``true_peak`` at this rate (``b2a_true_peak_factor``); raises for a bad rate."""
+        L = self.lib.b2a_true_peak_factor(float(sample_rate))
+        self.lib.check(min(L, 0))
+        return L
+
     def true_peak_taps(self, sample_rate: float) -> np.ndarray:
         """The float32 taps ``true_peak`` interpolates with at this rate: [L - 1, 12] (phase p = 1 .. L-1, tap
         d = -6 .. 5), empty for L = 1 (``b2a_true_peak_taps``)."""
-        L = self.lib.b2a_true_peak_factor(float(sample_rate))
-        self.lib.check(min(L, 0))
+        L = self._true_peak_factor(sample_rate)
         taps = np.zeros((L - 1, 12), dtype=np.float32)
         self.lib.check(self.lib.b2a_true_peak_taps(L, taps.ctypes.data_as(ctypes.c_void_p)))
         return taps
@@ -578,8 +583,7 @@ class Engine:
         x = self._prep(x, "x")
         assert x.ndim == 3, "x must be [B, C, T]"
         B, C, T = x.shape
-        L = self.lib.b2a_true_peak_factor(float(sample_rate))
-        self.lib.check(min(L, 0))
+        L = self._true_peak_factor(sample_rate)
         rows = torch.empty(B, C, dtype=torch.float32, device=x.device)
         db = torch.empty(B, dtype=torch.float32, device=x.device)
         self._call(self.lib.b2a_true_peak_f32, _dptr(x), B, C, T, L, _dptr(rows), _dptr(db), self._stream(x))
@@ -591,8 +595,7 @@ class Engine:
         """What ``limit`` hands to ``b2a_limiter_f32``: the oversampling factor, the linear ceiling [B] (float32 on
         ``device``; a Python number is filled in without a host copy), the look-ahead in samples and the float32
         release coefficient exp(-1 / (release * rate))."""
-        L = self.lib.b2a_true_peak_factor(float(sample_rate))
-        self.lib.check(min(L, 0))
+        L = self._true_peak_factor(sample_rate)
         A = int(round(float(lookahead) * float(sample_rate)))
         if not 0 <= A <= self.LIMITER_MAX_LOOKAHEAD:
             raise ValueError(f"limit: a lookahead of {lookahead} s is {A} samples at {sample_rate} Hz; "
