@@ -370,7 +370,8 @@ stretch_copy_kernel(const float* __restrict__ sbuf, const float* __restrict__ x,
   out[(size_t)row * (size_t)out_len + i] = v;
 }
 
-static int geometry(int64_t rows, int64_t T, int sr, float semitones, Geo* g) {
+// min_len: the least number of stretched samples s[0 .. Ls) to produce (time_stretch's output length; 0 otherwise)
+static int geometry(int64_t rows, int64_t T, int sr, float semitones, int64_t min_len, Geo* g) {
   (void)rows;
   const double r = pow(2.0, (double)semitones / 12.0);
   int W = 1;
@@ -384,7 +385,8 @@ static int geometry(int64_t rows, int64_t T, int sr, float semitones, Geo* g) {
   const double c = 0.95 * (r > 1.0 ? 1.0 / r : 1.0);
   g->half = (int)ceil(8.0 / c);
   g->H = (g->half + 3) & ~3;
-  const int64_t Ls = (int64_t)ceil((double)T * r) + g->half + 2;  // samples s[0 .. Ls)
+  int64_t Ls = (int64_t)ceil((double)T * r) + g->half + 2;  // samples s[0 .. Ls): what the rate change reads
+  if (Ls < min_len) Ls = min_len;
   g->SL = (g->H + Ls + 3) / 4 * 4;
   const int drift = (int)ceil(fabs((double)g->Hs / r - (double)g->Hs)) + 1;
   g->rcap = (2 * g->D + 2 * g->Lc + drift + 48 + 63) / 64 * 64;
@@ -400,11 +402,12 @@ static int geometry(int64_t rows, int64_t T, int sr, float semitones, Geo* g) {
   return 0;
 }
 
-static int build_table(int64_t rows, int64_t T, int sr, const float* semitones_h, int n_groups, GeoTable* tab) {
+static int build_table(int64_t rows, int64_t T, int sr, const float* semitones_h, int n_groups, GeoTable* tab,
+                       int64_t min_len = 0) {
   memset(tab, 0, sizeof(*tab));
   tab->n = n_groups;
   for (int i = 0; i < n_groups; ++i) {
-    geometry(rows, T, sr, semitones_h[i], &tab->g[i]);
+    geometry(rows, T, sr, semitones_h[i], min_len, &tab->g[i]);
     if (tab->g[i].J > tab->Jmax) tab->Jmax = tab->g[i].J;
     if (tab->g[i].SL > tab->SLmax) tab->SLmax = tab->g[i].SL;
   }
@@ -475,7 +478,7 @@ extern "C" int b2a_pitch_shift_multi_f32(const float* x, int64_t rows, int64_t T
 extern "C" int b2a_pitch_shift_num_frames(int64_t T, int sr, float semitones) {
   if (T < 1 || sr < 1 || !(fabsf(semitones) <= 24.f)) return -1;
   Geo g;
-  geometry(1, T, sr, semitones, &g);
+  geometry(1, T, sr, semitones, 0, &g);
   return g.J;
 }
 
@@ -488,10 +491,19 @@ extern "C" int64_t b2a_time_stretch_out_len(int64_t T, double factor) {
   return (int64_t)floor((double)T / factor + 0.5);
 }
 
+// The stretched rows cover the whole output, round(T / factor) samples: r is 2^(semitones / 12) with the semitones
+// rounded to float32, so T r alone can fall short of T / factor by more than the rate change's half + 2 samples of
+// slack (by 20 samples at T = 2^28 - 1, factor 0.26875).  Frames past the last one read as 0 there.
+static void stretch_table(int64_t rows, int64_t T, int sr, double factor, GeoTable* tab) {
+  const float st = (factor == 1.0) ? 0.0f : stretch_semitones(factor);
+  build_table(rows, T, sr, &st, 1, tab, b2a_time_stretch_out_len(T, factor));
+}
+
 extern "C" size_t b2a_time_stretch_workspace_bytes(int64_t rows, int64_t T, int sr, double factor) {
-  if (!(factor >= 0.25 && factor <= 4.0)) return 0;
-  const float st = stretch_semitones(factor);
-  return b2a_pitch_shift_multi_workspace_bytes(rows, T, sr, &st, 1);
+  if (rows < 1 || T < 1 || sr < 1 || !(factor >= 0.25 && factor <= 4.0)) return 0;
+  GeoTable tab;
+  stretch_table(rows, T, sr, factor, &tab);
+  return pos_bytes(rows, tab) + (size_t)rows * (size_t)tab.SLmax * 4;
 }
 
 extern "C" int b2a_time_stretch_f32(const float* x, int64_t rows, int64_t T, int sr, double factor, float* out,
@@ -502,10 +514,9 @@ extern "C" int b2a_time_stretch_f32(const float* x, int64_t rows, int64_t T, int
   B2A_REQUIRE(rows * T < ((int64_t)1 << 40) && T < ((int64_t)1 << 28) && rows <= 65535, B2A_E_UNSUPPORTED,
               "time_stretch: too large");
   B2A_REQUIRE(((uintptr_t)ws & 15) == 0, B2A_E_INVALID, "time_stretch: workspace must be 16-byte aligned");
-  const float st = (factor == 1.0) ? 0.0f : stretch_semitones(factor);
   const int64_t out_len = b2a_time_stretch_out_len(T, factor);
   GeoTable tab;
-  build_table(rows, T, sr, &st, 1, &tab);
+  stretch_table(rows, T, sr, factor, &tab);
   const size_t pb = pos_bytes(rows, tab);
   B2A_REQUIRE(ws_bytes >= pb + (size_t)rows * (size_t)tab.SLmax * 4, B2A_E_INVALID, "time_stretch: workspace too small");
   int* pos = (int*)ws;

@@ -18,7 +18,7 @@ code with the kernels -- so the CUDA path is compared with something other than 
              else p_j = clamp(a_j, 0, max(T - W, 0)).
   2. overlap-add   s[u] = h x[p_J + t] + (1 - h) x[p_{J-1} + t + Hs],  J = u // Hs, t = u % Hs,
              h = 1/2 - 1/2 cos(pi t / Hs); samples outside [0, T) and frames outside [0, J) read as 0;
-             u in [0, ceil(T r) + half + 2)
+             u in [0, ceil(T r) + half + 2) (time_stretch: u in [0, round(T / factor)))
   3. rate    y[n] = sum_k w_k s[ip + k - half + 1] / sum_k w_k,  P = n r, ip = int(P), f = P - ip, k = 0 .. 2 half - 1,
              t_k = 1 - half - f + k,  w_k = (1/2 + 1/2 cos(pi t_k / half)) sin(pi c t_k) / t_k  (-> pi c at t_k = 0),
              c = 0.95 min(1, 1/r), half = ceil(8 / c); s[u] = 0 for u < 0.
@@ -86,10 +86,11 @@ def splice_positions(x: np.ndarray, geo: Geometry):
     return pos, margin
 
 
-def overlap_add(x: np.ndarray, pos: np.ndarray, geo: Geometry) -> np.ndarray:
+def overlap_add(x: np.ndarray, pos: np.ndarray, geo: Geometry, n=None) -> np.ndarray:
+    """s[0 .. n), n = Ls unless given (frames outside [0, J) read as 0, so s is defined at every u >= 0)."""
     x = np.asarray(x, dtype=np.float64)
     T, g = len(x), geo
-    u = np.arange(g.Ls)
+    u = np.arange(g.Ls if n is None else n)
     Jn, t = u // g.Hs, u % g.Hs
     h = 0.5 - 0.5 * np.cos(np.pi * t / g.Hs)
 
@@ -140,8 +141,5 @@ def time_stretch_row(x: np.ndarray, sr: int, factor: float, positions=None):
     geo = Geometry(T, sr, stretch_semitones(factor))
     pos, margin = splice_positions(x, geo)
     use = pos if positions is None else np.asarray(positions[: geo.J], dtype=np.int64)
-    s = overlap_add(x, use, geo)
-    out = np.zeros(out_len)
-    m = min(out_len, len(s))
-    out[:m] = s[:m]
-    return out, pos, margin
+    # T r (r from float32 semitones) can fall short of T / factor: the overlap-add runs on to out_len
+    return overlap_add(x, use, geo, out_len), pos, margin
