@@ -167,6 +167,49 @@ class EffectMixin:
         self.stft_data = None
         return self
 
+    def sos_filter(self, sos, _bypass=None):
+        """Filter every item with a cascade of second-order sections (an extension; DESIGN.md K19):
+        ``scipy.signal.sosfilt(sos, x)`` with zero initial state, run exactly (no warm-up, no FIR approximation) on
+        the GPU.  ``sos`` is [S, 6] for the whole batch or [B, S, 6] per item (1 <= S <= 8), rows
+        ``b0 b1 b2 a0 a1 a2``; each row is divided by its a0 and rounded to float32 once.  All channels of an item use
+        its sections.  An item with a section whose poles are not strictly inside the unit circle comes back all NaN;
+        a NaN or inf sample makes its row non-finite from that sample on.  A gain deferred by ``normalize`` /
+        ``volume_change`` is applied inside the filter's own passes.  Differentiable with respect to ``audio_data``
+        (the backward is the same cascade run backwards in time); ``sos`` is a constant.  ``_bypass`` [B]: items
+        given identity sections, which return their samples unchanged."""
+        _grad.refuse_param_grad("sos_filter", "sos", sos)
+        x = self._audio_data
+        eng = _engine()
+        sos = eng.sos_coefficients(sos, self.batch_size, x.device)
+        if _bypass is not None:
+            ident = (torch.arange(6, device=sos.device) % 3 == 0).to(sos.dtype)  # 1 0 0 1 0 0, built without a copy
+            byp = torch.as_tensor(_bypass).to(sos.device).bool().reshape(-1, 1, 1)
+            sos = torch.where(byp, ident, sos.expand(self.batch_size, -1, -1)).contiguous()
+        gain = self._pending_gain
+        if _grad.wants_grad(x):
+            y = _grad.SOSFilter.apply(x, sos, gain)
+        else:
+            y = eng.sos_filter(x, sos, gain=gain)
+        self.audio_data = y  # the setter drops the consumed gain and the loudness cache
+        self.stft_data = None
+        return self
+
+    def parametric_eq(self, kind, freq, gain_db=0.0, q=0.7071, _bypass=None):
+        """Parametric equaliser (an extension): one RBJ Audio EQ Cookbook biquad per band and per item
+        (``core/biquad.py``), run as one :meth:`sos_filter` cascade.  ``kind``: one of ``peaking``, ``low_shelf``,
+        ``high_shelf``, ``low_pass``, ``high_pass``, ``band_pass``, ``notch``, ``all_pass``, or a list of n_bands of
+        them.  ``freq`` (Hz, in (0, sr/2)), ``gain_db`` (peaking and shelves) and ``q`` (> 0): numbers, [n_bands] or
+        [B, n_bands]; they are checked on host values, so a transform's parameter table costs no synchronisation.
+        Gradients reach ``audio_data`` only: a parameter that requires one raises ``NotImplementedError``."""
+        from . import biquad
+
+        for name, v in (("freq", freq), ("gain_db", gain_db), ("q", q)):
+            _grad.refuse_param_grad("parametric_eq", name, v)
+        kinds = [kind] if isinstance(kind, str) else list(kind)
+        biquad.check(kinds, freq, q, self.sample_rate)
+        sos = biquad.design(kinds, freq, gain_db, q, self.sample_rate, self.batch_size, self.device)
+        return self.sos_filter(sos, _bypass=_bypass)
+
     def volume_change(self, db, _bypass=None):
         """Multiply every item by ``10**(db/20)`` (ref :222-238)."""
         db = util.ensure_tensor(db, ndim=1).to(self.device).float()

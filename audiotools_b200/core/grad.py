@@ -1,7 +1,7 @@
 """``torch.autograd.Function``s over the engine: the differentiable forms of the spectral front end
 (ref:audiotools/core/audio_signal.py:1123-1296, 1333-1426 and effects.py:200-238, differentiable through torch there;
 ref:tests/core/test_grad.py) and of the time-domain effects (resample, equalizer, convolve, apply_ir,
-ensure_max_of_audio, mix, quantization; gradients with respect to the waveform only) and of the spectral masks and the
+ensure_max_of_audio, mix, quantization, sos_filter; gradients with respect to the waveform only) and of the spectral masks and the
 spectral gate (ref:audiotools/core/dsp.py:217-334, ml/layers/spectral_gate.py:58-127; gradients to the spectrogram)
 and of STOI (``metrics.quality.STOILoss``; gradients to the estimates).  ``AudioSignal`` uses them only when grad mode is on and the input requires a gradient;
 otherwise it calls the engine directly, with exactly the launches it always made.
@@ -309,6 +309,23 @@ class STOI(torch.autograd.Function):
     def backward(ctx, g):
         shape, sample_rate, extended = ctx.args
         return _engine().stoi_backward(g, ctx.ws, shape, sample_rate, extended), None, None, None
+
+
+class SOSFilter(torch.autograd.Function):
+    """x [B, C, T] -> the cascade of second-order sections (``Engine.sos_filter``), after an optional per-item gain.
+    The adjoint of a zero-state linear time-invariant filter is the same filter run backwards in time, so the backward
+    is ``Engine.sos_filter(g, sos, gain, reverse=True)``; the sections and the gain are constants."""
+
+    @staticmethod
+    def forward(ctx, x, sos, gain):
+        ctx.args = (sos, gain)
+        return _engine().sos_filter(x, sos, gain=gain)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        sos, gain = ctx.args
+        return _engine().sos_filter(g, sos, gain=gain, reverse=True), None, None
 
 
 def refuse_param_grad(method: str, name: str, t) -> None:

@@ -313,6 +313,32 @@ class Limiter(BaseTransform):
         return signal.limit(ceiling, lookahead=self.lookahead, release=self.release)
 
 
+class ParametricEQ(BaseTransform):
+    """``signal.parametric_eq(kinds, freq, gain_db, q)`` -- a random parametric equaliser (an extension; the reference
+    has none).  Each band is ``(kind, freq, gain_db, q)``: a cookbook kind (``core/biquad.py``) and three distribution
+    tuples, drawn per item and per band.  Frequencies are drawn in Hz and kept below 0.45 of the signal's rate.  Items
+    the mask does not select get identity sections and come back unchanged."""
+
+    DEFAULT_BANDS = (("low_shelf", ("uniform", 40.0, 300.0), ("uniform", -12.0, 12.0), ("const", 0.7071)),
+                     ("peaking", ("uniform", 200.0, 2000.0), ("uniform", -12.0, 12.0), ("uniform", 0.5, 4.0)),
+                     ("peaking", ("uniform", 1000.0, 8000.0), ("uniform", -12.0, 12.0), ("uniform", 0.5, 4.0)),
+                     ("high_shelf", ("uniform", 4000.0, 12000.0), ("uniform", -12.0, 12.0), ("const", 0.7071)))
+
+    def __init__(self, bands: tuple = DEFAULT_BANDS, name: str = None, prob: float = 1.0):
+        super().__init__(name=name, prob=prob)
+        self.bands = tuple(bands)
+
+    def _instantiate(self, state: RandomState, signal: AudioSignal):
+        top = 0.45 * signal.sample_rate
+        freq = [min(float(util.sample_from_dist(b[1], state)), top) for b in self.bands]
+        gain_db = [float(util.sample_from_dist(b[2], state)) for b in self.bands]
+        q = [float(util.sample_from_dist(b[3], state)) for b in self.bands]
+        return {"freq": np.array(freq), "gain_db": np.array(gain_db), "q": np.array(q)}
+
+    def _transform(self, signal, freq, gain_db, q, _bypass=None):
+        return signal.parametric_eq([b[0] for b in self.bands], freq, gain_db, q, _bypass=_bypass)
+
+
 class GlobalVolumeNorm(BaseTransform):
     """Normalise using the loudness of the whole source file, read from
     ``signal.metadata["loudness"]`` (ref :1006-1050)."""

@@ -34,7 +34,8 @@ class Engine:
     # ------------------------------------------------------------------ helpers
     DIFFERENTIABLE = ("AudioSignal.stft", "istft", "mel_spectrogram", "mfcc", "normalize", "volume_change",
                       "and magnitude / phase / log_magnitude through stft_data; resample, equalizer, convolve, apply_ir, "
-                      "ensure_max_of_audio, mix, quantization, mulaw_quantization (gradients to audio_data); "
+                      "ensure_max_of_audio, mix, quantization, mulaw_quantization, sos_filter, parametric_eq (gradients to "
+                      "audio_data); "
                       "mask_frequencies, mask_timesteps, mask_low_magnitudes, ml.layers.SpectralGate (gradients to "
                       "stft_data / the gated signal)")
 
@@ -638,6 +639,48 @@ class Engine:
         self._call(self.lib.b2a_limiter_f32, _dptr(x), _dptr(gain), B, C, T, L, _dptr(ceiling), A, a, _dptr(out),
                    _dptr(red), _dptr(ws), self._stream(x))
         return (out, red) if want_reduction else out
+
+    SOS_MAX_SECTIONS = 8  # csrc/iir.cu
+
+    def sos_coefficients(self, sos, B: int, device) -> torch.Tensor:
+        """``sos`` ([S, 6] or [1 or B, S, 6], rows b0 b1 b2 a0 a1 a2) as the kernels take it: every row divided by
+        its a0 in float64 and rounded to float32 once, [1 or B, S, 6] contiguous on ``device``."""
+        sos = torch.as_tensor(sos)
+        self._refuse_grad(sos, "sos")
+        if sos.ndim == 2:
+            sos = sos.unsqueeze(0)
+        if sos.ndim != 3 or sos.shape[-1] != 6 or sos.shape[0] not in (1, B):
+            raise ValueError(f"sos_filter: sos must be [S, 6] or [1 or {B}, S, 6], got {tuple(sos.shape)}")
+        if not 1 <= sos.shape[1] <= self.SOS_MAX_SECTIONS:
+            raise ValueError(f"sos_filter: {sos.shape[1]} sections; 1 .. {self.SOS_MAX_SECTIONS} are supported")
+        sos = sos.to(device=device, dtype=torch.float64, non_blocking=True)
+        return (sos / sos[..., 3:4]).to(torch.float32).contiguous()
+
+    def sos_filter(self, x: torch.Tensor, sos, gain: Optional[torch.Tensor] = None, reverse: bool = False,
+                   out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``scipy.signal.sosfilt(sos, x)`` with zero initial state for x [B, C, T] (``b2a_sos_filter_f32``, DESIGN.md
+        K19): ``sos`` [S, 6] for the whole batch or [B, S, 6] per item, 1 <= S <= 8, normalised by a0 and rounded to
+        float32 (``sos_coefficients``).  ``gain`` [B]: the item is ``float32(gain * x)``.  ``reverse`` runs every row
+        back to front (the adjoint).  An item with a section whose poles are not strictly inside the unit circle comes
+        back all NaN.  ``out`` may be ``x``.  Three launches."""
+        x = self._prep(x, "x")
+        assert x.ndim == 3, "x must be [B, C, T]"
+        B, C, T = x.shape
+        sos = self.sos_coefficients(sos, B, x.device)
+        if gain is not None:
+            gain = self._prep(gain.reshape(-1), "gain")
+            assert gain.numel() == B
+        if out is None:
+            out = torch.empty_like(x)
+        assert out.shape == x.shape and out.dtype == torch.float32 and out.is_contiguous() and out.device == x.device
+        S = sos.shape[1]
+        ws_bytes = int(self.lib.b2a_sos_filter_workspace_bytes(B, C, T, S))
+        if ws_bytes == 0:
+            raise _lib.B2AError(f"sos_filter: unsupported shape {tuple(x.shape)}")
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        self._call(self.lib.b2a_sos_filter_f32, _dptr(x), _dptr(gain), B, C, T, _dptr(sos), sos.shape[0], S,
+                   int(bool(reverse)), _dptr(out), _dptr(ws), self._stream(x))
+        return out
 
     def gain(self, x: torch.Tensor, gain: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``x[b] * gain[b]`` (ref:audiotools/core/effects.py:219,237)."""

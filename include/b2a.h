@@ -348,6 +348,19 @@ size_t b2a_limiter_workspace_bytes(int64_t B, int C, int64_t T);
 int b2a_limiter_f32(const float* x, const float* gain, int64_t B, int C, int64_t T, int factor, const float* ceiling,
                     int lookahead, float release_a, float* out, float* reduction, void* ws, void* stream);
 
+/* ---- per-item IIR biquad cascades (csrc/iir.cu) ---------------------------------------------------------------------
+ * scipy.signal.sosfilt with zero initial state, per item.  x [B, C, T]; gain nullable [B] (x means float(gain[b] x));
+ * sos [sos_items, S, 6] float32, rows b0 b1 b2 a0 a1 a2, used as b / a0 and a / a0 in float32; sos_items 1 (one set
+ * for the batch) or B (set b for item b, all its channels); 1 <= S <= 8 sections, run in order, each in the transposed
+ * direct form II, in double (each output rounded to float32 once).  reverse != 0 reads and writes every row back to front (the adjoint of the forward filter).
+ * A section that fails |a2| < 1 and |a1| < 1 + a2 makes its item's output all NaN; a NaN or inf sample makes its row
+ * non-finite from that sample on; other rows and items are unaffected.  out [B, C, T] may alias x.
+ * ws: b2a_sos_filter_workspace_bytes(B, C, T, S) bytes of scratch (0 for a bad shape).  Three launches, no host sync;
+ * reruns and batch-versus-single calls are bit-identical. */
+size_t b2a_sos_filter_workspace_bytes(int64_t B, int C, int64_t T, int S);
+int b2a_sos_filter_f32(const float* x, const float* gain, int64_t B, int C, int64_t T, const float* sos,
+                       int64_t sos_items, int S, int reverse, float* out, void* ws, void* stream);
+
 /* ---- per-item gain ---------------------------------------------------------------------
  * x[b, :, :] * gain[b]  (EffectMixin.normalize / volume_change, effects.py:219,237).
  * out may alias x.  per_item = C*T. */
