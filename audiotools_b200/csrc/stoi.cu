@@ -54,6 +54,14 @@ __device__ __forceinline__ double hann(int n) {
   return 0.5 + 0.5 * c;
 }
 
+// np.minimum / np.max: a NaN operand gives NaN (fmin and fmax return the other operand)
+__device__ __forceinline__ double min_nan(double a, double b) { return isnan(a) || isnan(b) ? a + b : fmin(a, b); }
+__device__ __forceinline__ double max_nan(double a, double b) { return isnan(a) || isnan(b) ? a + b : fmax(a, b); }
+// d min(a, b) / d a: 1, 1/2 at a tie (as torch.minimum), 0; NaN when either operand is NaN
+__device__ __forceinline__ double tie_mask(double a, double b) {
+  return isnan(a) || isnan(b) ? a + b : (a < b ? 1.0 : (a == b ? 0.5 : 0.0));
+}
+
 __device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -136,13 +144,14 @@ mask_kernel(const float* __restrict__ ref10, int64_t n10, int n_fr, double* __re
     }
     const double ef = 20.0 * log10(sqrt(warp_sum_d(s)) + EPS);
     if (lane == 0) e[f] = ef;
-    emax = fmax(emax, ef);
+    emax = max_nan(emax, ef);
   }
   if (lane == 0) red[warp] = emax;
   __syncthreads();  // also orders the energies written above before the reads below
   emax = red[0];
-  for (int i = 1; i < THREADS / 32; ++i) emax = fmax(emax, red[i]);
-  // 2. keep flags -> exclusive scan -> indices of the kept frames, in order
+  for (int i = 1; i < THREADS / 32; ++i) emax = max_nan(emax, red[i]);
+  // 2. keep flags -> exclusive scan -> indices of the kept frames, in order (a NaN energy makes emax NaN and keeps
+  //    no frame, as pystoi's np.max: the item is short)
   int carry = 0;
   for (int f0 = 0; f0 < n_fr; f0 += THREADS) {
     const int f = f0 + tid;
@@ -283,14 +292,14 @@ score_kernel(const float* __restrict__ tob, int B, int n_fr, const int32_t* __re
       for (int t = 0; t < SEG; ++t) {
         const double xv = xr[t];
         mx += xv;
-        my += fmin((double)yr[t] * c, xv * clip);
+        my += min_nan((double)yr[t] * c, xv * clip);
       }
       mx /= SEG;
       my /= SEG;
       double sxy = 0.0, sx2 = 0.0, sy2 = 0.0;
       for (int t = 0; t < SEG; ++t) {
         const double xv = xr[t];
-        const double dx = xv - mx, dy = fmin((double)yr[t] * c, xv * clip) - my;
+        const double dx = xv - mx, dy = min_nan((double)yr[t] * c, xv * clip) - my;
         sxy = fma(dx, dy, sxy);
         sx2 = fma(dx, dx, sx2);
         sy2 = fma(dy, dy, sy2);
@@ -390,14 +399,14 @@ score_bwd_kernel(const double* __restrict__ grad_score, const float* __restrict_
       for (int t = 0; t < SEG; ++t) {
         const double xv = xr[t];
         mx += xv;
-        my += fmin((double)yr[t] * c, xv * clip);
+        my += min_nan((double)yr[t] * c, xv * clip);
       }
       mx /= SEG;
       my /= SEG;
       double sxy = 0.0, sx2 = 0.0, sy2 = 0.0;
       for (int t = 0; t < SEG; ++t) {
         const double xv = xr[t];
-        const double dx = xv - mx, dy = fmin((double)yr[t] * c, xv * clip) - my;
+        const double dx = xv - mx, dy = min_nan((double)yr[t] * c, xv * clip) - my;
         sxy = fma(dx, dy, sxy);
         sx2 = fma(dx, dx, sx2);
         sy2 = fma(dy, dy, sy2);
@@ -411,8 +420,8 @@ score_bwd_kernel(const double* __restrict__ grad_score, const float* __restrict_
       for (int t = 0; t < SEG; ++t) {
         const double xv = xr[t], yv = yr[t];
         const double cy = yv * c, kx = xv * clip;
-        const double A = (xv - mx) * iuv - rv * (fmin(cy, kx) - my);
-        const double mt = cy < kx ? 1.0 : (cy == kx ? 0.5 : 0.0);
+        const double A = (xv - mx) * iuv - rv * (min_nan(cy, kx) - my);
+        const double mt = tie_mask(cy, kx);
         S = fma(mt * yv, A, S);
       }
       const double q = ny > 0.0 ? nx * S / (ny * (ny + EPS) * (ny + EPS)) : 0.0;  // -d c / d y_s = q' y_s
@@ -420,8 +429,8 @@ score_bwd_kernel(const double* __restrict__ grad_score, const float* __restrict_
       for (int t = 0; t < SEG; ++t) {
         const double xv = xr[t], yv = yr[t];
         const double cy = yv * c, kx = xv * clip;
-        const double A = (xv - mx) * iuv - rv * (fmin(cy, kx) - my);
-        const double mt = cy < kx ? 1.0 : (cy == kx ? 0.5 : 0.0);
+        const double A = (xv - mx) * iuv - rv * (min_nan(cy, kx) - my);
+        const double mt = tie_mask(cy, kx);
         o[t] = (float)(c * mt * A - q * yv);
       }
     }

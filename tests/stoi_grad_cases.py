@@ -46,8 +46,11 @@ def resample(x: torch.Tensor, sample_rate: int) -> torch.Tensor:
         return x
     taps = Engine.stoi_taps(sample_rate)
     n, t, valid = _resample_index(x.shape[-1], up, down, taps.size)
-    w = torch.from_numpy(np.where(valid, taps[t], 0.0)).to(x)
-    return (x[..., torch.from_numpy(n).to(x.device)] * w).sum(-1)
+    w = torch.from_numpy(taps[t]).to(x)
+    # the padding slots are a where, not a zero weight: autograd then sends them nothing, where 0 * a NaN gradient
+    # would reach sample 0
+    v = torch.from_numpy(valid).to(x.device)
+    return torch.where(v, x[..., torch.from_numpy(n).to(x.device)] * w, 0.0).sum(-1)
 
 
 def _window(like):
