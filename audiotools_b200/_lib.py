@@ -48,6 +48,13 @@ SIGNATURES = {
     "b2a_sos_filter_workspace_bytes": (c_size_t, [c_int64, c_int, c_int64, c_int]),
     "b2a_sos_filter_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int64, c_void_p, c_int64, c_int, c_int,
                                    c_void_p, c_void_p, c_void_p]),
+    "b2a_sos_filter_zi_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int64, c_void_p, c_int64, c_int, c_void_p,
+                                      c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2a_sos_filtfilt_workspace_bytes": (c_size_t, [c_int64, c_int, c_int64, c_int, c_int, c_int64]),
+    "b2a_sos_filtfilt_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int64, c_void_p, c_int64, c_int, c_int,
+                                     c_int64, c_void_p, c_void_p, c_void_p]),
+    "b2a_sos_filtfilt_backward_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int64, c_void_p, c_int64, c_int,
+                                              c_int, c_int64, c_void_p, c_void_p, c_void_p]),
     "b2a_gain_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
     "b2a_fftconv_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64, c_int64]),
     "b2a_fftconv_f32": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int,

@@ -167,16 +167,18 @@ class EffectMixin:
         self.stft_data = None
         return self
 
-    def sos_filter(self, sos, _bypass=None):
+    def sos_filter(self, sos, zero_phase: bool = False, _bypass=None):
         """Filter every item with a cascade of second-order sections (an extension; DESIGN.md K19):
         ``scipy.signal.sosfilt(sos, x)`` with zero initial state, run exactly (no warm-up, no FIR approximation) on
         the GPU.  ``sos`` is [S, 6] for the whole batch or [B, S, 6] per item (1 <= S <= 8), rows
         ``b0 b1 b2 a0 a1 a2``; each row is divided by its a0 and rounded to float32 once.  All channels of an item use
         its sections.  An item with a section whose poles are not strictly inside the unit circle comes back all NaN;
-        a NaN or inf sample makes its row non-finite from that sample on.  A gain deferred by ``normalize`` /
-        ``volume_change`` is applied inside the filter's own passes.  Differentiable with respect to ``audio_data``
-        (the backward is the same cascade run backwards in time); ``sos`` is a constant.  ``_bypass`` [B]: items
-        given identity sections, which return their samples unchanged."""
+        a NaN or inf sample makes its row non-finite from that sample on.  ``zero_phase=True`` runs
+        ``scipy.signal.sosfiltfilt(sos, x)`` with scipy's defaults instead (odd extension, each item's default
+        padlen; the signal must be longer than 3 (2S + 1) samples): forwards and backwards, so no sample moves, and a
+        NaN or inf sample makes its whole row non-finite.  A gain deferred by ``normalize`` / ``volume_change`` is
+        applied inside the filter's own passes.  Differentiable with respect to ``audio_data``; ``sos`` is a constant.
+        ``_bypass`` [B]: items given identity sections, which return their samples unchanged."""
         _grad.refuse_param_grad("sos_filter", "sos", sos)
         x = self._audio_data
         eng = _engine()
@@ -186,7 +188,12 @@ class EffectMixin:
             byp = torch.as_tensor(_bypass).to(sos.device).bool().reshape(-1, 1, 1)
             sos = torch.where(byp, ident, sos.expand(self.batch_size, -1, -1)).contiguous()
         gain = self._pending_gain
-        if _grad.wants_grad(x):
+        if zero_phase:
+            if _grad.wants_grad(x):
+                y = _grad.SOSFiltFilt.apply(x, sos, gain, "odd", None)
+            else:
+                y = eng.sos_filtfilt(x, sos, gain=gain)
+        elif _grad.wants_grad(x):
             y = _grad.SOSFilter.apply(x, sos, gain)
         else:
             y = eng.sos_filter(x, sos, gain=gain)

@@ -1,7 +1,7 @@
 """``torch.autograd.Function``s over the engine: the differentiable forms of the spectral front end
 (ref:audiotools/core/audio_signal.py:1123-1296, 1333-1426 and effects.py:200-238, differentiable through torch there;
 ref:tests/core/test_grad.py) and of the time-domain effects (resample, equalizer, convolve, apply_ir,
-ensure_max_of_audio, mix, quantization, sos_filter; gradients with respect to the waveform only) and of the spectral masks and the
+ensure_max_of_audio, mix, quantization, sos_filter, sosfiltfilt; gradients with respect to the waveform only) and of the spectral masks and the
 spectral gate (ref:audiotools/core/dsp.py:217-334, ml/layers/spectral_gate.py:58-127; gradients to the spectrogram)
 and of STOI (``metrics.quality.STOILoss``; gradients to the estimates).  ``AudioSignal`` uses them only when grad mode is on and the input requires a gradient;
 otherwise it calls the engine directly, with exactly the launches it always made.
@@ -326,6 +326,24 @@ class SOSFilter(torch.autograd.Function):
     def backward(ctx, g):
         sos, gain = ctx.args
         return _engine().sos_filter(g, sos, gain=gain, reverse=True), None, None
+
+
+class SOSFiltFilt(torch.autograd.Function):
+    """x [B, C, T] -> the zero-phase cascade (``Engine.sos_filtfilt``), after an optional per-item gain.  The backward
+    (``Engine.sos_filtfilt_backward``) composes the adjoints of the two passes, the rank-one terms of their start
+    states (each is linear in one sample) and the fold of the edge extension; the sections and the gain are
+    constants."""
+
+    @staticmethod
+    def forward(ctx, x, sos, gain, padtype, padlen):
+        ctx.args = (sos, gain, padtype, padlen)
+        return _engine().sos_filtfilt(x, sos, padtype, padlen, gain=gain)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        sos, gain, padtype, padlen = ctx.args
+        return _engine().sos_filtfilt_backward(g, sos, padtype, padlen, gain=gain), None, None, None, None
 
 
 def refuse_param_grad(method: str, name: str, t) -> None:

@@ -1,4 +1,5 @@
-// iir.cu -- per-item IIR biquad cascades of a batch (K19 in DESIGN.md): scipy.signal.sosfilt with zero initial state.
+// iir.cu -- per-item IIR biquad cascades of a batch (K19 in DESIGN.md): scipy.signal.sosfilt with zero or given
+// initial state, and scipy.signal.sosfiltfilt (method "pad") with its gradient.
 //
 //   sos [sos_items, S, 6] float32, rows b0 b1 b2 a0 a1 a2; the kernels use b / a0 and a / a0 in float32 (exact when
 //   a0 = 1, which is what Engine.sos_filter passes).  Item b uses set b when sos_items = B, else set 0, for all its
@@ -13,14 +14,19 @@
 //   item's output all NaN.  A NaN or inf sample makes its row non-finite from that sample on.
 //
 // The cascade's state s = (z1, z2) of every section is 2S numbers.  With the input set to 0 one sample maps s to A s,
-// and a chunk of CHUNK samples maps it to M = A^CHUNK.  Three launches, no host sync, exact carries (no warm-up):
+// and a chunk of CHUNK samples maps it to M = A^CHUNK.  A pass is three launches, no host sync, exact carries (no
+// warm-up):
 //   chunk_state_kernel   a warp per (row, 32 consecutive chunks), a lane per chunk: the recursion over the chunk
 //                        from zero state gives the chunk's end state e_k.  Samples travel through a 32 x 32
 //                        shared tile per warp, so every global access is a coalesced row of 32 floats.
 //   carry_kernel         a warp per row: A from the item's coefficients in double, M and M^2, M^4, M^8, M^16 by
-//                        squaring, then the affine scan s_{k+1} = M s_k + e_k, s_0 = 0, 32 chunks at a time as a
-//                        warp scan in double; writes every chunk's start state s_k.
+//                        squaring, then the affine scan s_{k+1} = M s_k + e_k from the start state s_0, 32 chunks at
+//                        a time as a warp scan in double; writes every chunk's start state s_k.
 //   filter_kernel        the layout of the first kernel: the recursion over the chunk from s_k writes y.
+// A pass walks a virtual row v[m], m in [0, L) (struct Pass): the samples of x, or of the intermediate between the two
+// passes of sosfiltfilt, read forwards or backwards, with scipy's edge extension applied in the loads.  s_0 is 0, a
+// given zi, or sosfilt_zi(sos) v[0] (read on the device).  The filter kernel can also write the state after v[L - 1]
+// (zf) and, per warp, G sum(v) - sum(y) (G: the cascade's DC gain), the rank-one term of the sosfiltfilt backward.
 // Nothing depends on the launch geometry or on other items: reruns and batch-versus-single calls are bit-identical.
 #include "b2a_common.h"
 
@@ -31,6 +37,31 @@ constexpr int CHUNK = 1024;   // samples of a row per chunk (one lane's sequenti
 constexpr int TILE = 32;      // samples per lane per shared-memory tile
 constexpr int WARPS = 8;      // warps per CTA of the chunk kernels
 constexpr int SMAX = 8;       // largest number of sections
+
+// padtype of b2a_sos_filtfilt_f32 (b2a.h); PAD_ZERO (outside [0, T) reads 0) is the backward's crop adjoint
+enum { PAD_NONE = 0, PAD_ODD = 1, PAD_EVEN = 2, PAD_CONST = 3, PAD_ZERO = 4 };
+
+// One pass of the cascade over every row.  Row r of length L = T + 2 pl: m in [0, L) is the extended position
+// e = (reverse ? L - 1 - m : m) - pl in [-pl, T + pl).  A source or destination row is either a row of T samples (x /
+// out: e outside [0, T) is extended on load by padtype and dropped on store) or the intermediate, Lmax samples per row
+// (index e + pl).
+struct Pass {
+  const float* src;         // [rows, T] or the intermediate
+  const float* gain;        // [B] or null; scales rows of x only
+  float* dst;               // [rows, T] or the intermediate
+  const float* sos;
+  int64_t sos_items;
+  int C;
+  int64_t T, Lmax;          // samples of a row of x; row stride of the intermediate, T + 2 max(pl)
+  int64_t n_chunks, work;   // chunks of Lmax; warps of the chunk kernels
+  int src_mid, dst_mid, reverse, padtype;
+  int64_t padlen;           // >= 0, or < 0: scipy's default for the item's sections
+  const double* zi;         // [S, rows, 2] start states, or null
+  int zi_unit;              // start from sosfilt_zi(sos) v[0]
+  double* zf;               // [S, rows, 2]: the state after v[L - 1], or null
+  double* part;             // [rows, n_groups]: G sum(v) - sum(y) over a warp's chunks, or null
+  const double* add_first;  // [rows, n_groups]: their sum is added to v[0], or null
+};
 
 template <int S>
 struct Coef {
@@ -54,6 +85,75 @@ __device__ __forceinline__ Coef<S> load_coef(const float* __restrict__ sos) {
   return c;
 }
 
+// scipy's default padlen, 3 (2S + 1 - min(#{b2 == 0}, #{a2 == 0})), or the given one
+__device__ __forceinline__ int64_t row_padlen(const float* so, int S, int64_t padlen) {
+  if (padlen >= 0) return padlen;
+  int nb = 0, na = 0;
+  for (int s = 0; s < S; ++s) {
+    const float a0 = so[6 * s + 3];
+    nb += so[6 * s + 2] / a0 == 0.f;
+    na += so[6 * s + 5] / a0 == 0.f;
+  }
+  return 3 * (2 * S + 1 - (nb < na ? nb : na));
+}
+
+// One row of a pass: pointers at the row, its padding and length
+struct Row {
+  const float* src;
+  float* dst;
+  int64_t T, L, pl;
+  float g, first, last;  // gain; the gained first and last samples of a row of x (the extension's edges)
+  int src_mid, dst_mid, reverse, padtype;
+};
+
+__device__ __forceinline__ Row make_row(const Pass& p, int S, int64_t row, int64_t b) {
+  Row r;
+  const int64_t pl = row_padlen(p.sos + (p.sos_items > 1 ? b : 0) * 6 * S, S, p.padlen);
+  r.src = p.src + row * (p.src_mid ? p.Lmax : p.T);
+  r.dst = p.dst ? p.dst + row * (p.dst_mid ? p.Lmax : p.T) : nullptr;
+  r.T = p.T, r.pl = pl, r.L = p.T + 2 * pl;
+  r.g = p.gain ? __ldg(p.gain + b) : 1.f;
+  r.first = p.src_mid ? 0.f : r.src[0] * r.g;
+  r.last = p.src_mid ? 0.f : r.src[p.T - 1] * r.g;
+  r.src_mid = p.src_mid, r.dst_mid = p.dst_mid, r.reverse = p.reverse, r.padtype = p.padtype;
+  return r;
+}
+
+// v[m]: 0 past the row's end.  EXT = false: a row of x without padding (pl = 0, L = T), the zero-state filter's own
+// index expression.  EXT: one predicated load and selects, no divergent branch, so a tile's 32 loads issue together.
+template <bool EXT>
+__device__ __forceinline__ float load(const Row& r, int64_t m) {
+  if (!EXT) return m < r.L ? r.src[r.reverse ? r.L - 1 - m : m] * r.g : 0.f;
+  const int64_t e = (r.reverse ? r.L - 1 - m : m) - r.pl;
+  const bool inside = r.src_mid || (e >= 0 && e < r.T);
+  const bool mirror = r.padtype == PAD_ODD || r.padtype == PAD_EVEN;
+  const int64_t i = r.src_mid ? e + r.pl : e < 0 ? -e : e >= r.T ? 2 * (r.T - 1) - e : e;
+  const float v = m < r.L && (inside || mirror) ? r.src[i] * (r.src_mid ? 1.f : r.g) : 0.f;
+  if (inside || m >= r.L) return v;
+  const float edge = e < 0 ? r.first : r.last;
+  return r.padtype == PAD_ODD ? 2.f * edge - v : r.padtype == PAD_EVEN ? v : r.padtype == PAD_CONST ? edge : 0.f;
+}
+
+template <bool EXT>
+__device__ __forceinline__ void store(const Row& r, int64_t m, float y) {
+  if (!EXT) {
+    if (m < r.L) r.dst[r.reverse ? r.L - 1 - m : m] = y;
+    return;
+  }
+  const int64_t e = (r.reverse ? r.L - 1 - m : m) - r.pl;
+  if (m < r.L && (r.dst_mid || (e >= 0 && e < r.T))) r.dst[r.dst_mid ? e + r.pl : e] = y;
+}
+
+// The sum of a row's n warp partials, the same order in every warp that asks
+__device__ __forceinline__ double warp_sum(const double* v, int64_t n) {
+  const int lane = threadIdx.x & 31;
+  double a = 0.0;
+  for (int64_t i = lane; i < n; i += 32) a += v[i];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+  return a;
+}
+
 // One sample through the cascade in double; z holds (z1, z2) of every section
 template <int S>
 __device__ __forceinline__ double step(const Coef<S>& c, double (&z)[2 * S], double u) {
@@ -67,31 +167,49 @@ __device__ __forceinline__ double step(const Coef<S>& c, double (&z)[2 * S], dou
   return u;
 }
 
-// Walk the warp's chunks tile by tile: lane l runs chunk g * 32 + l of row `row` from state z.  WRITE: y replaces the
-// tile and goes to out.  Flat indices are 64-bit.
-template <int S, bool WRITE>
-__device__ __forceinline__ void run_chunks(const float* x, float* out, int64_t row_off, int64_t T, int64_t first,
-                                           float g0, bool reverse, const Coef<S>& c, double (&z)[2 * S], float* tile) {
+// What the filter kernel gathers besides y (EXTRA): the state after v[L - 1] and the sums of v and y over m < L
+struct Extra {
+  double* zf;           // this row's zf (section stride zf_stride), or null
+  int64_t zf_stride;
+  double sum_v, sum_y;
+};
+
+// Walk the warp's chunks tile by tile: lane l runs chunk g * 32 + l of the row from state z.  WRITE: y replaces the
+// tile and is stored.  add0 (when `add`) is added to v[0].  Flat indices are 64-bit.
+template <int S, bool WRITE, bool EXT, bool EXTRA>
+__device__ __forceinline__ void run_chunks(const Row& rw, int64_t first, bool add, double add0, const Coef<S>& c,
+                                           double (&z)[2 * S], float* tile, Extra& ex) {
   const int lane = threadIdx.x & 31;
-  const int64_t len = T < CHUNK ? T : CHUNK;
+  const int64_t len = rw.L < CHUNK ? rw.L : CHUNK;
   const int n_tiles = (int)((len + TILE - 1) / TILE);
   for (int t = 0; t < n_tiles; ++t) {
     for (int r = 0; r < 32; ++r) {
       const int64_t n = first + (int64_t)r * CHUNK + t * TILE + lane;
-      tile[r * (TILE + 1) + lane] = n < T ? x[row_off + (reverse ? T - 1 - n : n)] * g0 : 0.f;
+      float v = load<EXT>(rw, n);
+      if (EXT && add && n == 0) v = (float)((double)v + add0);
+      tile[r * (TILE + 1) + lane] = v;
     }
     __syncwarp();
     float* mine = tile + lane * (TILE + 1);
+    const int64_t base = first + (int64_t)lane * CHUNK + t * TILE;  // position of mine[0]
 #pragma unroll 4
     for (int k = 0; k < TILE; ++k) {
-      const double y = step<S>(c, z, (double)mine[k]);
+      const double u = (double)mine[k];
+      const double y = step<S>(c, z, u);
       if (WRITE) mine[k] = (float)y;
+      if (EXTRA) {
+        if (base + k < rw.L) ex.sum_v += u, ex.sum_y += y;
+        if (ex.zf && base + k == rw.L - 1) {
+#pragma unroll
+          for (int i = 0; i < 2 * S; ++i) ex.zf[(i >> 1) * ex.zf_stride + (i & 1)] = z[i];
+        }
+      }
     }
     __syncwarp();
     if (WRITE) {
       for (int r = 0; r < 32; ++r) {
         const int64_t n = first + (int64_t)r * CHUNK + t * TILE + lane;
-        if (n < T) out[row_off + (reverse ? T - 1 - n : n)] = tile[r * (TILE + 1) + lane];
+        store<EXT>(rw, n, tile[r * (TILE + 1) + lane]);
       }
       __syncwarp();
     }
@@ -99,23 +217,22 @@ __device__ __forceinline__ void run_chunks(const float* x, float* out, int64_t r
 }
 
 // ws_e [rows, n_chunks, 2S]: end state of every chunk from zero state.
-template <int S>
-__global__ void __launch_bounds__(WARPS * 32) chunk_state_kernel(const float* __restrict__ x,
-                                                                 const float* __restrict__ gain, int C, int64_t T,
-                                                                 const float* __restrict__ sos, int64_t sos_items,
-                                                                 int64_t n_chunks, int64_t work, int reverse,
-                                                                 double* __restrict__ ws_e) {
+template <int S, bool EXT>
+__global__ void __launch_bounds__(WARPS * 32) chunk_state_kernel(const Pass p, double* __restrict__ ws_e) {
   __shared__ float s_tile[WARPS][32 * (TILE + 1)];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int64_t n_groups = (n_chunks + 31) / 32;
-  for (int64_t w = (int64_t)blockIdx.x * WARPS + wid; w < work; w += (int64_t)gridDim.x * WARPS) {
-    const int64_t row = w / n_groups, g = w - row * n_groups, b = row / C;
-    const Coef<S> c = load_coef<S>(sos + (sos_items > 1 ? b : 0) * 6 * S);
-    const float g0 = gain ? __ldg(gain + b) : 1.f;
+  const int64_t n_chunks = p.n_chunks, n_groups = (n_chunks + 31) / 32;
+  for (int64_t w = (int64_t)blockIdx.x * WARPS + wid; w < p.work; w += (int64_t)gridDim.x * WARPS) {
+    const int64_t row = w / n_groups, g = w - row * n_groups, b = row / p.C;
+    const Coef<S> c = load_coef<S>(p.sos + (p.sos_items > 1 ? b : 0) * 6 * S);
+    const Row rw = make_row(p, S, row, b);
+    const bool add = p.add_first && g == 0;
+    const double add0 = add ? warp_sum(p.add_first + row * n_groups, n_groups) : 0.0;
     double z[2 * S];
 #pragma unroll
     for (int i = 0; i < 2 * S; ++i) z[i] = 0.0;
-    run_chunks<S, false>(x, nullptr, row * T, T, g * 32 * CHUNK, g0, reverse, c, z, s_tile[wid]);
+    Extra ex{};
+    run_chunks<S, false, EXT, false>(rw, g * 32 * CHUNK, add, add0, c, z, s_tile[wid], ex);
     const int64_t k = g * 32 + lane;
     if (k < n_chunks) {
 #pragma unroll
@@ -150,17 +267,42 @@ __device__ __forceinline__ void square(const double* src, double* dst) {
   __syncwarp();
 }
 
+// s_0 of a row: the given zi, or sosfilt_zi(sos) v[0] -- each section's lfilter_zi, (I - A_s)^-1 B_s in closed form,
+// times the DC gains of the sections before it, in double from the float32 coefficients
+template <int S>
+__device__ __forceinline__ void start_state(const Pass& p, int64_t row, int64_t b, int64_t rows, double (&s0)[2 * S]) {
+  if (p.zi) {
+#pragma unroll
+    for (int i = 0; i < 2 * S; ++i) s0[i] = p.zi[((i >> 1) * rows + row) * 2 + (i & 1)];
+    return;
+  }
+  const float* so = p.sos + (p.sos_items > 1 ? b : 0) * 6 * S;
+  const double v = (double)load<true>(make_row(p, S, row, b), 0);
+  double scale = v;
+#pragma unroll
+  for (int s = 0; s < S; ++s) {
+    const float a0 = so[6 * s + 3];
+    const double b0 = (double)(so[6 * s] / a0), b1 = (double)(so[6 * s + 1] / a0), b2 = (double)(so[6 * s + 2] / a0),
+                 a1 = (double)(so[6 * s + 4] / a0), a2 = (double)(so[6 * s + 5] / a0);
+    const double B1 = b1 - a1 * b0, B2 = b2 - a2 * b0, z1 = (B1 + B2) / (1.0 + a1 + a2);
+    s0[2 * s] = scale * z1;
+    s0[2 * s + 1] = scale * (B2 - a2 * z1);
+    scale *= (b0 + b1 + b2) / (1.0 + a1 + a2);
+  }
+}
+
 // One warp (one CTA) per row.  ws_s [rows, n_chunks, 2S]: the start state of every chunk.
 template <int S>
-__global__ void __launch_bounds__(32) carry_kernel(const float* __restrict__ sos, int64_t sos_items, int C,
-                                                   int64_t rows, int64_t n_chunks, const double* __restrict__ ws_e,
+__global__ void __launch_bounds__(32) carry_kernel(const Pass p, const double* __restrict__ ws_e,
                                                    double* __restrict__ ws_s) {
   constexpr int N = 2 * S;
   __shared__ double s_pow[6][N * N];  // M, M^2, M^4, M^8, M^16; [5] scratch
   const int lane = threadIdx.x;
+  const int64_t rows = p.work / ((p.n_chunks + 31) / 32), n_chunks = p.n_chunks;
+  const bool has_s0 = p.zi || p.zi_unit;
   for (int64_t row = blockIdx.x; row < rows; row += gridDim.x) {
-    const int64_t b = row / C;
-    const float* so = sos + (sos_items > 1 ? b : 0) * 6 * S;
+    const int64_t b = row / p.C;
+    const float* so = p.sos + (p.sos_items > 1 ? b : 0) * 6 * S;
     if (n_chunks > 1) {
       // A, row by row: Y is the previous section's output as a linear form of the state (0 before section 0)
       if (lane == 0) {
@@ -182,7 +324,7 @@ __global__ void __launch_bounds__(32) carry_kernel(const float* __restrict__ sos
       __syncwarp();
       // A^CHUNK: log2(CHUNK) squarings, alternating between slots 0 and 5
       int cur = 0;
-      for (int p = 1; p < CHUNK; p *= 2) {
+      for (int p2 = 1; p2 < CHUNK; p2 *= 2) {
         square<N>(s_pow[cur], s_pow[5 - cur]);
         cur = 5 - cur;
       }
@@ -190,28 +332,29 @@ __global__ void __launch_bounds__(32) carry_kernel(const float* __restrict__ sos
         for (int o = lane; o < N * N; o += 32) s_pow[0][o] = s_pow[cur][o];
         __syncwarp();
       }
-      for (int p = 1; p < 5; ++p) square<N>(s_pow[p - 1], s_pow[p]);
-    }
-    if (lane == 0) {
-#pragma unroll
-      for (int i = 0; i < N; ++i) ws_s[row * n_chunks * N + i] = 0.0;  // s_0
+      for (int q = 1; q < 5; ++q) square<N>(s_pow[q - 1], s_pow[q]);
     }
     double carry[N];  // start state of the batch's first chunk
 #pragma unroll
     for (int i = 0; i < N; ++i) carry[i] = 0.0;
+    if (has_s0) start_state<S>(p, row, b, rows, carry);
+    if (lane == 0) {
+#pragma unroll
+      for (int i = 0; i < N; ++i) ws_s[row * n_chunks * N + i] = carry[i];  // s_0
+    }
     for (int64_t base = 0; base + 1 < n_chunks; base += 32) {  // the last chunk's end state is not needed
       const int64_t k = base + lane;
       double v[N], w[N];
 #pragma unroll
       for (int i = 0; i < N; ++i) v[i] = k < n_chunks ? ws_e[(row * n_chunks + k) * N + i] : 0.0;
-      if (lane == 0 && base > 0) matvec_add<N>(s_pow[0], carry, v);
+      if (lane == 0 && (base > 0 || has_s0)) matvec_add<N>(s_pow[0], carry, v);
       // inclusive scan: lane l ends with the end state of chunk base + l, i.e. the start state of chunk base + l + 1
 #pragma unroll
-      for (int p = 0; p < 5; ++p) {
-        const int o = 1 << p;
+      for (int q = 0; q < 5; ++q) {
+        const int o = 1 << q;
 #pragma unroll
         for (int i = 0; i < N; ++i) w[i] = __shfl_up_sync(0xffffffffu, v[i], o);
-        if (lane >= o) matvec_add<N>(s_pow[p], w, v);
+        if (lane >= o) matvec_add<N>(s_pow[q], w, v);
       }
       if (k + 1 < n_chunks) {
 #pragma unroll
@@ -224,28 +367,85 @@ __global__ void __launch_bounds__(32) carry_kernel(const float* __restrict__ sos
   }
 }
 
-template <int S>
-__global__ void __launch_bounds__(WARPS * 32) filter_kernel(const float* x, const float* __restrict__ gain, int C,
-                                                            int64_t T, const float* __restrict__ sos,
-                                                            int64_t sos_items, int64_t n_chunks, int64_t work,
-                                                            int reverse, const double* __restrict__ ws_s, float* out) {
+template <int S, bool EXT, bool EXTRA>
+__global__ void __launch_bounds__(WARPS * 32) filter_kernel(const Pass p, const double* __restrict__ ws_s) {
   __shared__ float s_tile[WARPS][32 * (TILE + 1)];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int64_t n_groups = (n_chunks + 31) / 32;
-  for (int64_t w = (int64_t)blockIdx.x * WARPS + wid; w < work; w += (int64_t)gridDim.x * WARPS) {
-    const int64_t row = w / n_groups, g = w - row * n_groups, b = row / C;
-    const Coef<S> c = load_coef<S>(sos + (sos_items > 1 ? b : 0) * 6 * S);
+  const int64_t n_chunks = p.n_chunks, n_groups = (n_chunks + 31) / 32, rows = p.work / n_groups;
+  for (int64_t w = (int64_t)blockIdx.x * WARPS + wid; w < p.work; w += (int64_t)gridDim.x * WARPS) {
+    const int64_t row = w / n_groups, g = w - row * n_groups, b = row / p.C;
+    const Coef<S> c = load_coef<S>(p.sos + (p.sos_items > 1 ? b : 0) * 6 * S);
+    const Row rw = make_row(p, S, row, b);
+    const int64_t lo = g * 32 * CHUNK, hi = lo + 32 * CHUNK < rw.L ? lo + 32 * CHUNK : rw.L;
     if (!c.stable) {  // warp-uniform: the whole item is NaN
-      const int64_t lo = g * 32 * CHUNK, hi = lo + 32 * CHUNK < T ? lo + 32 * CHUNK : T;
-      for (int64_t n = lo + lane; n < hi; n += 32) out[row * T + n] = __int_as_float(0x7fffffff);
+      const float nan = __int_as_float(0x7fffffff);
+      for (int64_t m = lo + lane; m < hi; m += 32) store<EXT>(rw, m, nan);
+      if (EXTRA && lane == 0) {
+        if (p.zf && rw.L - 1 >= lo && rw.L - 1 < hi) {
+          for (int i = 0; i < 2 * S; ++i) p.zf[((i >> 1) * rows + row) * 2 + (i & 1)] = (double)nan;
+        }
+        if (p.part) p.part[row * n_groups + g] = (double)nan;
+      }
       continue;
     }
-    const float g0 = gain ? __ldg(gain + b) : 1.f;
+    const bool add = p.add_first && g == 0;
+    const double add0 = add ? warp_sum(p.add_first + row * n_groups, n_groups) : 0.0;
     const int64_t k = g * 32 + lane;
     double z[2 * S];
 #pragma unroll
     for (int i = 0; i < 2 * S; ++i) z[i] = k < n_chunks ? __ldg(ws_s + (row * n_chunks + k) * 2 * S + i) : 0.0;
-    run_chunks<S, true>(x, out, row * T, T, g * 32 * CHUNK, g0, reverse, c, z, s_tile[wid]);
+    Extra ex{p.zf ? p.zf + row * 2 : nullptr, rows * 2, 0.0, 0.0};
+    run_chunks<S, true, EXT, EXTRA>(rw, lo, add, add0, c, z, s_tile[wid], ex);
+    if (EXTRA && p.part) {
+      double sv = ex.sum_v, sy = ex.sum_y;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        sv += __shfl_xor_sync(0xffffffffu, sv, o);
+        sy += __shfl_xor_sync(0xffffffffu, sy, o);
+      }
+      double G = 1.0;  // the cascade's gain at DC, as start_state's scale
+#pragma unroll
+      for (int s = 0; s < S; ++s) G *= (c.b0[s] + c.b1[s] + c.b2[s]) / (1.0 + c.a1[s] + c.a2[s]);
+      if (lane == 0) p.part[row * n_groups + g] = G * sv - sy;
+    }
+  }
+}
+
+// The sosfiltfilt backward's last step: grad_x = gain E^T f, E the edge extension, f the intermediate with the sum of
+// `part` added to its first sample (f = K^T ..., K = H + c e_0^T)
+__global__ void __launch_bounds__(256) fold_kernel(const Pass p, int S, const double* __restrict__ part,
+                                                   const float* __restrict__ f, float* __restrict__ gx) {
+  const int64_t n_groups = (p.n_chunks + 31) / 32, rows = p.work / n_groups, T = p.T, total = rows * T;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t row = i / T, n = i - row * T, b = row / p.C;
+    const int64_t pl = row_padlen(p.sos + (p.sos_items > 1 ? b : 0) * 6 * S, S, p.padlen);
+    const float* fr = f + row * p.Lmax;
+    const double* pr = part + row * n_groups;
+    auto F = [&](int64_t j) -> double {
+      double v = (double)fr[j];
+      if (j == 0) {
+        for (int64_t q = 0; q < n_groups; ++q) v += pr[q];
+      }
+      return v;
+    };
+    double acc = F(pl + n);
+    if (pl > 0) {
+      if (p.padtype == PAD_ODD || p.padtype == PAD_EVEN) {  // the mirrored samples
+        const double sgn = p.padtype == PAD_ODD ? -1.0 : 1.0;
+        if (n >= 1 && n <= pl) acc += sgn * F(pl - n);
+        if (T - 1 - n >= 1 && T - 1 - n <= pl) acc += sgn * F(2 * T - 2 + pl - n);
+      }
+      if (p.padtype == PAD_ODD || p.padtype == PAD_CONST) {  // the edge sample, 2 x[0] (odd) or x[0] (constant)
+        const double wt = p.padtype == PAD_ODD ? 2.0 : 1.0;
+        if (n == 0) {
+          for (int64_t q = 1; q <= pl; ++q) acc += wt * F(pl - q);
+        }
+        if (n == T - 1) {
+          for (int64_t q = 1; q <= pl; ++q) acc += wt * F(pl + T - 1 + q);
+        }
+      }
+    }
+    gx[i] = (float)(acc * (double)(p.gain ? __ldg(p.gain + b) : 1.f));
   }
 }
 
@@ -261,44 +461,166 @@ extern "C" size_t b2a_sos_filter_workspace_bytes(int64_t B, int C, int64_t T, in
   return (size_t)(2 * B * C * iir_chunks(T) * 2 * S) * sizeof(double);
 }
 
-template <int S>
-static int sos_launch(const float* x, const float* gain, int64_t B, int C, int64_t T, const float* sos,
-                      int64_t sos_items, int reverse, float* out, float* ws, void* stream) {
-  const int64_t rows = B * C, n_chunks = iir_chunks(T), work = rows * ((n_chunks + 31) / 32);
-  double* ws_e = reinterpret_cast<double*>(ws);
-  double* ws_s = ws_e + rows * n_chunks * 2 * S;
-  const int64_t g13 = (work + WARPS - 1) / WARPS;
+// The three launches of one pass; ws_e / ws_s: [rows, n_chunks, 2S] doubles each
+// EXT: rows padded or read from the intermediate (sosfiltfilt); else rows of x as they are (sosfilt)
+template <int S, bool EXT>
+static int run_pass(const Pass& p, double* ws_e, double* ws_s, void* stream) {
+  const int64_t rows = p.work / ((p.n_chunks + 31) / 32);
+  const int64_t g13 = (p.work + WARPS - 1) / WARPS;
   const unsigned grid13 = (unsigned)(g13 < INT32_MAX ? g13 : INT32_MAX);
   const unsigned grid2 = (unsigned)(rows < INT32_MAX ? rows : INT32_MAX);
-  B2A_LAUNCH(chunk_state_kernel<S>, dim3(grid13), dim3(WARPS * 32), 0, stream, x, gain, C, T, sos, sos_items, n_chunks,
-             work, reverse, ws_e);
+  void (*chunk_state)(const Pass, double*) = chunk_state_kernel<S, EXT>;
+  B2A_LAUNCH(chunk_state, dim3(grid13), dim3(WARPS * 32), 0, stream, p, ws_e);
   B2A_CUDA_OK(cudaGetLastError());
-  B2A_LAUNCH(carry_kernel<S>, dim3(grid2), dim3(32), 0, stream, sos, sos_items, C, rows, n_chunks, ws_e, ws_s);
+  B2A_LAUNCH(carry_kernel<S>, dim3(grid2), dim3(32), 0, stream, p, ws_e, ws_s);
   B2A_CUDA_OK(cudaGetLastError());
-  B2A_LAUNCH(filter_kernel<S>, dim3(grid13), dim3(WARPS * 32), 0, stream, x, gain, C, T, sos, sos_items, n_chunks, work,
-             reverse, ws_s, out);
+  void (*filter)(const Pass, const double*) =
+      p.zf || p.part ? filter_kernel<S, EXT, true> : filter_kernel<S, EXT, false>;
+  B2A_LAUNCH(filter, dim3(grid13), dim3(WARPS * 32), 0, stream, p, ws_s);
   B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
+}
+
+template <bool EXT>
+static int pass_launch(int S, const Pass& p, double* ws_e, double* ws_s, void* stream) {
+  switch (S) {
+    case 1: return run_pass<1, EXT>(p, ws_e, ws_s, stream);
+    case 2: return run_pass<2, EXT>(p, ws_e, ws_s, stream);
+    case 3: return run_pass<3, EXT>(p, ws_e, ws_s, stream);
+    case 4: return run_pass<4, EXT>(p, ws_e, ws_s, stream);
+    case 5: return run_pass<5, EXT>(p, ws_e, ws_s, stream);
+    case 6: return run_pass<6, EXT>(p, ws_e, ws_s, stream);
+    case 7: return run_pass<7, EXT>(p, ws_e, ws_s, stream);
+    default: return run_pass<8, EXT>(p, ws_e, ws_s, stream);
+  }
+}
+
+// A pass over rows of T samples padded by up to pmax on either side: everything but the buffers
+static Pass make_pass(int64_t B, int C, int64_t T, int64_t pmax, const float* sos, int64_t sos_items) {
+  Pass p{};
+  p.sos = sos, p.sos_items = sos_items, p.C = C, p.T = T, p.Lmax = T + 2 * pmax;
+  p.n_chunks = iir_chunks(p.Lmax);
+  p.work = B * C * ((p.n_chunks + 31) / 32);
+  return p;
+}
+
+static int check_args(const char* name, const void* x, const float* sos, const void* out, const void* ws, int64_t B,
+                      int C, int64_t T, int S, int64_t sos_items) {
+  B2A_REQUIRE(x && sos && out && ws, B2A_E_INVALID, "%s: null pointer", name);
+  B2A_REQUIRE(B >= 1 && C >= 1 && T >= 1, B2A_E_INVALID, "%s: bad shape B=%lld C=%d T=%lld", name, (long long)B, C,
+              (long long)T);
+  B2A_REQUIRE(T <= INT64_MAX / 8 / B / C, B2A_E_INVALID, "%s: B * C * T overflows", name);
+  B2A_REQUIRE(S >= 1 && S <= SMAX, B2A_E_INVALID, "%s: %d sections; 1 .. %d are supported", name, S, SMAX);
+  B2A_REQUIRE(sos_items == 1 || sos_items == B, B2A_E_INVALID, "%s: sos_items must be 1 or B=%lld, got %lld", name,
+              (long long)B, (long long)sos_items);
   return B2A_OK;
 }
 
 extern "C" int b2a_sos_filter_f32(const float* x, const float* gain, int64_t B, int C, int64_t T, const float* sos,
                                   int64_t sos_items, int S, int reverse, float* out, void* ws, void* stream) {
-  B2A_REQUIRE(x && sos && out && ws, B2A_E_INVALID, "sos_filter: null pointer");
-  B2A_REQUIRE(B >= 1 && C >= 1 && T >= 1, B2A_E_INVALID, "sos_filter: bad shape B=%lld C=%d T=%lld", (long long)B, C,
-              (long long)T);
-  B2A_REQUIRE(T <= INT64_MAX / 8 / B / C, B2A_E_INVALID, "sos_filter: B * C * T overflows");
-  B2A_REQUIRE(S >= 1 && S <= SMAX, B2A_E_INVALID, "sos_filter: %d sections; 1 .. %d are supported", S, SMAX);
-  B2A_REQUIRE(sos_items == 1 || sos_items == B, B2A_E_INVALID,
-              "sos_filter: sos_items must be 1 or B=%lld, got %lld", (long long)B, (long long)sos_items);
-  float* w = static_cast<float*>(ws);
-  switch (S) {
-    case 1: return sos_launch<1>(x, gain, B, C, T, sos, sos_items, reverse, out, w, stream);
-    case 2: return sos_launch<2>(x, gain, B, C, T, sos, sos_items, reverse, out, w, stream);
-    case 3: return sos_launch<3>(x, gain, B, C, T, sos, sos_items, reverse, out, w, stream);
-    case 4: return sos_launch<4>(x, gain, B, C, T, sos, sos_items, reverse, out, w, stream);
-    case 5: return sos_launch<5>(x, gain, B, C, T, sos, sos_items, reverse, out, w, stream);
-    case 6: return sos_launch<6>(x, gain, B, C, T, sos, sos_items, reverse, out, w, stream);
-    case 7: return sos_launch<7>(x, gain, B, C, T, sos, sos_items, reverse, out, w, stream);
-    default: return sos_launch<8>(x, gain, B, C, T, sos, sos_items, reverse, out, w, stream);
-  }
+  const int rc = check_args("sos_filter", x, sos, out, ws, B, C, T, S, sos_items);
+  if (rc != B2A_OK) return rc;
+  Pass p = make_pass(B, C, T, 0, sos, sos_items);
+  p.src = x, p.gain = gain, p.dst = out, p.reverse = reverse;
+  double* ws_e = static_cast<double*>(ws);
+  return pass_launch<false>(S, p, ws_e, ws_e + B * C * p.n_chunks * 2 * S, stream);
+}
+
+extern "C" int b2a_sos_filter_zi_f32(const float* x, const float* gain, int64_t B, int C, int64_t T, const float* sos,
+                                     int64_t sos_items, int S, const double* zi, float* out, double* zf, void* ws,
+                                     void* stream) {
+  const int rc = check_args("sos_filter_zi", x, sos, out, ws, B, C, T, S, sos_items);
+  if (rc != B2A_OK) return rc;
+  B2A_REQUIRE(zi, B2A_E_INVALID, "sos_filter_zi: null pointer");
+  Pass p = make_pass(B, C, T, 0, sos, sos_items);
+  p.src = x, p.gain = gain, p.dst = out, p.zi = zi, p.zf = zf;
+  double* ws_e = static_cast<double*>(ws);
+  return pass_launch<false>(S, p, ws_e, ws_e + B * C * p.n_chunks * 2 * S, stream);
+}
+
+// Largest padding of a call: none, the given padlen, or scipy's default at its largest, 3 (2S + 1); -1 when invalid
+static int64_t filtfilt_pmax(int S, int padtype, int64_t padlen) {
+  if (padtype < PAD_NONE || padtype > PAD_CONST) return -1;
+  if (padtype == PAD_NONE) return 0;
+  return padlen >= 0 ? padlen : 3 * (2 * S + 1);
+}
+
+// Workspace of sosfiltfilt and its backward, doubles first: ws_e, ws_s [rows, n_chunks, 2S], two partial arrays
+// [rows, n_groups], then the intermediate [rows, Lmax] floats
+struct FiltFiltWs {
+  double *e, *s, *part_a, *part_b;
+  float* mid;
+  size_t bytes;
+};
+
+static FiltFiltWs filtfilt_ws(const Pass& p, int S, int64_t rows, void* ws) {
+  FiltFiltWs w;
+  const int64_t n_groups = (p.n_chunks + 31) / 32, states = rows * p.n_chunks * 2 * S;
+  double* d = static_cast<double*>(ws);
+  w.e = d, w.s = d + states, w.part_a = d + 2 * states, w.part_b = w.part_a + rows * n_groups;
+  w.mid = reinterpret_cast<float*>(w.part_b + rows * n_groups);
+  w.bytes = (size_t)(2 * states + 2 * rows * n_groups) * sizeof(double) + (size_t)(rows * p.Lmax) * sizeof(float);
+  return w;
+}
+
+extern "C" size_t b2a_sos_filtfilt_workspace_bytes(int64_t B, int C, int64_t T, int S, int padtype, int64_t padlen) {
+  const int64_t pmax = filtfilt_pmax(S, padtype, padlen);
+  if (B < 1 || C < 1 || T < 1 || S < 1 || S > SMAX || pmax < 0 || T > INT64_MAX / 32 / B / C || T <= pmax) return 0;
+  return filtfilt_ws(make_pass(B, C, T, pmax, nullptr, 1), S, B * C, nullptr).bytes;
+}
+
+static int filtfilt_check(const char* name, const float* x, const float* sos, const float* out, const void* ws,
+                          int64_t B, int C, int64_t T, int S, int64_t sos_items, int padtype, int64_t padlen) {
+  const int rc = check_args(name, x, sos, out, ws, B, C, T, S, sos_items);
+  if (rc != B2A_OK) return rc;
+  B2A_REQUIRE(T <= INT64_MAX / 32 / B / C, B2A_E_INVALID, "%s: B * C * T overflows", name);
+  const int64_t pmax = filtfilt_pmax(S, padtype, padlen);
+  B2A_REQUIRE(pmax >= 0, B2A_E_INVALID, "%s: padtype %d; 0 (none), 1 (odd), 2 (even) or 3 (constant)", name, padtype);
+  B2A_REQUIRE(T > pmax, B2A_E_INVALID, "%s: T=%lld must exceed the padding %lld", name, (long long)T, (long long)pmax);
+  return B2A_OK;
+}
+
+extern "C" int b2a_sos_filtfilt_f32(const float* x, const float* gain, int64_t B, int C, int64_t T, const float* sos,
+                                    int64_t sos_items, int S, int padtype, int64_t padlen, float* out, void* ws,
+                                    void* stream) {
+  const int rc = filtfilt_check("sos_filtfilt", x, sos, out, ws, B, C, T, S, sos_items, padtype, padlen);
+  if (rc != B2A_OK) return rc;
+  const int64_t pmax = filtfilt_pmax(S, padtype, padlen);
+  Pass p = make_pass(B, C, T, pmax, sos, sos_items);
+  const FiltFiltWs w = filtfilt_ws(p, S, B * C, ws);
+  p.padtype = padtype, p.padlen = padtype == PAD_NONE ? 0 : padlen, p.zi_unit = 1;
+  // forward over the extended row into the intermediate, from sosfilt_zi * ext[0]
+  p.src = x, p.gain = gain, p.dst = w.mid, p.dst_mid = 1;
+  int r = pass_launch<true>(S, p, w.e, w.s, stream);
+  if (r != B2A_OK) return r;
+  // backwards over the intermediate, from sosfilt_zi * its last sample, cropped into out
+  p.src = w.mid, p.src_mid = 1, p.gain = nullptr, p.dst = out, p.dst_mid = 0, p.reverse = 1;
+  return pass_launch<true>(S, p, w.e, w.s, stream);
+}
+
+extern "C" int b2a_sos_filtfilt_backward_f32(const float* grad_y, const float* gain, int64_t B, int C, int64_t T,
+                                             const float* sos, int64_t sos_items, int S, int padtype, int64_t padlen,
+                                             float* grad_x, void* ws, void* stream) {
+  const int rc = filtfilt_check("sos_filtfilt_backward", grad_y, sos, grad_x, ws, B, C, T, S, sos_items, padtype,
+                                padlen);
+  if (rc != B2A_OK) return rc;
+  const int64_t pmax = filtfilt_pmax(S, padtype, padlen);
+  Pass p = make_pass(B, C, T, pmax, sos, sos_items);
+  const FiltFiltWs w = filtfilt_ws(p, S, B * C, ws);
+  p.padlen = padtype == PAD_NONE ? 0 : padlen;
+  // H P^T g into the intermediate (the crop's adjoint pads with zeros), and r1 = G sum(g) - sum(H P^T g)
+  p.src = grad_y, p.padtype = PAD_ZERO, p.dst = w.mid, p.dst_mid = 1, p.part = w.part_a;
+  int r = pass_launch<true>(S, p, w.e, w.s, stream);
+  if (r != B2A_OK) return r;
+  // H^T (w + r1 e_last), in place, and r2 = G sum(w') - sum(H^T w')
+  p.src = w.mid, p.src_mid = 1, p.reverse = 1, p.add_first = w.part_a, p.part = w.part_b;
+  r = pass_launch<true>(S, p, w.e, w.s, stream);
+  if (r != B2A_OK) return r;
+  // grad_x = gain E^T (f + r2 e_0)
+  p.padtype = padtype, p.gain = gain;
+  const int64_t total = B * C * T, blocks = (total + 255) / 256;
+  B2A_LAUNCH(fold_kernel, dim3((unsigned)(blocks < 65536 * 16 ? blocks : 65536 * 16)), dim3(256), 0, stream, p, S,
+             w.part_b, w.mid, grad_x);
+  B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
 }

@@ -34,7 +34,7 @@ class Engine:
     # ------------------------------------------------------------------ helpers
     DIFFERENTIABLE = ("AudioSignal.stft", "istft", "mel_spectrogram", "mfcc", "normalize", "volume_change",
                       "and magnitude / phase / log_magnitude through stft_data; resample, equalizer, convolve, apply_ir, "
-                      "ensure_max_of_audio, mix, quantization, mulaw_quantization, sos_filter, parametric_eq (gradients to "
+                      "ensure_max_of_audio, mix, quantization, mulaw_quantization, sos_filter, parametric_eq, core.iir.sosfiltfilt (gradients to "
                       "audio_data); "
                       "mask_frequencies, mask_timesteps, mask_low_magnitudes, ml.layers.SpectralGate (gradients to "
                       "stft_data / the gated signal)")
@@ -681,6 +681,91 @@ class Engine:
         self._call(self.lib.b2a_sos_filter_f32, _dptr(x), _dptr(gain), B, C, T, _dptr(sos), sos.shape[0], S,
                    int(bool(reverse)), _dptr(out), _dptr(ws), self._stream(x))
         return out
+
+    def _sos_args(self, x, sos, gain, out, name):
+        """The shared marshalling of the stateful and zero-phase cascades: x [B, C, T], sos as the kernels take it,
+        the gain [B] or None, out."""
+        x = self._prep(x, name)
+        if x.ndim != 3:
+            raise ValueError(f"{name}: x must be [B, C, T], got {tuple(x.shape)}")
+        B = x.shape[0]
+        sos = self.sos_coefficients(sos, B, x.device)
+        if gain is not None:
+            gain = self._prep(gain.reshape(-1), "gain")
+            assert gain.numel() == B
+        if out is None:
+            out = torch.empty_like(x)
+        assert out.shape == x.shape and out.dtype == torch.float32 and out.is_contiguous() and out.device == x.device
+        return x, sos, gain, out
+
+    def sos_filter_zi(self, x: torch.Tensor, sos, zi, gain: Optional[torch.Tensor] = None,
+                      out: Optional[torch.Tensor] = None):
+        """``scipy.signal.sosfilt(sos, x, zi=zi)`` for x [B, C, T] (``b2a_sos_filter_zi_f32``, DESIGN.md K19) ->
+        (y float32, zf float64 [S, B, C, 2]).  ``zi`` is scipy's layout for this x, [S, B, C, 2], float64 or float32;
+        the state stays in double, so ``zf`` chained into the next segment's ``zi`` gives one pass over the whole row.
+        ``sos`` and ``gain`` as in ``sos_filter``.  Three launches, no host sync."""
+        x, sos, gain, out = self._sos_args(x, sos, gain, out, "x")
+        B, C, T = x.shape
+        S = sos.shape[1]
+        zi = torch.as_tensor(zi)
+        self._refuse_grad(zi, "zi")
+        if tuple(zi.shape) != (S, B, C, 2):
+            raise ValueError(f"sosfilt: zi must be [{S}, {B}, {C}, 2] for x {tuple(x.shape)}, got {tuple(zi.shape)}")
+        zi = zi.to(device=x.device, dtype=torch.float64).contiguous()
+        zf = torch.empty(S, B, C, 2, dtype=torch.float64, device=x.device)
+        ws_bytes = int(self.lib.b2a_sos_filter_workspace_bytes(B, C, T, S))
+        if ws_bytes == 0:
+            raise _lib.B2AError(f"sosfilt: unsupported shape {tuple(x.shape)}")
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        self._call(self.lib.b2a_sos_filter_zi_f32, _dptr(x), _dptr(gain), B, C, T, _dptr(sos), sos.shape[0], S,
+                   _dptr(zi), _dptr(out), _dptr(zf), _dptr(ws), self._stream(x))
+        return out, zf
+
+    SOS_PADTYPES = {None: 0, "odd": 1, "even": 2, "constant": 3}  # b2a_sos_filtfilt_f32
+
+    def _filtfilt_args(self, x, sos, padtype, padlen, gain, out, name):
+        if padtype not in self.SOS_PADTYPES:
+            raise ValueError(f"sosfiltfilt: padtype must be 'odd', 'even', 'constant' or None, got {padtype!r}")
+        if padlen is not None and int(padlen) < 0:
+            raise ValueError(f"sosfiltfilt: padlen must be >= 0, got {padlen}")
+        x, sos, gain, out = self._sos_args(x, sos, gain, out, name)
+        B, C, T = x.shape
+        S = sos.shape[1]
+        pt = self.SOS_PADTYPES[padtype]
+        pl = -1 if padlen is None else int(padlen)
+        # the default is checked at its largest, 3 (2S + 1): the per-item value lives on the device
+        edge = 0 if padtype is None else (3 * (2 * S + 1) if pl < 0 else pl)
+        if T <= edge:
+            raise ValueError(f"sosfiltfilt: the length of the input ({T}) must be greater than the padding ({edge})"
+                             + (", the largest default for these sections" if pl < 0 else ""))
+        ws_bytes = int(self.lib.b2a_sos_filtfilt_workspace_bytes(B, C, T, S, pt, pl))
+        if ws_bytes == 0:
+            raise _lib.B2AError(f"sosfiltfilt: unsupported shape {tuple(x.shape)}")
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        return x, sos, gain, out, pt, pl, ws
+
+    def sos_filtfilt(self, x: torch.Tensor, sos, padtype="odd", padlen: Optional[int] = None,
+                     gain: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``scipy.signal.sosfiltfilt(sos, x, padtype=padtype, padlen=padlen)`` (method "pad") for x [B, C, T]
+        (``b2a_sos_filtfilt_f32``, DESIGN.md K19).  ``padlen=None`` is scipy's default for each item's sections,
+        3 (2S + 1 - min(#{b2 = 0}, #{a2 = 0})); T must exceed the padding, checked against 3 (2S + 1) for the default
+        so that nothing is read back (this refuses rows of at most 51 samples that scipy would take).  ``sos`` and
+        ``gain`` as in ``sos_filter``.  Six launches, no host sync."""
+        x, sos, gain, out, pt, pl, ws = self._filtfilt_args(x, sos, padtype, padlen, gain, out, "x")
+        B, C, T = x.shape
+        self._call(self.lib.b2a_sos_filtfilt_f32, _dptr(x), _dptr(gain), B, C, T, _dptr(sos), sos.shape[0],
+                   sos.shape[1], pt, pl, _dptr(out), _dptr(ws), self._stream(x))
+        return out
+
+    def sos_filtfilt_backward(self, grad_y: torch.Tensor, sos, padtype="odd", padlen: Optional[int] = None,
+                              gain: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The gradient of ``sos_filtfilt`` with respect to x for the upstream gradient ``grad_y`` [B, C, T]
+        (``b2a_sos_filtfilt_backward_f32``).  Seven launches, no host sync."""
+        g, sos, gain, gx, pt, pl, ws = self._filtfilt_args(grad_y, sos, padtype, padlen, gain, None, "grad_y")
+        B, C, T = g.shape
+        self._call(self.lib.b2a_sos_filtfilt_backward_f32, _dptr(g), _dptr(gain), B, C, T, _dptr(sos), sos.shape[0],
+                   sos.shape[1], pt, pl, _dptr(gx), _dptr(ws), self._stream(g))
+        return gx
 
     def gain(self, x: torch.Tensor, gain: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``x[b] * gain[b]`` (ref:audiotools/core/effects.py:219,237)."""

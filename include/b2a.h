@@ -361,6 +361,31 @@ size_t b2a_sos_filter_workspace_bytes(int64_t B, int C, int64_t T, int S);
 int b2a_sos_filter_f32(const float* x, const float* gain, int64_t B, int C, int64_t T, const float* sos,
                        int64_t sos_items, int S, int reverse, float* out, void* ws, void* stream);
 
+/* scipy.signal.sosfilt(sos, x, zi=zi), per item: as b2a_sos_filter_f32 (reverse = 0), started from zi [S, B, C, 2]
+ * float64 (scipy's layout for x [B, C, T]); zf nullable [S, B, C, 2] float64 receives the state after sample T - 1
+ * (NaN for an unstable item).  The state is carried in double, so chaining zf into the next segment's zi gives one
+ * pass over the whole row.  ws: b2a_sos_filter_workspace_bytes(B, C, T, S) bytes.  Three launches, no host sync. */
+int b2a_sos_filter_zi_f32(const float* x, const float* gain, int64_t B, int C, int64_t T, const float* sos,
+                          int64_t sos_items, int S, const double* zi, float* out, double* zf, void* ws, void* stream);
+
+/* scipy.signal.sosfiltfilt(sos, x, padtype, padlen), method "pad", per item; x, gain and sos as b2a_sos_filter_f32.
+ * padtype 0 (None: no extension), 1 (odd), 2 (even) or 3 (constant); padlen >= 0, or -1 for scipy's default per item,
+ * 3 (2S + 1 - min(#{b2 = 0}, #{a2 = 0})).  The row is extended by padlen samples on either side in the loads, filtered
+ * forwards from sosfilt_zi(sos) ext[0] into a float32 intermediate, backwards from sosfilt_zi(sos) times its last
+ * sample, and cropped.  T must exceed the padding: padlen, or 3 (2S + 1) with the default.  An unstable item is all
+ * NaN; a NaN or inf sample makes its whole row non-finite.  out may alias x.
+ * ws: b2a_sos_filtfilt_workspace_bytes(B, C, T, S, padtype, padlen) bytes (0 for a bad shape or padding), shared with
+ * the backward.  Six launches, no host sync. */
+size_t b2a_sos_filtfilt_workspace_bytes(int64_t B, int C, int64_t T, int S, int padtype, int64_t padlen);
+int b2a_sos_filtfilt_f32(const float* x, const float* gain, int64_t B, int C, int64_t T, const float* sos,
+                         int64_t sos_items, int S, int padtype, int64_t padlen, float* out, void* ws, void* stream);
+/* The gradient of b2a_sos_filtfilt_f32 with respect to x for the upstream gradient grad_y [B, C, T]: the adjoints of
+ * the two passes, the rank-one terms of their start states and the fold of the edge extension.  Same arguments and
+ * workspace; grad_x may alias grad_y.  Seven launches, no host sync. */
+int b2a_sos_filtfilt_backward_f32(const float* grad_y, const float* gain, int64_t B, int C, int64_t T,
+                                  const float* sos, int64_t sos_items, int S, int padtype, int64_t padlen,
+                                  float* grad_x, void* ws, void* stream);
+
 /* ---- per-item gain ---------------------------------------------------------------------
  * x[b, :, :] * gain[b]  (EffectMixin.normalize / volume_change, effects.py:219,237).
  * out may alias x.  per_item = C*T. */
