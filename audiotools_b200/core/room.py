@@ -1,0 +1,132 @@
+"""Shoebox-room impulse responses by the image-source method (Allen & Berkley 1979) for a whole batch on the GPU
+(csrc/rir.cu, DESIGN.md K20).
+
+``image_source_ir(room, source, mics, sample_rate, length, beta=... | rt60=...)`` returns an ``AudioSignal``
+[B, C, length]: channel c of item b is the response from item b's source to its microphone c, ready for
+``AudioSignal.apply_ir``.  Lengths are in metres, the sound speed in m/s.  Each image of the source adds a
+Hann-windowed fractional delay of 2 floor(0.004 sample_rate + 1/2) samples, centred on its distance, scaled by the
+product of the wall reflection coefficients it meets over 4 pi times its distance in metres; ``high_pass`` then
+applies Allen & Berkley's 100 Hz high-pass as one second-order section.  ``rt60`` in place of ``beta`` gives all six
+walls the reflection coefficient of Sabine's formula (``sabine_beta``).
+
+The geometry is checked on host values (``util.host_view`` reads a table's host mirror, so no device sync is needed)
+and is a constant: a geometry tensor that requires a gradient raises ``NotImplementedError``.
+"""
+import math
+
+import numpy as np
+import torch
+
+from . import grad as _grad
+from . import util
+
+MIN_SAMPLE_RATE = 125.0     # below it the window 2 floor(0.004 fs + 1/2) is empty
+MAX_SAMPLE_RATE = 384000.0  # csrc/rir.cu's largest window table
+MIN_DISTANCE = 1e-3         # metres between the source and a microphone
+
+
+def _host(name: str, v) -> np.ndarray:
+    _grad.refuse_param_grad("image_source_ir", name, v)
+    if torch.is_tensor(v):
+        v = util.host_view(v).detach().cpu().numpy()  # the host mirror belongs to v itself, not to a detached view
+    return np.asarray(v, dtype=np.float64)
+
+
+def _room_sizes(room: np.ndarray):
+    """Volume and surface of rooms [..., 3]."""
+    lx, ly, lz = room[..., 0], room[..., 1], room[..., 2]
+    return lx * ly * lz, 2.0 * (lx * ly + lx * lz + ly * lz)
+
+
+def min_rt60(room, sound_speed: float = 343.0) -> np.ndarray:
+    """The smallest RT60 Sabine's formula gives a room [..., 3]: every wall fully absorbing (alpha = 1)."""
+    vol, surf = _room_sizes(np.asarray(room, dtype=np.float64))
+    return 24.0 * math.log(10.0) * vol / (sound_speed * surf)
+
+
+def sabine_beta(room, rt60, sound_speed: float = 343.0) -> np.ndarray:
+    """Wall reflection coefficients [..., 6] for rooms [..., 3] and reverberation times ``rt60`` (seconds, scalar or
+    [...]) by Sabine: alpha = 24 ln 10 V / (c S rt60), beta = sqrt(1 - alpha), the same for all six walls; rt60 = 0
+    gives beta = 0.  A time below the room's smallest feasible RT60 (alpha > 1) raises ``ValueError``."""
+    room = np.asarray(room, dtype=np.float64)
+    rt60 = np.asarray(rt60, dtype=np.float64)
+    if not (np.all(np.isfinite(rt60)) and np.all(rt60 >= 0)):
+        raise ValueError(f"rt60 must be finite and >= 0, got {rt60}")
+    vol, surf = _room_sizes(room)
+    pos = rt60 > 0
+    alpha = np.where(pos, 24.0 * math.log(10.0) * vol / (sound_speed * surf * np.where(pos, rt60, 1.0)), 1.0)
+    bad = alpha > 1.0
+    if np.any(bad):
+        lo = np.broadcast_to(min_rt60(room, sound_speed), alpha.shape)[bad].flat[0]
+        t = np.broadcast_to(rt60, alpha.shape)[bad].flat[0]
+        raise ValueError(f"rt60 = {t:.6g} s is below the room's smallest feasible RT60, {lo:.6g} s (Sabine, every "
+                         "wall fully absorbing)")
+    return np.repeat(np.sqrt(1.0 - alpha)[..., None], 6, axis=-1)
+
+
+def _batch(name: str, v: np.ndarray, item_ndim: int, B: int) -> np.ndarray:
+    if v.ndim == item_ndim:
+        return np.broadcast_to(v, (B,) + v.shape)
+    if v.ndim == item_ndim + 1 and v.shape[0] in (1, B):
+        return np.broadcast_to(v, (B,) + v.shape[1:])
+    raise ValueError(f"image_source_ir: {name} of shape {v.shape} does not fit a batch of {B}")
+
+
+def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta=None, rt60=None,
+                    max_order: int = -1, sound_speed: float = 343.0, high_pass: bool = True, device="cuda"):
+    """Impulse responses [B, C, length] of shoebox rooms by the image-source method, as an ``AudioSignal`` at
+    ``sample_rate``.
+
+    ``room`` [3] or [B, 3] (Lx, Ly, Lz), ``source`` [3] or [B, 3], ``mics`` [C, 3] or [B, C, 3]; exactly one of
+    ``beta`` ([6] or [B, 6]: the walls x = 0, x = Lx, y = 0, y = Ly, z = 0, z = Lz, each in [0, 1]) and ``rt60``
+    (seconds, scalar or [B]; ``sabine_beta``).  ``max_order`` >= 0 keeps the images of at most that order (the number
+    of wall reflections); -1 keeps every image that arrives within ``length`` samples.  One kernel launch, three more
+    with ``high_pass``; no host sync."""
+    from ..engine import get_engine
+    from .audio_signal import AudioSignal
+
+    if (beta is None) == (rt60 is None):
+        raise ValueError("image_source_ir: give exactly one of beta and rt60")
+    room_h, src_h, mics_h = _host("room", room), _host("source", source), _host("mics", mics)
+    wall_h = _host("beta" if rt60 is None else "rt60", beta if rt60 is None else rt60)
+    sample_rate, length, max_order, sound_speed = float(sample_rate), int(length), int(max_order), float(sound_speed)
+    if not MIN_SAMPLE_RATE <= sample_rate <= MAX_SAMPLE_RATE:
+        raise ValueError(f"image_source_ir: sample_rate = {sample_rate:g}; {MIN_SAMPLE_RATE:g} .. "
+                         f"{MAX_SAMPLE_RATE:g} Hz are supported (below 125 Hz the window 2 round(0.004 fs) is empty)")
+    if length < 1:
+        raise ValueError(f"image_source_ir: length = {length} must be >= 1")
+    if max_order < -1:
+        raise ValueError(f"image_source_ir: max_order = {max_order} must be >= -1 (-1: every image)")
+    if not (math.isfinite(sound_speed) and sound_speed > 0):
+        raise ValueError(f"image_source_ir: sound_speed = {sound_speed} must be positive")
+    B = max(room_h.shape[0] if room_h.ndim == 2 else 1, src_h.shape[0] if src_h.ndim == 2 else 1,
+            mics_h.shape[0] if mics_h.ndim == 3 else 1,
+            (wall_h.shape[0] if wall_h.ndim == 2 else 1) if rt60 is None else (wall_h.size if wall_h.ndim else 1))
+    room_h = _batch("room", room_h, 1, B)
+    src_h = _batch("source", src_h, 1, B)
+    mics_h = _batch("mics", mics_h, 2, B)
+    if room_h.shape[-1] != 3 or src_h.shape[-1] != 3 or mics_h.shape[-1] != 3:
+        raise ValueError("image_source_ir: room, source and microphone positions have 3 coordinates")
+    if not (np.all(np.isfinite(room_h)) and np.all(room_h > 0)):
+        raise ValueError(f"image_source_ir: room dimensions must be positive, got {room_h.min(axis=0)} at least")
+    for name, p in (("source", src_h[:, None]), ("microphone", mics_h)):
+        if not (np.all(np.isfinite(p)) and np.all(p > 0) and np.all(p < room_h[:, None])):
+            raise ValueError(f"image_source_ir: every {name} must be strictly inside its room")
+    gap = np.sqrt(((mics_h - src_h[:, None]) ** 2).sum(-1))
+    if np.any(gap < MIN_DISTANCE):
+        raise ValueError(f"image_source_ir: a microphone is {gap.min():.3g} m from the source; at least "
+                         f"{MIN_DISTANCE:g} m is needed")
+    if rt60 is None:
+        beta_h = _batch("beta", wall_h, 1, B)
+        if beta_h.shape[-1] != 6:
+            raise ValueError(f"image_source_ir: beta must have 6 walls, got {beta_h.shape}")
+    else:
+        beta_h = sabine_beta(room_h, _batch("rt60", wall_h.reshape(-1) if wall_h.ndim else wall_h, 0, B),
+                             sound_speed)
+    if not (np.all(beta_h >= 0) and np.all(beta_h <= 1)):
+        raise ValueError("image_source_ir: every reflection coefficient beta must be in [0, 1]")
+    dev = torch.device(device)
+    tab = [torch.from_numpy(np.array(a, dtype=np.float64)).to(dev, non_blocking=True)
+           for a in (room_h, src_h, mics_h, beta_h)]
+    ir = get_engine().image_source_ir(*tab, length, sample_rate, sound_speed, max_order, high_pass)
+    return AudioSignal(ir, sample_rate)

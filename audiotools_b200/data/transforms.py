@@ -552,6 +552,68 @@ class RoomImpulseResponse(BaseTransform):
         return signal.apply_ir(ir_signal.clone(), drr, eq, use_original_phase=self.use_original_phase, _bypass=_bypass)
 
 
+class SyntheticRoomImpulseResponse(BaseTransform):
+    """``signal.apply_ir(ir)`` with one simulated shoebox room per item (an extension; ``core.room.image_source_ir``):
+    no impulse-response collection is needed.  The signal's C channels are C microphones on a horizontal line.
+
+    Per item, in this order: the room's x, y and z (``room``, three distribution tuples, metres); ``rt60`` (seconds),
+    raised to 1.01 times the room's smallest feasible RT60 (``core.room.min_rt60``); the source, one
+    ``state.uniform`` call for x, y, z inside the room shrunk by ``margin`` on every side; the microphone spacing
+    (``mic_spacing``, metres); the array's azimuth, ``uniform(0, 2 pi)``; the array's centre, one ``state.uniform``
+    call inside the room shrunk by ``margin`` plus half the array's extent along x and y.  A room too small for the
+    margin or the array raises ``ValueError``.  The IR is ``duration`` seconds long when given, else the batch's
+    longest RT60, and never longer than the signal.  All walls absorb alike (Sabine); ``max_order`` and ``high_pass``
+    are passed to ``image_source_ir``."""
+    _bypass_pays = False  # FFT convolution
+
+    DEFAULT_ROOM = (("uniform", 3.0, 10.0), ("uniform", 3.0, 8.0), ("uniform", 2.4, 4.0))
+
+    def __init__(self, room: tuple = DEFAULT_ROOM, rt60: tuple = ("uniform", 0.2, 0.8), margin: float = 0.5,
+                 mic_spacing: tuple = ("uniform", 0.05, 0.2), max_order: int = -1, duration: float = None,
+                 high_pass: bool = True, name: str = None, prob: float = 1.0, use_original_phase: bool = False):
+        super().__init__(name=name, prob=prob)
+        self.room = tuple(room)
+        self.rt60 = rt60
+        self.margin = float(margin)
+        self.mic_spacing = mic_spacing
+        self.max_order = int(max_order)
+        self.duration = duration
+        self.high_pass = high_pass
+        self.use_original_phase = use_original_phase
+
+    def _instantiate(self, state: RandomState, signal: AudioSignal):
+        from ..core import room as _room
+
+        dims = np.array([float(util.sample_from_dist(d, state)) for d in self.room])
+        rt60 = float(util.sample_from_dist(self.rt60, state))
+        lo, hi = np.full(3, self.margin), dims - self.margin
+        if np.any(lo >= hi):
+            raise ValueError(f"SyntheticRoomImpulseResponse: room {dims} m is too small for a {self.margin} m margin")
+        source = state.uniform(lo, hi)
+        spacing = float(util.sample_from_dist(self.mic_spacing, state))
+        azimuth = state.uniform(0.0, 2.0 * np.pi)
+        C = signal.num_channels
+        axis = np.array([np.cos(azimuth), np.sin(azimuth), 0.0])
+        ext = 0.5 * (C - 1) * spacing * np.abs(axis)
+        if np.any(lo + ext > hi - ext):
+            raise ValueError(f"SyntheticRoomImpulseResponse: room {dims} m is too small for {C} microphones "
+                             f"{spacing} m apart and a {self.margin} m margin")
+        centre = state.uniform(lo + ext, hi - ext)
+        mics = centre + (np.arange(C) - 0.5 * (C - 1))[:, None] * spacing * axis
+        rt60 = max(rt60, 1.01 * float(_room.min_rt60(dims)))
+        return {"room": dims, "rt60": np.float64(rt60), "source": source, "mics": mics}
+
+    def _transform(self, signal, room, rt60, source, mics, _bypass=None):
+        from ..core.room import image_source_ir
+
+        sr, T = signal.sample_rate, signal.signal_length
+        seconds = self.duration if self.duration is not None else float(util.host_view(rt60).max())
+        length = max(1, min(T, int(np.ceil(seconds * sr))))
+        ir = image_source_ir(room, source, mics, sr, length, rt60=rt60, max_order=self.max_order,
+                             high_pass=self.high_pass, device=signal.device)
+        return signal.apply_ir(ir, use_original_phase=self.use_original_phase, _bypass=_bypass)
+
+
 class PitchShift(BaseTransform):
     """``signal.pitch_shift(n_semitones)``.  NEW: the reference has no PitchShift transform (only the
     ``AudioSignal.pitch_shift`` method, ref:audiotools/core/effects.py:247-277, which takes ONE shift

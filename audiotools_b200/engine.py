@@ -767,6 +767,34 @@ class Engine:
                    sos.shape[1], pt, pl, _dptr(gx), _dptr(ws), self._stream(g))
         return gx
 
+    RIR_MAX_ROWS = 65535  # items x microphones of one b2a_rir_ism_f32 launch (grid y)
+
+    def image_source_ir(self, room: torch.Tensor, src: torch.Tensor, mics: torch.Tensor, beta: torch.Tensor,
+                        length: int, sample_rate: float, sound_speed: float = 343.0, max_order: int = -1,
+                        high_pass: bool = True) -> torch.Tensor:
+        """Shoebox-room impulse responses by the image-source method (``b2a_rir_ism_f32``, DESIGN.md K20) -> [B, C,
+        length] float32.  room [B, 3], src [B, 3], mics [B, C, 3] (metres) and beta [B, 6] are float64 tensors on the
+        device, already checked (``core.room.image_source_ir``).  ``high_pass`` applies Allen & Berkley's 100 Hz
+        high-pass as one second-order section through ``sos_filter``.  One launch, three more with the high-pass."""
+        if mics.ndim != 3 or mics.shape[-1] != 3:
+            raise ValueError(f"image_source_ir: mics must be [B, C, 3], got {tuple(mics.shape)}")
+        B, C = mics.shape[:2]
+        if tuple(room.shape) != (B, 3) or tuple(src.shape) != (B, 3) or tuple(beta.shape) != (B, 6):
+            raise ValueError(f"image_source_ir: room / source / beta must be [{B}, 3] / [{B}, 3] / [{B}, 6], got "
+                             f"{tuple(room.shape)} / {tuple(src.shape)} / {tuple(beta.shape)}")
+        if B * C > self.RIR_MAX_ROWS:
+            raise ValueError(f"image_source_ir: {B * C} rows (items x microphones); at most {self.RIR_MAX_ROWS}")
+        room, src, mics, beta = (self._prep(t, n, torch.float64) for t, n in
+                                 ((room, "room"), (src, "source"), (mics, "mics"), (beta, "beta")))
+        out = torch.empty(B, C, int(length), dtype=torch.float32, device=room.device)
+        self._call(self.lib.b2a_rir_ism_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), B, C, int(length),
+                   float(sample_rate), float(sound_speed), int(max_order), _dptr(out), self._stream(room))
+        if high_pass:
+            w = 2 * math.pi * 100.0 / sample_rate
+            r = math.exp(-w)
+            out = self.sos_filter(out, [[1.0, -(1.0 + r), r, 1.0, -2.0 * r * math.cos(w), r * r]], out=out)
+        return out
+
     def gain(self, x: torch.Tensor, gain: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``x[b] * gain[b]`` (ref:audiotools/core/effects.py:219,237)."""
         x = self._prep(x, "x")

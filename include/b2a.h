@@ -386,6 +386,18 @@ int b2a_sos_filtfilt_backward_f32(const float* grad_y, const float* gain, int64_
                                   const float* sos, int64_t sos_items, int S, int padtype, int64_t padlen,
                                   float* grad_x, void* ws, void* stream);
 
+/* ---- shoebox-room impulse responses by the image-source method (csrc/rir.cu) ----------------------------------------
+ * out [B, C, L] float32: the impulse response from item b's source to its microphone c (DESIGN.md K20).  Geometry is
+ * float64 on the device: room [B, 3] (Lx, Ly, Lz, metres), src [B, 3], mics [B, C, 3], beta [B, 6] (reflection
+ * coefficients of the walls x = 0, x = Lx, y = 0, y = Ly, z = 0, z = Lz).  fs in [125, 384000] Hz, c > 0 m/s;
+ * max_order >= 0 keeps images of at most that order, -1 keeps every image that reaches the first L samples.  Each image
+ * adds g h(i - d) at the Tw = 2 floor(0.004 fs + 1/2) samples around its distance d (samples), h a Hann-windowed
+ * sinc.  B C <= 65535, L <= 2^30; the arguments are not checked against each other (positions inside the room, beta in
+ * [0, 1]): core/room.py does that.  One launch, no host sync, no atomics: reruns and a batch against its items one at a
+ * time are bit-identical. */
+int b2a_rir_ism_f32(const double* room, const double* src, const double* mics, const double* beta, int64_t B, int C,
+                    int64_t L, double fs, double c, int max_order, float* out, void* stream);
+
 /* ---- per-item gain ---------------------------------------------------------------------
  * x[b, :, :] * gain[b]  (EffectMixin.normalize / volume_change, effects.py:219,237).
  * out may alias x.  per_item = C*T. */
