@@ -9,6 +9,13 @@ product of the wall reflection coefficients it meets over 4 pi times its distanc
 applies Allen & Berkley's 100 Hz high-pass as one second-order section.  ``rt60`` in place of ``beta`` gives all six
 walls the reflection coefficient of Sabine's formula (``sabine_beta``).
 
+``diffuse_after`` (seconds, scalar or [B]) with ``seed`` (int or [B] ints) makes a hybrid response: the images
+arriving before sample n_d = ceil(diffuse_after sample_rate) only, and from n_d - Tw/2 on a diffuse tail, Gaussian
+noise under the energy envelope the same room's images have on average (a raised-cosine crossfade over the Tw samples
+centred on n_d).  The image count up to a time t grows with t^3, so a short ``diffuse_after`` makes long responses
+cheap.  The tail is frequency-flat like the walls, and the tails of different microphones are independent; it depends
+only on the item's geometry, its seed and the microphone, so a batch equals its items one at a time.
+
 The geometry is checked on host values (``util.host_view`` reads a table's host mirror, so no device sync is needed)
 and is a constant: a geometry tensor that requires a gradient raises ``NotImplementedError``.
 """
@@ -73,7 +80,8 @@ def _batch(name: str, v: np.ndarray, item_ndim: int, B: int) -> np.ndarray:
 
 
 def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta=None, rt60=None,
-                    max_order: int = -1, sound_speed: float = 343.0, high_pass: bool = True, device="cuda"):
+                    max_order: int = -1, sound_speed: float = 343.0, high_pass: bool = True, diffuse_after=None,
+                    seed=None, device="cuda"):
     """Impulse responses [B, C, length] of shoebox rooms by the image-source method, as an ``AudioSignal`` at
     ``sample_rate``.
 
@@ -81,7 +89,11 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
     ``beta`` ([6] or [B, 6]: the walls x = 0, x = Lx, y = 0, y = Ly, z = 0, z = Lz, each in [0, 1]) and ``rt60``
     (seconds, scalar or [B]; ``sabine_beta``).  ``max_order`` >= 0 keeps the images of at most that order (the number
     of wall reflections); -1 keeps every image that arrives within ``length`` samples.  One kernel launch, three more
-    with ``high_pass``; no host sync."""
+    with ``high_pass``; no host sync.
+
+    ``diffuse_after`` (seconds > 0, scalar or [B]) and ``seed`` (an int or [B] ints in [0, 2^63)) add the diffuse tail
+    (module docstring; DESIGN.md K20 "Hybrid"): two kernel launches before the high-pass.  It needs ``max_order =
+    -1`` (the tail stands for images of every order); ``None`` leaves the images-only path untouched."""
     from ..engine import get_engine
     from .audio_signal import AudioSignal
 
@@ -99,9 +111,27 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
         raise ValueError(f"image_source_ir: max_order = {max_order} must be >= -1 (-1: every image)")
     if not (math.isfinite(sound_speed) and sound_speed > 0):
         raise ValueError(f"image_source_ir: sound_speed = {sound_speed} must be positive")
+    n_tail = 1
+    if diffuse_after is None and seed is not None:
+        raise ValueError("image_source_ir: seed is for the diffuse tail; give diffuse_after too")
+    if diffuse_after is not None:
+        td_h = _host("diffuse_after", diffuse_after).reshape(-1)
+        if not (td_h.size and np.all(np.isfinite(td_h)) and np.all(td_h > 0)):
+            raise ValueError(f"image_source_ir: diffuse_after = {td_h} must be finite and > 0 seconds")
+        if max_order != -1:
+            raise ValueError(f"image_source_ir: max_order = {max_order} with diffuse_after; the diffuse tail stands "
+                             "for images of every order, so it needs max_order = -1")
+        if seed is None:
+            raise ValueError("image_source_ir: diffuse_after needs a seed (an int or one per item)")
+        sd = np.asarray(util.host_view(seed).detach().cpu().numpy() if torch.is_tensor(seed) else seed).reshape(-1)
+        if sd.dtype.kind not in "iu" or not (sd.size and np.all(sd >= 0) and np.all(sd < 2 ** 63)):
+            raise ValueError(f"image_source_ir: seed = {sd} must be integers in [0, 2^63)")
+        sd = sd.astype(np.int64)
+        n_tail = max(td_h.size, sd.size)
     B = max(room_h.shape[0] if room_h.ndim == 2 else 1, src_h.shape[0] if src_h.ndim == 2 else 1,
             mics_h.shape[0] if mics_h.ndim == 3 else 1,
-            (wall_h.shape[0] if wall_h.ndim == 2 else 1) if rt60 is None else (wall_h.size if wall_h.ndim else 1))
+            (wall_h.shape[0] if wall_h.ndim == 2 else 1) if rt60 is None else (wall_h.size if wall_h.ndim else 1),
+            n_tail)
     room_h = _batch("room", room_h, 1, B)
     src_h = _batch("source", src_h, 1, B)
     mics_h = _batch("mics", mics_h, 2, B)
@@ -128,5 +158,11 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
     dev = torch.device(device)
     tab = [torch.from_numpy(np.array(a, dtype=np.float64)).to(dev, non_blocking=True)
            for a in (room_h, src_h, mics_h, beta_h)]
-    ir = get_engine().image_source_ir(*tab, length, sample_rate, sound_speed, max_order, high_pass)
+    tail = {}
+    if diffuse_after is not None:
+        td_h = _batch("diffuse_after", td_h, 0, B)
+        sd = _batch("seed", sd, 0, B)
+        tail = dict(diffuse_after=torch.from_numpy(np.array(td_h, dtype=np.float64)).to(dev, non_blocking=True),
+                    seed=torch.from_numpy(np.array(sd, dtype=np.int64)).to(dev, non_blocking=True))
+    ir = get_engine().image_source_ir(*tab, length, sample_rate, sound_speed, max_order, high_pass, **tail)
     return AudioSignal(ir, sample_rate)

@@ -24,6 +24,18 @@
 // with cos / sin(pi k / Tw) from a per-CTA table, so the large argument pi (k - e) is never rounded; (-1)^i is applied
 // once per sample at the end.  A sample's sum depends only on its row's geometry and the tile size: reruns and a batch
 // against its items one at a time are bit-identical.
+//
+// Hybrid (b2a_rir_hybrid_f32): the image sources for the early part only, a statistical tail after it.  With n_d =
+// ceil(t_d fs), ism_kernel keeps the images with floor(d) < min(L, n_d); tail_kernel then adds, at every sample
+// n >= n_d - Tw/2, w(n) sqrt(E(n)) xi(seed, c, n):
+//   E(n) = c / (4 pi V fs) (1/4pi) int exp(-n sum_a lambda_a |u_a|) dOmega(u),  lambda_a = -(ln b_a0 + ln b_a1) / L_a
+// (L_a in samples), the expected energy per sample of the image arrivals at n; w^2 = 1/2 (1 - cos(pi x)), x = (n - n_d
+// + Tw/2 + 1/2) / Tw, over the Tw samples centred on n_d, then 1; xi a standard normal from a SplitMix64 counter
+// (key = mix(mix(seed) + c), z = mix(key + n gamma)) by Box-Muller.  A wall with beta = 0 gives E = 0.
+//   ln E is evaluated in double at nodes n_k = tau (1.1^k - 1), tau = max(1, 1 / sum lambda) samples, by a tanh-sinh
+// rule (65 x 65 points) in u_z (uniform on [0, 1]) and the azimuth over one octant, with its derivative, and
+// interpolated between nodes by a cubic Hermite (relative error below 1e-5: (ln E)'''' falls off like 12 / n^4).  Each
+// CTA evaluates the nodes its tile spans, so the tail too depends only on its row's geometry, seed and microphone.
 #include "b2a_common.h"
 
 namespace b2a {
@@ -40,6 +52,8 @@ constexpr int FAR = -(1 << 30);  // floor(d) of a staged slot that holds no imag
 
 struct Geo {
   const double *room, *src, *mics, *beta;
+  const double* td;        // per item: the diffuse tail starts at ceil(td fs); null: images only
+  const uint64_t* seed;    // per item: the tail's noise
   int C, L, Tw, max_order;
   double fs, c;
   float* out;
@@ -84,7 +98,12 @@ __global__ void __launch_bounds__(NT) ism_kernel(const Geo g) {
   }
   // the shell: floor(d) in [dlo, dhi)
   const double dlo = (double)t0 - half;
-  const double dhi = fmin((double)t0 + TT + half - 1, (double)g.L);
+  const double lim = g.td ? fmin((double)g.L, ceil(g.td[b] * g.fs)) : (double)g.L;  // images with floor(d) < lim
+  const double dhi = fmin((double)t0 + TT + half - 1, lim);
+  if (dhi <= dlo) {  // a tile past the images (only with a diffuse tail)
+    for (int i = t0 + tid; i < min(t0 + TT, g.L); i += NT) g.out[row * (int64_t)g.L + i] = 0.f;
+    return;
+  }
   const double reach = dhi * (1.0 + 1e-12) + 1e-6;  // lines with rho >= reach have no image in the shell
   int64_t Mx = (int64_t)ceil(dhi / (2 * Lx)) + 1, My = (int64_t)ceil(dhi / (2 * Ly)) + 1;
   if (g.max_order >= 0) {  // |2 mx - q| <= max_order
@@ -202,27 +221,153 @@ __global__ void __launch_bounds__(NT) ism_kernel(const Geo g) {
   }
 }
 
+
+constexpr int QK = 32;                // tanh-sinh: 2 QK + 1 points per dimension, steps of 3 / QK
+constexpr int QM = 2 * QK + 1;
+constexpr int QN = QM * QM;
+constexpr double GROW = 1.1;          // envelope nodes n_k = tau (GROW^k - 1)
+constexpr int NK = 72;                // nodes one tile spans: at most ln(TT + 1) / ln(GROW) + 3
+constexpr uint64_t GAMMA = 0x9E3779B97F4A7C15ull;
+
+__device__ __forceinline__ uint64_t mix64(uint64_t z) {  // the SplitMix64 finaliser
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+__device__ __forceinline__ int node_of(double n, double tau, double lr) { return (int)floor(log1p(n / tau) / lr); }
+
+__global__ void __launch_bounds__(NT) tail_kernel(const Geo g) {
+  __shared__ double qa[QM], qr[QM], qw[QM], pb[QM], pw[QM];  // z: lambda_z z, sqrt(1 - z^2), weight; azimuth
+  __shared__ double nn[NK], nf[NK], nd[NK];                  // node, ln of the direction mean, its derivative
+  __shared__ double part[WARPS][2];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int64_t row = blockIdx.y, b = row / g.C;
+  const int c = (int)(row % g.C), t0 = blockIdx.x * TT, half = g.Tw / 2;
+  const double n_d = ceil(g.td[b] * g.fs), s_d = fmax(n_d - half, 0.0);  // the tail's first sample
+  const int end = min(t0 + TT, g.L);
+  if ((double)end <= s_d) return;
+  const int start = (int)s_d;
+  const double* be = g.beta + 6 * b;
+  for (int a = 0; a < 6; ++a)
+    if (be[a] == 0.0) return;  // E = 0
+  const double ks = g.fs / g.c;
+  const double lx = -(log(be[0]) + log(be[1])) / (g.room[3 * b] * ks);
+  const double ly = -(log(be[2]) + log(be[3])) / (g.room[3 * b + 1] * ks);
+  const double lz = -(log(be[4]) + log(be[5])) / (g.room[3 * b + 2] * ks);
+  const double m = fmin(lx, fmin(ly, lz));  // sum lambda_a |u_a| >= m on the unit sphere
+  const double tau = fmax(1.0, fmin(1.0 / (lx + ly + lz), (double)g.L)), lr = log(GROW);
+  const double scale = g.c / (4.0 * M_PI * g.room[3 * b] * g.room[3 * b + 1] * g.room[3 * b + 2] * g.fs);
+  const int first = max(t0, start);
+  const int k_lo = node_of(first, tau, lr);
+  const int k_hi = max(k_lo + 1, min(node_of(end - 1, tau, lr) + 1, k_lo + NK - 1));
+
+  for (int i = tid; i < QM; i += NT) {
+    const double h = 3.0 / QK, t = (i - QK) * h, a = 0.5 * M_PI * sinh(t), ch = cosh(a);
+    const double x = 0.5 * (1.0 + tanh(a)), w = 0.25 * M_PI * h * cosh(t) / (ch * ch);
+    double s, co;
+    sincospi(0.5 * x, &s, &co);
+    qa[i] = lz * x, qr[i] = sqrt(fmax(0.0, 1.0 - x * x)), qw[i] = w * (2.0 / M_PI);
+    pb[i] = lx * co + ly * s, pw[i] = 0.5 * M_PI * w;
+  }
+  __syncthreads();
+  for (int k = k_lo; k <= k_hi; ++k) {
+    const double n = tau * expm1(k * lr);
+    double s0 = 0.0, s1 = 0.0;
+    for (int q = tid; q < QN; q += NT) {
+      const int i = q / QM, j = q - i * QM;
+      const double sg = qa[i] + qr[i] * pb[j] - m;
+      const double e = qw[i] * pw[j] * exp(-n * sg);
+      s0 += e, s1 += e * sg;
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+      s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+    }
+    if (lane == 0) part[warp][0] = s0, part[warp][1] = s1;
+    __syncthreads();
+    if (tid == 0) {
+      double S0 = 0.0, S1 = 0.0;
+      for (int w = 0; w < WARPS; ++w) S0 += part[w][0], S1 += part[w][1];
+      const bool ok = S0 > 0.0;  // else every term underflowed: E is 0 to double precision
+      nn[k - k_lo] = n, nf[k - k_lo] = ok ? log(S0) - n * m : -1e300, nd[k - k_lo] = ok ? -m - S1 / S0 : 0.0;
+    }
+    __syncthreads();
+  }
+
+  const uint64_t key = mix64(mix64(g.seed[b]) + (uint64_t)c);
+  float* o = g.out + row * (int64_t)g.L;
+  for (int i = first + tid; i < end; i += NT) {
+    const int k = min(max(node_of(i, tau, lr), k_lo), k_hi - 1) - k_lo;
+    const double h = nn[k + 1] - nn[k], t = (i - nn[k]) / h, t2 = t * t, t3 = t2 * t;
+    const double f = (2 * t3 - 3 * t2 + 1) * nf[k] + (t3 - 2 * t2 + t) * h * nd[k] + (3 * t2 - 2 * t3) * nf[k + 1] +
+                     (t3 - t2) * h * nd[k + 1];
+    double amp = sqrt(scale * exp(f));
+    const double x = (i - n_d + half + 0.5) / g.Tw;
+    if (x < 1.0) {
+      double s, co;
+      sincospi(x, &s, &co);
+      amp *= sqrt(0.5 * (1.0 - co));
+    }
+    const uint64_t z = mix64(key + (uint64_t)i * GAMMA);
+    const double u1 = ((double)(z >> 32) + 0.5) * 0x1p-32, u2 = (double)(z & 0xffffffffull) * 0x1p-32;
+    double s, co;
+    sincospi(2.0 * u2, &s, &co);
+    o[i] += (float)(amp * sqrt(-2.0 * log(u1)) * co);
+  }
+}
+
 }  // namespace rir
 }  // namespace b2a
 
 using namespace b2a::rir;
 
+static int check(const char* fn, const double* room, const double* src, const double* mics, const double* beta,
+                 int64_t B, int C, int64_t L, double fs, double c, float* out) {
+  B2A_REQUIRE(room && src && mics && beta && out, B2A_E_INVALID, "%s: null pointer", fn);
+  B2A_REQUIRE(B >= 1 && C >= 1 && L >= 1, B2A_E_INVALID, "%s: bad shape B=%lld C=%d L=%lld", fn, (long long)B, C,
+              (long long)L);
+  B2A_REQUIRE(B * C <= 65535, B2A_E_INVALID, "%s: %lld rows (items x microphones); at most 65535 per call", fn,
+              (long long)(B * C));
+  B2A_REQUIRE(L <= (1 << 30), B2A_E_INVALID, "%s: L=%lld; at most 2^30 samples", fn, (long long)L);
+  B2A_REQUIRE(fs >= 125.0 && fs <= 384000.0, B2A_E_INVALID, "%s: fs=%g; 125 .. 384000 Hz are supported", fn, fs);
+  B2A_REQUIRE(c > 0.0 && c < 1e30, B2A_E_INVALID, "%s: sound speed %g must be positive and finite", fn, c);
+  return B2A_OK;
+}
+
+static Geo geo(const double* room, const double* src, const double* mics, const double* beta, int C, int64_t L,
+               double fs, double c, int max_order, float* out) {
+  Geo g;
+  g.room = room, g.src = src, g.mics = mics, g.beta = beta, g.td = nullptr, g.seed = nullptr, g.C = C, g.L = (int)L;
+  g.max_order = max_order, g.Tw = 2 * (int)floor(0.004 * fs + 0.5), g.fs = fs, g.c = c, g.out = out;
+  return g;
+}
+
 extern "C" int b2a_rir_ism_f32(const double* room, const double* src, const double* mics, const double* beta, int64_t B,
                                int C, int64_t L, double fs, double c, int max_order, float* out, void* stream) {
-  B2A_REQUIRE(room && src && mics && beta && out, B2A_E_INVALID, "rir_ism: null pointer");
-  B2A_REQUIRE(B >= 1 && C >= 1 && L >= 1, B2A_E_INVALID, "rir_ism: bad shape B=%lld C=%d L=%lld", (long long)B, C,
-              (long long)L);
-  B2A_REQUIRE(B * C <= 65535, B2A_E_INVALID, "rir_ism: %lld rows (items x microphones); at most 65535 per call",
-              (long long)(B * C));
-  B2A_REQUIRE(L <= (1 << 30), B2A_E_INVALID, "rir_ism: L=%lld; at most 2^30 samples", (long long)L);
-  B2A_REQUIRE(fs >= 125.0 && fs <= 384000.0, B2A_E_INVALID, "rir_ism: fs=%g; 125 .. 384000 Hz are supported", fs);
-  B2A_REQUIRE(c > 0.0 && c < 1e30, B2A_E_INVALID, "rir_ism: sound speed %g must be positive and finite", c);
+  const int rc = check("rir_ism", room, src, mics, beta, B, C, L, fs, c, out);
+  if (rc != B2A_OK) return rc;
   B2A_REQUIRE(max_order >= -1, B2A_E_INVALID, "rir_ism: max_order=%d must be >= -1", max_order);
-  Geo g;
-  g.room = room, g.src = src, g.mics = mics, g.beta = beta, g.C = C, g.L = (int)L, g.max_order = max_order;
-  g.Tw = 2 * (int)floor(0.004 * fs + 0.5), g.fs = fs, g.c = c, g.out = out;
+  const Geo g = geo(room, src, mics, beta, C, L, fs, c, max_order, out);
   const dim3 grid((unsigned)((L + TT - 1) / TT), (unsigned)(B * C));
   B2A_LAUNCH(ism_kernel, grid, dim3(NT), 0, stream, g);
+  B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
+}
+
+extern "C" int b2a_rir_hybrid_f32(const double* room, const double* src, const double* mics, const double* beta,
+                                  const double* t_d, const uint64_t* seed, int64_t B, int C, int64_t L, double fs,
+                                  double c, float* out, void* stream) {
+  const int rc = check("rir_hybrid", room, src, mics, beta, B, C, L, fs, c, out);
+  if (rc != B2A_OK) return rc;
+  B2A_REQUIRE(t_d && seed, B2A_E_INVALID, "rir_hybrid: null pointer");
+  Geo g = geo(room, src, mics, beta, C, L, fs, c, -1, out);
+  g.td = t_d, g.seed = seed;
+  const dim3 grid((unsigned)((L + TT - 1) / TT), (unsigned)(B * C));
+  B2A_LAUNCH(ism_kernel, grid, dim3(NT), 0, stream, g);
+  B2A_CUDA_OK(cudaGetLastError());
+  B2A_LAUNCH(tail_kernel, grid, dim3(NT), 0, stream, g);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }

@@ -563,16 +563,25 @@ class SyntheticRoomImpulseResponse(BaseTransform):
     call inside the room shrunk by ``margin`` plus half the array's extent along x and y.  A room too small for the
     margin or the array raises ``ValueError``.  The IR is ``duration`` seconds long when given, else the batch's
     longest RT60, and never longer than the signal.  All walls absorb alike (Sabine); ``max_order`` and ``high_pass``
-    are passed to ``image_source_ir``."""
+    are passed to ``image_source_ir``.
+
+    ``diffuse_after`` (seconds: a float or a distribution tuple) makes hybrid responses, images before it and a diffuse
+    tail after it (``image_source_ir(..., diffuse_after=, seed=)``), much cheaper for long RT60s.  Only then two more
+    draws follow the ones above: the time (when it is a tuple), then the tail's seed, ``state.randint(0, 2**31 - 1)``.
+    It needs ``max_order = -1``."""
     _bypass_pays = False  # FFT convolution
 
     DEFAULT_ROOM = (("uniform", 3.0, 10.0), ("uniform", 3.0, 8.0), ("uniform", 2.4, 4.0))
 
     def __init__(self, room: tuple = DEFAULT_ROOM, rt60: tuple = ("uniform", 0.2, 0.8), margin: float = 0.5,
                  mic_spacing: tuple = ("uniform", 0.05, 0.2), max_order: int = -1, duration: float = None,
-                 high_pass: bool = True, name: str = None, prob: float = 1.0, use_original_phase: bool = False):
+                 high_pass: bool = True, name: str = None, prob: float = 1.0, use_original_phase: bool = False,
+                 diffuse_after=None):
         super().__init__(name=name, prob=prob)
+        if diffuse_after is None:  # no tail: neither draw is made, so neither key is expected
+            self.keys = [k for k in self.keys if k not in ("diffuse_after", "seed")]
         self.room = tuple(room)
+        self.diffuse_after = diffuse_after
         self.rt60 = rt60
         self.margin = float(margin)
         self.mic_spacing = mic_spacing
@@ -601,16 +610,21 @@ class SyntheticRoomImpulseResponse(BaseTransform):
         centre = state.uniform(lo + ext, hi - ext)
         mics = centre + (np.arange(C) - 0.5 * (C - 1))[:, None] * spacing * axis
         rt60 = max(rt60, 1.01 * float(_room.min_rt60(dims)))
-        return {"room": dims, "rt60": np.float64(rt60), "source": source, "mics": mics}
+        out = {"room": dims, "rt60": np.float64(rt60), "source": source, "mics": mics}
+        if self.diffuse_after is not None:
+            td = self.diffuse_after
+            out["diffuse_after"] = np.float64(util.sample_from_dist(td, state) if isinstance(td, tuple) else td)
+            out["seed"] = np.int64(state.randint(0, 2 ** 31 - 1))
+        return out
 
-    def _transform(self, signal, room, rt60, source, mics, _bypass=None):
+    def _transform(self, signal, room, rt60, source, mics, diffuse_after=None, seed=None, _bypass=None):
         from ..core.room import image_source_ir
 
         sr, T = signal.sample_rate, signal.signal_length
         seconds = self.duration if self.duration is not None else float(util.host_view(rt60).max())
         length = max(1, min(T, int(np.ceil(seconds * sr))))
         ir = image_source_ir(room, source, mics, sr, length, rt60=rt60, max_order=self.max_order,
-                             high_pass=self.high_pass, device=signal.device)
+                             high_pass=self.high_pass, diffuse_after=diffuse_after, seed=seed, device=signal.device)
         return signal.apply_ir(ir, use_original_phase=self.use_original_phase, _bypass=_bypass)
 
 

@@ -771,11 +771,16 @@ class Engine:
 
     def image_source_ir(self, room: torch.Tensor, src: torch.Tensor, mics: torch.Tensor, beta: torch.Tensor,
                         length: int, sample_rate: float, sound_speed: float = 343.0, max_order: int = -1,
-                        high_pass: bool = True) -> torch.Tensor:
+                        high_pass: bool = True, diffuse_after: Optional[torch.Tensor] = None,
+                        seed: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Shoebox-room impulse responses by the image-source method (``b2a_rir_ism_f32``, DESIGN.md K20) -> [B, C,
         length] float32.  room [B, 3], src [B, 3], mics [B, C, 3] (metres) and beta [B, 6] are float64 tensors on the
         device, already checked (``core.room.image_source_ir``).  ``high_pass`` applies Allen & Berkley's 100 Hz
-        high-pass as one second-order section through ``sos_filter``.  One launch, three more with the high-pass."""
+        high-pass as one second-order section through ``sos_filter``.  One launch, three more with the high-pass.
+
+        ``diffuse_after`` (float64 [B], seconds > 0) with ``seed`` (int64 [B], >= 0) keeps the images arriving before
+        ceil(diffuse_after sample_rate) only and adds a diffuse tail after them (``b2a_rir_hybrid_f32``): two launches,
+        then the high-pass.  ``max_order`` must be -1 then."""
         if mics.ndim != 3 or mics.shape[-1] != 3:
             raise ValueError(f"image_source_ir: mics must be [B, C, 3], got {tuple(mics.shape)}")
         B, C = mics.shape[:2]
@@ -787,8 +792,20 @@ class Engine:
         room, src, mics, beta = (self._prep(t, n, torch.float64) for t, n in
                                  ((room, "room"), (src, "source"), (mics, "mics"), (beta, "beta")))
         out = torch.empty(B, C, int(length), dtype=torch.float32, device=room.device)
-        self._call(self.lib.b2a_rir_ism_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), B, C, int(length),
-                   float(sample_rate), float(sound_speed), int(max_order), _dptr(out), self._stream(room))
+        if diffuse_after is None:
+            self._call(self.lib.b2a_rir_ism_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), B, C, int(length),
+                       float(sample_rate), float(sound_speed), int(max_order), _dptr(out), self._stream(room))
+        else:
+            if max_order != -1:
+                raise ValueError(f"image_source_ir: max_order = {max_order} with a diffuse tail; the tail has every "
+                                 "order")
+            if seed is None or tuple(diffuse_after.shape) != (B,) or tuple(seed.shape) != (B,):
+                raise ValueError(f"image_source_ir: diffuse_after and seed must be [{B}]")
+            td = self._prep(diffuse_after, "diffuse_after", torch.float64)
+            sd = self._prep(seed, "seed", torch.int64)
+            self._call(self.lib.b2a_rir_hybrid_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), _dptr(td),
+                       _dptr(sd), B, C, int(length), float(sample_rate), float(sound_speed), _dptr(out),
+                       self._stream(room))
         if high_pass:
             w = 2 * math.pi * 100.0 / sample_rate
             r = math.exp(-w)

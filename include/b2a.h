@@ -398,6 +398,16 @@ int b2a_sos_filtfilt_backward_f32(const float* grad_y, const float* gain, int64_
 int b2a_rir_ism_f32(const double* room, const double* src, const double* mics, const double* beta, int64_t B, int C,
                     int64_t L, double fs, double c, int max_order, float* out, void* stream);
 
+/* The same impulse responses with a diffuse late tail (DESIGN.md K20, "Hybrid"): the images with floor(d) <
+ * min(L, n_d), n_d = ceil(t_d[b] fs), t_d [B] float64 seconds > 0 on the device; then, at every sample n >= n_d - Tw/2,
+ * w(n) sqrt(E_b(n)) xi(seed[b], c, n) is added: E_b the expected energy per sample of the image arrivals of item b's
+ * room, w a raised-cosine ramp over the Tw samples centred on n_d, xi a standard normal from a stateless counter-based
+ * generator (SplitMix64, Box-Muller).  seed [B] uint64 on the device.  Every image order is kept.  Two launches, no
+ * host sync, no atomics; a batch equals its items one at a time, bit for bit. */
+int b2a_rir_hybrid_f32(const double* room, const double* src, const double* mics, const double* beta,
+                       const double* t_d, const uint64_t* seed, int64_t B, int C, int64_t L, double fs, double c,
+                       float* out, void* stream);
+
 /* ---- per-item gain ---------------------------------------------------------------------
  * x[b, :, :] * gain[b]  (EffectMixin.normalize / volume_change, effects.py:219,237).
  * out may alias x.  per_item = C*T. */
