@@ -59,6 +59,11 @@ SIGNATURES = {
                                 c_int, c_void_p, c_void_p]),
     "b2a_rir_hybrid_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64,
                                    c_double, c_double, c_void_p, c_void_p]),
+    "b2a_rir_bands_kept": (c_int, [c_int, c_double]),
+    "b2a_rir_bands_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
+                                  c_int, c_int64, c_double, c_double, c_int, c_void_p, c_void_p]),
+    "b2a_rir_band_sum_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_double, c_double, c_int,
+                                     c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "b2a_gain_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
     "b2a_fftconv_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64, c_int64]),
     "b2a_fftconv_f32": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int,

@@ -16,6 +16,15 @@ centred on n_d).  The image count up to a time t grows with t^3, so a short ``di
 cheap.  The tail is frequency-flat like the walls, and the tails of different microphones are independent; it depends
 only on the item's geometry, its seed and the microphone, so a batch equals its items one at a time.
 
+``bands=K`` gives every wall, and with ``air_absorption`` the air, its own value in each of K octave bands centred on
+f_k = 125 2^k Hz: r_k is the response (images, and the tail with ``diffuse_after``) with band k's reflection
+coefficients, every image also scaled by 10^(-a_k d / 20) (d in metres, a_k in dB/m) and the tail's envelope by
+10^(-a_k (c n / fs) / 10); the tails of all bands share one noise.  The bands are joined by zero-phase windowed-sinc
+low-passes LP_k at the crossovers e_k = 125 2^(k + 1/2) Hz, y = r_{K'-1} + sum_{k < K'-1} LP_k * (r_k - r_{k+1}),
+where K' counts the bands whose lower crossover is below sample_rate / 2.  The crossovers are 2 half_0 + 1 taps long,
+half_0 = int(8 fs / e_0 / 2), and zero-phase, so a response can start up to half_0 samples before its first arrival
+(the window's Tw / 2 comes on top).  Equal bands without air give the ``bands=None`` response bit for bit.
+
 The geometry is checked on host values (``util.host_view`` reads a table's host mirror, so no device sync is needed)
 and is a constant: a geometry tensor that requires a gradient raises ``NotImplementedError``.
 """
@@ -30,6 +39,8 @@ from . import util
 MIN_SAMPLE_RATE = 125.0     # below it the window 2 floor(0.004 fs + 1/2) is empty
 MAX_SAMPLE_RATE = 384000.0  # csrc/rir.cu's largest window table
 MIN_DISTANCE = 1e-3         # metres between the source and a microphone
+MAX_BANDS = 8               # octave bands centred on 125 2^k Hz, k < 8 (up to 16 kHz)
+MAX_ROWS = 65535            # items x microphones x bands of one call (csrc/rir.cu's grid)
 
 
 def _host(name: str, v) -> np.ndarray:
@@ -81,7 +92,7 @@ def _batch(name: str, v: np.ndarray, item_ndim: int, B: int) -> np.ndarray:
 
 def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta=None, rt60=None,
                     max_order: int = -1, sound_speed: float = 343.0, high_pass: bool = True, diffuse_after=None,
-                    seed=None, device="cuda"):
+                    seed=None, bands=None, air_absorption=None, device="cuda"):
     """Impulse responses [B, C, length] of shoebox rooms by the image-source method, as an ``AudioSignal`` at
     ``sample_rate``.
 
@@ -93,7 +104,14 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
 
     ``diffuse_after`` (seconds > 0, scalar or [B]) and ``seed`` (an int or [B] ints in [0, 2^63)) add the diffuse tail
     (module docstring; DESIGN.md K20 "Hybrid"): two kernel launches before the high-pass.  It needs ``max_order =
-    -1`` (the tail stands for images of every order); ``None`` leaves the images-only path untouched."""
+    -1`` (the tail stands for images of every order); ``None`` leaves the images-only path untouched.
+
+    ``bands=K`` (1 .. 8) makes the walls, and with ``air_absorption`` the air, frequency-dependent over K octave bands
+    centred on 125 2^k Hz (module docstring; DESIGN.md K20 "Bands"): ``beta`` is then [6, K] or [B, 6, K], ``rt60``
+    [K] or [B, K] (``sabine_beta`` per band) and ``air_absorption`` (dB/m, finite, >= 0) [K] or [B, K].  Bands whose
+    lower crossover is at or above sample_rate / 2 are checked but not computed.  One launch (two with the tail), the
+    crossovers' ``fftconv`` and one launch for their sum when more than one band is computed, then the high-pass.
+    ``bands=None`` leaves the frequency-flat paths untouched."""
     from ..engine import get_engine
     from .audio_signal import AudioSignal
 
@@ -112,6 +130,13 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
     if not (math.isfinite(sound_speed) and sound_speed > 0):
         raise ValueError(f"image_source_ir: sound_speed = {sound_speed} must be positive")
     n_tail = 1
+    if bands is None and air_absorption is not None:
+        raise ValueError("image_source_ir: air_absorption is per octave band; give bands too")
+    if bands is not None:
+        if isinstance(bands, bool) or not isinstance(bands, (int, np.integer)) or not 1 <= bands <= MAX_BANDS:
+            raise ValueError(f"image_source_ir: bands = {bands!r}; an int in 1 .. {MAX_BANDS} (octaves from 125 Hz)")
+        bands = int(bands)
+        air_h = None if air_absorption is None else _host("air_absorption", air_absorption)
     if diffuse_after is None and seed is not None:
         raise ValueError("image_source_ir: seed is for the diffuse tail; give diffuse_after too")
     if diffuse_after is not None:
@@ -128,10 +153,13 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
             raise ValueError(f"image_source_ir: seed = {sd} must be integers in [0, 2^63)")
         sd = sd.astype(np.int64)
         n_tail = max(td_h.size, sd.size)
+    if bands is None:
+        n_wall = (wall_h.shape[0] if wall_h.ndim == 2 else 1) if rt60 is None else (wall_h.size if wall_h.ndim else 1)
+    else:  # the item axis leads a [B, 6, K] beta, a [B, K] rt60 and a [B, K] air absorption
+        n_wall = max(wall_h.shape[0] if wall_h.ndim == (3 if rt60 is None else 2) else 1,
+                     air_h.shape[0] if air_h is not None and air_h.ndim == 2 else 1)
     B = max(room_h.shape[0] if room_h.ndim == 2 else 1, src_h.shape[0] if src_h.ndim == 2 else 1,
-            mics_h.shape[0] if mics_h.ndim == 3 else 1,
-            (wall_h.shape[0] if wall_h.ndim == 2 else 1) if rt60 is None else (wall_h.size if wall_h.ndim else 1),
-            n_tail)
+            mics_h.shape[0] if mics_h.ndim == 3 else 1, n_wall, n_tail)
     room_h = _batch("room", room_h, 1, B)
     src_h = _batch("source", src_h, 1, B)
     mics_h = _batch("mics", mics_h, 2, B)
@@ -146,7 +174,29 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
     if np.any(gap < MIN_DISTANCE):
         raise ValueError(f"image_source_ir: a microphone is {gap.min():.3g} m from the source; at least "
                          f"{MIN_DISTANCE:g} m is needed")
-    if rt60 is None:
+    if bands is not None:
+        if rt60 is None:
+            beta_h = _batch("beta", wall_h, 2, B)
+            if beta_h.shape[1:] != (6, bands):
+                raise ValueError(f"image_source_ir: beta must be [6, {bands}] or [B, 6, {bands}] with bands = "
+                                 f"{bands}, got {wall_h.shape}")
+        else:
+            rt_h = _batch("rt60", wall_h, 1, B)
+            if rt_h.shape[1:] != (bands,):
+                raise ValueError(f"image_source_ir: rt60 must be [{bands}] or [B, {bands}] with bands = {bands}, "
+                                 f"got {wall_h.shape}")
+            beta_h = np.swapaxes(sabine_beta(room_h[:, None], rt_h, sound_speed), 1, 2)  # [B, 6, K]
+        if air_h is not None:
+            air_h = _batch("air_absorption", air_h, 1, B)
+            if air_h.shape[1:] != (bands,):
+                raise ValueError(f"image_source_ir: air_absorption must be [{bands}] or [B, {bands}] dB/m with bands "
+                                 f"= {bands}, got {air_h.shape}")
+            if not (np.all(np.isfinite(air_h)) and np.all(air_h >= 0)):
+                raise ValueError("image_source_ir: air_absorption must be finite and >= 0 dB/m")
+        if B * mics_h.shape[1] * bands > MAX_ROWS:
+            raise ValueError(f"image_source_ir: {B * mics_h.shape[1] * bands} rows (items x microphones x bands); "
+                             f"at most {MAX_ROWS}")
+    elif rt60 is None:
         beta_h = _batch("beta", wall_h, 1, B)
         if beta_h.shape[-1] != 6:
             raise ValueError(f"image_source_ir: beta must have 6 walls, got {beta_h.shape}")
@@ -164,5 +214,10 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
         sd = _batch("seed", sd, 0, B)
         tail = dict(diffuse_after=torch.from_numpy(np.array(td_h, dtype=np.float64)).to(dev, non_blocking=True),
                     seed=torch.from_numpy(np.array(sd, dtype=np.int64)).to(dev, non_blocking=True))
-    ir = get_engine().image_source_ir(*tab, length, sample_rate, sound_speed, max_order, high_pass, **tail)
+    if bands is None:
+        ir = get_engine().image_source_ir(*tab, length, sample_rate, sound_speed, max_order, high_pass, **tail)
+    else:
+        air = None if air_h is None else torch.from_numpy(np.array(air_h, dtype=np.float64)).to(dev, non_blocking=True)
+        ir = get_engine().image_source_ir_bands(*tab, length, sample_rate, sound_speed, max_order, high_pass, air=air,
+                                                **tail)
     return AudioSignal(ir, sample_rate)

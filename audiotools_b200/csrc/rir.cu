@@ -36,6 +36,12 @@
 // rule (65 x 65 points) in u_z (uniform on [0, 1]) and the azimuth over one octant, with its derivative, and
 // interpolated between nodes by a cubic Hermite (relative error below 1e-5: (ln E)'''' falls off like 12 / n^4).  Each
 // CTA evaluates the nodes its tile spans, so the tail too depends only on its row's geometry, seed and microphone.
+//
+// Bands (b2a_rir_bands_f32): K octave bands with their own beta [B, 6, K] and air absorption [B, K] (dB/m).  The
+// first K' bands (lower crossover below fs / 2) are computed in one pass: ism_tile<K'> enumerates each tile's images
+// once and keeps K' compensated sums per sample, and the rows it writes are r_k - r_{k+1} (k < K' - 1) and r_{K'-1};
+// tail_kernel adds each band's tail the same way.  The crossovers (Engine.fftconv) and band_sum_kernel then form
+// y = r_{K'-1} + sum_k LP_k * (r_k - r_{k+1}) (DESIGN.md K20 "Bands").
 #include "b2a_common.h"
 
 namespace b2a {
@@ -49,14 +55,17 @@ constexpr int TT = NT * PER;     // samples per CTA (tile)
 constexpr int CAP = 256;         // images staged in shared memory at a time
 constexpr int TW_MAX = 3072;     // largest window: fs up to 384 kHz
 constexpr int FAR = -(1 << 30);  // floor(d) of a staged slot that holds no image
+constexpr int MAX_BANDS = 8;     // octave bands, 125 Hz .. 16 kHz
 
 struct Geo {
-  const double *room, *src, *mics, *beta;
+  const double *room, *src, *mics, *beta;  // beta [B, 6, K]
   const double* td;        // per item: the diffuse tail starts at ceil(td fs); null: images only
   const uint64_t* seed;    // per item: the tail's noise
+  const double* air;       // [B, K] air absorption in dB/m; null: none
   int C, L, Tw, max_order;
+  int K, KB;               // bands per item in beta / air (1: frequency-flat); bands computed (the first KB)
   double fs, c;
-  float* out;
+  float* out;              // [KB, B C, L]: rows k < KB - 1 hold r_k - r_{k+1}, row KB - 1 holds r_{KB-1}
 };
 
 struct __align__(16) Img {
@@ -76,21 +85,29 @@ __device__ __forceinline__ double ipow(double b, int64_t n) {
 
 __device__ __forceinline__ int64_t floor_div2(int64_t a) { return a >= 0 ? a / 2 : -((-a + 1) / 2); }
 
-__global__ void __launch_bounds__(NT) ism_kernel(const Geo g) {
+// The image sum of one tile for the first NB bands of a row.  The images are enumerated once; each staged image carries
+// the last band's gains in its Img record and the other bands' in bgs, and every band keeps its own compensated sums.
+// A band skips an image whose gain rounds to 0 in float, so band NB - 1 adds exactly the images ism_kernel adds for its
+// beta, in the same order and with the same arithmetic: with one band this is ism_kernel.
+template <int NB>
+__device__ __forceinline__ void ism_tile(const Geo& g) {
   __shared__ float2 tab[TW_MAX + 1];
   __shared__ Img img[CAP];
+  __shared__ float2 bgs[NB > 1 ? NB - 1 : 1][CAP];  // bands 0 .. NB - 2: (gs, g0) of the staged images
+  __shared__ double wall[6][NB], att[NB];             // beta per wall and band; air absorption per sample of distance
   __shared__ int64_t wtot[WARPS];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int64_t row = blockIdx.y, b = row / g.C;
+  const int64_t row = blockIdx.y, b = row / g.C, rows = gridDim.y;
   const int t0 = blockIdx.x * TT, Tw = g.Tw, half = Tw / 2;
   const double ks = g.fs / g.c;  // samples per metre
   const double Lx = g.room[3 * b] * ks, Ly = g.room[3 * b + 1] * ks, Lz = g.room[3 * b + 2] * ks;
   const double sx = g.src[3 * b] * ks, sy = g.src[3 * b + 1] * ks, sz = g.src[3 * b + 2] * ks;
   const double rx = g.mics[3 * row] * ks, ry = g.mics[3 * row + 1] * ks, rz = g.mics[3 * row + 2] * ks;
-  const double* be = g.beta + 6 * b;
-  const double bx0 = be[0], bx1 = be[1], by0 = be[2], by1 = be[3], bz0 = be[4], bz1 = be[5];
   const double gscale = ks / (4.0 * M_PI);  // g = product of the betas * gscale / d
 
+  for (int i = tid; i < 6 * NB; i += NT) wall[i / NB][i % NB] = g.beta[(6 * b + i / NB) * g.K + i % NB];
+  // 10^(-a d_m / 20) = exp(-att d), d in samples
+  for (int i = tid; i < NB; i += NT) att[i] = g.air ? g.air[b * g.K + i] * (M_LN10 / 20.0) / ks : 0.0;
   for (int i = tid; i <= Tw; i += NT) {
     double s, c;
     sincospi((double)(i - half) / Tw, &s, &c);
@@ -101,7 +118,8 @@ __global__ void __launch_bounds__(NT) ism_kernel(const Geo g) {
   const double lim = g.td ? fmin((double)g.L, ceil(g.td[b] * g.fs)) : (double)g.L;  // images with floor(d) < lim
   const double dhi = fmin((double)t0 + TT + half - 1, lim);
   if (dhi <= dlo) {  // a tile past the images (only with a diffuse tail)
-    for (int i = t0 + tid; i < min(t0 + TT, g.L); i += NT) g.out[row * (int64_t)g.L + i] = 0.f;
+    for (int bd = 0; bd < NB; ++bd)
+      for (int i = t0 + tid; i < min(t0 + TT, g.L); i += NT) g.out[(bd * rows + row) * g.L + i] = 0.f;
     return;
   }
   const double reach = dhi * (1.0 + 1e-12) + 1e-6;  // lines with rho >= reach have no image in the shell
@@ -113,9 +131,11 @@ __global__ void __launch_bounds__(NT) ism_kernel(const Geo g) {
   const int64_t ny = 2 * (2 * My + 1), n_lines = 2 * (2 * Mx + 1) * ny * 2;
   const int wb = t0 + warp * WS;  // the warp's first sample
 
-  float acc[PER], cmp[PER];
+  float acc[NB][PER], cmp[NB][PER];
 #pragma unroll
-  for (int s = 0; s < PER; ++s) acc[s] = 0.f, cmp[s] = 0.f;
+  for (int bd = 0; bd < NB; ++bd)
+#pragma unroll
+    for (int s = 0; s < PER; ++s) acc[bd][s] = 0.f, cmp[bd][s] = 0.f;
   __syncthreads();
 
   for (int64_t l0 = 0; l0 < n_lines; l0 += NT) {
@@ -123,7 +143,9 @@ __global__ void __launch_bounds__(NT) ism_kernel(const Geo g) {
     const int64_t line = l0 + tid;
     int64_t za = 0, zb = -1, zc = 0, zd = -1, mx = 0, my = 0;
     int q = 0, j = 0, k = 0;
-    double X = 0, Y = 0, Zc = 0, pxy = 0;
+    double X = 0, Y = 0, Zc = 0, pxy[NB];
+#pragma unroll
+    for (int bd = 0; bd < NB; ++bd) pxy[bd] = 0;
     if (line < n_lines) {
       k = (int)(line & 1);
       const int64_t r2 = line >> 1, ix = r2 / ny, iy = r2 % ny;
@@ -148,7 +170,10 @@ __global__ void __launch_bounds__(NT) ism_kernel(const Geo g) {
         zc = (int64_t)floor((zmin - Zc) * inv) - 1, zd = (int64_t)ceil((zmax - Zc) * inv) + 1;
         if (zb >= zc - 1) zb = zd, zc = 0, zd = -1;  // one run
         za = max(za, olo), zb = min(zb, ohi), zc = max(zc, olo), zd = min(zd, ohi);
-        pxy = ipow(bx0, mx - q) * ipow(bx1, mx) * ipow(by0, my - j) * ipow(by1, my) * gscale;
+#pragma unroll
+        for (int bd = 0; bd < NB; ++bd)
+          pxy[bd] = ipow(wall[0][bd], mx - q) * ipow(wall[1][bd], mx) * ipow(wall[2][bd], my - j) *
+                    ipow(wall[3][bd], my) * gscale;
       }
     }
     const int64_t n1 = zb >= za ? zb - za + 1 : 0, cnt = n1 + (zd >= zc ? zd - zc + 1 : 0);
@@ -174,15 +199,28 @@ __global__ void __launch_bounds__(NT) ism_kernel(const Geo g) {
         const double Z = Zc + 2.0 * mz * Lz;
         const double d = sqrt(X * X + Y * Y + Z * Z);
         const double fl = floor(d);
-        const double gd = pxy * ipow(bz0, mz - k) * ipow(bz1, mz) / d;
+        double gd[NB];
+        bool live = false;
+#pragma unroll
+        for (int bd = 0; bd < NB; ++bd) {
+          gd[bd] = pxy[bd] * ipow(wall[4][bd], mz - k) * ipow(wall[5][bd], mz) / d;
+          if (g.air) gd[bd] *= exp(-att[bd] * d);
+          live = live || (float)gd[bd] != 0.f;
+        }
         Img im;
         im.fl = FAR;
-        if (fl >= dlo && fl < dhi && (float)gd != 0.f) {
+        if (fl >= dlo && fl < dhi && live) {
           const double D = d - fl > 0.5 ? fl + 1 : fl, e = d - D;
-          const double sg = fmod(D, 2.0) != 0.0 ? -gd : gd;  // (-1)^D g
+          const bool odd = fmod(D, 2.0) != 0.0;
           double se, ce, sw, cw;
           sincospi(e, &se, &ce);
           sincospi(e / Tw, &sw, &cw);
+#pragma unroll
+          for (int bd = 0; bd < NB - 1; ++bd) {
+            const double sg = odd ? -gd[bd] : gd[bd];  // (-1)^D g
+            bgs[bd][sl - c0] = make_float2((float)(-sg * se / M_PI), (float)sg);
+          }
+          const double sg = odd ? -gd[NB - 1] : gd[NB - 1];
           im.fl = (int)fl, im.D = (int)D, im.e = (float)e, im.gs = (float)(-sg * se / M_PI), im.g0 = (float)sg;
           im.ce = (float)cw, im.se = (float)sw, im.pad = 0.f;
         }
@@ -193,6 +231,10 @@ __global__ void __launch_bounds__(NT) ism_kernel(const Geo g) {
       for (int m = 0; m < n_img; ++m) {
         const Img im = img[m];
         if (im.fl + half < wb || im.fl - half + 1 >= wb + WS) continue;  // warp-uniform
+        float2 gb[NB];
+#pragma unroll
+        for (int bd = 0; bd < NB - 1; ++bd) gb[bd] = bgs[bd][m];
+        gb[NB - 1] = make_float2(im.gs, im.g0);
         const int i0 = wb + lane, u0 = i0 - im.fl + half - 1, k0 = i0 - im.D;
         const float kf0 = (float)k0;
 #pragma unroll
@@ -201,11 +243,16 @@ __global__ void __launch_bounds__(NT) ism_kernel(const Geo g) {
             const float2 cs = tab[k0 + 32 * s + half];
             const float t = (kf0 + (float)(32 * s)) - im.e;
             const float w = cs.x * im.ce + cs.y * im.se;
-            const float x = t == 0.f ? im.g0 : im.gs * __fdividef(w * w, t);
-            // Kahan: cmp carries the low part the running sum lost
-            const float y = x - cmp[s], tsum = acc[s] + y;
-            cmp[s] = (tsum - acc[s]) - y;
-            acc[s] = tsum;
+            const float r = __fdividef(w * w, t);
+#pragma unroll
+            for (int bd = 0; bd < NB; ++bd) {
+              if (NB > 1 && gb[bd].y == 0.f) continue;  // this band's gain is 0 in float: not added
+              const float x = t == 0.f ? gb[bd].y : gb[bd].x * r;
+              // Kahan: cmp carries the low part the running sum lost
+              const float y = x - cmp[bd][s], tsum = acc[bd][s] + y;
+              cmp[bd][s] = (tsum - acc[bd][s]) - y;
+              acc[bd][s] = tsum;
+            }
           }
         }
       }
@@ -213,13 +260,25 @@ __global__ void __launch_bounds__(NT) ism_kernel(const Geo g) {
     }
     __syncthreads();  // wtot is rewritten by the next round
   }
-  float* o = g.out + row * (int64_t)g.L;
 #pragma unroll
   for (int s = 0; s < PER; ++s) {
     const int i = wb + lane + 32 * s;
-    if (i < g.L) o[i] = (i & 1) ? 0.f - acc[s] : acc[s];
+    if (i < g.L) {
+      float v[NB];
+#pragma unroll
+      for (int bd = 0; bd < NB; ++bd) v[bd] = (i & 1) ? 0.f - acc[bd][s] : acc[bd][s];
+      g.out[((NB - 1) * rows + row) * g.L + i] = v[NB - 1];
+#pragma unroll
+      for (int bd = 0; bd < NB - 1; ++bd) g.out[(bd * rows + row) * g.L + i] = v[bd] - v[bd + 1];
+    }
   }
 }
+
+__global__ void __launch_bounds__(NT) ism_kernel(const Geo g) { ism_tile<1>(g); }
+
+// one CTA per SM is enough to let ptxas keep every band's sums in registers (no spills up to NB = 8)
+template <int NB>
+__global__ void __launch_bounds__(NT, 1) ism_bands_kernel(const Geo g) { ism_tile<NB>(g); }
 
 
 constexpr int QK = 32;                // tanh-sinh: 2 QK + 1 points per dimension, steps of 3 / QK
@@ -237,84 +296,147 @@ __device__ __forceinline__ uint64_t mix64(uint64_t z) {  // the SplitMix64 final
 
 __device__ __forceinline__ int node_of(double n, double tau, double lr) { return (int)floor(log1p(n / tau) / lr); }
 
+// Adds the tail of every computed band to the rows ism_tile wrote: band k's envelope is E(n; beta_k) exp(-2 att_k n)
+// (the air's 10^(-a_k (c n / fs) / 10), added to ln E at the sample, exactly), its noise xi(seed, c, n) is shared by the
+// bands, so row KB - 1 gets v_{KB-1} and row k < KB - 1 gets v_k - v_{k+1}.  The bands are walked from the last one
+// down, each with the node evaluation of the flat tail; with one band this is the flat tail.
 __global__ void __launch_bounds__(NT) tail_kernel(const Geo g) {
   __shared__ double qa[QM], qr[QM], qw[QM], pb[QM], pw[QM];  // z: lambda_z z, sqrt(1 - z^2), weight; azimuth
   __shared__ double nn[NK], nf[NK], nd[NK];                  // node, ln of the direction mean, its derivative
   __shared__ double part[WARPS][2];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int64_t row = blockIdx.y, b = row / g.C;
+  const int64_t row = blockIdx.y, b = row / g.C, rows = gridDim.y;
   const int c = (int)(row % g.C), t0 = blockIdx.x * TT, half = g.Tw / 2;
   const double n_d = ceil(g.td[b] * g.fs), s_d = fmax(n_d - half, 0.0);  // the tail's first sample
   const int end = min(t0 + TT, g.L);
   if ((double)end <= s_d) return;
   const int start = (int)s_d;
-  const double* be = g.beta + 6 * b;
-  for (int a = 0; a < 6; ++a)
-    if (be[a] == 0.0) return;  // E = 0
   const double ks = g.fs / g.c;
-  const double lx = -(log(be[0]) + log(be[1])) / (g.room[3 * b] * ks);
-  const double ly = -(log(be[2]) + log(be[3])) / (g.room[3 * b + 1] * ks);
-  const double lz = -(log(be[4]) + log(be[5])) / (g.room[3 * b + 2] * ks);
-  const double m = fmin(lx, fmin(ly, lz));  // sum lambda_a |u_a| >= m on the unit sphere
-  const double tau = fmax(1.0, fmin(1.0 / (lx + ly + lz), (double)g.L)), lr = log(GROW);
   const double scale = g.c / (4.0 * M_PI * g.room[3 * b] * g.room[3 * b + 1] * g.room[3 * b + 2] * g.fs);
   const int first = max(t0, start);
-  const int k_lo = node_of(first, tau, lr);
-  const int k_hi = max(k_lo + 1, min(node_of(end - 1, tau, lr) + 1, k_lo + NK - 1));
+  const double lr = log(GROW);
 
-  for (int i = tid; i < QM; i += NT) {
-    const double h = 3.0 / QK, t = (i - QK) * h, a = 0.5 * M_PI * sinh(t), ch = cosh(a);
-    const double x = 0.5 * (1.0 + tanh(a)), w = 0.25 * M_PI * h * cosh(t) / (ch * ch);
-    double s, co;
-    sincospi(0.5 * x, &s, &co);
-    qa[i] = lz * x, qr[i] = sqrt(fmax(0.0, 1.0 - x * x)), qw[i] = w * (2.0 / M_PI);
-    pb[i] = lx * co + ly * s, pw[i] = 0.5 * M_PI * w;
-  }
-  __syncthreads();
-  for (int k = k_lo; k <= k_hi; ++k) {
-    const double n = tau * expm1(k * lr);
-    double s0 = 0.0, s1 = 0.0;
-    for (int q = tid; q < QN; q += NT) {
-      const int i = q / QM, j = q - i * QM;
-      const double sg = qa[i] + qr[i] * pb[j] - m;
-      const double e = qw[i] * pw[j] * exp(-n * sg);
-      s0 += e, s1 += e * sg;
-    }
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-      s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-    }
-    if (lane == 0) part[warp][0] = s0, part[warp][1] = s1;
-    __syncthreads();
-    if (tid == 0) {
-      double S0 = 0.0, S1 = 0.0;
-      for (int w = 0; w < WARPS; ++w) S0 += part[w][0], S1 += part[w][1];
-      const bool ok = S0 > 0.0;  // else every term underflowed: E is 0 to double precision
-      nn[k - k_lo] = n, nf[k - k_lo] = ok ? log(S0) - n * m : -1e300, nd[k - k_lo] = ok ? -m - S1 / S0 : 0.0;
-    }
-    __syncthreads();
-  }
-
+  // this thread's samples first + tid + NT s: the Box-Muller radius and cosine of each
   const uint64_t key = mix64(mix64(g.seed[b]) + (uint64_t)c);
-  float* o = g.out + row * (int64_t)g.L;
-  for (int i = first + tid; i < end; i += NT) {
-    const int k = min(max(node_of(i, tau, lr), k_lo), k_hi - 1) - k_lo;
-    const double h = nn[k + 1] - nn[k], t = (i - nn[k]) / h, t2 = t * t, t3 = t2 * t;
-    const double f = (2 * t3 - 3 * t2 + 1) * nf[k] + (t3 - 2 * t2 + t) * h * nd[k] + (3 * t2 - 2 * t3) * nf[k + 1] +
-                     (t3 - t2) * h * nd[k + 1];
-    double amp = sqrt(scale * exp(f));
-    const double x = (i - n_d + half + 0.5) / g.Tw;
-    if (x < 1.0) {
-      double s, co;
-      sincospi(x, &s, &co);
-      amp *= sqrt(0.5 * (1.0 - co));
-    }
+  double rad[PER], cosv[PER];
+  float prev[PER];
+#pragma unroll
+  for (int s = 0; s < PER; ++s) {
+    const int i = first + tid + NT * s;
     const uint64_t z = mix64(key + (uint64_t)i * GAMMA);
     const double u1 = ((double)(z >> 32) + 0.5) * 0x1p-32, u2 = (double)(z & 0xffffffffull) * 0x1p-32;
-    double s, co;
-    sincospi(2.0 * u2, &s, &co);
-    o[i] += (float)(amp * sqrt(-2.0 * log(u1)) * co);
+    double sn, co;
+    sincospi(2.0 * u2, &sn, &co);
+    rad[s] = sqrt(-2.0 * log(u1)), cosv[s] = co, prev[s] = 0.f;
+  }
+
+  for (int bd = g.KB - 1; bd >= 0; --bd) {
+    double be[6];
+    bool zero = false;
+    for (int a = 0; a < 6; ++a) {
+      be[a] = g.beta[(6 * b + a) * g.K + bd];
+      zero = zero || be[a] == 0.0;  // E = 0
+    }
+    const double ea = g.air ? 2.0 * g.air[b * g.K + bd] * (M_LN10 / 20.0) / ks : 0.0;  // energy, per sample
+    int k_lo = 0, k_hi = 1;
+    double tau = 1.0;
+    if (!zero) {
+      const double lx = -(log(be[0]) + log(be[1])) / (g.room[3 * b] * ks);
+      const double ly = -(log(be[2]) + log(be[3])) / (g.room[3 * b + 1] * ks);
+      const double lz = -(log(be[4]) + log(be[5])) / (g.room[3 * b + 2] * ks);
+      const double m = fmin(lx, fmin(ly, lz));  // sum lambda_a |u_a| >= m on the unit sphere
+      tau = fmax(1.0, fmin(1.0 / (lx + ly + lz), (double)g.L));
+      k_lo = node_of(first, tau, lr);
+      k_hi = max(k_lo + 1, min(node_of(end - 1, tau, lr) + 1, k_lo + NK - 1));
+
+      for (int i = tid; i < QM; i += NT) {
+        const double h = 3.0 / QK, t = (i - QK) * h, a = 0.5 * M_PI * sinh(t), ch = cosh(a);
+        const double x = 0.5 * (1.0 + tanh(a)), w = 0.25 * M_PI * h * cosh(t) / (ch * ch);
+        double s, co;
+        sincospi(0.5 * x, &s, &co);
+        qa[i] = lz * x, qr[i] = sqrt(fmax(0.0, 1.0 - x * x)), qw[i] = w * (2.0 / M_PI);
+        pb[i] = lx * co + ly * s, pw[i] = 0.5 * M_PI * w;
+      }
+      __syncthreads();
+      for (int k = k_lo; k <= k_hi; ++k) {
+        const double n = tau * expm1(k * lr);
+        double s0 = 0.0, s1 = 0.0;
+        for (int q = tid; q < QN; q += NT) {
+          const int i = q / QM, j = q - i * QM;
+          const double sg = qa[i] + qr[i] * pb[j] - m;
+          const double e = qw[i] * pw[j] * exp(-n * sg);
+          s0 += e, s1 += e * sg;
+        }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+          s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+          s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+        }
+        if (lane == 0) part[warp][0] = s0, part[warp][1] = s1;
+        __syncthreads();
+        if (tid == 0) {
+          double S0 = 0.0, S1 = 0.0;
+          for (int w = 0; w < WARPS; ++w) S0 += part[w][0], S1 += part[w][1];
+          const bool ok = S0 > 0.0;  // else every term underflowed: E is 0 to double precision
+          nn[k - k_lo] = n, nf[k - k_lo] = ok ? log(S0) - n * m : -1e300, nd[k - k_lo] = ok ? -m - S1 / S0 : 0.0;
+        }
+        __syncthreads();
+      }
+    }
+
+#pragma unroll
+    for (int s = 0; s < PER; ++s) {
+      const int i = first + tid + NT * s;
+      if (i >= end) break;
+      float v = 0.f;
+      if (!zero) {
+        const int k = min(max(node_of(i, tau, lr), k_lo), k_hi - 1) - k_lo;
+        const double h = nn[k + 1] - nn[k], t = (i - nn[k]) / h, t2 = t * t, t3 = t2 * t;
+        const double f = (2 * t3 - 3 * t2 + 1) * nf[k] + (t3 - 2 * t2 + t) * h * nd[k] + (3 * t2 - 2 * t3) * nf[k + 1] +
+                         (t3 - t2) * h * nd[k + 1];
+        double amp = sqrt(scale * exp(f - ea * i));
+        const double x = (i - n_d + half + 0.5) / g.Tw;
+        if (x < 1.0) {
+          double sn, co;
+          sincospi(x, &sn, &co);
+          amp *= sqrt(0.5 * (1.0 - co));
+        }
+        v = (float)(amp * rad[s] * cosv[s]);
+      }
+      float* o = g.out + (bd * rows + row) * (int64_t)g.L;
+      if (bd == g.KB - 1) {
+        if (!zero) o[i] += v;
+      } else {
+        o[i] += v - prev[s];
+      }
+      prev[s] = v;
+    }
+    __syncthreads();  // the next band rewrites the tables and the nodes
+  }
+}
+
+// y = r_last + conv_0 + conv_1 + ... (the crossovers' outputs, added in band order), one row per blockIdx.y.  The
+// crossovers run on the FFT engine, whose rounding spreads over whole blocks, so the samples before the first one any
+// band can reach are written as the exact zeros they are: every image is at least as far as the direct path d, so
+// nothing reaches n < floor(d) - Tw/2 + 1 - half, nor, with a tail, n < n_d - Tw/2 - half; one sample of margin is
+// kept for the rounding of d.
+__global__ void __launch_bounds__(256) band_sum_kernel(const Geo g, int half, const float* __restrict__ conv,
+                                                       int n_conv, float* __restrict__ y) {
+  const int64_t row = blockIdx.y, b = row / g.C, rows = gridDim.y, n = rows * (int64_t)g.L;
+  const double ks = g.fs / g.c;
+  const double X = (g.src[3 * b] - g.mics[3 * row]) * ks, Y = (g.src[3 * b + 1] - g.mics[3 * row + 1]) * ks;
+  const double Z = (g.src[3 * b + 2] - g.mics[3 * row + 2]) * ks;
+  double z0 = floor(sqrt(X * X + Y * Y + Z * Z)) - g.Tw / 2 - half;
+  if (g.td) z0 = fmin(z0, fmax(ceil(g.td[b] * g.fs) - g.Tw / 2, 0.0) - half - 1);
+  const float* last = g.out + (int64_t)n_conv * n + row * (int64_t)g.L;
+  float* o = y + row * (int64_t)g.L;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < g.L; i += gridDim.x * blockDim.x) {
+    float v = 0.f;
+    if ((double)i >= z0) {
+      v = last[i];
+      for (int k = 0; k < n_conv; ++k) v += conv[k * n + row * (int64_t)g.L + i];
+    }
+    o[i] = v;
   }
 }
 
@@ -339,8 +461,8 @@ static int check(const char* fn, const double* room, const double* src, const do
 static Geo geo(const double* room, const double* src, const double* mics, const double* beta, int C, int64_t L,
                double fs, double c, int max_order, float* out) {
   Geo g;
-  g.room = room, g.src = src, g.mics = mics, g.beta = beta, g.td = nullptr, g.seed = nullptr, g.C = C, g.L = (int)L;
-  g.max_order = max_order, g.Tw = 2 * (int)floor(0.004 * fs + 0.5), g.fs = fs, g.c = c, g.out = out;
+  g.room = room, g.src = src, g.mics = mics, g.beta = beta, g.td = nullptr, g.seed = nullptr, g.air = nullptr;
+  g.C = C, g.L = (int)L, g.K = 1, g.KB = 1, g.max_order = max_order, g.Tw = 2 * (int)floor(0.004 * fs + 0.5), g.fs = fs, g.c = c, g.out = out;
   return g;
 }
 
@@ -368,6 +490,73 @@ extern "C" int b2a_rir_hybrid_f32(const double* room, const double* src, const d
   B2A_LAUNCH(ism_kernel, grid, dim3(NT), 0, stream, g);
   B2A_CUDA_OK(cudaGetLastError());
   B2A_LAUNCH(tail_kernel, grid, dim3(NT), 0, stream, g);
+  B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
+}
+
+// Bands whose lower crossover 125 2^(k - 1/2) Hz is below fs / 2 (band 0 always)
+static int bands_kept(int K, double fs) {
+  int kb = 1;
+  while (kb < K && 125.0 * exp2(kb - 0.5) < 0.5 * fs) ++kb;
+  return kb;
+}
+
+template <int NB>
+static void launch_bands(const dim3& grid, const Geo& g, void* stream) {
+  B2A_LAUNCH(ism_bands_kernel<NB>, grid, dim3(NT), 0, stream, g);
+}
+
+extern "C" int b2a_rir_bands_kept(int K, double fs) {
+  if (K < 1 || K > MAX_BANDS || !(fs > 0.0)) return 0;
+  return bands_kept(K, fs);
+}
+
+extern "C" int b2a_rir_bands_f32(const double* room, const double* src, const double* mics, const double* beta,
+                                 const double* air, const double* t_d, const uint64_t* seed, int64_t B, int C, int K,
+                                 int64_t L, double fs, double c, int max_order, float* out, void* stream) {
+  const int rc = check("rir_bands", room, src, mics, beta, B, C, L, fs, c, out);
+  if (rc != B2A_OK) return rc;
+  B2A_REQUIRE(K >= 1 && K <= MAX_BANDS, B2A_E_INVALID, "rir_bands: K=%d bands; 1 .. %d are supported", K, MAX_BANDS);
+  B2A_REQUIRE(B * C * K <= 65535, B2A_E_INVALID, "rir_bands: %lld rows (items x microphones x bands); at most 65535",
+              (long long)(B * C * K));
+  B2A_REQUIRE(max_order >= -1, B2A_E_INVALID, "rir_bands: max_order=%d must be >= -1", max_order);
+  B2A_REQUIRE(!t_d == !seed, B2A_E_INVALID, "rir_bands: a diffuse tail needs both t_d and seed");
+  B2A_REQUIRE(!t_d || max_order == -1, B2A_E_INVALID, "rir_bands: max_order=%d with a diffuse tail", max_order);
+  Geo g = geo(room, src, mics, beta, C, L, fs, c, max_order, out);
+  g.air = air, g.td = t_d, g.seed = seed, g.K = K, g.KB = bands_kept(K, fs);
+  const dim3 grid((unsigned)((L + TT - 1) / TT), (unsigned)(B * C));
+  switch (g.KB) {
+    case 1: B2A_LAUNCH(ism_kernel, grid, dim3(NT), 0, stream, g); break;
+    case 2: launch_bands<2>(grid, g, stream); break;
+    case 3: launch_bands<3>(grid, g, stream); break;
+    case 4: launch_bands<4>(grid, g, stream); break;
+    case 5: launch_bands<5>(grid, g, stream); break;
+    case 6: launch_bands<6>(grid, g, stream); break;
+    case 7: launch_bands<7>(grid, g, stream); break;
+    default: launch_bands<8>(grid, g, stream); break;
+  }
+  B2A_CUDA_OK(cudaGetLastError());
+  if (t_d) {
+    B2A_LAUNCH(tail_kernel, grid, dim3(NT), 0, stream, g);
+    B2A_CUDA_OK(cudaGetLastError());
+  }
+  return B2A_OK;
+}
+
+extern "C" int b2a_rir_band_sum_f32(const double* src, const double* mics, const double* t_d, int64_t B, int C,
+                                    int64_t L, double fs, double c, int half, const float* bands, const float* conv,
+                                    int n_conv, float* out, void* stream) {
+  B2A_REQUIRE(src && mics && bands && conv && out, B2A_E_INVALID, "rir_band_sum: null pointer");
+  B2A_REQUIRE(B >= 1 && C >= 1 && L >= 1 && B * C <= 65535 && L <= (1 << 30) && n_conv >= 1 && n_conv < MAX_BANDS &&
+                  half >= 0,
+              B2A_E_INVALID, "rir_band_sum: bad shape B=%lld C=%d L=%lld n_conv=%d half=%d", (long long)B, C,
+              (long long)L, n_conv, half);
+  B2A_REQUIRE(fs >= 125.0 && fs <= 384000.0 && c > 0.0 && c < 1e30, B2A_E_INVALID, "rir_band_sum: fs=%g c=%g", fs, c);
+  Geo g = geo(nullptr, src, mics, nullptr, C, L, fs, c, -1, const_cast<float*>(bands));
+  g.td = t_d;
+  const int64_t bx = (L + 255) / 256;
+  const dim3 grid((unsigned)(bx < 64 ? bx : 64), (unsigned)(B * C));
+  B2A_LAUNCH(band_sum_kernel, grid, dim3(256), 0, stream, g, half, conv, n_conv, out);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }

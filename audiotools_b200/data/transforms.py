@@ -568,7 +568,13 @@ class SyntheticRoomImpulseResponse(BaseTransform):
     ``diffuse_after`` (seconds: a float or a distribution tuple) makes hybrid responses, images before it and a diffuse
     tail after it (``image_source_ir(..., diffuse_after=, seed=)``), much cheaper for long RT60s.  Only then two more
     draws follow the ones above: the time (when it is a tuple), then the tail's seed, ``state.randint(0, 2**31 - 1)``.
-    It needs ``max_order = -1``."""
+    It needs ``max_order = -1``.
+
+    ``bands=K`` makes the rooms frequency-dependent over K octave bands (``image_source_ir(..., bands=)``):
+    ``band_rt60`` is K distribution tuples, each band's RT60 as a ratio to the item's ``rt60`` (None: 1 for every band),
+    each raised like ``rt60`` to 1.01 times the room's smallest feasible RT60; ``air_absorption`` is K constants in
+    dB/m (None: no air absorption).  Only then K more draws follow all the ones above, one per band in order, and the
+    IR is as long as the longest band RT60 when no ``duration`` is given."""
     _bypass_pays = False  # FFT convolution
 
     DEFAULT_ROOM = (("uniform", 3.0, 10.0), ("uniform", 3.0, 8.0), ("uniform", 2.4, 4.0))
@@ -576,10 +582,31 @@ class SyntheticRoomImpulseResponse(BaseTransform):
     def __init__(self, room: tuple = DEFAULT_ROOM, rt60: tuple = ("uniform", 0.2, 0.8), margin: float = 0.5,
                  mic_spacing: tuple = ("uniform", 0.05, 0.2), max_order: int = -1, duration: float = None,
                  high_pass: bool = True, name: str = None, prob: float = 1.0, use_original_phase: bool = False,
-                 diffuse_after=None):
+                 diffuse_after=None, bands: int = None, band_rt60=None, air_absorption=None):
         super().__init__(name=name, prob=prob)
         if diffuse_after is None:  # no tail: neither draw is made, so neither key is expected
             self.keys = [k for k in self.keys if k not in ("diffuse_after", "seed")]
+        if bands is None:
+            if band_rt60 is not None or air_absorption is not None:
+                raise ValueError("SyntheticRoomImpulseResponse: band_rt60 and air_absorption need bands")
+            self.keys = [k for k in self.keys if k != "band_rt60"]
+        else:
+            from ..core.room import MAX_BANDS
+
+            if isinstance(bands, bool) or not isinstance(bands, (int, np.integer)) or not 1 <= bands <= MAX_BANDS:
+                raise ValueError(f"SyntheticRoomImpulseResponse: bands = {bands!r}; an int in 1 .. {MAX_BANDS}")
+            band_rt60 = tuple(band_rt60) if band_rt60 is not None else (("const", 1.0),) * bands
+            if len(band_rt60) != bands:
+                raise ValueError(f"SyntheticRoomImpulseResponse: band_rt60 has {len(band_rt60)} entries for {bands} "
+                                 "bands")
+            if air_absorption is not None:
+                air_absorption = np.asarray(air_absorption, dtype=np.float64)
+                if air_absorption.shape != (bands,):
+                    raise ValueError(f"SyntheticRoomImpulseResponse: air_absorption must be {bands} values (dB/m), "
+                                     f"got shape {air_absorption.shape}")
+        self.bands = None if bands is None else int(bands)
+        self.band_rt60 = band_rt60
+        self.air_absorption = air_absorption
         self.room = tuple(room)
         self.diffuse_after = diffuse_after
         self.rt60 = rt60
@@ -615,16 +642,24 @@ class SyntheticRoomImpulseResponse(BaseTransform):
             td = self.diffuse_after
             out["diffuse_after"] = np.float64(util.sample_from_dist(td, state) if isinstance(td, tuple) else td)
             out["seed"] = np.int64(state.randint(0, 2 ** 31 - 1))
+        if self.bands is not None:
+            floor = 1.01 * float(_room.min_rt60(dims))
+            out["band_rt60"] = np.array([max(float(util.sample_from_dist(r, state)) * rt60, floor)
+                                         for r in self.band_rt60])
         return out
 
-    def _transform(self, signal, room, rt60, source, mics, diffuse_after=None, seed=None, _bypass=None):
+    def _transform(self, signal, room, rt60, source, mics, diffuse_after=None, seed=None, band_rt60=None,
+                   _bypass=None):
         from ..core.room import image_source_ir
 
         sr, T = signal.sample_rate, signal.signal_length
-        seconds = self.duration if self.duration is not None else float(util.host_view(rt60).max())
+        walls = rt60 if band_rt60 is None else band_rt60
+        seconds = self.duration if self.duration is not None else float(util.host_view(walls).max())
         length = max(1, min(T, int(np.ceil(seconds * sr))))
-        ir = image_source_ir(room, source, mics, sr, length, rt60=rt60, max_order=self.max_order,
-                             high_pass=self.high_pass, diffuse_after=diffuse_after, seed=seed, device=signal.device)
+        bands = {} if self.bands is None else dict(bands=self.bands, air_absorption=self.air_absorption)
+        ir = image_source_ir(room, source, mics, sr, length, rt60=walls, max_order=self.max_order,
+                             high_pass=self.high_pass, diffuse_after=diffuse_after, seed=seed, device=signal.device,
+                             **bands)
         return signal.apply_ir(ir, use_original_phase=self.use_original_phase, _bypass=_bypass)
 
 

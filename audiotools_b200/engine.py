@@ -30,6 +30,7 @@ class Engine:
         self.launches = 0  # kernels of libb2a launched through this engine (bench.py reports it)
         self._packed_cache = {}
         self._routes = {}
+        self._crossovers = {}  # octave_crossovers: (rate, bands, device) -> (taps, half)
 
     # ------------------------------------------------------------------ helpers
     DIFFERENTIABLE = ("AudioSignal.stft", "istft", "mel_spectrogram", "mfcc", "normalize", "volume_change",
@@ -806,11 +807,93 @@ class Engine:
             self._call(self.lib.b2a_rir_hybrid_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), _dptr(td),
                        _dptr(sd), B, C, int(length), float(sample_rate), float(sound_speed), _dptr(out),
                        self._stream(room))
-        if high_pass:
-            w = 2 * math.pi * 100.0 / sample_rate
-            r = math.exp(-w)
-            out = self.sos_filter(out, [[1.0, -(1.0 + r), r, 1.0, -2.0 * r * math.cos(w), r * r]], out=out)
-        return out
+        return self._rir_high_pass(out, sample_rate) if high_pass else out
+
+    def _rir_high_pass(self, out: torch.Tensor, sample_rate: float) -> torch.Tensor:
+        """Allen & Berkley's 100 Hz high-pass, one second-order section, in place (three launches)."""
+        w = 2 * math.pi * 100.0 / sample_rate
+        r = math.exp(-w)
+        return self.sos_filter(out, [[1.0, -(1.0 + r), r, 1.0, -2.0 * r * math.cos(w), r * r]], out=out)
+
+    RIR_MAX_BANDS = 8  # octave bands centred on 125 2^k Hz, k < 8
+
+    def rir_bands_kept(self, n_bands: int, sample_rate: float) -> int:
+        """The octave bands of ``image_source_ir_bands`` that are computed: those whose lower crossover 125 2^(k - 1/2)
+        Hz is below sample_rate / 2 (``b2a_rir_bands_kept``)."""
+        kept = self.lib.b2a_rir_bands_kept(int(n_bands), float(sample_rate))
+        if kept < 1:
+            raise ValueError(f"image_source_ir: bands = {n_bands}; 1 .. {self.RIR_MAX_BANDS} are supported")
+        return kept
+
+    def octave_crossovers(self, sample_rate: float, n_bands: int, device):
+        """(taps [n_bands - 1, 2 half + 1] float32 convolution taps, half) of the zero-phase windowed-sinc low-passes
+        at the octave crossovers 125 2^(k + 1/2) Hz, k < n_bands - 1 (``_lowpass_bank``, julius arithmetic), all with
+        the half-length julius.SplitBands(zeros=8) gives its lowest cutoff: int(8 / (e_0 / fs) / 2).  Designed once per
+        (rate, band count, device) and cached, so the response path does no tensor arithmetic after the first call."""
+        key = (float(sample_rate), int(n_bands), torch.device(device))
+        hit = self._crossovers.get(key)
+        if hit is None:
+            import numpy as _np
+
+            c = 125.0 * 2.0 ** (_np.arange(n_bands - 1) + 0.5) / float(sample_rate)
+            half = int(8 / c[0] / 2)
+            lp = self._lowpass_bank(torch.from_numpy(c).float(), torch.full((len(c),), half, dtype=torch.int64),
+                                    device)
+            hit = self._crossovers[key] = (torch.flip(lp, dims=[1]).contiguous(), half)
+        return hit
+
+    def image_source_ir_bands(self, room: torch.Tensor, src: torch.Tensor, mics: torch.Tensor, beta: torch.Tensor,
+                              length: int, sample_rate: float, sound_speed: float = 343.0, max_order: int = -1,
+                              high_pass: bool = True, air: Optional[torch.Tensor] = None,
+                              diffuse_after: Optional[torch.Tensor] = None,
+                              seed: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Octave-band shoebox-room impulse responses (DESIGN.md K20 "Bands") -> [B, C, length] float32.  beta [B, 6,
+        K] per wall and band, ``air`` [B, K] dB/m or None, the rest as ``image_source_ir``; everything already checked
+        (``core.room.image_source_ir``).  ``b2a_rir_bands_f32`` writes the K' kept bands' differences r_k - r_{k+1} and
+        the last band r_{K'-1}; the differences go through the zero-phase crossovers LP_k (``fftconv``, zero padding)
+        and ``b2a_rir_band_sum_f32`` adds them to the last band: y = r_{K'-1} + sum_k LP_k * (r_k - r_{k+1}), exactly
+        0 before the first sample the direct path (or the tail) reaches through the crossovers.  With K' = 1 nothing
+        is filtered.  No host sync."""
+        if mics.ndim != 3 or mics.shape[-1] != 3:
+            raise ValueError(f"image_source_ir: mics must be [B, C, 3], got {tuple(mics.shape)}")
+        B, C = mics.shape[:2]
+        K = beta.shape[-1] if beta.ndim == 3 else 0
+        if (tuple(room.shape) != (B, 3) or tuple(src.shape) != (B, 3) or tuple(beta.shape) != (B, 6, K)
+                or (air is not None and tuple(air.shape) != (B, K))):
+            raise ValueError(f"image_source_ir: room / source / beta / air must be [{B}, 3] / [{B}, 3] / [{B}, 6, K] "
+                             f"/ [{B}, K], got {tuple(room.shape)} / {tuple(src.shape)} / {tuple(beta.shape)} / "
+                             f"{None if air is None else tuple(air.shape)}")
+        kept = self.rir_bands_kept(K, sample_rate)
+        if B * C * K > self.RIR_MAX_ROWS:
+            raise ValueError(f"image_source_ir: {B * C * K} rows (items x microphones x bands); at most "
+                             f"{self.RIR_MAX_ROWS}")
+        if (diffuse_after is None) != (seed is None):
+            raise ValueError("image_source_ir: diffuse_after and seed go together")
+        if diffuse_after is not None:
+            if max_order != -1:
+                raise ValueError(f"image_source_ir: max_order = {max_order} with a diffuse tail; the tail has every "
+                                 "order")
+            if tuple(diffuse_after.shape) != (B,) or tuple(seed.shape) != (B,):
+                raise ValueError(f"image_source_ir: diffuse_after and seed must be [{B}]")
+        room, src, mics, beta = (self._prep(t, n, torch.float64) for t, n in
+                                 ((room, "room"), (src, "source"), (mics, "mics"), (beta, "beta")))
+        air = None if air is None else self._prep(air, "air", torch.float64)
+        td = None if diffuse_after is None else self._prep(diffuse_after, "diffuse_after", torch.float64)
+        sd = None if seed is None else self._prep(seed, "seed", torch.int64)
+        L = int(length)
+        bands = torch.empty(kept, B, C, L, dtype=torch.float32, device=room.device)
+        self._call(self.lib.b2a_rir_bands_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), _dptr(air), _dptr(td),
+                   _dptr(sd), B, C, K, L, float(sample_rate), float(sound_speed), int(max_order), _dptr(bands),
+                   self._stream(room))
+        if kept == 1:
+            out = bands[0]
+        else:
+            taps, half = self.octave_crossovers(sample_rate, kept, room.device)
+            conv = self.fftconv(bands[:kept - 1], taps, rows_per_filt=B * C, offset0=half, pad_mode="constant")
+            out = torch.empty(B, C, L, dtype=torch.float32, device=room.device)
+            self._call(self.lib.b2a_rir_band_sum_f32, _dptr(src), _dptr(mics), _dptr(td), B, C, L, float(sample_rate),
+                       float(sound_speed), half, _dptr(bands), _dptr(conv), kept - 1, _dptr(out), self._stream(room))
+        return self._rir_high_pass(out, sample_rate) if high_pass else out
 
     def gain(self, x: torch.Tensor, gain: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``x[b] * gain[b]`` (ref:audiotools/core/effects.py:219,237)."""

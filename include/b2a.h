@@ -408,6 +408,28 @@ int b2a_rir_hybrid_f32(const double* room, const double* src, const double* mics
                        const double* t_d, const uint64_t* seed, int64_t B, int C, int64_t L, double fs, double c,
                        float* out, void* stream);
 
+/* Octave-band responses (DESIGN.md K20, "Bands"): band k (centre 125 2^k Hz) of item b uses the reflection
+ * coefficients beta[b, :, k] (beta [B, 6, K] float64) and, when air [B, K] (dB/m, float64) is given, every image is
+ * also scaled by 10^(-air[b, k] d / 20) (d in metres) and the tail's envelope by 10^(-air[b, k] (c n / fs) / 10).
+ * t_d and seed as in b2a_rir_hybrid_f32, both null for images only (then max_order >= -1; with a tail it must be -1).
+ * Only the first K' = b2a_rir_bands_kept(K, fs) bands are computed: those whose lower crossover 125 2^(k - 1/2) Hz is
+ * below fs / 2.  out [K', B, C, L] float32, band-major: row k < K' - 1 holds r_k - r_{k+1}, row K' - 1 holds r_{K'-1},
+ * r_k the band's response before the crossovers.  The images are enumerated once for all bands; with equal bands and
+ * no air the differences are exactly 0 and r_{K'-1} is b2a_rir_ism_f32's / b2a_rir_hybrid_f32's output, bit for bit.
+ * 1 <= K <= 8, B C K <= 65535.  One launch, two with a tail; no host sync, no atomics. */
+int b2a_rir_bands_kept(int K, double fs);
+int b2a_rir_bands_f32(const double* room, const double* src, const double* mics, const double* beta, const double* air,
+                      const double* t_d, const uint64_t* seed, int64_t B, int C, int K, int64_t L, double fs, double c,
+                      int max_order, float* out, void* stream);
+
+/* y[b, c] = bands[n_conv, b, c] + sum_{k < n_conv} conv[k, b, c] (added in k order): the crossover outputs of the
+ * octave-band differences added to the last band (bands [n_conv + 1, B, C, L] from b2a_rir_bands_f32, conv [n_conv, B,
+ * C, L]).  Samples before the first one any band can reach through crossovers of half-length `half` (the direct path's
+ * window, or with t_d the tail's start, less half and one sample) are written as 0.  1 <= n_conv < 8.  One launch. */
+int b2a_rir_band_sum_f32(const double* src, const double* mics, const double* t_d, int64_t B, int C, int64_t L,
+                         double fs, double c, int half, const float* bands, const float* conv, int n_conv, float* out,
+                         void* stream);
+
 /* ---- per-item gain ---------------------------------------------------------------------
  * x[b, :, :] * gain[b]  (EffectMixin.normalize / volume_change, effects.py:219,237).
  * out may alias x.  per_item = C*T. */
