@@ -9,7 +9,7 @@
 //                      fill = val * exp(1j * val).  No loads of the spectrogram; one CTA per (row, bin) line.
 //   rotate_kernel      shift_phase (:335-351): X *= exp(1j * shift), shift per item or per cell -- one read, one write.
 //   maxpow_kernel +    mask_low_magnitudes (:308-333): log_magnitude()'s top_db floor needs the global maximum of
-//   mask_low_kernel    |X|^2 (one read-only pass, float atomicMax on the bit pattern), then cells whose
+//   mask_low_kernel    |X|^2 (one read-only pass, atomicMax on the bit pattern), then cells whose
 //                      10 log10(max(|X|^2, 1e-10)) (floored at max - 80 dB) is below the item's cut-off get
 //                      magnitude `val` and keep their phase; only those cells are written.
 // The gradient path (a spectrogram that requires a gradient) cannot write in place: autograd may have saved the input
@@ -94,31 +94,41 @@ __device__ __forceinline__ float power_of(float2 z) {
   return mag * mag;                    // .pow(2)
 }
 
+// max(a, b) as torch.maximum and clamp compute it: NaN if either is NaN (fmaxf would drop the NaN).  Equal to fmaxf
+// for any other pair.
+__device__ __forceinline__ float max_nan(float a, float b) { return (a != a || b != b) ? a + b : fmaxf(a, b); }
+
+// The maximum of |X|^2 as an unsigned max of bit patterns: |X|^2 is +0 or positive, and those order like their bits.
+// Every NaN pattern, of either sign, ranks above +inf's 0x7f800000, so a NaN anywhere in the batch wins, as in
+// log_spec.max(); it is stored as the positive quiet NaN 0x7fffffff.
 __global__ void __launch_bounds__(256)
 maxpow_kernel(const float2* __restrict__ spec, long long total, unsigned* __restrict__ max_bits) {
-  float m = 0.f;
+  unsigned m = 0u;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
-    m = fmaxf(m, power_of(spec[i]));
-  m = warp_max(m);
-  __shared__ float sm[8];
+    m = max(m, __float_as_uint(power_of(spec[i])));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+  __shared__ unsigned sm[8];
   if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = m;
   __syncthreads();
   if (threadIdx.x == 0) {
-    for (int w = 1; w < 8; ++w) m = fmaxf(m, sm[w]);
-    atomicMax(max_bits, __float_as_uint(m));  // non-negative floats order like their bit patterns
+    for (int w = 1; w < 8; ++w) m = max(m, sm[w]);
+    atomicMax(max_bits, m > 0x7f800000u ? 0x7fffffffu : m);
   }
 }
 
-// log_magnitude()'s top_db floor from the maximum maxpow_kernel found
+// log_magnitude()'s top_db floor from the maximum maxpow_kernel found (NaN when the batch holds a NaN)
 __device__ __forceinline__ float mask_low_floor(const unsigned* max_bits, float amin2, float top_db) {
-  return 10.0f * log10f(fmaxf(__uint_as_float(*max_bits), amin2)) - top_db;
+  return 10.0f * log10f(max_nan(__uint_as_float(*max_bits), amin2)) - top_db;
 }
 
-// the mask decision of mask_low_magnitudes, shared by the forwards and the backward
+// the mask decision of mask_low_magnitudes, shared by the forwards and the backward.  torch.maximum(log_spec, NaN) is
+// NaN and NaN < cut is false: a NaN floor masks nothing.  A NaN cell makes the floor NaN (it enters the batch's
+// maximum), so the cell's own power needs no test, and the floor's is the same for every cell of a launch.
 __device__ __forceinline__ bool mask_low_cell(float2 z, float floor_db, float cut, float amin2) {
   float db = 10.0f * log10f(fmaxf(power_of(z), amin2));
   db = fmaxf(db, floor_db);
-  return db < cut;
+  return db < cut && floor_db == floor_db;
 }
 
 // magnitude := val, phase kept: val * exp(1j * atan2(im, re))
@@ -189,7 +199,9 @@ mask_low_bwd_kernel(const float2* __restrict__ g, const float2* __restrict__ spe
 //                      Y = X in the forward; Y = g in the backward (S is a constant of the gradient: the reference
 //                      builds it from a comparison), which reads X again and the saved thresholds.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float gate_db(float2 z) { return 20.0f * log10f(fmaxf(hypotf(z.x, z.y), 1e-4f)); }
+// clamp(1e-4) keeps a NaN: a NaN cell of the signal is never below its threshold, and one in the noise makes its
+// bin's threshold NaN, so that bin is never gated
+__device__ __forceinline__ float gate_db(float2 z) { return 20.0f * log10f(max_nan(hypotf(z.x, z.y), 1e-4f)); }
 
 __global__ void __launch_bounds__(256)
 gate_stats_kernel(const float2* __restrict__ nz, int lines, int N, float n_std, float* __restrict__ thresh) {
