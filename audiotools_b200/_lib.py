@@ -34,6 +34,10 @@ SIGNATURES = {
                              POINTER(c_double), POINTER(c_double), c_int, c_double,
                              POINTER(c_double), c_void_p, c_void_p, c_void_p,
                              c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "b2a_lufs_backward_workspace_bytes": (c_size_t, [c_int64, c_int, c_int64, c_double, c_double]),
+    "b2a_lufs_backward_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int64, c_double,
+                                      POINTER(c_double), POINTER(c_double), c_int, c_double, POINTER(c_double),
+                                      c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "b2a_loudness_stats_num_short_term": (c_int64, [c_int64, c_double]),
     "b2a_loudness_stats_workspace_bytes": (c_size_t, [c_int64, c_int, c_int64, c_double]),
     "b2a_loudness_stats_f32": (c_int, [c_void_p, c_int64, c_int, c_int64, c_int64, c_double,

@@ -3,7 +3,8 @@
 ref:tests/core/test_grad.py) and of the time-domain effects (resample, equalizer, convolve, apply_ir,
 ensure_max_of_audio, mix, quantization, sos_filter, sosfiltfilt; gradients with respect to the waveform only) and of the spectral masks and the
 spectral gate (ref:audiotools/core/dsp.py:217-334, ml/layers/spectral_gate.py:58-127; gradients to the spectrogram)
-and of STOI (``metrics.quality.STOILoss``; gradients to the estimates).  ``AudioSignal`` uses them only when grad mode is on and the input requires a gradient;
+and of STOI and the integrated loudness (``metrics.quality.STOILoss``, ``metrics.LoudnessLoss``; gradients to the
+estimates).  ``AudioSignal`` uses them only when grad mode is on and the input requires a gradient;
 otherwise it calls the engine directly, with exactly the launches it always made.
 
 Each forward is the engine call of the no-gradient path; each backward is one launch sequence of csrc/grad.cu (or an
@@ -309,6 +310,31 @@ class STOI(torch.autograd.Function):
     def backward(ctx, g):
         shape, sample_rate, extended = ctx.args
         return _engine().stoi_backward(g, ctx.ws, shape, sample_rate, extended), None, None, None
+
+
+class Loudness(torch.autograd.Function):
+    """(x [B, C, T], gain [B] or None) -> loud [B] = max(lufs, -70), bit for bit ``loudness()``'s value of the samples
+    float32(gain x) zero-extended to ``padded_length`` (``Engine.lufs`` with its block energies).  The forward keeps
+    x, the block energies and the unclamped loudness; the backward (``Engine.lufs_backward``) rebuilds the gate
+    decisions from them (constants of the backward: they are piecewise constant) and recomputes the K-weighted
+    signal.  The gain is a constant."""
+
+    @staticmethod
+    def forward(ctx, x, gain, sample_rate, padded_length):
+        eng = _engine()
+        xs = x if gain is None else eng.gain(x, gain)
+        out = eng.lufs(xs, sample_rate, padded_length=padded_length, want_blocks=True)
+        ctx.save_for_backward(x)
+        ctx.args = (gain, sample_rate, padded_length, out["blocks"], out["lufs"])
+        return out["loud"]
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (x,) = ctx.saved_tensors
+        gain, sample_rate, padded_length, blocks, lufs = ctx.args
+        gx = _engine().lufs_backward(g, x, sample_rate, blocks, lufs, padded_length=padded_length, gain=gain)
+        return gx, None, None, None
 
 
 class SOSFilter(torch.autograd.Function):

@@ -28,7 +28,13 @@
 // given zi, or sosfilt_zi(sos) v[0] (read on the device).  The filter kernel can also write the state after v[L - 1]
 // (zf) and, per warp, G sum(v) - sum(y) (G: the cascade's DC gain), the rank-one term of the sosfiltfilt backward.
 // Nothing depends on the launch geometry or on other items: reruns and batch-versus-single calls are bit-identical.
+//
+// The loudness backward (b2a_lufs_backward_f32, K21) runs two passes of the K-weighting on the LOUDNESS layout: the
+// forward pass over a row of x zero-extended to Lmax samples stores u = wt[row] * m[e] * y (m[e]: the gating blocks
+// kept by the forward that contain sample e) into the intermediate, and the reverse pass over the intermediate stores
+// its first T samples (the adjoint of the zero extension) into grad_x.
 #include "b2a_common.h"
+#include "iir_internal.h"
 
 namespace b2a {
 namespace iir {
@@ -40,6 +46,11 @@ constexpr int SMAX = 8;       // largest number of sections
 
 // padtype of b2a_sos_filtfilt_f32 (b2a.h); PAD_ZERO (outside [0, T) reads 0) is the backward's crop adjoint
 enum { PAD_NONE = 0, PAD_ODD = 1, PAD_EVEN = 2, PAD_CONST = 3, PAD_ZERO = 4 };
+
+// Row layouts of a pass: rows of x as they are (sosfilt); rows padded by the edge extension or read from the
+// intermediate (sosfiltfilt); the loudness backward's rows (a row of x zero-extended to Lmax samples, or a row of the
+// intermediate, with the gating weight applied on the store of the forward pass)
+enum { ROWS = 0, EXTENDED = 1, LOUDNESS = 2 };
 
 // One pass of the cascade over every row.  Row r of length L = T + 2 pl: m in [0, L) is the extended position
 // e = (reverse ? L - 1 - m : m) - pl in [-pl, T + pl).  A source or destination row is either a row of T samples (x /
@@ -61,6 +72,9 @@ struct Pass {
   double* zf;               // [S, rows, 2]: the state after v[L - 1], or null
   double* part;             // [rows, n_groups]: G sum(v) - sum(y) over a warp's chunks, or null
   const double* add_first;  // [rows, n_groups]: their sum is added to v[0], or null
+  const double* wt;         // LOUDNESS: [rows] weight of the store, or null (no weight)
+  const int* kept;          // LOUDNESS: [B, nblk + 1] running count of the kept gating blocks
+  int nblk, blk_stride, blk_len;
 };
 
 template <int S>
@@ -104,6 +118,9 @@ struct Row {
   int64_t T, L, pl;
   float g, first, last;  // gain; the gained first and last samples of a row of x (the extension's edges)
   int src_mid, dst_mid, reverse, padtype;
+  double w;              // LOUDNESS: the row's weight (kept != null)
+  const int* kept;       // LOUDNESS: the item's running count of kept blocks, or null
+  int nblk, bs, bk;      // LOUDNESS: blocks, their stride and length in samples
 };
 
 __device__ __forceinline__ Row make_row(const Pass& p, int S, int64_t row, int64_t b) {
@@ -119,11 +136,35 @@ __device__ __forceinline__ Row make_row(const Pass& p, int S, int64_t row, int64
   return r;
 }
 
-// v[m]: 0 past the row's end.  EXT = false: a row of x without padding (pl = 0, L = T), the zero-state filter's own
-// index expression.  EXT: one predicated load and selects, no divergent branch, so a tile's 32 loads issue together.
-template <bool EXT>
+// make_row, and for LOUDNESS the virtual length Lmax and the store's weight
+template <int LAY>
+__device__ __forceinline__ Row make_row_as(const Pass& p, int S, int64_t row, int64_t b) {
+  Row r = make_row(p, S, row, b);
+  if (LAY == LOUDNESS) {
+    r.L = p.Lmax;
+    r.kept = p.wt ? p.kept + b * (p.nblk + 1) : nullptr;
+    r.w = p.wt ? p.wt[row] : 0.0;
+    r.nblk = p.nblk, r.bs = p.blk_stride, r.bk = p.blk_len;
+  }
+  return r;
+}
+
+// LOUDNESS: the number of kept blocks [i stride, i stride + len), 0 <= i < nblk, that contain sample e
+__device__ __forceinline__ int kept_blocks(const Row& r, int64_t e) {
+  const int64_t hi = e / r.bs < r.nblk - 1 ? e / r.bs : r.nblk - 1, lo = e < r.bk ? 0 : (e - r.bk) / r.bs + 1;
+  return hi >= lo ? r.kept[hi + 1] - r.kept[lo] : 0;
+}
+
+// v[m]: 0 past the row's end.  ROWS: a row of x without padding (pl = 0, L = T), the zero-state filter's own index
+// expression.  EXTENDED: one predicated load and selects, no divergent branch, so a tile's 32 loads issue together.
+// LOUDNESS: a row of x reads 0 from T on.
+template <int LAY>
 __device__ __forceinline__ float load(const Row& r, int64_t m) {
-  if (!EXT) return m < r.L ? r.src[r.reverse ? r.L - 1 - m : m] * r.g : 0.f;
+  if (LAY == ROWS) return m < r.L ? r.src[r.reverse ? r.L - 1 - m : m] * r.g : 0.f;
+  if (LAY == LOUDNESS) {
+    const int64_t e = r.reverse ? r.L - 1 - m : m;
+    return m < r.L && (r.src_mid || e < r.T) ? r.src[e] * r.g : 0.f;
+  }
   const int64_t e = (r.reverse ? r.L - 1 - m : m) - r.pl;
   const bool inside = r.src_mid || (e >= 0 && e < r.T);
   const bool mirror = r.padtype == PAD_ODD || r.padtype == PAD_EVEN;
@@ -134,10 +175,15 @@ __device__ __forceinline__ float load(const Row& r, int64_t m) {
   return r.padtype == PAD_ODD ? 2.f * edge - v : r.padtype == PAD_EVEN ? v : r.padtype == PAD_CONST ? edge : 0.f;
 }
 
-template <bool EXT>
+template <int LAY>
 __device__ __forceinline__ void store(const Row& r, int64_t m, float y) {
-  if (!EXT) {
+  if (LAY == ROWS) {
     if (m < r.L) r.dst[r.reverse ? r.L - 1 - m : m] = y;
+    return;
+  }
+  if (LAY == LOUDNESS) {
+    const int64_t e = r.reverse ? r.L - 1 - m : m;
+    if (m < r.L && (r.dst_mid || e < r.T)) r.dst[e] = r.kept ? (float)((double)y * r.w * kept_blocks(r, e)) : y;
     return;
   }
   const int64_t e = (r.reverse ? r.L - 1 - m : m) - r.pl;
@@ -176,7 +222,7 @@ struct Extra {
 
 // Walk the warp's chunks tile by tile: lane l runs chunk g * 32 + l of the row from state z.  WRITE: y replaces the
 // tile and is stored.  add0 (when `add`) is added to v[0].  Flat indices are 64-bit.
-template <int S, bool WRITE, bool EXT, bool EXTRA>
+template <int S, bool WRITE, int LAY, bool EXTRA>
 __device__ __forceinline__ void run_chunks(const Row& rw, int64_t first, bool add, double add0, const Coef<S>& c,
                                            double (&z)[2 * S], float* tile, Extra& ex) {
   const int lane = threadIdx.x & 31;
@@ -185,8 +231,8 @@ __device__ __forceinline__ void run_chunks(const Row& rw, int64_t first, bool ad
   for (int t = 0; t < n_tiles; ++t) {
     for (int r = 0; r < 32; ++r) {
       const int64_t n = first + (int64_t)r * CHUNK + t * TILE + lane;
-      float v = load<EXT>(rw, n);
-      if (EXT && add && n == 0) v = (float)((double)v + add0);
+      float v = load<LAY>(rw, n);
+      if (LAY == EXTENDED && add && n == 0) v = (float)((double)v + add0);
       tile[r * (TILE + 1) + lane] = v;
     }
     __syncwarp();
@@ -209,7 +255,7 @@ __device__ __forceinline__ void run_chunks(const Row& rw, int64_t first, bool ad
     if (WRITE) {
       for (int r = 0; r < 32; ++r) {
         const int64_t n = first + (int64_t)r * CHUNK + t * TILE + lane;
-        store<EXT>(rw, n, tile[r * (TILE + 1) + lane]);
+        store<LAY>(rw, n, tile[r * (TILE + 1) + lane]);
       }
       __syncwarp();
     }
@@ -217,7 +263,7 @@ __device__ __forceinline__ void run_chunks(const Row& rw, int64_t first, bool ad
 }
 
 // ws_e [rows, n_chunks, 2S]: end state of every chunk from zero state.
-template <int S, bool EXT>
+template <int S, int LAY>
 __global__ void __launch_bounds__(WARPS * 32) chunk_state_kernel(const Pass p, double* __restrict__ ws_e) {
   __shared__ float s_tile[WARPS][32 * (TILE + 1)];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -225,14 +271,14 @@ __global__ void __launch_bounds__(WARPS * 32) chunk_state_kernel(const Pass p, d
   for (int64_t w = (int64_t)blockIdx.x * WARPS + wid; w < p.work; w += (int64_t)gridDim.x * WARPS) {
     const int64_t row = w / n_groups, g = w - row * n_groups, b = row / p.C;
     const Coef<S> c = load_coef<S>(p.sos + (p.sos_items > 1 ? b : 0) * 6 * S);
-    const Row rw = make_row(p, S, row, b);
+    const Row rw = make_row_as<LAY>(p, S, row, b);
     const bool add = p.add_first && g == 0;
     const double add0 = add ? warp_sum(p.add_first + row * n_groups, n_groups) : 0.0;
     double z[2 * S];
 #pragma unroll
     for (int i = 0; i < 2 * S; ++i) z[i] = 0.0;
     Extra ex{};
-    run_chunks<S, false, EXT, false>(rw, g * 32 * CHUNK, add, add0, c, z, s_tile[wid], ex);
+    run_chunks<S, false, LAY, false>(rw, g * 32 * CHUNK, add, add0, c, z, s_tile[wid], ex);
     const int64_t k = g * 32 + lane;
     if (k < n_chunks) {
 #pragma unroll
@@ -277,7 +323,7 @@ __device__ __forceinline__ void start_state(const Pass& p, int64_t row, int64_t 
     return;
   }
   const float* so = p.sos + (p.sos_items > 1 ? b : 0) * 6 * S;
-  const double v = (double)load<true>(make_row(p, S, row, b), 0);
+  const double v = (double)load<EXTENDED>(make_row(p, S, row, b), 0);
   double scale = v;
 #pragma unroll
   for (int s = 0; s < S; ++s) {
@@ -367,7 +413,7 @@ __global__ void __launch_bounds__(32) carry_kernel(const Pass p, const double* _
   }
 }
 
-template <int S, bool EXT, bool EXTRA>
+template <int S, int LAY, bool EXTRA>
 __global__ void __launch_bounds__(WARPS * 32) filter_kernel(const Pass p, const double* __restrict__ ws_s) {
   __shared__ float s_tile[WARPS][32 * (TILE + 1)];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -375,11 +421,11 @@ __global__ void __launch_bounds__(WARPS * 32) filter_kernel(const Pass p, const 
   for (int64_t w = (int64_t)blockIdx.x * WARPS + wid; w < p.work; w += (int64_t)gridDim.x * WARPS) {
     const int64_t row = w / n_groups, g = w - row * n_groups, b = row / p.C;
     const Coef<S> c = load_coef<S>(p.sos + (p.sos_items > 1 ? b : 0) * 6 * S);
-    const Row rw = make_row(p, S, row, b);
+    const Row rw = make_row_as<LAY>(p, S, row, b);
     const int64_t lo = g * 32 * CHUNK, hi = lo + 32 * CHUNK < rw.L ? lo + 32 * CHUNK : rw.L;
     if (!c.stable) {  // warp-uniform: the whole item is NaN
       const float nan = __int_as_float(0x7fffffff);
-      for (int64_t m = lo + lane; m < hi; m += 32) store<EXT>(rw, m, nan);
+      for (int64_t m = lo + lane; m < hi; m += 32) store<LAY>(rw, m, nan);
       if (EXTRA && lane == 0) {
         if (p.zf && rw.L - 1 >= lo && rw.L - 1 < hi) {
           for (int i = 0; i < 2 * S; ++i) p.zf[((i >> 1) * rows + row) * 2 + (i & 1)] = (double)nan;
@@ -395,7 +441,7 @@ __global__ void __launch_bounds__(WARPS * 32) filter_kernel(const Pass p, const 
 #pragma unroll
     for (int i = 0; i < 2 * S; ++i) z[i] = k < n_chunks ? __ldg(ws_s + (row * n_chunks + k) * 2 * S + i) : 0.0;
     Extra ex{p.zf ? p.zf + row * 2 : nullptr, rows * 2, 0.0, 0.0};
-    run_chunks<S, true, EXT, EXTRA>(rw, lo, add, add0, c, z, s_tile[wid], ex);
+    run_chunks<S, true, LAY, EXTRA>(rw, lo, add, add0, c, z, s_tile[wid], ex);
     if (EXTRA && p.part) {
       double sv = ex.sum_v, sy = ex.sum_y;
 #pragma unroll
@@ -462,36 +508,36 @@ extern "C" size_t b2a_sos_filter_workspace_bytes(int64_t B, int C, int64_t T, in
 }
 
 // The three launches of one pass; ws_e / ws_s: [rows, n_chunks, 2S] doubles each
-// EXT: rows padded or read from the intermediate (sosfiltfilt); else rows of x as they are (sosfilt)
-template <int S, bool EXT>
+// LAY: ROWS (rows of x as they are: sosfilt), EXTENDED (sosfiltfilt) or LOUDNESS
+template <int S, int LAY>
 static int run_pass(const Pass& p, double* ws_e, double* ws_s, void* stream) {
   const int64_t rows = p.work / ((p.n_chunks + 31) / 32);
   const int64_t g13 = (p.work + WARPS - 1) / WARPS;
   const unsigned grid13 = (unsigned)(g13 < INT32_MAX ? g13 : INT32_MAX);
   const unsigned grid2 = (unsigned)(rows < INT32_MAX ? rows : INT32_MAX);
-  void (*chunk_state)(const Pass, double*) = chunk_state_kernel<S, EXT>;
+  void (*chunk_state)(const Pass, double*) = chunk_state_kernel<S, LAY>;
   B2A_LAUNCH(chunk_state, dim3(grid13), dim3(WARPS * 32), 0, stream, p, ws_e);
   B2A_CUDA_OK(cudaGetLastError());
   B2A_LAUNCH(carry_kernel<S>, dim3(grid2), dim3(32), 0, stream, p, ws_e, ws_s);
   B2A_CUDA_OK(cudaGetLastError());
   void (*filter)(const Pass, const double*) =
-      p.zf || p.part ? filter_kernel<S, EXT, true> : filter_kernel<S, EXT, false>;
+      p.zf || p.part ? filter_kernel<S, LAY, true> : filter_kernel<S, LAY, false>;
   B2A_LAUNCH(filter, dim3(grid13), dim3(WARPS * 32), 0, stream, p, ws_s);
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }
 
-template <bool EXT>
+template <int LAY>
 static int pass_launch(int S, const Pass& p, double* ws_e, double* ws_s, void* stream) {
   switch (S) {
-    case 1: return run_pass<1, EXT>(p, ws_e, ws_s, stream);
-    case 2: return run_pass<2, EXT>(p, ws_e, ws_s, stream);
-    case 3: return run_pass<3, EXT>(p, ws_e, ws_s, stream);
-    case 4: return run_pass<4, EXT>(p, ws_e, ws_s, stream);
-    case 5: return run_pass<5, EXT>(p, ws_e, ws_s, stream);
-    case 6: return run_pass<6, EXT>(p, ws_e, ws_s, stream);
-    case 7: return run_pass<7, EXT>(p, ws_e, ws_s, stream);
-    default: return run_pass<8, EXT>(p, ws_e, ws_s, stream);
+    case 1: return run_pass<1, LAY>(p, ws_e, ws_s, stream);
+    case 2: return run_pass<2, LAY>(p, ws_e, ws_s, stream);
+    case 3: return run_pass<3, LAY>(p, ws_e, ws_s, stream);
+    case 4: return run_pass<4, LAY>(p, ws_e, ws_s, stream);
+    case 5: return run_pass<5, LAY>(p, ws_e, ws_s, stream);
+    case 6: return run_pass<6, LAY>(p, ws_e, ws_s, stream);
+    case 7: return run_pass<7, LAY>(p, ws_e, ws_s, stream);
+    default: return run_pass<8, LAY>(p, ws_e, ws_s, stream);
   }
 }
 
@@ -523,7 +569,7 @@ extern "C" int b2a_sos_filter_f32(const float* x, const float* gain, int64_t B, 
   Pass p = make_pass(B, C, T, 0, sos, sos_items);
   p.src = x, p.gain = gain, p.dst = out, p.reverse = reverse;
   double* ws_e = static_cast<double*>(ws);
-  return pass_launch<false>(S, p, ws_e, ws_e + B * C * p.n_chunks * 2 * S, stream);
+  return pass_launch<ROWS>(S, p, ws_e, ws_e + B * C * p.n_chunks * 2 * S, stream);
 }
 
 extern "C" int b2a_sos_filter_zi_f32(const float* x, const float* gain, int64_t B, int C, int64_t T, const float* sos,
@@ -535,7 +581,7 @@ extern "C" int b2a_sos_filter_zi_f32(const float* x, const float* gain, int64_t 
   Pass p = make_pass(B, C, T, 0, sos, sos_items);
   p.src = x, p.gain = gain, p.dst = out, p.zi = zi, p.zf = zf;
   double* ws_e = static_cast<double*>(ws);
-  return pass_launch<false>(S, p, ws_e, ws_e + B * C * p.n_chunks * 2 * S, stream);
+  return pass_launch<ROWS>(S, p, ws_e, ws_e + B * C * p.n_chunks * 2 * S, stream);
 }
 
 // Largest padding of a call: none, the given padlen, or scipy's default at its largest, 3 (2S + 1); -1 when invalid
@@ -591,11 +637,11 @@ extern "C" int b2a_sos_filtfilt_f32(const float* x, const float* gain, int64_t B
   p.padtype = padtype, p.padlen = padtype == PAD_NONE ? 0 : padlen, p.zi_unit = 1;
   // forward over the extended row into the intermediate, from sosfilt_zi * ext[0]
   p.src = x, p.gain = gain, p.dst = w.mid, p.dst_mid = 1;
-  int r = pass_launch<true>(S, p, w.e, w.s, stream);
+  int r = pass_launch<EXTENDED>(S, p, w.e, w.s, stream);
   if (r != B2A_OK) return r;
   // backwards over the intermediate, from sosfilt_zi * its last sample, cropped into out
   p.src = w.mid, p.src_mid = 1, p.gain = nullptr, p.dst = out, p.dst_mid = 0, p.reverse = 1;
-  return pass_launch<true>(S, p, w.e, w.s, stream);
+  return pass_launch<EXTENDED>(S, p, w.e, w.s, stream);
 }
 
 extern "C" int b2a_sos_filtfilt_backward_f32(const float* grad_y, const float* gain, int64_t B, int C, int64_t T,
@@ -610,11 +656,11 @@ extern "C" int b2a_sos_filtfilt_backward_f32(const float* grad_y, const float* g
   p.padlen = padtype == PAD_NONE ? 0 : padlen;
   // H P^T g into the intermediate (the crop's adjoint pads with zeros), and r1 = G sum(g) - sum(H P^T g)
   p.src = grad_y, p.padtype = PAD_ZERO, p.dst = w.mid, p.dst_mid = 1, p.part = w.part_a;
-  int r = pass_launch<true>(S, p, w.e, w.s, stream);
+  int r = pass_launch<EXTENDED>(S, p, w.e, w.s, stream);
   if (r != B2A_OK) return r;
   // H^T (w + r1 e_last), in place, and r2 = G sum(w') - sum(H^T w')
   p.src = w.mid, p.src_mid = 1, p.reverse = 1, p.add_first = w.part_a, p.part = w.part_b;
-  r = pass_launch<true>(S, p, w.e, w.s, stream);
+  r = pass_launch<EXTENDED>(S, p, w.e, w.s, stream);
   if (r != B2A_OK) return r;
   // grad_x = gain E^T (f + r2 e_0)
   p.padtype = padtype, p.gain = gain;
@@ -624,3 +670,35 @@ extern "C" int b2a_sos_filtfilt_backward_f32(const float* grad_y, const float* g
   B2A_CUDA_OK(cudaGetLastError());
   return B2A_OK;
 }
+
+// ---- the loudness backward's two passes (iir_internal.h)
+namespace b2a {
+namespace iir {
+
+size_t loudness_adjoint_workspace_bytes(int64_t rows, int64_t Tp, int S) {
+  return (size_t)(2 * rows * iir_chunks(Tp) * 2 * S) * sizeof(double) + (size_t)(rows * Tp) * sizeof(float);
+}
+
+int loudness_adjoint(const float* x, const float* gain, int64_t B, int C, int64_t T, int64_t Tp, const float* sos,
+                     int S, const double* wt, const int* kept, int nblk, int blk_stride, int blk_len, float* grad_x,
+                     void* ws, void* stream) {
+  B2A_REQUIRE(S == 1 || S == 2, B2A_E_UNSUPPORTED, "lufs_backward: %d sections (1 or 2)", S);
+  Pass p = make_pass(B, C, T, 0, sos, 1);
+  p.Lmax = Tp, p.n_chunks = iir_chunks(Tp), p.work = B * C * ((p.n_chunks + 31) / 32);
+  p.kept = kept, p.nblk = nblk, p.blk_stride = blk_stride, p.blk_len = blk_len;
+  const int64_t states = B * C * p.n_chunks * 2 * S;
+  double* ws_e = static_cast<double*>(ws);
+  float* u = reinterpret_cast<float*>(ws_e + 2 * states);
+  // u = wt m K x over the zero-extended row, into the intermediate
+  p.src = x, p.gain = gain, p.dst = u, p.dst_mid = 1, p.wt = wt;
+  int r = S == 1 ? run_pass<1, LOUDNESS>(p, ws_e, ws_e + states, stream)
+                 : run_pass<2, LOUDNESS>(p, ws_e, ws_e + states, stream);
+  if (r != B2A_OK) return r;
+  // grad_x = the first T samples of K^T u
+  p.src = u, p.src_mid = 1, p.gain = nullptr, p.dst = grad_x, p.dst_mid = 0, p.reverse = 1, p.wt = nullptr;
+  return S == 1 ? run_pass<1, LOUDNESS>(p, ws_e, ws_e + states, stream)
+                : run_pass<2, LOUDNESS>(p, ws_e, ws_e + states, stream);
+}
+
+}  // namespace iir
+}  // namespace b2a

@@ -45,7 +45,11 @@
 // Kernel 3  loudness_stats_kernel        (one CTA per item; b2a_loudness_stats_f32 only)
 //   EBU R128 loudness range from the same interval bins: 3 s short-term loudness (30 strides), both gates, and the
 //   10 % / 95 % nearest-rank percentiles by radix selection -- no host synchronisation, no sort.
+// Kernel 4  lufs_grad_gate_kernel        (one CTA per item; b2a_lufs_backward_f32 only, K21 in DESIGN.md)
+//   the gate decisions of lufs_gate_kernel rebuilt from its z, through the same device functions, as a running count
+//   of the kept blocks and the weight of every row; the rest of the backward is two K-weighting passes of csrc/iir.cu.
 #include "b2a_common.h"
+#include "iir_internal.h"
 
 namespace b2a {
 namespace lufs {
@@ -549,6 +553,67 @@ struct GateParams {
   int C, nblk, nbins, q;
 };
 
+// l of block i: -0.691 + 10 log10(sum_c G_c z_c,i)
+__device__ __forceinline__ double block_loudness(const GateParams& gp, const float* z, int i) {
+  double acc = 0.0;
+  for (int c = 0; c < gp.C; ++c) acc += gp.G[c] * (double)z[c * gp.nblk + i];
+  return -0.691 + 10.0 * log10(acc);
+}
+
+constexpr double GAMMA_A = -70.0;
+
+// The gate decision of a block of loudness l under the relative gate Gamma_r.  The reference zeroes z where l <= Ga or
+// l <= Gr (a NaN l survives) and counts the blocks where l > Ga and l > Gr (a NaN l is not counted); the two agree on
+// every finite l.  lufs_gate_kernel and lufs_grad_gate_kernel both decide here.
+struct Verdict {
+  bool summed, counted;
+};
+__device__ __forceinline__ Verdict gate(double l, double Gamma_r) {
+  return {!((l <= GAMMA_A) || (l <= Gamma_r)), (l > GAMMA_A) && (l > Gamma_r)};
+}
+
+// Pass 1 of the gating, by the GT threads of one CTA: the absolute gate, then Gamma_r from the mean z of the blocks
+// above it (float32 sums, 0 / 0 -> NaN, as the reference).  mom (nullable) [nblk]: every block's l.  *n1t: the
+// blocks above the absolute gate.
+__device__ __forceinline__ double relative_gate(const GateParams& gp, const float* z, float* mom, double* sd, int* si,
+                                                int* n1t) {
+  const int C = gp.C, nblk = gp.nblk;
+  double sum1[8];
+  for (int c = 0; c < C; ++c) sum1[c] = 0.0;
+  int n1 = 0;
+  for (int i = threadIdx.x; i < nblk; i += GT) {
+    const double l = block_loudness(gp, z, i);
+    if (mom) mom[i] = (float)l;
+    // z[l <= Ga] = 0 (a NaN l is NOT zeroed), masked = l > Ga (a NaN l is NOT counted)
+    if (!(l <= GAMMA_A))
+      for (int c = 0; c < C; ++c) sum1[c] += (double)z[c * nblk + i];
+    if (l > GAMMA_A) n1++;
+  }
+  *n1t = block_sum<int>(n1, si);
+  double gr_acc = 0.0;
+  for (int c = 0; c < C; ++c) {
+    float zs = (float)block_sum<double>(sum1[c], sd);  // float32 sum in the reference
+    float zavg = zs / (float)*n1t;                     // 0/0 -> NaN as in the reference
+    gr_acc += (double)zavg * gp.G[c];
+  }
+  return -0.691 + 10.0 * log10(gr_acc) - 10.0;
+}
+
+// E = sum_c G_c zavg_c of the n2t blocks that passed both gates (sum2: this thread's per-channel sums of their z), with
+// the reference's NaN / inf scrubbing of zavg
+__device__ __forceinline__ double gated_energy(const GateParams& gp, const double (&sum2)[8], int n2t, double* sd) {
+  double lacc = 0.0;
+  for (int c = 0; c < gp.C; ++c) {
+    float zs = (float)block_sum<double>(sum2[c], sd);
+    float zavg = zs / (float)n2t;
+    if (zavg != zavg) zavg = 0.f;                              // nan -> 0          (:240-242)
+    if (zavg == INFINITY) zavg = 3.4028234663852886e38f;       // +inf -> f32 max   (:243)
+    if (zavg == -INFINITY) zavg = -3.4028234663852886e38f;     // -inf -> f32 min   (:244)
+    lacc += gp.G[c] * (double)zavg;
+  }
+  return lacc;
+}
+
 // gr_out (nullable) [B]: the relative gate Gamma_r, -inf when no block passes the absolute gate; mom_out (nullable)
 // [B, nblk]: the momentary loudness l of every block (loudness_stats)
 __global__ void __launch_bounds__(GT)
@@ -573,54 +638,22 @@ lufs_gate_kernel(const double* __restrict__ bins, GateParams gp, float* __restri
     if (z_out) z_out[(size_t)b * C * nblk + idx] = zf;
   }
   __syncthreads();
-  const double Gamma_a = -70.0;
   // pass 1: absolute gate
-  double sum1[8];
-  for (int c = 0; c < C; ++c) sum1[c] = 0.0;
-  int n1 = 0;
-  for (int i = tid; i < nblk; i += GT) {
-    double acc = 0.0;
-    for (int c = 0; c < C; ++c) acc += gp.G[c] * (double)z[c * nblk + i];
-    double l = -0.691 + 10.0 * log10(acc);
-    if (mom_out) mom_out[(size_t)b * nblk + i] = (float)l;
-    // z[l <= Ga] = 0 (a NaN l is NOT zeroed), masked = l > Ga (a NaN l is NOT counted)
-    if (!(l <= Gamma_a))
-      for (int c = 0; c < C; ++c) sum1[c] += (double)z[c * nblk + i];
-    if (l > Gamma_a) n1++;
-  }
-  int n1t = block_sum<int>(n1, si);
-  double gr_acc = 0.0;
-  for (int c = 0; c < C; ++c) {
-    float zs = (float)block_sum<double>(sum1[c], sd);  // float32 sum in the reference
-    float zavg = zs / (float)n1t;                      // 0/0 -> NaN as in the reference
-    gr_acc += (double)zavg * gp.G[c];
-  }
-  const double Gamma_r = -0.691 + 10.0 * log10(gr_acc) - 10.0;
+  int n1t;
+  const double Gamma_r = relative_gate(gp, z, mom_out ? mom_out + (size_t)b * nblk : nullptr, sd, si, &n1t);
   if (gr_out && tid == 0) gr_out[b] = n1t > 0 ? (float)Gamma_r : -INFINITY;  // 0 / 0 gives NaN above
   // pass 2: absolute + relative gate (comparisons with NaN are false, as in torch)
   double sum2[8];
   for (int c = 0; c < C; ++c) sum2[c] = 0.0;
   int n2 = 0;
   for (int i = tid; i < nblk; i += GT) {
-    double acc = 0.0;
-    for (int c = 0; c < C; ++c) acc += gp.G[c] * (double)z[c * nblk + i];
-    double l = -0.691 + 10.0 * log10(acc);
-    // z[l <= Ga] = 0; z[l <= Gr] = 0  ->  a block survives iff !(l <= Ga) && !(l <= Gr)
-    bool zeroed = (l <= Gamma_a) || (l <= Gamma_r);
-    if (!zeroed)
+    const Verdict v = gate(block_loudness(gp, z, i), Gamma_r);
+    if (v.summed)
       for (int c = 0; c < C; ++c) sum2[c] += (double)z[c * nblk + i];
-    if ((l > Gamma_a) && (l > Gamma_r)) n2++;
+    if (v.counted) n2++;
   }
   int n2t = block_sum<int>(n2, si);
-  double lacc = 0.0;
-  for (int c = 0; c < C; ++c) {
-    float zs = (float)block_sum<double>(sum2[c], sd);
-    float zavg = zs / (float)n2t;
-    if (zavg != zavg) zavg = 0.f;                              // nan -> 0          (:240-242)
-    if (zavg == INFINITY) zavg = 3.4028234663852886e38f;       // +inf -> f32 max   (:243)
-    if (zavg == -INFINITY) zavg = -3.4028234663852886e38f;     // -inf -> f32 min   (:244)
-    lacc += gp.G[c] * (double)zavg;
-  }
+  const double lacc = gated_energy(gp, sum2, n2t, sd);
   if (tid == 0) {
     float lufs = (float)(-0.691 + 10.0 * log10(lacc));
     lufs_out[b] = lufs;
@@ -631,6 +664,76 @@ lufs_gate_kernel(const double* __restrict__ bins, GateParams gp, float* __restri
       float gdb = db - loud;
       gain_out[b] = expf(gdb * 0.11512925464970229f);  // GAIN_FACTOR = ln(10)/20 (effects.py:12)
     }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// the gradient of loud = max(lufs, -70) (K21): the gates of lufs_gate_kernel, rebuilt from the z it wrote
+// ---------------------------------------------------------------------------------------------
+struct GradSos {  // the cascade as csrc/iir.cu reads it: [n / 6][b0 b1 b2 1 a1 a2] float32
+  float v[MAX_STAGES * 6];
+  int n;
+};
+
+// One CTA per item, on the z [C, nblk] that lufs_gate_kernel wrote for it (z_blocks):
+//   kept [B, nblk + 1]: kept[i] = the number of blocks among 0 .. i - 1 that passed both gates (J; the decisions are
+//        made by gate() on relative_gate()'s Gamma_r, the forward's own functions on the forward's own z);
+//   wt [B, C]: d loud / d y_c[t] = wt m[t] y_c[t], wt = grad_loud (10 / ln 10) G_c 2 scale gain / (E n), n = |J|;
+//        NaN for an item with a non-finite z (a NaN or inf sample), 0 for an item at or below -70 LUFS (clamped).
+// Block 0 also writes the cascade to sos_out.
+__global__ void __launch_bounds__(GT)
+lufs_grad_gate_kernel(const float* __restrict__ zb, const float* __restrict__ lufs,
+                      const float* __restrict__ grad_loud, const float* __restrict__ gain, GateParams gp, GradSos sos,
+                      float* __restrict__ sos_out, int* __restrict__ kept, double* __restrict__ wt) {
+  __shared__ double sd[GT];
+  __shared__ int si[GT];
+  const int b = blockIdx.x, C = gp.C, nblk = gp.nblk, tid = threadIdx.x;
+  if (b == 0 && tid < sos.n) sos_out[tid] = sos.v[tid];
+  const float* z = zb + (size_t)b * C * nblk;
+  int n1t;
+  const double Gamma_r = relative_gate(gp, z, nullptr, sd, si, &n1t);
+  int* kb = kept + (size_t)b * (nblk + 1);
+  double sum2[8];
+  for (int c = 0; c < C; ++c) sum2[c] = 0.0;
+  int n2 = 0, bad = 0;
+  for (int i = tid; i < nblk; i += GT) {
+    const Verdict v = gate(block_loudness(gp, z, i), Gamma_r);
+    if (v.summed)
+      for (int c = 0; c < C; ++c) sum2[c] += (double)z[c * nblk + i];
+    if (v.counted) n2++;
+    kb[i + 1] = v.counted ? 1 : 0;  // read back below by this same thread
+    for (int c = 0; c < C; ++c) bad |= !isfinite(z[c * nblk + i]);
+  }
+  const int n2t = block_sum<int>(n2, si);
+  const double E = gated_energy(gp, sum2, n2t, sd);
+  const int n_bad = block_sum<int>(bad, si);
+  // the flags -> their running count, GT blocks at a time (an inclusive scan in shared memory)
+  int carry = 0;
+  for (int i0 = 0; i0 < nblk; i0 += GT) {
+    const int i = i0 + tid;
+    __syncthreads();
+    si[tid] = i < nblk ? kb[i + 1] : 0;
+    __syncthreads();
+    for (int o = 1; o < GT; o <<= 1) {
+      const int t = tid >= o ? si[tid - o] : 0;
+      __syncthreads();
+      si[tid] += t;
+      __syncthreads();
+    }
+    if (i < nblk) kb[i + 1] = carry + si[tid];
+    carry += si[GT - 1];
+  }
+  if (tid == 0) kb[0] = 0;
+  if (tid < C) {
+    double w = 0.0;
+    if (n_bad > 0) {
+      w = (double)__int_as_float(0x7fffffff);  // NaN: the whole row's gradient
+    } else if (lufs[b] > -70.f) {
+      const double db_per_rel = 10.0 / 2.302585092994046;  // d(10 log10 E) / (dE / E)
+      w = (double)grad_loud[b] * db_per_rel * gp.G[tid] * 2.0 * (double)gp.scale * (gain ? (double)gain[b] : 1.0) /
+          (E * (double)n2t);
+    }
+    wt[(size_t)b * C + tid] = w;
   }
 }
 
@@ -905,6 +1008,21 @@ static StatsWs stats_ws_layout(int64_t B, int C, const Geometry& g, int64_t n_st
   return s;
 }
 
+// ---- the loudness backward: the iir passes' scratch, then wt [B, C] doubles, kept [B, nblk + 1] ints, the cascade
+struct GradWs {
+  size_t iir, wt, kept, sos, total;
+};
+static GradWs grad_ws_layout(int64_t B, int C, int64_t Tp, const Geometry& g) {
+  GradWs w;
+  size_t o = 0;
+  w.iir = o; o = align256(o + b2a::iir::loudness_adjoint_workspace_bytes(B * C, Tp, MAX_STAGES));
+  w.wt = o; o = align256(o + sizeof(double) * B * C);
+  w.kept = o; o = align256(o + sizeof(int) * B * (g.nblk + 1));
+  w.sos = o; o = align256(o + sizeof(float) * MAX_STAGES * 6);
+  w.total = o;
+  return w;
+}
+
 }  // namespace lufs
 }  // namespace b2a
 
@@ -941,6 +1059,53 @@ extern "C" int b2a_lufs_f32(const float* x, int64_t B, int C, int64_t T, int64_t
   if (re != B2A_OK) return re;
   return gate(B, C, g, rate, block_s, chan_gain_h, w, ws, z_blocks, lufs_out, loud_out, target_db, n_target, gain_out,
               nullptr, nullptr, stream);
+}
+
+extern "C" size_t b2a_lufs_backward_workspace_bytes(int64_t B, int C, int64_t T_padded, double rate, double block_s) {
+  Geometry g;
+  if (B < 1 || C < 1 || T_padded < 1 || geometry(T_padded, rate, block_s, &g) != 0) return 0;
+  return grad_ws_layout(B, C, T_padded, g).total;
+}
+
+extern "C" int b2a_lufs_backward_f32(const float* grad_loud, const float* x, const float* gain, int64_t B, int C,
+                                     int64_t T, int64_t T_padded, double rate, const double* sos_h,
+                                     const double* stage_gain_h, int n_stage, double block_s, const double* chan_gain_h,
+                                     const float* z_blocks, const float* lufs, float* grad_x, void* ws,
+                                     size_t ws_bytes, void* stream) {
+  B2A_REQUIRE(grad_loud && x && z_blocks && lufs && grad_x && ws && sos_h && stage_gain_h && chan_gain_h,
+              B2A_E_INVALID, "lufs_backward: null pointer");
+  int rc = check_input(B, C, T, T_padded, n_stage);
+  if (rc != B2A_OK) return rc;
+  Geometry g;
+  rc = check_geometry(T_padded, rate, block_s, &g);
+  if (rc != B2A_OK) return rc;
+  const GradWs w = grad_ws_layout(B, C, T_padded, g);
+  B2A_REQUIRE(ws_bytes >= w.total, B2A_E_INVALID, "lufs_backward: workspace too small (%zu < %zu)", ws_bytes,
+              w.total);
+  // the float32 coefficients of energy(), b with the stage gain folded in, a0 = 1
+  GradSos sos;
+  sos.n = 6 * n_stage;
+  for (int s = 0; s < n_stage; ++s) {
+    const double* c = sos_h + 6 * s;
+    B2A_REQUIRE(c[3] != 0.0, B2A_E_INVALID, "lufs_backward: a0 == 0 in stage %d", s);
+    const float a0 = (float)c[3], sg = (float)stage_gain_h[s];
+    float* r = sos.v + 6 * s;
+    r[0] = (float)c[0] / a0 * sg; r[1] = (float)c[1] / a0 * sg; r[2] = (float)c[2] / a0 * sg;
+    r[3] = 1.f; r[4] = (float)c[4] / a0; r[5] = (float)c[5] / a0;
+  }
+  GateParams gp;
+  for (int c = 0; c < 8; ++c) gp.G[c] = c < C ? chan_gain_h[c] : 0.0;
+  gp.scale = (float)(1.0 / (block_s * rate));
+  gp.C = C; gp.nblk = g.nblk; gp.nbins = g.nbins; gp.q = g.q;
+  char* base = (char*)ws;
+  float* sos_d = (float*)(base + w.sos);
+  int* kept = (int*)(base + w.kept);
+  double* wt = (double*)(base + w.wt);
+  B2A_LAUNCH(lufs_grad_gate_kernel, dim3((unsigned)B), dim3(GT), 0, stream, z_blocks, lufs, grad_loud, gain, gp, sos,
+             sos_d, kept, wt);
+  B2A_CUDA_OK(cudaGetLastError());
+  return b2a::iir::loudness_adjoint(x, gain, B, C, T, T_padded, sos_d, n_stage, wt, kept, g.nblk, g.stride, g.K, grad_x,
+                                    base + w.iir, stream);
 }
 
 extern "C" int64_t b2a_loudness_stats_num_short_term(int64_t T_padded, double rate) {

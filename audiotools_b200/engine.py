@@ -38,7 +38,8 @@ class Engine:
                       "ensure_max_of_audio, mix, quantization, mulaw_quantization, sos_filter, parametric_eq, core.iir.sosfiltfilt (gradients to "
                       "audio_data); "
                       "mask_frequencies, mask_timesteps, mask_low_magnitudes, ml.layers.SpectralGate (gradients to "
-                      "stft_data / the gated signal)")
+                      "stft_data / the gated signal); metrics.STOILoss, metrics.LoudnessLoss (gradients to the "
+                      "estimates)")
 
     @classmethod
     def _refuse_grad(cls, t: torch.Tensor, name: str):
@@ -528,6 +529,42 @@ class Engine:
                    _dptr(lufs), _dptr(loud), _dptr(target_db), n_target, _dptr(gain), _dptr(ws), ws_bytes,
                    self._stream(x))
         return {"lufs": lufs, "loud": loud, "gain": gain, "blocks": blocks}
+
+    def lufs_backward(self, grad_loud: torch.Tensor, x: torch.Tensor, sample_rate: float, blocks: torch.Tensor,
+                      lufs: torch.Tensor, padded_length: Optional[int] = None, gain: Optional[torch.Tensor] = None,
+                      block_size: float = 0.400) -> torch.Tensor:
+        """dL/dx [B, C, T] float32 of ``loud`` = max(lufs, -70) that :meth:`lufs` returned for ``x`` (times ``gain``
+        [B] when given: the forward measured float32(gain x)), from that call's ``blocks`` and ``lufs`` and dL/dloud
+        ``grad_loud`` [B] (``b2a_lufs_backward_f32``, DESIGN.md K21).  The gate decisions are the forward's.  Items
+        clamped at -70 get zeros, items with a NaN or inf sample NaN.  K-weighting only; seven launches, no host
+        sync."""
+        x = self._prep(x, "x")
+        assert x.ndim == 3, "x must be [B, C, T]"
+        B, C, T = x.shape
+        if C > len(kweighting.CHANNEL_GAINS):
+            raise ValueError(f"loudness supports at most 5 channels, got {C}")
+        Tp = T if padded_length is None else int(padded_length)
+        g = self._prep(grad_loud.reshape(-1), "grad_loud")
+        assert g.numel() == B, (g.numel(), B)
+        if gain is not None:
+            gain = self._prep(gain.reshape(-1), "gain")
+            assert gain.numel() == B
+        blocks, lufs = self._prep(blocks, "blocks"), self._prep(lufs.reshape(-1), "lufs")
+        sos, sgain = kweighting.design(float(sample_rate))
+        G = np.ascontiguousarray(kweighting.CHANNEL_GAINS[:C], dtype=np.float64)
+        L = self.lib
+        nblk = L.b2a_lufs_num_blocks(Tp, float(sample_rate), float(block_size))
+        assert blocks.shape == (B, C, nblk) and lufs.numel() == B, (tuple(blocks.shape), (B, C, nblk))
+        ws_bytes = int(L.b2a_lufs_backward_workspace_bytes(B, C, Tp, float(sample_rate), float(block_size)))
+        if ws_bytes == 0:
+            raise _lib.B2AError(f"lufs_backward: unsupported geometry (T={Tp}, rate={sample_rate}, block={block_size})")
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        gx = torch.empty_like(x)
+        dp = ctypes.POINTER(ctypes.c_double)
+        self._call(L.b2a_lufs_backward_f32, _dptr(g), _dptr(x), _dptr(gain), B, C, T, Tp, float(sample_rate),
+                   sos.ctypes.data_as(dp), sgain.ctypes.data_as(dp), sos.shape[0], float(block_size),
+                   G.ctypes.data_as(dp), _dptr(blocks), _dptr(lufs), _dptr(gx), _dptr(ws), ws_bytes, self._stream(x))
+        return gx
 
     LOUDNESS_STATS = ("I", "I Threshold", "LRA", "LRA Threshold", "LRA Low", "LRA High")
 

@@ -291,6 +291,28 @@ int b2a_lufs_f32(const float* x, int64_t B, int C, int64_t T, int64_t T_padded, 
                  const float* target_db, int n_target, float* gain_out,
                  void* ws, size_t ws_bytes, void* stream);
 
+/* ---- gradient of the integrated loudness (K21) -------------------------------------------
+ * grad_x [B, C, T] float32 = grad_loud[b] d loud_b / d x, loud = max(lufs, -70) of b2a_lufs_f32, for the same
+ * x [B, C, T], T_padded, rate, sos_h, stage_gain_h, n_stage, block_s and chan_gain_h as that call:
+ *   d loud / d x_c = K^T u_c,  u_c[t] = (10 / ln 10) G_c scale gain / (E n) * 2 y_c[t] * m[t]
+ * y_c = K x_c on the row zero-extended to T_padded (K: the cascade, float32 coefficients as b2a_lufs_f32 rounds them),
+ * scale = float32(1 / (block_s rate)), J the blocks that passed both gates, n = |J|, E = sum_c G_c zavg_c, m[t] the
+ * number of blocks of J that contain t, K^T the cascade run backwards in time over [0, T_padded), cropped to [0, T).
+ *   grad_loud [B] float32 on the device.
+ *   gain nullable [B]: the forward measured float32(gain[b] x) (a deferred normalize() gain); grad_x is then with
+ *        respect to x.
+ *   z_blocks [B, C, nblk], lufs [B]: the z_blocks and lufs_out of the forward call.  The gate decisions are rebuilt
+ *        from them by the forward's own functions; they are constants of the backward (piecewise-constant).
+ *   An item with lufs <= -70 gets an exactly zero row; an item with a non-finite block energy (a NaN or inf sample)
+ *   gets an all-NaN row.  Other items are unaffected; reruns and batch-versus-single calls are bit-identical.
+ *   ws: b2a_lufs_backward_workspace_bytes(B, C, T_padded, rate, block_s) bytes of scratch.
+ * Seven launches (one per-item gate kernel, two three-launch passes of csrc/iir.cu), no host sync. */
+size_t b2a_lufs_backward_workspace_bytes(int64_t B, int C, int64_t T_padded, double rate, double block_s);
+int b2a_lufs_backward_f32(const float* grad_loud, const float* x, const float* gain, int64_t B, int C, int64_t T,
+                          int64_t T_padded, double rate, const double* sos_h, const double* stage_gain_h,
+                          int n_stage, double block_s, const double* chan_gain_h, const float* z_blocks,
+                          const float* lufs, float* grad_x, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- EBU R128 loudness statistics ------------------------------------------------------
  * The six numbers of audiotools/core/ffmpeg.py:13-62 (r128stats) for every item, in one
  * K-weighting pass of the GPU instead of one ffmpeg process per item.  BS.1770 arithmetic of
