@@ -104,14 +104,14 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
 
     ``diffuse_after`` (seconds > 0, scalar or [B]) and ``seed`` (an int or [B] ints in [0, 2^63)) add the diffuse tail
     (module docstring; DESIGN.md K20 "Hybrid"): two kernel launches before the high-pass.  It needs ``max_order =
-    -1`` (the tail stands for images of every order); ``None`` leaves the images-only path untouched.
+    -1`` (the tail stands for images of every order).
 
     ``bands=K`` (1 .. 8) makes the walls, and with ``air_absorption`` the air, frequency-dependent over K octave bands
     centred on 125 2^k Hz (module docstring; DESIGN.md K20 "Bands"): ``beta`` is then [6, K] or [B, 6, K], ``rt60``
     [K] or [B, K] (``sabine_beta`` per band) and ``air_absorption`` (dB/m, finite, >= 0) [K] or [B, K].  Bands whose
     lower crossover is at or above sample_rate / 2 are checked but not computed.  One launch (two with the tail), the
     crossovers' ``fftconv`` and one launch for their sum when more than one band is computed, then the high-pass.
-    ``bands=None`` leaves the frequency-flat paths untouched."""
+    ``bands=None`` is the frequency-flat room, computed as one band."""
     from ..engine import get_engine
     from .audio_signal import AudioSignal
 
@@ -136,7 +136,7 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
         if isinstance(bands, bool) or not isinstance(bands, (int, np.integer)) or not 1 <= bands <= MAX_BANDS:
             raise ValueError(f"image_source_ir: bands = {bands!r}; an int in 1 .. {MAX_BANDS} (octaves from 125 Hz)")
         bands = int(bands)
-        air_h = None if air_absorption is None else _host("air_absorption", air_absorption)
+    air_h = None if air_absorption is None else _host("air_absorption", air_absorption)
     if diffuse_after is None and seed is not None:
         raise ValueError("image_source_ir: seed is for the diffuse tail; give diffuse_after too")
     if diffuse_after is not None:
@@ -205,19 +205,18 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
                              sound_speed)
     if not (np.all(beta_h >= 0) and np.all(beta_h <= 1)):
         raise ValueError("image_source_ir: every reflection coefficient beta must be in [0, 1]")
+    if bands is None:
+        beta_h = beta_h[..., None]  # a frequency-flat room is one band: [B, 6, 1]
     dev = torch.device(device)
-    tab = [torch.from_numpy(np.array(a, dtype=np.float64)).to(dev, non_blocking=True)
-           for a in (room_h, src_h, mics_h, beta_h)]
+
+    def upload(a, dtype=np.float64):
+        return None if a is None else torch.from_numpy(np.array(a, dtype=dtype)).to(dev, non_blocking=True)
+
+    tab = [upload(a) for a in (room_h, src_h, mics_h, beta_h)]
     tail = {}
     if diffuse_after is not None:
-        td_h = _batch("diffuse_after", td_h, 0, B)
-        sd = _batch("seed", sd, 0, B)
-        tail = dict(diffuse_after=torch.from_numpy(np.array(td_h, dtype=np.float64)).to(dev, non_blocking=True),
-                    seed=torch.from_numpy(np.array(sd, dtype=np.int64)).to(dev, non_blocking=True))
-    if bands is None:
-        ir = get_engine().image_source_ir(*tab, length, sample_rate, sound_speed, max_order, high_pass, **tail)
-    else:
-        air = None if air_h is None else torch.from_numpy(np.array(air_h, dtype=np.float64)).to(dev, non_blocking=True)
-        ir = get_engine().image_source_ir_bands(*tab, length, sample_rate, sound_speed, max_order, high_pass, air=air,
-                                                **tail)
+        tail = dict(diffuse_after=upload(_batch("diffuse_after", td_h, 0, B)),
+                    seed=upload(_batch("seed", sd, 0, B), np.int64))
+    ir = get_engine().image_source_ir(*tab, length, sample_rate, sound_speed, max_order, high_pass,
+                                      air=upload(air_h), **tail)
     return AudioSignal(ir, sample_rate)

@@ -25,7 +25,7 @@
 // once per sample at the end.  A sample's sum depends only on its row's geometry and the tile size: reruns and a batch
 // against its items one at a time are bit-identical.
 //
-// Hybrid (b2a_rir_hybrid_f32): the image sources for the early part only, a statistical tail after it.  With n_d =
+// Hybrid (t_d and seed given): the image sources for the early part only, a statistical tail after it.  With n_d =
 // ceil(t_d fs), ism_kernel keeps the images with floor(d) < min(L, n_d); tail_kernel then adds, at every sample
 // n >= n_d - Tw/2, w(n) sqrt(E(n)) xi(seed, c, n):
 //   E(n) = c / (4 pi V fs) (1/4pi) int exp(-n sum_a lambda_a |u_a|) dOmega(u),  lambda_a = -(ln b_a0 + ln b_a1) / L_a
@@ -37,7 +37,7 @@
 // interpolated between nodes by a cubic Hermite (relative error below 1e-5: (ln E)'''' falls off like 12 / n^4).  Each
 // CTA evaluates the nodes its tile spans, so the tail too depends only on its row's geometry, seed and microphone.
 //
-// Bands (b2a_rir_bands_f32): K octave bands with their own beta [B, 6, K] and air absorption [B, K] (dB/m).  The
+// Bands (K > 1): K octave bands with their own beta [B, 6, K] and air absorption [B, K] (dB/m).  The
 // first K' bands (lower crossover below fs / 2) are computed in one pass: ism_tile<K'> enumerates each tile's images
 // once and keeps K' compensated sums per sample, and the rows it writes are r_k - r_{k+1} (k < K' - 1) and r_{K'-1};
 // tail_kernel adds each band's tail the same way.  The crossovers (Engine.fftconv) and band_sum_kernel then form
@@ -445,53 +445,12 @@ __global__ void __launch_bounds__(256) band_sum_kernel(const Geo g, int half, co
 
 using namespace b2a::rir;
 
-static int check(const char* fn, const double* room, const double* src, const double* mics, const double* beta,
-                 int64_t B, int C, int64_t L, double fs, double c, float* out) {
-  B2A_REQUIRE(room && src && mics && beta && out, B2A_E_INVALID, "%s: null pointer", fn);
-  B2A_REQUIRE(B >= 1 && C >= 1 && L >= 1, B2A_E_INVALID, "%s: bad shape B=%lld C=%d L=%lld", fn, (long long)B, C,
-              (long long)L);
-  B2A_REQUIRE(B * C <= 65535, B2A_E_INVALID, "%s: %lld rows (items x microphones); at most 65535 per call", fn,
-              (long long)(B * C));
-  B2A_REQUIRE(L <= (1 << 30), B2A_E_INVALID, "%s: L=%lld; at most 2^30 samples", fn, (long long)L);
-  B2A_REQUIRE(fs >= 125.0 && fs <= 384000.0, B2A_E_INVALID, "%s: fs=%g; 125 .. 384000 Hz are supported", fn, fs);
-  B2A_REQUIRE(c > 0.0 && c < 1e30, B2A_E_INVALID, "%s: sound speed %g must be positive and finite", fn, c);
-  return B2A_OK;
-}
-
 static Geo geo(const double* room, const double* src, const double* mics, const double* beta, int C, int64_t L,
                double fs, double c, int max_order, float* out) {
   Geo g;
   g.room = room, g.src = src, g.mics = mics, g.beta = beta, g.td = nullptr, g.seed = nullptr, g.air = nullptr;
   g.C = C, g.L = (int)L, g.K = 1, g.KB = 1, g.max_order = max_order, g.Tw = 2 * (int)floor(0.004 * fs + 0.5), g.fs = fs, g.c = c, g.out = out;
   return g;
-}
-
-extern "C" int b2a_rir_ism_f32(const double* room, const double* src, const double* mics, const double* beta, int64_t B,
-                               int C, int64_t L, double fs, double c, int max_order, float* out, void* stream) {
-  const int rc = check("rir_ism", room, src, mics, beta, B, C, L, fs, c, out);
-  if (rc != B2A_OK) return rc;
-  B2A_REQUIRE(max_order >= -1, B2A_E_INVALID, "rir_ism: max_order=%d must be >= -1", max_order);
-  const Geo g = geo(room, src, mics, beta, C, L, fs, c, max_order, out);
-  const dim3 grid((unsigned)((L + TT - 1) / TT), (unsigned)(B * C));
-  B2A_LAUNCH(ism_kernel, grid, dim3(NT), 0, stream, g);
-  B2A_CUDA_OK(cudaGetLastError());
-  return B2A_OK;
-}
-
-extern "C" int b2a_rir_hybrid_f32(const double* room, const double* src, const double* mics, const double* beta,
-                                  const double* t_d, const uint64_t* seed, int64_t B, int C, int64_t L, double fs,
-                                  double c, float* out, void* stream) {
-  const int rc = check("rir_hybrid", room, src, mics, beta, B, C, L, fs, c, out);
-  if (rc != B2A_OK) return rc;
-  B2A_REQUIRE(t_d && seed, B2A_E_INVALID, "rir_hybrid: null pointer");
-  Geo g = geo(room, src, mics, beta, C, L, fs, c, -1, out);
-  g.td = t_d, g.seed = seed;
-  const dim3 grid((unsigned)((L + TT - 1) / TT), (unsigned)(B * C));
-  B2A_LAUNCH(ism_kernel, grid, dim3(NT), 0, stream, g);
-  B2A_CUDA_OK(cudaGetLastError());
-  B2A_LAUNCH(tail_kernel, grid, dim3(NT), 0, stream, g);
-  B2A_CUDA_OK(cudaGetLastError());
-  return B2A_OK;
 }
 
 // Bands whose lower crossover 125 2^(k - 1/2) Hz is below fs / 2 (band 0 always)
@@ -511,17 +470,21 @@ extern "C" int b2a_rir_bands_kept(int K, double fs) {
   return bands_kept(K, fs);
 }
 
-extern "C" int b2a_rir_bands_f32(const double* room, const double* src, const double* mics, const double* beta,
-                                 const double* air, const double* t_d, const uint64_t* seed, int64_t B, int C, int K,
-                                 int64_t L, double fs, double c, int max_order, float* out, void* stream) {
-  const int rc = check("rir_bands", room, src, mics, beta, B, C, L, fs, c, out);
-  if (rc != B2A_OK) return rc;
-  B2A_REQUIRE(K >= 1 && K <= MAX_BANDS, B2A_E_INVALID, "rir_bands: K=%d bands; 1 .. %d are supported", K, MAX_BANDS);
-  B2A_REQUIRE(B * C * K <= 65535, B2A_E_INVALID, "rir_bands: %lld rows (items x microphones x bands); at most 65535",
+extern "C" int b2a_rir_f32(const double* room, const double* src, const double* mics, const double* beta,
+                           const double* air, const double* t_d, const uint64_t* seed, int64_t B, int C, int K,
+                           int64_t L, double fs, double c, int max_order, float* out, void* stream) {
+  B2A_REQUIRE(room && src && mics && beta && out, B2A_E_INVALID, "rir: null pointer");
+  B2A_REQUIRE(B >= 1 && C >= 1 && L >= 1, B2A_E_INVALID, "rir: bad shape B=%lld C=%d L=%lld", (long long)B, C,
+              (long long)L);
+  B2A_REQUIRE(K >= 1 && K <= MAX_BANDS, B2A_E_INVALID, "rir: K=%d bands; 1 .. %d are supported", K, MAX_BANDS);
+  B2A_REQUIRE(B * C * K <= 65535, B2A_E_INVALID, "rir: %lld rows (items x microphones x bands); at most 65535",
               (long long)(B * C * K));
-  B2A_REQUIRE(max_order >= -1, B2A_E_INVALID, "rir_bands: max_order=%d must be >= -1", max_order);
-  B2A_REQUIRE(!t_d == !seed, B2A_E_INVALID, "rir_bands: a diffuse tail needs both t_d and seed");
-  B2A_REQUIRE(!t_d || max_order == -1, B2A_E_INVALID, "rir_bands: max_order=%d with a diffuse tail", max_order);
+  B2A_REQUIRE(L <= (1 << 30), B2A_E_INVALID, "rir: L=%lld; at most 2^30 samples", (long long)L);
+  B2A_REQUIRE(fs >= 125.0 && fs <= 384000.0, B2A_E_INVALID, "rir: fs=%g; 125 .. 384000 Hz are supported", fs);
+  B2A_REQUIRE(c > 0.0 && c < 1e30, B2A_E_INVALID, "rir: sound speed %g must be positive and finite", c);
+  B2A_REQUIRE(max_order >= -1, B2A_E_INVALID, "rir: max_order=%d must be >= -1", max_order);
+  B2A_REQUIRE(!t_d == !seed, B2A_E_INVALID, "rir: a diffuse tail needs both t_d and seed");
+  B2A_REQUIRE(!t_d || max_order == -1, B2A_E_INVALID, "rir: max_order=%d with a diffuse tail", max_order);
   Geo g = geo(room, src, mics, beta, C, L, fs, c, max_order, out);
   g.air = air, g.td = t_d, g.seed = seed, g.K = K, g.KB = bands_kept(K, fs);
   const dim3 grid((unsigned)((L + TT - 1) / TT), (unsigned)(B * C));

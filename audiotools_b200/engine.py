@@ -17,6 +17,7 @@ import torch
 
 from . import _lib
 from .core import kweighting
+from .core import room as _room
 
 
 def _dptr(t: Optional[torch.Tensor]):
@@ -805,61 +806,18 @@ class Engine:
                    sos.shape[1], pt, pl, _dptr(gx), _dptr(ws), self._stream(g))
         return gx
 
-    RIR_MAX_ROWS = 65535  # items x microphones of one b2a_rir_ism_f32 launch (grid y)
-
-    def image_source_ir(self, room: torch.Tensor, src: torch.Tensor, mics: torch.Tensor, beta: torch.Tensor,
-                        length: int, sample_rate: float, sound_speed: float = 343.0, max_order: int = -1,
-                        high_pass: bool = True, diffuse_after: Optional[torch.Tensor] = None,
-                        seed: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Shoebox-room impulse responses by the image-source method (``b2a_rir_ism_f32``, DESIGN.md K20) -> [B, C,
-        length] float32.  room [B, 3], src [B, 3], mics [B, C, 3] (metres) and beta [B, 6] are float64 tensors on the
-        device, already checked (``core.room.image_source_ir``).  ``high_pass`` applies Allen & Berkley's 100 Hz
-        high-pass as one second-order section through ``sos_filter``.  One launch, three more with the high-pass.
-
-        ``diffuse_after`` (float64 [B], seconds > 0) with ``seed`` (int64 [B], >= 0) keeps the images arriving before
-        ceil(diffuse_after sample_rate) only and adds a diffuse tail after them (``b2a_rir_hybrid_f32``): two launches,
-        then the high-pass.  ``max_order`` must be -1 then."""
-        if mics.ndim != 3 or mics.shape[-1] != 3:
-            raise ValueError(f"image_source_ir: mics must be [B, C, 3], got {tuple(mics.shape)}")
-        B, C = mics.shape[:2]
-        if tuple(room.shape) != (B, 3) or tuple(src.shape) != (B, 3) or tuple(beta.shape) != (B, 6):
-            raise ValueError(f"image_source_ir: room / source / beta must be [{B}, 3] / [{B}, 3] / [{B}, 6], got "
-                             f"{tuple(room.shape)} / {tuple(src.shape)} / {tuple(beta.shape)}")
-        if B * C > self.RIR_MAX_ROWS:
-            raise ValueError(f"image_source_ir: {B * C} rows (items x microphones); at most {self.RIR_MAX_ROWS}")
-        room, src, mics, beta = (self._prep(t, n, torch.float64) for t, n in
-                                 ((room, "room"), (src, "source"), (mics, "mics"), (beta, "beta")))
-        out = torch.empty(B, C, int(length), dtype=torch.float32, device=room.device)
-        if diffuse_after is None:
-            self._call(self.lib.b2a_rir_ism_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), B, C, int(length),
-                       float(sample_rate), float(sound_speed), int(max_order), _dptr(out), self._stream(room))
-        else:
-            if max_order != -1:
-                raise ValueError(f"image_source_ir: max_order = {max_order} with a diffuse tail; the tail has every "
-                                 "order")
-            if seed is None or tuple(diffuse_after.shape) != (B,) or tuple(seed.shape) != (B,):
-                raise ValueError(f"image_source_ir: diffuse_after and seed must be [{B}]")
-            td = self._prep(diffuse_after, "diffuse_after", torch.float64)
-            sd = self._prep(seed, "seed", torch.int64)
-            self._call(self.lib.b2a_rir_hybrid_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), _dptr(td),
-                       _dptr(sd), B, C, int(length), float(sample_rate), float(sound_speed), _dptr(out),
-                       self._stream(room))
-        return self._rir_high_pass(out, sample_rate) if high_pass else out
-
     def _rir_high_pass(self, out: torch.Tensor, sample_rate: float) -> torch.Tensor:
         """Allen & Berkley's 100 Hz high-pass, one second-order section, in place (three launches)."""
         w = 2 * math.pi * 100.0 / sample_rate
         r = math.exp(-w)
         return self.sos_filter(out, [[1.0, -(1.0 + r), r, 1.0, -2.0 * r * math.cos(w), r * r]], out=out)
 
-    RIR_MAX_BANDS = 8  # octave bands centred on 125 2^k Hz, k < 8
-
     def rir_bands_kept(self, n_bands: int, sample_rate: float) -> int:
-        """The octave bands of ``image_source_ir_bands`` that are computed: those whose lower crossover 125 2^(k - 1/2)
-        Hz is below sample_rate / 2 (``b2a_rir_bands_kept``)."""
+        """The octave bands of ``image_source_ir`` that are computed: those whose lower crossover 125 2^(k - 1/2) Hz is
+        below sample_rate / 2 (``b2a_rir_bands_kept``)."""
         kept = self.lib.b2a_rir_bands_kept(int(n_bands), float(sample_rate))
         if kept < 1:
-            raise ValueError(f"image_source_ir: bands = {n_bands}; 1 .. {self.RIR_MAX_BANDS} are supported")
+            raise ValueError(f"image_source_ir: bands = {n_bands}; 1 .. {_room.MAX_BANDS} are supported")
         return kept
 
     def octave_crossovers(self, sample_rate: float, n_bands: int, device):
@@ -879,18 +837,25 @@ class Engine:
             hit = self._crossovers[key] = (torch.flip(lp, dims=[1]).contiguous(), half)
         return hit
 
-    def image_source_ir_bands(self, room: torch.Tensor, src: torch.Tensor, mics: torch.Tensor, beta: torch.Tensor,
-                              length: int, sample_rate: float, sound_speed: float = 343.0, max_order: int = -1,
-                              high_pass: bool = True, air: Optional[torch.Tensor] = None,
-                              diffuse_after: Optional[torch.Tensor] = None,
-                              seed: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Octave-band shoebox-room impulse responses (DESIGN.md K20 "Bands") -> [B, C, length] float32.  beta [B, 6,
-        K] per wall and band, ``air`` [B, K] dB/m or None, the rest as ``image_source_ir``; everything already checked
-        (``core.room.image_source_ir``).  ``b2a_rir_bands_f32`` writes the K' kept bands' differences r_k - r_{k+1} and
-        the last band r_{K'-1}; the differences go through the zero-phase crossovers LP_k (``fftconv``, zero padding)
-        and ``b2a_rir_band_sum_f32`` adds them to the last band: y = r_{K'-1} + sum_k LP_k * (r_k - r_{k+1}), exactly
-        0 before the first sample the direct path (or the tail) reaches through the crossovers.  With K' = 1 nothing
-        is filtered.  No host sync."""
+    def image_source_ir(self, room: torch.Tensor, src: torch.Tensor, mics: torch.Tensor, beta: torch.Tensor,
+                        length: int, sample_rate: float, sound_speed: float = 343.0, max_order: int = -1,
+                        high_pass: bool = True, air: Optional[torch.Tensor] = None,
+                        diffuse_after: Optional[torch.Tensor] = None,
+                        seed: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Shoebox-room impulse responses by the image-source method (``b2a_rir_f32``, DESIGN.md K20) -> [B, C, length]
+        float32.  room [B, 3], src [B, 3], mics [B, C, 3] (metres), beta [B, 6, K] per wall and octave band (K = 1: a
+        frequency-flat room) and ``air`` [B, K] dB/m or None are float64 tensors on the device, already checked
+        (``core.room.image_source_ir``).  ``high_pass`` applies Allen & Berkley's 100 Hz high-pass as one second-order
+        section through ``sos_filter`` (three launches).  No host sync.
+
+        ``diffuse_after`` (float64 [B], seconds > 0) with ``seed`` (int64 [B], >= 0) keeps the images arriving before
+        ceil(diffuse_after sample_rate) only and adds a diffuse tail after them; ``max_order`` must be -1 then.  One
+        launch, two with the tail.
+
+        ``b2a_rir_f32`` writes the K' kept bands' differences r_k - r_{k+1} and the last band r_{K'-1}; when K' > 1 the
+        differences go through the zero-phase crossovers LP_k (``fftconv``, zero padding) and ``b2a_rir_band_sum_f32``
+        adds them to the last band: y = r_{K'-1} + sum_k LP_k * (r_k - r_{k+1}), exactly 0 before the first sample the
+        direct path (or the tail) reaches through the crossovers."""
         if mics.ndim != 3 or mics.shape[-1] != 3:
             raise ValueError(f"image_source_ir: mics must be [B, C, 3], got {tuple(mics.shape)}")
         B, C = mics.shape[:2]
@@ -900,10 +865,10 @@ class Engine:
             raise ValueError(f"image_source_ir: room / source / beta / air must be [{B}, 3] / [{B}, 3] / [{B}, 6, K] "
                              f"/ [{B}, K], got {tuple(room.shape)} / {tuple(src.shape)} / {tuple(beta.shape)} / "
                              f"{None if air is None else tuple(air.shape)}")
-        kept = self.rir_bands_kept(K, sample_rate)
-        if B * C * K > self.RIR_MAX_ROWS:
-            raise ValueError(f"image_source_ir: {B * C * K} rows (items x microphones x bands); at most "
-                             f"{self.RIR_MAX_ROWS}")
+        kept = 1 if K == 1 else self.rir_bands_kept(K, sample_rate)
+        if B * C * K > _room.MAX_ROWS:
+            raise ValueError(f"image_source_ir: {B * C * K} rows (items x microphones{' x bands' if K > 1 else ''}); "
+                             f"at most {_room.MAX_ROWS}")
         if (diffuse_after is None) != (seed is None):
             raise ValueError("image_source_ir: diffuse_after and seed go together")
         if diffuse_after is not None:
@@ -919,7 +884,7 @@ class Engine:
         sd = None if seed is None else self._prep(seed, "seed", torch.int64)
         L = int(length)
         bands = torch.empty(kept, B, C, L, dtype=torch.float32, device=room.device)
-        self._call(self.lib.b2a_rir_bands_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), _dptr(air), _dptr(td),
+        self._call(self.lib.b2a_rir_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), _dptr(air), _dptr(td),
                    _dptr(sd), B, C, K, L, float(sample_rate), float(sound_speed), int(max_order), _dptr(bands),
                    self._stream(room))
         if kept == 1:

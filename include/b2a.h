@@ -409,43 +409,38 @@ int b2a_sos_filtfilt_backward_f32(const float* grad_y, const float* gain, int64_
                                   float* grad_x, void* ws, void* stream);
 
 /* ---- shoebox-room impulse responses by the image-source method (csrc/rir.cu) ----------------------------------------
- * out [B, C, L] float32: the impulse response from item b's source to its microphone c (DESIGN.md K20).  Geometry is
- * float64 on the device: room [B, 3] (Lx, Ly, Lz, metres), src [B, 3], mics [B, C, 3], beta [B, 6] (reflection
- * coefficients of the walls x = 0, x = Lx, y = 0, y = Ly, z = 0, z = Lz).  fs in [125, 384000] Hz, c > 0 m/s;
- * max_order >= 0 keeps images of at most that order, -1 keeps every image that reaches the first L samples.  Each image
- * adds g h(i - d) at the Tw = 2 floor(0.004 fs + 1/2) samples around its distance d (samples), h a Hann-windowed
- * sinc.  B C <= 65535, L <= 2^30; the arguments are not checked against each other (positions inside the room, beta in
- * [0, 1]): core/room.py does that.  One launch, no host sync, no atomics: reruns and a batch against its items one at a
- * time are bit-identical. */
-int b2a_rir_ism_f32(const double* room, const double* src, const double* mics, const double* beta, int64_t B, int C,
-                    int64_t L, double fs, double c, int max_order, float* out, void* stream);
-
-/* The same impulse responses with a diffuse late tail (DESIGN.md K20, "Hybrid"): the images with floor(d) <
- * min(L, n_d), n_d = ceil(t_d[b] fs), t_d [B] float64 seconds > 0 on the device; then, at every sample n >= n_d - Tw/2,
- * w(n) sqrt(E_b(n)) xi(seed[b], c, n) is added: E_b the expected energy per sample of the image arrivals of item b's
- * room, w a raised-cosine ramp over the Tw samples centred on n_d, xi a standard normal from a stateless counter-based
- * generator (SplitMix64, Box-Muller).  seed [B] uint64 on the device.  Every image order is kept.  Two launches, no
- * host sync, no atomics; a batch equals its items one at a time, bit for bit. */
-int b2a_rir_hybrid_f32(const double* room, const double* src, const double* mics, const double* beta,
-                       const double* t_d, const uint64_t* seed, int64_t B, int C, int64_t L, double fs, double c,
-                       float* out, void* stream);
-
-/* Octave-band responses (DESIGN.md K20, "Bands"): band k (centre 125 2^k Hz) of item b uses the reflection
- * coefficients beta[b, :, k] (beta [B, 6, K] float64) and, when air [B, K] (dB/m, float64) is given, every image is
- * also scaled by 10^(-air[b, k] d / 20) (d in metres) and the tail's envelope by 10^(-air[b, k] (c n / fs) / 10).
- * t_d and seed as in b2a_rir_hybrid_f32, both null for images only (then max_order >= -1; with a tail it must be -1).
+ * The impulse responses from item b's source to its microphone c (DESIGN.md K20), in K octave bands; K = 1 is the
+ * frequency-flat room.  Geometry is float64 on the device: room [B, 3] (Lx, Ly, Lz, metres), src [B, 3],
+ * mics [B, C, 3], beta [B, 6, K] (reflection coefficients of the walls x = 0, x = Lx, y = 0, y = Ly, z = 0, z = Lz;
+ * band k, centred on 125 2^k Hz, uses beta[b, :, k]).  fs in [125, 384000] Hz, c > 0 m/s; max_order >= 0 keeps images
+ * of at most that order, -1 keeps every image that reaches the first L samples.  Each image adds g h(i - d) at the
+ * Tw = 2 floor(0.004 fs + 1/2) samples around its distance d (samples), h a Hann-windowed sinc.
+ *
+ * air [B, K] (dB/m, float64) or null: every image of band k is also scaled by 10^(-air[b, k] d / 20) (d in metres)
+ * and the tail's envelope by 10^(-air[b, k] (c n / fs) / 10).
+ *
+ * t_d [B] (float64 seconds > 0) and seed [B] (uint64), both on the device or both null, add a diffuse late tail
+ * (DESIGN.md K20, "Hybrid"): the images with floor(d) < min(L, n_d), n_d = ceil(t_d[b] fs), then, at every sample
+ * n >= n_d - Tw/2, w(n) sqrt(E_b(n)) xi(seed[b], c, n): E_b the expected energy per sample of the image arrivals of
+ * item b's room, w a raised-cosine ramp over the Tw samples centred on n_d, xi a standard normal from a stateless
+ * counter-based generator (SplitMix64, Box-Muller) shared by the bands.  Every image order is kept: max_order must be
+ * -1 with a tail.
+ *
  * Only the first K' = b2a_rir_bands_kept(K, fs) bands are computed: those whose lower crossover 125 2^(k - 1/2) Hz is
- * below fs / 2.  out [K', B, C, L] float32, band-major: row k < K' - 1 holds r_k - r_{k+1}, row K' - 1 holds r_{K'-1},
- * r_k the band's response before the crossovers.  The images are enumerated once for all bands; with equal bands and
- * no air the differences are exactly 0 and r_{K'-1} is b2a_rir_ism_f32's / b2a_rir_hybrid_f32's output, bit for bit.
- * 1 <= K <= 8, B C K <= 65535.  One launch, two with a tail; no host sync, no atomics. */
+ * below fs / 2 (DESIGN.md K20, "Bands").  out [K', B, C, L] float32, band-major: row k < K' - 1 holds r_k - r_{k+1},
+ * row K' - 1 holds r_{K'-1}, r_k the band's response before the crossovers.  The images are enumerated once for all
+ * bands; with equal bands and no air the differences are exactly 0 and r_{K'-1} is the K = 1 output, bit for bit.
+ *
+ * 1 <= K <= 8, B C K <= 65535, L <= 2^30; the arguments are not checked against each other (positions inside the room,
+ * beta in [0, 1]): core/room.py does that.  One launch, two with a tail; no host sync, no atomics: reruns and a batch
+ * against its items one at a time are bit-identical. */
 int b2a_rir_bands_kept(int K, double fs);
-int b2a_rir_bands_f32(const double* room, const double* src, const double* mics, const double* beta, const double* air,
-                      const double* t_d, const uint64_t* seed, int64_t B, int C, int K, int64_t L, double fs, double c,
-                      int max_order, float* out, void* stream);
+int b2a_rir_f32(const double* room, const double* src, const double* mics, const double* beta, const double* air,
+                const double* t_d, const uint64_t* seed, int64_t B, int C, int K, int64_t L, double fs, double c,
+                int max_order, float* out, void* stream);
 
 /* y[b, c] = bands[n_conv, b, c] + sum_{k < n_conv} conv[k, b, c] (added in k order): the crossover outputs of the
- * octave-band differences added to the last band (bands [n_conv + 1, B, C, L] from b2a_rir_bands_f32, conv [n_conv, B,
+ * octave-band differences added to the last band (bands [n_conv + 1, B, C, L] from b2a_rir_f32, conv [n_conv, B,
  * C, L]).  Samples before the first one any band can reach through crossovers of half-length `half` (the direct path's
  * window, or with t_d the tail's start, less half and one sample) are written as 0.  1 <= n_conv < 8.  One launch. */
 int b2a_rir_band_sum_f32(const double* src, const double* mics, const double* t_d, int64_t B, int C, int64_t L,

@@ -26,7 +26,7 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 K_BUDGET = 8.0   # u, per sample, relative to G[n]; worst measured 4.96 (48 kHz) on an H100 80GB HBM3 at 700 W
 TILE = 512       # csrc/rir.cu: samples per CTA
-LAUNCHES = 1     # b2a_rir_ism_f32; the high-pass adds K19's three
+LAUNCHES = 1     # b2a_rir_f32; the high-pass adds K19's three
 WORST = {}       # the largest K seen per rate (printed by test_report_worst_k)
 
 
@@ -245,18 +245,18 @@ def check_api(eng, fs=8000):
     z = torch.zeros(1, 3, dtype=torch.float64, device=DEV)
     with pytest.raises(ValueError, match="rows"):
         eng.image_source_ir(z.expand(70000, 3), z.expand(70000, 3), torch.zeros(70000, 1, 3, dtype=torch.float64,
-                            device=DEV), torch.zeros(70000, 6, dtype=torch.float64, device=DEV), 10, fs)
+                            device=DEV), torch.zeros(70000, 6, 1, dtype=torch.float64, device=DEV), 10, fs)
     p = z.data_ptr()
-    for args, msg in (((None, p, p, p, 1, 1, 10, fs, 343.0, -1, p, None), b"null pointer"),
-                      ((p, p, p, p, 0, 1, 10, fs, 343.0, -1, p, None), b"bad shape"),
-                      ((p, p, p, p, 1, 1, 0, fs, 343.0, -1, p, None), b"bad shape"),
-                      ((p, p, p, p, 300, 300, 10, fs, 343.0, -1, p, None), b"65535"),
-                      ((p, p, p, p, 1, 1, (1 << 30) + 1, fs, 343.0, -1, p, None), b"2^30"),
-                      ((p, p, p, p, 1, 1, 10, 100.0, 343.0, -1, p, None), b"fs="),
-                      ((p, p, p, p, 1, 1, 10, 400000.0, 343.0, -1, p, None), b"fs="),
-                      ((p, p, p, p, 1, 1, 10, fs, 0.0, -1, p, None), b"sound speed"),
-                      ((p, p, p, p, 1, 1, 10, fs, 343.0, -2, p, None), b"max_order")):
-        assert lib.b2a_rir_ism_f32(*args) == -1 and msg in lib.b2a_last_error(), msg
+    for args, msg in (((None, p, p, p, None, None, None, 1, 1, 1, 10, fs, 343.0, -1, p, None), b"null pointer"),
+                      ((p, p, p, p, None, None, None, 0, 1, 1, 10, fs, 343.0, -1, p, None), b"bad shape"),
+                      ((p, p, p, p, None, None, None, 1, 1, 1, 0, fs, 343.0, -1, p, None), b"bad shape"),
+                      ((p, p, p, p, None, None, None, 300, 300, 1, 10, fs, 343.0, -1, p, None), b"65535"),
+                      ((p, p, p, p, None, None, None, 1, 1, 1, (1 << 30) + 1, fs, 343.0, -1, p, None), b"2^30"),
+                      ((p, p, p, p, None, None, None, 1, 1, 1, 10, 100.0, 343.0, -1, p, None), b"fs="),
+                      ((p, p, p, p, None, None, None, 1, 1, 1, 10, 400000.0, 343.0, -1, p, None), b"fs="),
+                      ((p, p, p, p, None, None, None, 1, 1, 1, 10, fs, 0.0, -1, p, None), b"sound speed"),
+                      ((p, p, p, p, None, None, None, 1, 1, 1, 10, fs, 343.0, -2, p, None), b"max_order")):
+        assert lib.b2a_rir_f32(*args) == -1 and msg in lib.b2a_last_error(), msg
     assert lib.kernel_launches.value == k0
     # the transform: seeded draws against a numpy restatement of the documented order
     T, C = 4000, 2

@@ -295,8 +295,8 @@ def check_api(eng, fs=8000):
                       ((p, p, p, p, None, p, None, 1, 1, 3, 10, fs, 343.0, -1, p, None), b"t_d and seed"),
                       ((p, p, p, p, None, p, p, 1, 1, 3, 10, fs, 343.0, 2, p, None), b"max_order"),
                       ((p, p, p, p, None, None, None, 1, 1, 3, 10, 100.0, 343.0, -1, p, None), b"fs=")):
-        assert lib.b2a_rir_bands_f32(*args) == -1 and msg in lib.b2a_last_error(), msg
-        assert lib.b2a_last_error().startswith(b"rir_bands")
+        assert lib.b2a_rir_f32(*args) == -1 and msg in lib.b2a_last_error(), msg
+        assert lib.b2a_last_error().startswith(b"rir:")
     assert lib.b2a_rir_band_sum_f32(p, p, None, 1, 1, 10, fs, 343.0, 5, p, p, 0, p, None) == -1
     assert lib.b2a_rir_band_sum_f32(None, p, None, 1, 1, 10, fs, 343.0, 5, p, p, 1, p, None) == -1
     assert lib.kernel_launches.value == k0
@@ -350,7 +350,7 @@ def fftconv_launches(eng, rows, L, taps):
 
 
 def check_launches(eng, fs=8000):
-    """b2a_rir_bands_f32: 1 launch (2 with a tail); K' > 1 adds fftconv's and the sum's 1; the high-pass 3."""
+    """b2a_rir_f32: 1 launch (2 with a tail); K' > 1 adds fftconv's and the sum's 1; the high-pass 3."""
     from audiotools_b200.core.room import image_source_ir
 
     room, src, mics = [4.0, 3.0, 2.5], [1.0, 1.0, 1.0], [[2.0, 2.0, 1.5], [2.5, 2.0, 1.5]]

@@ -32,7 +32,7 @@ DEV = "cuda:0"
 K_BUDGET = 8.0   # u, the images' per-sample bound (tests/test_gpu_rir.py)
 ENV_REL = 1e-4   # relative error of the tail's amplitude against the converged envelope
 TILE = 512       # csrc/rir.cu: samples per CTA
-LAUNCHES = 2     # b2a_rir_hybrid_f32: the images, then the tail; the high-pass adds K19's three
+LAUNCHES = 2     # b2a_rir_f32 with a tail: the images, then the tail; the high-pass adds K19's three
 
 
 @pytest.fixture(scope="module")
@@ -254,19 +254,19 @@ def check_api(eng, fs=8000):
                           diffuse_after=torch.tensor(0.05, dtype=torch.float64, requires_grad=True))
     z = torch.zeros(1, 3, dtype=torch.float64, device=DEV)
     with pytest.raises(ValueError, match="max_order"):
-        eng.image_source_ir(z, z, z[None], torch.zeros(1, 6, dtype=torch.float64, device=DEV), 10, fs, max_order=2,
+        eng.image_source_ir(z, z, z[None], torch.zeros(1, 6, 1, dtype=torch.float64, device=DEV), 10, fs, max_order=2,
                             diffuse_after=z[0, :1], seed=torch.zeros(1, dtype=torch.int64, device=DEV))
     p = z.data_ptr()
-    for args, msg in (((None, p, p, p, p, p, 1, 1, 10, fs, 343.0, p, None), b"null pointer"),
-                      ((p, p, p, p, None, p, 1, 1, 10, fs, 343.0, p, None), b"null pointer"),
-                      ((p, p, p, p, p, None, 1, 1, 10, fs, 343.0, p, None), b"null pointer"),
-                      ((p, p, p, p, p, p, 0, 1, 10, fs, 343.0, p, None), b"bad shape"),
-                      ((p, p, p, p, p, p, 300, 300, 10, fs, 343.0, p, None), b"65535"),
-                      ((p, p, p, p, p, p, 1, 1, (1 << 30) + 1, fs, 343.0, p, None), b"2^30"),
-                      ((p, p, p, p, p, p, 1, 1, 10, 100.0, 343.0, p, None), b"fs="),
-                      ((p, p, p, p, p, p, 1, 1, 10, fs, 0.0, p, None), b"sound speed")):
-        assert lib.b2a_rir_hybrid_f32(*args) == -1 and msg in lib.b2a_last_error(), msg
-        assert lib.b2a_last_error().startswith(b"rir_hybrid")
+    for args, msg in (((None, p, p, p, None, p, p, 1, 1, 1, 10, fs, 343.0, -1, p, None), b"null pointer"),
+                      ((p, p, p, p, None, None, p, 1, 1, 1, 10, fs, 343.0, -1, p, None), b"t_d and seed"),
+                      ((p, p, p, p, None, p, None, 1, 1, 1, 10, fs, 343.0, -1, p, None), b"t_d and seed"),
+                      ((p, p, p, p, None, p, p, 0, 1, 1, 10, fs, 343.0, -1, p, None), b"bad shape"),
+                      ((p, p, p, p, None, p, p, 300, 300, 1, 10, fs, 343.0, -1, p, None), b"65535"),
+                      ((p, p, p, p, None, p, p, 1, 1, 1, (1 << 30) + 1, fs, 343.0, -1, p, None), b"2^30"),
+                      ((p, p, p, p, None, p, p, 1, 1, 1, 10, 100.0, 343.0, -1, p, None), b"fs="),
+                      ((p, p, p, p, None, p, p, 1, 1, 1, 10, fs, 0.0, -1, p, None), b"sound speed")):
+        assert lib.b2a_rir_f32(*args) == -1 and msg in lib.b2a_last_error(), msg
+        assert lib.b2a_last_error().startswith(b"rir:")
     assert lib.kernel_launches.value == k0
     # the transform: with diffuse_after, two draws after the images-only ones
     T, C = 4000, 2

@@ -111,10 +111,10 @@ def test_bad_arguments_launch_nothing_in_the_real_library():
     buf = (ctypes.c_double * 64)()
     p = ctypes.cast(buf, ctypes.c_void_p)
     k0 = lib.kernel_launches.value
-    assert lib.b2a_rir_ism_f32(p, p, p, None, 1, 1, 16, 8000.0, 343.0, -1, p, None) == -1
-    assert lib.b2a_rir_ism_f32(p, p, p, p, 1, 1, 16, 124.0, 343.0, -1, p, None) == -1
-    assert lib.b2a_rir_ism_f32(p, p, p, p, 1, 1, 16, 8000.0, -1.0, -1, p, None) == -1
-    assert lib.b2a_rir_ism_f32(p, p, p, p, 65536, 1, 16, 8000.0, 343.0, -1, p, None) == -1
+    assert lib.b2a_rir_f32(p, p, p, None, None, None, None, 1, 1, 1, 16, 8000.0, 343.0, -1, p, None) == -1
+    assert lib.b2a_rir_f32(p, p, p, p, None, None, None, 1, 1, 1, 16, 124.0, 343.0, -1, p, None) == -1
+    assert lib.b2a_rir_f32(p, p, p, p, None, None, None, 1, 1, 1, 16, 8000.0, -1.0, -1, p, None) == -1
+    assert lib.b2a_rir_f32(p, p, p, p, None, None, None, 65536, 1, 1, 16, 8000.0, 343.0, -1, p, None) == -1
     assert lib.kernel_launches.value == k0
 
 

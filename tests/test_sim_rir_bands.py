@@ -83,9 +83,9 @@ def test_bad_arguments_launch_nothing_in_the_real_library():
     p = ctypes.cast(buf, ctypes.c_void_p)
     k0 = lib.kernel_launches.value
     assert lib.b2a_rir_bands_kept(8, 8000.0) == 6 and lib.b2a_rir_bands_kept(9, 8000.0) == 0
-    assert lib.b2a_rir_bands_f32(p, p, p, p, None, None, None, 1, 1, 9, 16, 8000.0, 343.0, -1, p, None) == -1
-    assert lib.b2a_rir_bands_f32(p, p, p, p, None, p, None, 1, 1, 3, 16, 8000.0, 343.0, -1, p, None) == -1
-    assert lib.b2a_rir_bands_f32(p, p, p, p, None, None, None, 21846, 1, 3, 16, 8000.0, 343.0, -1, p, None) == -1
+    assert lib.b2a_rir_f32(p, p, p, p, None, None, None, 1, 1, 9, 16, 8000.0, 343.0, -1, p, None) == -1
+    assert lib.b2a_rir_f32(p, p, p, p, None, p, None, 1, 1, 3, 16, 8000.0, 343.0, -1, p, None) == -1
+    assert lib.b2a_rir_f32(p, p, p, p, None, None, None, 21846, 1, 3, 16, 8000.0, 343.0, -1, p, None) == -1
     assert lib.b2a_rir_band_sum_f32(p, p, None, 1, 1, 16, 8000.0, 343.0, 5, p, p, 8, p, None) == -1
     assert lib.kernel_launches.value == k0
 
