@@ -127,6 +127,9 @@ SIGNATURES = {
     "b2a_circconv_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64, c_int64]),
     "b2a_circconv_f32": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p,
                                  c_void_p, c_size_t, c_void_p]),
+    "b2a_circconv_path_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int]),
+    "b2a_circconv_path_f32": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int, c_int, c_int,
+                                      c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "b2a_resample_backward_f32": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_int, c_void_p, c_void_p,
                                           c_void_p]),
     "b2a_fir_pad_fold_workspace_bytes": (c_size_t, [c_int64, c_int]),

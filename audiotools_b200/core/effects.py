@@ -68,13 +68,36 @@ class EffectMixin:
             ir = ir.equalizer(ir_eq)
         if drr is not None:
             ir = ir.alter_drr(drr)
+        return self._convolve_keeping_peak(lambda: self.convolve(ir, _bypass=_bypass), use_original_phase, _bypass)
+
+    def apply_moving_ir(self, irs, hop: int, use_original_phase: bool = False, _bypass=None):
+        """``apply_ir`` for a moving source or microphone (an extension; DESIGN.md K22): ``irs`` [B, K, C, L] (or
+        [B, K, 1, L], shared by the channels) holds one impulse response per waypoint, waypoint k at sample k ``hop``.
+        The output crossfades the K circular convolutions linearly between neighbouring waypoints, the last one
+        holding to the end; every waypoint of an (item, channel) row is rolled and scaled by the row's first waypoint,
+        so a change in delay along the path is heard.  Then each row's input peak is restored as ``apply_ir`` does.
+        ``hop`` >= 1024 samples and K = (T - 1) // hop + 1, else ``ValueError``.  There is no backward: a signal or
+        ``irs`` that requires a gradient raises ``NotImplementedError``.  ``_bypass`` [B]: items left untouched."""
+        for name, t in (("the signal", self._materialized()), ("the impulse responses", irs)):
+            if _grad.wants_grad(t):
+                raise NotImplementedError(f"apply_moving_ir: {name} requires a gradient, and the moving convolution "
+                                          "has no backward; call it under torch.no_grad() or on detached tensors")
+
+        def convolve():
+            self.audio_data = _engine().circular_convolve_moving(self._materialized(), irs, hop, bypass=_bypass)
+
+        return self._convolve_keeping_peak(convolve, use_original_phase, _bypass)
+
+    def _convolve_keeping_peak(self, convolve, use_original_phase: bool, _bypass):
+        """Run ``convolve()`` on this signal, optionally put the input's phase back, and scale every (item, channel)
+        row back to its input peak (ref :125-179)."""
         cuda = _on_engine(self._audio_data)
         x0 = self._materialized()
         # the peaks are values here; with a gradient, PeakScale's backward differentiates through them
         max_spk = _engine().row_absmax(x0.detach()) if cuda else \
             self.audio_data.abs().max(dim=-1, keepdims=True).values
         phase = self.phase if use_original_phase else None
-        self.convolve(ir, _bypass=_bypass)
+        convolve()
         if use_original_phase:
             self.stft()
             self.stft_data = self.magnitude * torch.exp(1j * phase)

@@ -108,6 +108,36 @@ struct InvParams {
   int off_tw, off_ut, off_buf;
 };
 
+// The packed complex input of the inverse real FFT of one block: bin k of the block spectrum is yr[k * fs] (times
+// hr[k] when hr is set).  Z[e] = Xe[e] + i Xo[e] from the real-FFT bins X[e], X[N-e]; the inverse transform is
+// conj(FFT(conj(Z)))/N, so z holds conj(Z).   e = l + 32 m
+template <int N>
+__device__ __forceinline__ void inverse_input(float2 (&z)[32], const float2* __restrict__ yr, size_t fs,
+                                              const float2* __restrict__ hr, const float2* ut, int l) {
+#pragma unroll
+  for (int m = 0; m < 32; ++m) {
+    const int e = l + 32 * m;
+    // for e > N/2 use the pair (k = N-e): Z[e] = conj(Xe[k]) + i conj(Xo[k])
+    const int k = (m < 16) ? e : N - e;
+    float2 xk = __ldg(yr + (size_t)k * fs);
+    float2 xn = __ldg(yr + (size_t)(N - k) * fs);
+    if (hr) {  // one partition: Y = H * X, multiplied here instead of in a pass of its own
+      xk = cmul(xk, __ldg(hr + k));
+      xn = cmul(xn, __ldg(hr + (N - k)));
+    }
+    // Xe = (X[k] + conj X[N-k])/2 ; T = (X[k] - conj X[N-k])/2 ; Xo = conj(W_k) T, W_k = exp(-i pi k/N)
+    const float2 xe = make_float2(0.5f * (xk.x + xn.x), 0.5f * (xk.y - xn.y));
+    const float2 tt = make_float2(0.5f * (xk.x - xn.x), 0.5f * (xk.y + xn.y));
+    float2 w;
+    if (k == N / 2) w = make_float2(0.f, -1.f);
+    else w = ut[(k >> 5) * 32 + (k & 31)];  // table index m' * LPF + l' with k = l' + 32 m'
+    const float2 xo = make_float2(fmaf(w.x, tt.x, w.y * tt.y), fmaf(w.x, tt.y, -w.y * tt.x));  // conj(w) * tt
+    float2 zz = make_float2(xe.x - xo.y, xe.y + xo.x);  // Xe + i Xo
+    if (m >= 16 && e != N / 2) zz = make_float2(xe.x + xo.y, -xe.y + xo.x);  // conj(Xe) + i conj(Xo)
+    z[m] = make_float2(zz.x, -zz.y);  // conj for the inverse-by-forward trick
+  }
+}
+
 // inverse real FFT of block spectra, one warp per block, keeping the last LP samples (overlap-save)
 __global__ void __launch_bounds__(256, 2) ifft_blocks_kernel(InvParams p) {
   using PL = WPlan<LOG2N>;
@@ -136,31 +166,8 @@ __global__ void __launch_bounds__(256, 2) ifft_blocks_kernel(InvParams p) {
     }
     const float2* yr = p.Y + (size_t)row * NF * p.NB + b;
     const float2* hr = p.H1 ? p.H1 + (size_t)((p.row0 + row) / p.rows_per_filt) * NF : nullptr;
-    // Z[e] = Xe[e] + i Xo[e] from the real-FFT bins X[e], X[N-e]; the inverse transform is
-    // conj(FFT(conj(Z)))/N, so feed conj(Z).   e = l + 32 m
     float2 z[32];
-#pragma unroll
-    for (int m = 0; m < 32; ++m) {
-      const int e = l + 32 * m;
-      // for e > N/2 use the pair (k = N-e): Z[e] = conj(Xe[k]) + i conj(Xo[k])
-      const int k = (m < 16) ? e : N - e;
-      float2 xk = __ldg(yr + (size_t)k * p.NB);
-      float2 xn = __ldg(yr + (size_t)(N - k) * p.NB);
-      if (hr) {  // one partition: Y = H * X, multiplied here instead of in a pass of its own
-        xk = cmul(xk, __ldg(hr + k));
-        xn = cmul(xn, __ldg(hr + (N - k)));
-      }
-      // Xe = (X[k] + conj X[N-k])/2 ; T = (X[k] - conj X[N-k])/2 ; Xo = conj(W_k) T, W_k = exp(-i pi k/N)
-      const float2 xe = make_float2(0.5f * (xk.x + xn.x), 0.5f * (xk.y - xn.y));
-      const float2 tt = make_float2(0.5f * (xk.x - xn.x), 0.5f * (xk.y + xn.y));
-      float2 w;
-      if (k == N / 2) w = make_float2(0.f, -1.f);
-      else w = ut[(k >> 5) * 32 + (k & 31)];  // table index m' * LPF + l' with k = l' + 32 m'
-      const float2 xo = make_float2(fmaf(w.x, tt.x, w.y * tt.y), fmaf(w.x, tt.y, -w.y * tt.x));  // conj(w) * tt
-      float2 zz = make_float2(xe.x - xo.y, xe.y + xo.x);  // Xe + i Xo
-      if (m >= 16 && e != N / 2) zz = make_float2(xe.x + xo.y, -xe.y + xo.x);  // conj(Xe) + i conj(Xo)
-      z[m] = make_float2(zz.x, -zz.y);  // conj for the inverse-by-forward trick
-    }
+    inverse_input<N>(z, yr, (size_t)p.NB, hr, ut, l);
     warp_fft<LOG2N>(z, xb, tw, l);
     // z[m] = conj(N * zt[n]), n = l + 32 m; samples x[2n] = Re zt, x[2n+1] = Im zt; keep n >= N/2
     const int grow = p.row0 + row;
@@ -185,13 +192,12 @@ __global__ void __launch_bounds__(256, 2) ifft_blocks_kernel(InvParams p) {
   }
 }
 
-// per item: first index of max|h| over the first Leff samples, and 1 / max(max|h|, 1e-5)
-__global__ void __launch_bounds__(256)
-ir_peak_kernel(const float* __restrict__ ir, int L, int Leff, int32_t* __restrict__ idx_out,
-               float* __restrict__ scale_out, int roll) {
+// per CTA of 256 threads: first index of max|h| over the first Leff samples, and 1 / max(max|h|, 1e-5), stored at
+// idx_out[blockIdx.x] and scale_out[blockIdx.x]
+__device__ __forceinline__ void ir_peak(const float* __restrict__ h, int Leff, int32_t* __restrict__ idx_out,
+                                        float* __restrict__ scale_out, int roll) {
   __shared__ float sv[256];
   __shared__ int si[256];
-  const float* h = ir + (size_t)blockIdx.x * L;
   float best = -1.f;
   int bi = 0;
   for (int i = threadIdx.x; i < Leff; i += 256) {
@@ -216,6 +222,13 @@ ir_peak_kernel(const float* __restrict__ ir, int L, int Leff, int32_t* __restric
     idx_out[blockIdx.x] = roll ? si[0] : 0;
     scale_out[blockIdx.x] = 1.0f / fmaxf(sv[0], 1e-5f);
   }
+}
+
+// per IR of rows L apart: ir_peak
+__global__ void __launch_bounds__(256)
+ir_peak_kernel(const float* __restrict__ ir, int L, int Leff, int32_t* __restrict__ idx_out,
+               float* __restrict__ scale_out, int roll) {
+  ir_peak(ir + (size_t)blockIdx.x * L, Leff, idx_out, scale_out, roll);
 }
 
 struct Layout {
@@ -407,4 +420,279 @@ extern "C" int b2a_circconv_backward_f32(const float* grad_out, int64_t rows, in
   B2A_LAUNCH(ir_peak_kernel, dim3((unsigned)n_ir), dim3(256), 0, stream, ir, (int)L, (int)L, pidx, pscale, roll_to_peak);
   B2A_LAUNCH(reverse_taps_kernel, dim3((unsigned)n_ir), dim3(256), 0, stream, ir, (int)L, (const int32_t*)pidx, rev, off);
   return run(grad_out, rows, T, rev, n_ir, L, rows_per_ir, off, 0, 3, pscale, 0, bypass, grad_x, base, w, stream);
+}
+
+/* b2a_circconv_path_f32: a circular convolution whose impulse response moves along a path of K waypoints, one IR
+ * every `hop` samples (DESIGN.md K22).  Waypoint k sits at tau_k = k hop; the output is the receiver-time crossfade
+ *     y[row][t] = s sum_k v_k(t) sum_j h_k[j] x[(t - j + idx) mod T],   v_k(t) = max(0, 1 - |t - tau_k| / hop),
+ * v_{K-1}(t) = 1 for t >= tau_{K-1}, with idx and s from waypoint 0 (ir_peak_kernel), so the weights sum to 1 and a
+ * change in propagation delay along the path stays in the output.
+ *
+ * It is the overlap-save engine above with the FIR stage split by waypoint.  X is computed once per row.  Waypoint k
+ * is non-zero on (tau_{k-1}, tau_{k+1}), so its FIR runs only over the output blocks that meet that span
+ * (path_blocks); hop >= LP means a block meets at most 3 waypoints, and waypoints k and k + 3 never share a block.
+ * Each waypoint therefore writes its own slot k % 3 of Y3 with no overlap, and the inverse kernel transforms the 2 or
+ * 3 slots of a block, weights each sample by v_k and sums them in waypoint order: no atomics, no read-modify-write. */
+namespace b2a {
+namespace fftconv {
+
+// The output blocks [lo, hi] on which waypoint k's weight is non-zero: those meeting (tau_{k-1}, tau_{k+1}), from block
+// 0 for the first waypoint and up to the last block for the last one.
+__device__ __forceinline__ void path_blocks(int k, int K, int hop, int NB, int& lo, int& hi) {
+  lo = k == 0 ? 0 : ((k - 1) * hop + 1) / LP;
+  hi = k == K - 1 ? NB - 1 : min(((k + 1) * hop - 1) / LP, NB - 1);
+}
+
+// v_k(t): hop - |t - tau_k| is exact, so the weights of two neighbours are each rounded once.
+__device__ __forceinline__ float path_weight(int k, int K, int hop, int t) {
+  const int d = t - k * hop;
+  if (k == K - 1 && d >= 0) return 1.0f;
+  const int a = d < 0 ? -d : d;
+  return a >= hop ? 0.0f : (float)(hop - a) / (float)hop;
+}
+
+constexpr int PATH_R = 8;  // output blocks per thread and register tile
+
+// Y3[row][k % 3][b][f] = sum_p H[item][k][c][f][p] * X[row][f][b + P-1 - p] over the blocks b of waypoint k, for the
+// row's IR ir = item * ir_channels + c.  One thread
+// per bin f walks the waypoint's blocks in tiles of PATH_R and slides a window over X, so each tap and each new X value
+// is loaded once per tile.  The sum runs in freq_fir_kernel's order (q = P-1-p ascending, one fmaf chain per output),
+// so a waypoint's block spectra are bit-identical to the static engine's.  The [b][f] layout makes the stores and the
+// inverse kernel's loads unit-stride.
+__global__ void __launch_bounds__(128)
+path_fir_kernel(const float2* __restrict__ X, const float2* __restrict__ H, float2* __restrict__ Y3, int NB, int NBX,
+                int P, int K, int hop, int rows_per_ir, int ir_channels, int row0) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= NF) return;
+  const int k = blockIdx.y, row = blockIdx.z;
+  int lo, hi;
+  path_blocks(k, K, hop, NB, lo, hi);
+  const int ir = (row0 + row) / rows_per_ir - row0 / rows_per_ir;  // chunks start on an item boundary
+  const int filt = ((ir / ir_channels) * K + k) * ir_channels + ir % ir_channels;
+  const float2* xr = X + ((size_t)row * NF + f) * NBX;
+  const float2* hr = H + ((size_t)filt * NF + f) * P;
+  float2* yr = Y3 + ((size_t)row * 3 + k % 3) * NB * NF + f;
+  const float2 zero = make_float2(0.f, 0.f);
+#pragma unroll 1
+  for (int b0 = lo; b0 <= hi; b0 += PATH_R) {
+    float2 w[PATH_R], a[PATH_R];
+#pragma unroll
+    for (int r = 0; r < PATH_R; ++r) {
+      w[r] = b0 + r < NBX ? __ldg(xr + b0 + r) : zero;  // w[r] = X[b0 + r + q]
+      a[r] = zero;
+    }
+#pragma unroll 2
+    for (int q = 0; q < P; ++q) {
+      const float2 g = __ldg(hr + (P - 1 - q));
+#pragma unroll
+      for (int r = 0; r < PATH_R; ++r) cmac(a[r], g, w[r]);
+#pragma unroll
+      for (int r = 0; r < PATH_R - 1; ++r) w[r] = w[r + 1];
+      const int i = b0 + PATH_R + q;
+      w[PATH_R - 1] = i < NBX ? __ldg(xr + i) : zero;
+    }
+#pragma unroll
+    for (int r = 0; r < PATH_R; ++r)
+      if (b0 + r <= hi) yr[(size_t)(b0 + r) * NF] = a[r];
+  }
+}
+
+struct PathInvParams {
+  const float2* Y3;      // [rows, 3, NB, NF]
+  const float* x;        // [rows_total, T]
+  const float* post;     // [n_ir]
+  const int32_t* bypass; // [n_ir] nullable: non-zero = out = x for the rows of this IR
+  float* out;            // [rows_total, T]
+  int rows, row0, T, NB, K, hop, rows_per_ir;
+  int off_tw, off_ut, off_buf;
+};
+
+// One warp per output block: the inverse FFT of each waypoint active on the block, weighted per sample by v_k and
+// summed in waypoint order, then scaled by the row's post.
+__global__ void __launch_bounds__(256, 2) path_ifft_kernel(PathInvParams p) {
+  using PL = WPlan<LOG2N>;
+  constexpr int N = PL::N;
+  B2A_DYN_SMEM(smem);
+  float2* tw = reinterpret_cast<float2*>(smem + p.off_tw);
+  float2* ut = reinterpret_cast<float2*>(smem + p.off_ut);
+  float* xbs = reinterpret_cast<float*>(smem + p.off_buf);
+  const int tid = threadIdx.x, l = tid & 31, warp = tid >> 5;
+  warp_fft_tables<LOG2N>(tw, ut);
+  __syncthreads();
+  float* xb = xbs + warp * PL::XB;
+  const int groups = (p.NB + 7) / 8;
+  const int total = p.rows * groups;
+  const float inv_n = 1.0f / (float)N;
+#pragma unroll 1
+  for (int t = blockIdx.x; t < total; t += gridDim.x) {
+    const int row = t / groups, b = (t - row * groups) * 8 + warp;
+    if (b >= p.NB) continue;  // warp-uniform
+    const int grow = p.row0 + row;
+    float* orow = p.out + (size_t)grow * p.T;
+    if (p.bypass && __ldg(p.bypass + grow / p.rows_per_ir)) {
+      const float* xs = p.x + (size_t)grow * p.T;
+      for (int i = l; i < LP; i += 32) { const int s = b * LP + i; if (s < p.T) orow[s] = __ldg(xs + s); }
+      continue;
+    }
+    float acc[32];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+    const int kc = b * LP / p.hop;  // the waypoints meeting block b are among kc - 1 .. kc + 2
+    const int k1 = min(kc + 2, p.K - 1);
+#pragma unroll 1
+    for (int k = max(kc - 1, 0); k <= k1; ++k) {
+      int lo, hi;
+      path_blocks(k, p.K, p.hop, p.NB, lo, hi);
+      if (b < lo || b > hi) continue;  // warp-uniform
+      float2 z[32];
+      inverse_input<N>(z, p.Y3 + (((size_t)row * 3 + k % 3) * p.NB + b) * NF, 1, nullptr, ut, l);
+      warp_fft<LOG2N>(z, xb, tw, l);
+      // z[m] = conj(N * zt[n]), n = l + 32 m; samples x[2n] = Re zt, x[2n+1] = Im zt; keep n >= N/2
+#pragma unroll
+      for (int m = 16; m < 32; ++m) {
+        const int s0 = b * LP + 2 * (l + 32 * m) - LP;
+        acc[2 * (m - 16)] += path_weight(k, p.K, p.hop, s0) * (z[m].x * inv_n);
+        acc[2 * (m - 16) + 1] += path_weight(k, p.K, p.hop, s0 + 1) * (-z[m].y * inv_n);
+      }
+      __syncwarp();
+    }
+    const float post = __ldg(p.post + grow / p.rows_per_ir);
+#pragma unroll
+    for (int m = 16; m < 32; ++m) {
+      const int s0 = b * LP + 2 * (l + 32 * m) - LP;
+      if (s0 < p.T) orow[s0] = acc[2 * (m - 16)] * post;
+      if (s0 + 1 < p.T) orow[s0 + 1] = acc[2 * (m - 16) + 1] * post;
+    }
+  }
+}
+
+// per IR i = item * ir_channels + c of an [items][K][ir_channels][L] bank: ir_peak of its first waypoint
+__global__ void __launch_bounds__(256)
+path_peak_kernel(const float* __restrict__ ir, int K, int ir_channels, int L, int32_t* __restrict__ idx_out,
+                 float* __restrict__ scale_out, int roll) {
+  const int item = blockIdx.x / ir_channels, c = blockIdx.x - item * ir_channels;
+  ir_peak(ir + ((size_t)item * K * ir_channels + c) * L, L, idx_out, scale_out, roll);
+}
+
+struct PathLayout {
+  size_t ones, half, H, X, Y3, rorg, peak_idx, peak_scale, total;
+  int P, NB, NBX, chunk;  // chunk: rows per chunk, whole items of ir_channels * rows_per_ir rows
+};
+
+// Per item: the spectra of its ir_channels x K waypoints; per row: X and the three Y3 slots.  A chunk of whole items
+// takes at most CHUNK_BUDGET_MB of spectra, or one item when a single one needs more.
+static PathLayout path_layout(int64_t rows, int64_t T, int64_t K, int64_t L, int64_t rows_per_ir,
+                              int64_t ir_channels) {
+  PathLayout w;
+  w.P = (int)((L + LP - 1) / LP);
+  w.NB = (int)((T + LP - 1) / LP);
+  w.NBX = w.NB + w.P - 1;
+  const int64_t n_ir = rows / rows_per_ir, item_rows = rows_per_ir * ir_channels, items = rows / item_rows;
+  const size_t per_item = ((size_t)ir_channels * K * w.P + (size_t)item_rows * (w.NBX + 3 * (size_t)w.NB)) * NF * 8;
+  int64_t chunk = (int64_t)((CHUNK_BUDGET_MB << 20) / per_item);
+  if (chunk < 1) chunk = 1;
+  if (chunk > items) chunk = items;
+  if (chunk * item_rows > 65535) chunk = 65535 / item_rows;
+  w.chunk = (int)(chunk * item_rows);
+  size_t o = 0;
+  w.ones = o; o = al(o + NFFT * 4);
+  w.half = o; o = al(o + NFFT * 4);
+  w.H = o; o = al(o + (size_t)chunk * ir_channels * K * w.P * NF * 8);
+  w.X = o; o = al(o + (size_t)w.chunk * NF * w.NBX * 8);
+  w.Y3 = o; o = al(o + (size_t)w.chunk * 3 * w.NB * NF * 8);
+  w.rorg = o; o = al(o + (size_t)w.chunk * 4);
+  w.peak_idx = o; o = al(o + (size_t)n_ir * 4);
+  w.peak_scale = o; o = al(o + (size_t)n_ir * 4);
+  w.total = o;
+  return w;
+}
+
+static int run_path(const float* x, int64_t rows, int64_t T, const float* ir, int64_t K, int64_t L, int rows_per_ir,
+                    int ir_channels, int hop, int roll_to_peak, const int32_t* bypass, float* out, char* ws,
+                    const PathLayout& w, void* stream) {
+  float* ones = (float*)(ws + w.ones);
+  float* half = (float*)(ws + w.half);
+  float2* H = (float2*)(ws + w.H);
+  float2* X = (float2*)(ws + w.X);
+  float2* Y3 = (float2*)(ws + w.Y3);
+  int32_t* rorg = (int32_t*)(ws + w.rorg);
+  int32_t* pidx = (int32_t*)(ws + w.peak_idx);
+  float* pscale = (float*)(ws + w.peak_scale);
+  const int64_t n_ir = rows / rows_per_ir, item_rows = (int64_t)rows_per_ir * ir_channels;
+  // roll and scale of every IR's first waypoint
+  B2A_LAUNCH(path_peak_kernel, dim3((unsigned)n_ir), dim3(256), 0, stream, ir, (int)K, ir_channels, (int)L, pidx,
+             pscale, roll_to_peak);
+  B2A_LAUNCH(fill_windows_kernel, dim3(NFFT / 256), dim3(256), 0, stream, ones, half);
+  using PL = WPlan<LOG2N>;
+  PathInvParams ip;
+  memset(&ip, 0, sizeof(ip));
+  int o = 0;
+  ip.off_tw = o; o += (PL::NTW * PL::LPF * 8 + 31) & ~15;
+  ip.off_ut = o; o += (16 * PL::LPF * 8 + 15) & ~15;
+  ip.off_buf = o; o += 8 * PL::XB * 4;
+  B2A_CUDA_OK(cudaFuncSetAttribute(path_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, o));
+  for (int64_t r0 = 0; r0 < rows; r0 += w.chunk) {
+    const int nr = (int)((rows - r0 < w.chunk) ? rows - r0 : w.chunk);
+    const int64_t b0 = r0 / item_rows, nb = nr / item_rows;
+    // 1. partitions of every waypoint of the chunk's items, a contiguous run of filters: [nb][K][ir_channels][NF][P]
+    int rc = frames_fft(ir + (size_t)b0 * K * ir_channels * L, (int)(nb * K * ir_channels), (int)L, NFFT, LP, half, 0,
+                        nullptr, B2A_PAD_CONSTANT, w.P, H, stream);
+    if (rc != B2A_OK) return rc;
+    // 2. block spectra of the rows, circular, shifted by waypoint 0's peak
+    B2A_LAUNCH(row_origin_kernel, dim3((nr + 255) / 256), dim3(256), 0, stream, (const int32_t*)pidx, 0, rows_per_ir,
+               nr, (int)r0, rorg);
+    rc = frames_fft(x + (size_t)r0 * T, nr, (int)T, NFFT, LP, ones, -w.P * LP, rorg, 3, w.NBX, X, stream);
+    if (rc != B2A_OK) return rc;
+    // 3. each waypoint's FIR over its own blocks
+    B2A_LAUNCH(path_fir_kernel, dim3((NF + 127) / 128, (unsigned)K, nr), dim3(128), 0, stream, (const float2*)X,
+               (const float2*)H, Y3, w.NB, w.NBX, w.P, (int)K, hop, rows_per_ir, ir_channels, (int)r0);
+    // 4. inverse FFTs, crossfade, scale
+    ip.Y3 = Y3; ip.x = x; ip.post = pscale; ip.bypass = bypass; ip.out = out;
+    ip.rows = nr; ip.row0 = (int)r0; ip.T = (int)T; ip.NB = w.NB; ip.K = (int)K; ip.hop = hop;
+    ip.rows_per_ir = rows_per_ir;
+    const int64_t total = (int64_t)nr * ((w.NB + 7) / 8);
+    const int64_t cap = (int64_t)num_sms() * 2;
+    B2A_LAUNCH(path_ifft_kernel, dim3((unsigned)(total < cap ? total : cap)), dim3(256), (size_t)o, stream, ip);
+  }
+  B2A_CUDA_OK(cudaGetLastError());
+  return B2A_OK;
+}
+
+}  // namespace fftconv
+}  // namespace b2a
+
+extern "C" size_t b2a_circconv_path_workspace_bytes(int64_t rows, int64_t T, int64_t K, int64_t L, int rows_per_ir,
+                                                    int ir_channels, int hop) {
+  if (rows < 1 || T < 1 || K < 1 || L < 1 || rows_per_ir < 1 || ir_channels < 1 ||
+      rows % ((int64_t)rows_per_ir * ir_channels) || hop < 1)
+    return 0;
+  return path_layout(rows, T, K, L < T ? L : T, rows_per_ir, ir_channels).total;
+}
+
+extern "C" int b2a_circconv_path_f32(const float* x, int64_t rows, int64_t T, const float* ir, int64_t K, int64_t L,
+                                     int rows_per_ir, int ir_channels, int hop, int roll_to_peak,
+                                     const int32_t* bypass, float* out, void* ws, size_t ws_bytes, void* stream) {
+  B2A_REQUIRE(x && ir && out && ws, B2A_E_INVALID, "circconv_path: null pointer");
+  B2A_REQUIRE(rows >= 1 && T >= 1 && K >= 1 && L >= 1 && rows_per_ir >= 1 && ir_channels >= 1, B2A_E_INVALID,
+              "circconv_path: bad shape");
+  B2A_REQUIRE(rows % ((int64_t)rows_per_ir * ir_channels) == 0, B2A_E_INVALID,
+              "circconv_path: %lld rows are not whole items of %d IRs of %d rows", (long long)rows, ir_channels,
+              rows_per_ir);
+  B2A_REQUIRE(T < ((int64_t)1 << 30), B2A_E_UNSUPPORTED, "circconv_path: too long");
+  B2A_REQUIRE(hop >= LP, B2A_E_INVALID, "circconv_path: hop %d < %d samples (a block would meet more than 3 waypoints)",
+              hop, LP);
+  B2A_REQUIRE(K == (T - 1) / hop + 1, B2A_E_INVALID,
+              "circconv_path: %lld waypoints %d samples apart do not cover T=%lld (need %lld)", (long long)K, hop,
+              (long long)T, (long long)((T - 1) / hop + 1));
+  B2A_REQUIRE(L <= T, B2A_E_INVALID,
+              "circconv_path: pass the IRs already truncated to the signal length (L=%lld > T=%lld)", (long long)L,
+              (long long)T);
+  B2A_REQUIRE(K <= 65535 && K * ir_channels * L < ((int64_t)1 << 31), B2A_E_UNSUPPORTED,
+              "circconv_path: %lld waypoints of %d x %lld samples are too many", (long long)K, ir_channels,
+              (long long)L);
+  B2A_REQUIRE(out != x, B2A_E_INVALID, "circconv_path: in-place is not supported");
+  const PathLayout w = path_layout(rows, T, K, L, rows_per_ir, ir_channels);
+  B2A_REQUIRE(ws_bytes >= w.total, B2A_E_INVALID, "circconv_path: workspace too small (%zu < %zu)", ws_bytes, w.total);
+  return run_path(x, rows, T, ir, K, L, rows_per_ir, ir_channels, hop, roll_to_peak, bypass, out, (char*)ws, w,
+                  stream);
 }

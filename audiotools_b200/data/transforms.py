@@ -61,6 +61,13 @@ def _stack_leaf(vals: list):
     return torch.as_tensor(arr).to(dtype) if arr.dtype != object else torch.stack([tt(v) for v in vals])
 
 
+def _host_values(v, dtype=np.float64) -> np.ndarray:
+    """A drawn parameter (host values, or a tensor read through its host mirror: no device sync) as a numpy array."""
+    if torch.is_tensor(v):
+        v = util.host_view(v).detach().cpu().numpy()
+    return np.asarray(v, dtype=dtype)
+
+
 def _collate_draws(draws: list):
     flats = [util.flatten(d) for d in draws]
     return util.unflatten({k: _stack_leaf([f[k] for f in flats]) for k in flats[0]})
@@ -574,7 +581,18 @@ class SyntheticRoomImpulseResponse(BaseTransform):
     ``band_rt60`` is K distribution tuples, each band's RT60 as a ratio to the item's ``rt60`` (None: 1 for every band),
     each raised like ``rt60`` to 1.01 times the room's smallest feasible RT60; ``air_absorption`` is K constants in
     dB/m (None: no air absorption).  Only then K more draws follow all the ones above, one per band in order, and the
-    IR is as long as the longest band RT60 when no ``duration`` is given."""
+    IR is as long as the longest band RT60 when no ``duration`` is given.
+
+    ``source_speed`` (a distribution tuple, m/s) makes the source move (``AudioSignal.apply_moving_ir``, DESIGN.md
+    K22): the drawn source is the start of a straight path that it follows at the drawn speed toward an end point, and
+    where it stops.  Only then two more draws follow all the ones above: the end point (``end``), one
+    ``state.uniform`` call inside the same margin box as the source, so the whole path stays in the box; then the speed
+    (``speed``), which must be >= 0 (a negative draw raises ``ValueError``).  One response is computed every
+    ``max(1024, round(waypoint_hop * sample_rate))`` samples at the source's position at that time (1024 is the
+    convolution's smallest hop, so below 20.48 kHz the default 0.05 s becomes 1024 samples), and the signal is
+    convolved with the path, crossfading between neighbouring waypoints.  With ``diffuse_after`` all waypoints of an item share its seed, so their tails are the same noise under
+    slightly different envelopes and a crossfade loses no tail power.  A smaller ``waypoint_hop`` reduces the comb
+    filtering a crossfade makes when the delay changes by more than a sample between waypoints."""
     _bypass_pays = False  # FFT convolution
 
     DEFAULT_ROOM = (("uniform", 3.0, 10.0), ("uniform", 3.0, 8.0), ("uniform", 2.4, 4.0))
@@ -582,8 +600,11 @@ class SyntheticRoomImpulseResponse(BaseTransform):
     def __init__(self, room: tuple = DEFAULT_ROOM, rt60: tuple = ("uniform", 0.2, 0.8), margin: float = 0.5,
                  mic_spacing: tuple = ("uniform", 0.05, 0.2), max_order: int = -1, duration: float = None,
                  high_pass: bool = True, name: str = None, prob: float = 1.0, use_original_phase: bool = False,
-                 diffuse_after=None, bands: int = None, band_rt60=None, air_absorption=None):
+                 diffuse_after=None, bands: int = None, band_rt60=None, air_absorption=None, source_speed=None,
+                 waypoint_hop: float = 0.05):
         super().__init__(name=name, prob=prob)
+        if source_speed is None:  # a static source: neither draw is made, so neither key is expected
+            self.keys = [k for k in self.keys if k not in ("end", "speed")]
         if diffuse_after is None:  # no tail: neither draw is made, so neither key is expected
             self.keys = [k for k in self.keys if k not in ("diffuse_after", "seed")]
         if bands is None:
@@ -616,6 +637,10 @@ class SyntheticRoomImpulseResponse(BaseTransform):
         self.duration = duration
         self.high_pass = high_pass
         self.use_original_phase = use_original_phase
+        self.source_speed = source_speed
+        self.waypoint_hop = float(waypoint_hop)
+        if not (np.isfinite(self.waypoint_hop) and self.waypoint_hop > 0):
+            raise ValueError(f"SyntheticRoomImpulseResponse: waypoint_hop = {waypoint_hop!r}; seconds > 0")
 
     def _instantiate(self, state: RandomState, signal: AudioSignal):
         from ..core import room as _room
@@ -646,10 +671,17 @@ class SyntheticRoomImpulseResponse(BaseTransform):
             floor = 1.01 * float(_room.min_rt60(dims))
             out["band_rt60"] = np.array([max(float(util.sample_from_dist(r, state)) * rt60, floor)
                                          for r in self.band_rt60])
+        if self.source_speed is not None:
+            out["end"] = state.uniform(lo, hi)
+            speed = float(util.sample_from_dist(self.source_speed, state))
+            if not (np.isfinite(speed) and speed >= 0):
+                raise ValueError(f"SyntheticRoomImpulseResponse: source_speed drew {speed} m/s; speeds must be "
+                                 "finite and >= 0")
+            out["speed"] = np.float64(speed)
         return out
 
-    def _transform(self, signal, room, rt60, source, mics, diffuse_after=None, seed=None, band_rt60=None,
-                   _bypass=None):
+    def _transform(self, signal, room, rt60, source, mics, diffuse_after=None, seed=None, band_rt60=None, end=None,
+                   speed=None, _bypass=None):
         from ..core.room import image_source_ir
 
         sr, T = signal.sample_rate, signal.signal_length
@@ -657,10 +689,51 @@ class SyntheticRoomImpulseResponse(BaseTransform):
         seconds = self.duration if self.duration is not None else float(util.host_view(walls).max())
         length = max(1, min(T, int(np.ceil(seconds * sr))))
         bands = {} if self.bands is None else dict(bands=self.bands, air_absorption=self.air_absorption)
-        ir = image_source_ir(room, source, mics, sr, length, rt60=walls, max_order=self.max_order,
-                             high_pass=self.high_pass, diffuse_after=diffuse_after, seed=seed, device=signal.device,
-                             **bands)
-        return signal.apply_ir(ir, use_original_phase=self.use_original_phase, _bypass=_bypass)
+        if end is None:
+            ir = image_source_ir(room, source, mics, sr, length, rt60=walls, max_order=self.max_order,
+                                 high_pass=self.high_pass, diffuse_after=diffuse_after, seed=seed,
+                                 device=signal.device, **bands)
+            return signal.apply_ir(ir, use_original_phase=self.use_original_phase, _bypass=_bypass)
+        from ..engine import Engine
+
+        hop = max(Engine.MOVING_IR_MIN_HOP, int(round(self.waypoint_hop * sr)))
+        K = (T - 1) // hop + 1
+        path = self.path(source, end, speed, K, hop / sr)  # [B, K, 3]
+        B, C = signal.batch_size, signal.num_channels
+
+        def per_waypoint(v, nd: int, dtype=np.float64):  # each item's value [..nd dims], repeated for its waypoints
+            if v is None:
+                return None
+            v = _host_values(v, dtype)
+            return np.repeat(np.broadcast_to(v, (B,) + v.shape[v.ndim - nd:]), K, axis=0)
+
+        from ..core.room import MAX_ROWS
+
+        room_k, mics_k = per_waypoint(room, 1), per_waypoint(mics, 2)
+        walls_k = per_waypoint(walls, 0 if band_rt60 is None else 1)
+        td_k, seed_k = per_waypoint(diffuse_after, 0), per_waypoint(seed, 0, np.int64)
+        step = max(1, MAX_ROWS // (C * (self.bands or 1)))  # items per call: items x microphones x bands <= MAX_ROWS
+        irs = []
+        for i in range(0, B * K, step):
+            s = slice(i, i + step)
+            irs.append(image_source_ir(room_k[s], path.reshape(-1, 3)[s], mics_k[s], sr, length, rt60=walls_k[s],
+                                       max_order=self.max_order, high_pass=self.high_pass,
+                                       diffuse_after=None if td_k is None else td_k[s],
+                                       seed=None if seed_k is None else seed_k[s], device=signal.device,
+                                       **bands).audio_data)
+        irs = torch.cat(irs).reshape(B, K, C, length)
+        return signal.apply_moving_ir(irs, hop, use_original_phase=self.use_original_phase, _bypass=_bypass)
+
+    @staticmethod
+    def path(source, end, speed, K: int, dt: float) -> np.ndarray:
+        """[B, K, 3] positions of sources moving from ``source`` [B, 3] toward ``end`` [B, 3] at ``speed`` [B] m/s,
+        stopping there, sampled every ``dt`` seconds from 0."""
+        source, end = _host_values(source).reshape(-1, 3), _host_values(end).reshape(-1, 3)
+        speed = _host_values(speed).reshape(-1, 1)
+        span = end - source
+        dist = np.linalg.norm(span, axis=-1, keepdims=True)
+        frac = speed * dt * np.arange(K)[None, :] / np.maximum(dist, 1e-300)  # [B, K]
+        return np.where(frac[..., None] >= 1.0, end[:, None], source[:, None] + frac[..., None] * span[:, None])
 
 
 class PitchShift(BaseTransform):

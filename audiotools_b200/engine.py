@@ -1415,6 +1415,45 @@ class Engine:
             bypass = self._bypass(bypass, n_ir, device)
         return ir, n_ir, L, rows_per_ir, bypass
 
+    MOVING_IR_MIN_HOP = 1024  # csrc/fftconv.cu's block: with a shorter hop a block would meet more than 3 waypoints
+
+    def circular_convolve_moving(self, x: torch.Tensor, irs: torch.Tensor, hop: int, roll_to_peak: bool = True,
+                                 bypass: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """:meth:`circular_convolve` along a path of K impulse responses (DESIGN.md K22): waypoint k sits at sample
+        k hop, and the output crossfades the K static convolutions linearly between neighbouring waypoints,
+        y = sum_k v_k(t) (h_k (*) x)(t), the last waypoint holding from its sample on.  Every waypoint of a row takes
+        the roll and scale of the row's first waypoint.  x: [B, C, T]; irs: [B, K, C or 1, L] (1: shared by the
+        channels), truncated to T; ``hop`` >= 1024 samples and K = (T - 1) // hop + 1.  ``bypass`` [B]: items left
+        untouched."""
+        x = self._prep(x, "x")
+        irs = self._prep(irs, "irs")
+        B, C, T = x.shape
+        if isinstance(hop, bool) or not isinstance(hop, (int, np.integer)):
+            raise ValueError(f"circular_convolve_moving: hop = {hop!r}; an int number of samples")
+        hop = int(hop)
+        if irs.ndim != 4 or irs.shape[0] != B or irs.shape[2] not in (1, C) or irs.shape[3] < 1:
+            raise ValueError(f"circular_convolve_moving: irs must be [{B}, K, {C} or 1, L] for x {tuple(x.shape)}, "
+                             f"got {tuple(irs.shape)}")
+        if hop < self.MOVING_IR_MIN_HOP:
+            raise ValueError(f"circular_convolve_moving: hop = {hop} samples; at least {self.MOVING_IR_MIN_HOP}")
+        K = irs.shape[1]
+        if K != (T - 1) // hop + 1:
+            raise ValueError(f"circular_convolve_moving: {K} waypoints every {hop} samples for T = {T}; the path "
+                             f"must cover the signal exactly, (T - 1) // hop + 1 = {(T - 1) // hop + 1} waypoints")
+        n_ch = irs.shape[2]
+        irs = irs[..., :T].contiguous()
+        L = irs.shape[-1]
+        rows_per_ir = 1 if n_ch == C else C
+        if bypass is not None:
+            bypass = torch.as_tensor(bypass).reshape(-1).to(x.device).repeat_interleave(n_ch)
+            bypass = self._bypass(bypass, B * n_ch, x.device)
+        ws_bytes = self.lib.b2a_circconv_path_workspace_bytes(B * C, T, K, L, rows_per_ir, n_ch, hop)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        out = torch.empty_like(x)
+        self._call(self.lib.b2a_circconv_path_f32, _dptr(x), B * C, T, _dptr(irs), K, L, rows_per_ir, n_ch, hop,
+                   int(bool(roll_to_peak)), _dptr(bypass), _dptr(out), _dptr(ws), ws_bytes, self._stream(x))
+        return out
+
     def circular_convolve_backward(self, grad_out: torch.Tensor, ir: torch.Tensor, roll_to_peak: bool = True,
                                    bypass: Optional[torch.Tensor] = None) -> torch.Tensor:
         """dL/dx of :meth:`circular_convolve` (the IR is a constant): circular correlation with the rolled, scaled IR,

@@ -508,6 +508,21 @@ size_t b2a_circconv_backward_workspace_bytes(int64_t rows, int64_t T, int64_t n_
 int b2a_circconv_backward_f32(const float* grad_out, int64_t rows, int64_t T, const float* ir, int64_t n_ir, int64_t L,
                               int rows_per_ir, int roll_to_peak, const int32_t* bypass, float* grad_x, void* ws,
                               size_t ws_bytes, void* stream);
+/* A moving impulse response: b2a_circconv_f32 along a path of K waypoints, waypoint k at sample tau_k = k hop.
+ *   out[row][t] = s sum_k v_k(t) sum_j h_{i,k}[j] x[row][(t - j + idx) mod T],   i = row / rows_per_ir,
+ * v_k(t) = max(0, 1 - |t - tau_k| / hop), except v_{K-1}(t) = 1 for t >= tau_{K-1}: the weights sum to 1.  idx and s
+ * are b2a_circconv_f32's roll and scale of waypoint 0's IR and serve the whole path, so a change in delay along it
+ * is kept.  ir: [items][K][ir_channels][L] with items = rows / (rows_per_ir ir_channels) and IR i = item ir_channels
+ * + c, so h_{i,k} = ir[item][k][c]; L <= T; hop >= 1024 (the engine's block: a block then meets at most 3
+ * waypoints); K = (T - 1) / hop + 1 exactly; K <= 65535 and K ir_channels L < 2^31.  bypass: nullable
+ * [rows / rows_per_ir], rows copied through.  No host sync, no atomics: rows are independent and reruns are
+ * bit-identical.  With K = 1 and L > 1024 the output is b2a_circconv_f32's bit for bit.  out must not alias x.
+ * ws: b2a_circconv_path_workspace_bytes() bytes. */
+size_t b2a_circconv_path_workspace_bytes(int64_t rows, int64_t T, int64_t K, int64_t L, int rows_per_ir,
+                                         int ir_channels, int hop);
+int b2a_circconv_path_f32(const float* x, int64_t rows, int64_t T, const float* ir, int64_t K, int64_t L,
+                          int rows_per_ir, int ir_channels, int hop, int roll_to_peak, const int32_t* bypass,
+                          float* out, void* ws, size_t ws_bytes, void* stream);
 
 /* ---- windowed-sinc polyphase resampling ------------------------------------------------------
  * AudioSignal.resample (audiotools/core/audio_signal.py:716-736 -> julius.resample_frac): old_r/new_r are
