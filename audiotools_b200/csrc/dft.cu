@@ -464,7 +464,9 @@ int b2a::dft::launch_fold(const float* frames, const float* window, int64_t rows
 extern "C" int b2a_mel_dct_f32(const float* logmel, int64_t rows, int n_mels, int64_t n_frames, const float* dct, int n_mfcc,
                                float* out, void* stream) {
   B2A_REQUIRE(logmel && dct && out, B2A_E_INVALID, "mel_dct: null pointer");
-  B2A_REQUIRE(rows >= 1 && rows <= 65535 && n_mels >= 1 && n_mfcc >= 1 && n_frames >= 1, B2A_E_INVALID, "mel_dct: bad shape");
+  // the kernel's frame index is an int that runs to the end of the last 128-frame tile
+  B2A_REQUIRE(rows >= 1 && rows <= 65535 && n_mels >= 1 && n_mfcc >= 1 && n_frames >= 1 && n_frames <= INT_MAX - 127,
+              B2A_E_INVALID, "mel_dct: bad shape");
   const size_t smem = (size_t)n_mels * n_mfcc * sizeof(float);
   B2A_REQUIRE(smem <= 200 * 1024, B2A_E_UNSUPPORTED, "mel_dct: %d x %d basis does not fit shared memory", n_mels, n_mfcc);
   B2A_CUDA_OK(cudaFuncSetAttribute(mel_dct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -42,27 +42,37 @@ __device__ __forceinline__ void map_row(const float* __restrict__ x, float* __re
        [&](int64_t i) { y[i] = f(x[i]); });
 }
 
-// peak must be zeroed by the caller (memset inside the entry point); |x| >= 0, so float bits order like ints
+// peak must be zeroed by the caller (memset inside the entry point).  |x| >= 0, so its float bits order like unsigned
+// ints, and every NaN pattern of |x| ranks above +inf's 0x7f800000: a NaN anywhere in the row is its peak, as in the
+// reference's x.abs().max(dim=-1) (fmaxf would drop it)
+__device__ __forceinline__ unsigned abs_bits(float v) { return __float_as_uint(v) & 0x7fffffffu; }
 __global__ void __launch_bounds__(TPB) absmax_kernel(const float* __restrict__ x, int64_t T, int vec_ok,
                                                      float* __restrict__ peak) {
   const int row = blockIdx.y;
   const float* xr = x + (size_t)row * (size_t)T;
-  float m = 0.f;
+  unsigned m = 0u;
   walk(T, vec_ok,
        [&](int64_t i) {
          const float4 v = ld_stream4(xr + i);
-         m = fmaxf(fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
+         m = max(max(m, max(abs_bits(v.x), abs_bits(v.y))), max(abs_bits(v.z), abs_bits(v.w)));
        },
-       [&](int64_t i) { m = fmaxf(m, fabsf(xr[i])); });
-  m = warp_max(m);
-  __shared__ float s[TPB / 32];
+       [&](int64_t i) { m = max(m, abs_bits(xr[i])); });
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+  __shared__ unsigned s[TPB / 32];
   if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = m;
   __syncthreads();
-  if (threadIdx.x < 32) {
-    m = threadIdx.x < TPB / 32 ? s[threadIdx.x] : 0.f;
-    m = warp_max(m);
-    if (threadIdx.x == 0) atomicMax(reinterpret_cast<int*>(peak + row), __float_as_int(m));
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < TPB / 32; ++w) m = max(m, s[w]);
+    atomicMax(reinterpret_cast<unsigned*>(peak + row), m);
   }
+}
+
+// x.clamp(lo, hi) as torch computes it with tensor bounds: a NaN sample or a NaN bound gives NaN (fminf / fmaxf alone
+// would return the other operand)
+__device__ __forceinline__ float clamp_nan(float v, float lo, float hi) {
+  const float r = fminf(fmaxf(v, lo), hi);
+  return (v != v || lo != lo || hi != hi) ? v + lo + hi : r;
 }
 
 // MODE 0: limit peak (scale = peak > lim ? lim / peak : 1)   MODE 1: clamp to [lo, hi] of the item
@@ -80,7 +90,7 @@ __global__ void __launch_bounds__(TPB) rows_kernel(const float* __restrict__ x, 
   } else {
     p0 = __ldg(a + row); p1 = __ldg(b + row);
   }
-  map_row(xr, yr, T, vec_ok, [&](float v) { return MODE == 0 ? v * p0 : fminf(fmaxf(v, p0), p1); });
+  map_row(xr, yr, T, vec_ok, [&](float v) { return MODE == 0 ? v * p0 : clamp_nan(v, p0, p1); });
 }
 
 __global__ void __launch_bounds__(TPB) gain_kernel(const float* __restrict__ x, float* __restrict__ out,
@@ -140,8 +150,11 @@ __global__ void __launch_bounds__(TPB) quantize_kernel(const float* __restrict__
   map_row(xr, yr, per_item, vec_ok, [&](float v) { return mulaw ? quant_mulaw(v, mu, l1p) : quant_linear(v, q); });
 }
 
-// ---- exact k-th smallest by 4-pass (8 bits each) radix selection: one CTA per requested order statistic
+// ---- exact k-th smallest by 4-pass (8 bits each) radix selection: one CTA per requested order statistic.  Every NaN,
+// of either sign, gets the largest key, so NaNs rank above +inf as in torch.sort, and a NaN statistic comes back as the
+// positive quiet NaN 0x7fffffff (ord_key alone would rank a NaN with the sign bit set below -inf).  -0 ranks before +0.
 constexpr int ST = 1024;
+__device__ __forceinline__ unsigned stat_key(float v) { return v != v ? 0xffffffffu : ord_key(v); }
 __global__ void __launch_bounds__(ST) order_stat_kernel(const float* __restrict__ row, int64_t T,
                                                         const int64_t* __restrict__ ks, float* __restrict__ out) {
   __shared__ unsigned hist[256];
@@ -157,7 +170,7 @@ __global__ void __launch_bounds__(ST) order_stat_kernel(const float* __restrict_
     for (int i = tid; i < 256; i += ST) hist[i] = 0;
     __syncthreads();
     for (int64_t i = tid; i < T; i += ST) {
-      const unsigned key = ord_key(__ldg(row + i));
+      const unsigned key = stat_key(__ldg(row + i));
       if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 0xff], 1u);
     }
     __syncthreads();
@@ -207,14 +220,21 @@ namespace effects {
 // ---------------------------------------------------------------------------------------------
 constexpr int DRR_T = 512;
 
+// torch.argmax's order: NaN above every number, then the larger value, then the smaller index
 struct ArgMax { float v; int i; };
-__device__ __forceinline__ ArgMax better(ArgMax a, ArgMax b) {  // larger value, then the smaller index
+__device__ __forceinline__ ArgMax better(ArgMax a, ArgMax b) {
+  const bool an = a.v != a.v, bn = b.v != b.v;
+  if (an || bn) return (bn && (!an || b.i < a.i)) ? b : a;
   return (b.v > a.v || (b.v == a.v && b.i < a.i)) ? b : a;
 }
+// T <= INT_MAX - DRR_T (checked by the entry point), so i += DRR_T cannot overflow
 __device__ ArgMax block_argmax(const float* __restrict__ x, int T, ArgMax* sm) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   ArgMax m{-INFINITY, 0x7fffffff};
-  for (int i = tid; i < T; i += DRR_T) { const float v = x[i]; if (v > m.v) { m.v = v; m.i = i; } }
+  for (int i = tid; i < T; i += DRR_T) {
+    const float v = x[i];
+    if (v > m.v || (v != v && m.v == m.v)) { m.v = v; m.i = i; }
+  }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     ArgMax t{__shfl_xor_sync(0xffffffffu, m.v, o), __shfl_xor_sync(0xffffffffu, m.i, o)};
@@ -372,8 +392,10 @@ extern "C" int b2a_order_stats_f32(const float* row, int64_t T, const int64_t* k
 extern "C" int b2a_alter_drr_f32(const float* ir, float* out, int64_t rows, int64_t T, int C, int t0, const float* drr,
                                  float max_abs, void* stream) {
   B2A_REQUIRE(ir && out && drr, B2A_E_INVALID, "alter_drr: null pointer");
-  B2A_REQUIRE(rows >= 1 && T >= 1 && T < ((int64_t)1 << 31) && C >= 1 && rows % C == 0 && t0 >= 0, B2A_E_INVALID,
-              "alter_drr: bad shape");
+  // the kernel's int sample index steps by DRR_T and reaches td + t0: both must stay below INT_MAX
+  B2A_REQUIRE(rows >= 1 && T >= 1 && T <= INT_MAX - DRR_T && C >= 1 && rows % C == 0 && t0 >= 0 &&
+                  (int64_t)t0 <= INT_MAX - T,
+              B2A_E_INVALID, "alter_drr: bad shape");
   B2A_REQUIRE(out != ir, B2A_E_INVALID, "alter_drr: out must not alias ir");
   B2A_LAUNCH(alter_drr_kernel, dim3((unsigned)rows), dim3(DRR_T), 0, stream, ir, out, (int)T, C, t0, drr, max_abs);
   B2A_CUDA_OK(cudaGetLastError());
@@ -393,30 +415,37 @@ extern "C" int b2a_alter_drr_f32(const float* ir, float* out, int64_t rows, int6
 namespace b2a {
 namespace effects {
 
-__device__ __forceinline__ void arg_better(float& v, int& i, float ov, int oi) {
+// The arg-max of |v| ranks the bits of |v| as unsigned ints, as absmax_kernel does: a NaN ranks above every number, as
+// in torch.max(dim).  Ties (equal bits) go to the smaller index.
+__device__ __forceinline__ void arg_better(unsigned& v, int& i, unsigned ov, int oi) {
   if (ov > v || (ov == v && oi < i)) { v = ov; i = oi; }
 }
 __device__ __forceinline__ float sgn(float v) { return v > 0.f ? 1.f : (v < 0.f ? -1.f : 0.f); }
+// clamp(v, 1e-8) as torch computes it: NaN stays NaN (fmaxf alone would return 1e-8)
+__device__ __forceinline__ float clamp_peak(float v) { return v != v ? v : fmaxf(v, 1e-8f); }
 
 __global__ void __launch_bounds__(TPB) peak_scale_bwd_kernel(const float* __restrict__ g, const float* __restrict__ y,
                                                              const float* __restrict__ xr_, int64_t T, float lim,
                                                              const int32_t* __restrict__ bypass, float* __restrict__ gy,
                                                              float* __restrict__ gxr) {
-  __shared__ float sv[TPB], sx[TPB], sd[TPB];
+  __shared__ unsigned sv[TPB], sx[TPB];
+  __shared__ float sd[TPB];
   __shared__ int si[TPB], sxi[TPB];
   const int row = blockIdx.x, tid = threadIdx.x;
   const float* gr = g + (size_t)row * T;
   const float* yr = y + (size_t)row * T;
   const float* xr = xr_ ? xr_ + (size_t)row * T : nullptr;
-  float bv = -1.f, bx = -1.f, d = 0.f;
-  int bi = 0, bxi = 0;
+  unsigned bv = 0u, bx = 0u;
+  float d = 0.f;
+  int bi = 0x7fffffff, bxi = 0x7fffffff;
   for (int64_t i = tid; i < T; i += TPB) {
     const float v = yr[i];
-    if (fabsf(v) > bv) { bv = fabsf(v); bi = (int)i; }
+    const unsigned av = abs_bits(v);
+    if (av > bv || bi == 0x7fffffff) { bv = av; bi = (int)i; }
     d = fmaf(gr[i], v, d);
     if (xr) {
-      const float a = fabsf(xr[i]);
-      if (a > bx) { bx = a; bxi = (int)i; }
+      const unsigned a = abs_bits(xr[i]);
+      if (a > bx || bxi == 0x7fffffff) { bx = a; bxi = (int)i; }
     }
   }
   sv[tid] = bv; si[tid] = bi; sx[tid] = bx; sxi[tid] = bxi; sd[tid] = d;
@@ -429,7 +458,9 @@ __global__ void __launch_bounds__(TPB) peak_scale_bwd_kernel(const float* __rest
     }
     __syncthreads();
   }
-  const float My = sv[0], dot = sd[0];
+  // A NaN peak: limit mode keeps the gain 1 (NaN > lim is false), as the reference's ensure_max_of_audio does; the
+  // restore's clamp keeps it, so S and the whole row's gradient are NaN, as in the reference
+  const float My = __uint_as_float(sv[0]), Mx = __uint_as_float(sx[0]), dot = sd[0];
   const int b = si[0];
   const bool byp = bypass && bypass[row];
   float S, cb = 0.f;
@@ -439,7 +470,7 @@ __global__ void __launch_bounds__(TPB) peak_scale_bwd_kernel(const float* __rest
   } else if (byp) {
     S = 1.0f;
   } else {
-    S = fmaxf(sx[0], 1e-8f) / fmaxf(My, 1e-8f);
+    S = clamp_peak(Mx) / clamp_peak(My);
     if (My >= 1e-8f) cb = -S * dot / My * sgn(yr[b]);
   }
   float* gyr = gy + (size_t)row * T;
@@ -451,7 +482,7 @@ __global__ void __launch_bounds__(TPB) peak_scale_bwd_kernel(const float* __rest
   __syncthreads();
   if (tid == 0) {
     gyr[b] = S * gr[b] + cb;
-    if (gxo && !byp && sx[0] >= 1e-8f) gxo[sxi[0]] = dot / fmaxf(My, 1e-8f) * sgn(xr[sxi[0]]);
+    if (gxo && !byp && Mx >= 1e-8f) gxo[sxi[0]] = dot / clamp_peak(My) * sgn(xr[sxi[0]]);
   }
 }
 

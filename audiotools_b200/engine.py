@@ -1013,16 +1013,21 @@ class Engine:
         return out
 
     def quantile(self, row: torch.Tensor, q: torch.Tensor) -> torch.Tensor:
-        """``torch.quantile(row, q)`` (linear interpolation; aten's float32 rank arithmetic and lerp) for a 1-D row."""
+        """``torch.quantile(row, q)`` (linear interpolation; aten's float32 rank arithmetic and lerp) for a 1-D row.
+        A row that holds a NaN gives NaN for every q, as in aten, which moves every rank to the last one: the largest
+        order statistic, computed in the same launch, is NaN exactly then."""
         n = row.numel()
         q = q.to(row.device).reshape(-1).float()
+        nq = q.numel()
         ranks = q * (n - 1)
         below = ranks.floor()
         w = ranks - below
-        ks = torch.cat([below, ranks.ceil()]).to(torch.int64)
+        ks = torch.cat([below.to(torch.int64), ranks.ceil().to(torch.int64),
+                        torch.full((1,), n - 1, dtype=torch.int64, device=ranks.device)])
         v = self.order_stats(row, ks)
-        a, b = v[: q.numel()], v[q.numel():]
-        return torch.where(w < 0.5, a + w * (b - a), b - (b - a) * (1 - w))
+        a, b, last = v[:nq], v[nq:2 * nq], v[2 * nq:]
+        out = torch.where(w < 0.5, a + w * (b - a), b - (b - a) * (1 - w))
+        return torch.where(last.isnan(), last, out)
 
     def clamp_items(self, x: torch.Tensor, lo: torch.Tensor, hi: torch.Tensor) -> torch.Tensor:
         """``x.clamp(lo[item], hi[item])`` (ref :459)."""
