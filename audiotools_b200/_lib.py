@@ -62,6 +62,9 @@ SIGNATURES = {
     "b2a_rir_bands_kept": (c_int, [c_int, c_double]),
     "b2a_rir_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int,
                             c_int64, c_double, c_double, c_int, c_void_p, c_void_p]),
+    "b2a_rir_directional_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_int64, c_int, c_int, c_int64, c_double, c_double, c_int, c_void_p,
+                                        c_void_p]),
     "b2a_rir_band_sum_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_double, c_double, c_int,
                                      c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "b2a_gain_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),

@@ -25,6 +25,15 @@ where K' counts the bands whose lower crossover is below sample_rate / 2.  The c
 half_0 = int(8 fs / e_0 / 2), and zero-phase, so a response can start up to half_0 samples before its first arrival
 (the window's Tw / 2 comes on top).  Equal bands without air give the ``bands=None`` response bit for bit.
 
+``mic_pattern`` / ``source_pattern`` with ``mic_orientation`` / ``source_orientation`` make the microphones and the
+sources directional (DESIGN.md K20 "Directivity"): a first-order pattern p in [0, 1] (a name of ``PATTERNS`` or a
+value) with an orientation v has the amplitude gain D(u) = p + (1 - p) u.v for a unit direction u, negative in a rear
+lobe and the same at every frequency.  Every image is scaled by the microphone's gain at the direction its sound
+arrives from and by the source's gain at the direction the source emitted it in (each wall reflection mirrors one
+axis), so swapping a source and a microphone together with their patterns gives the same response.  The diffuse tail
+follows the expected energy of those scaled arrivals.  An end whose p is 1 everywhere is omnidirectional whatever its
+orientation, and its response is the omnidirectional one bit for bit.
+
 The geometry is checked on host values (``util.host_view`` reads a table's host mirror, so no device sync is needed)
 and is a constant: a geometry tensor that requires a gradient raises ``NotImplementedError``.
 """
@@ -41,6 +50,10 @@ MAX_SAMPLE_RATE = 384000.0  # csrc/rir.cu's largest window table
 MIN_DISTANCE = 1e-3         # metres between the source and a microphone
 MAX_BANDS = 8               # octave bands centred on 125 2^k Hz, k < 8 (up to 16 kHz)
 MAX_ROWS = 65535            # items x microphones x bands of one call (csrc/rir.cu's grid)
+# first-order patterns D(u) = p + (1 - p) u.v by name: p = 1 / (1 + sqrt 3) = (sqrt 3 - 1) / 2 is the supercardioid
+# (the largest front-to-back energy ratio), 1/4 the hypercardioid (the largest directivity factor)
+PATTERNS = {"omni": 1.0, "subcardioid": 0.75, "cardioid": 0.5, "supercardioid": (math.sqrt(3.0) - 1.0) / 2.0,
+            "hypercardioid": 0.25, "figure8": 0.0}
 
 
 def _host(name: str, v) -> np.ndarray:
@@ -82,6 +95,44 @@ def sabine_beta(room, rt60, sound_speed: float = 343.0) -> np.ndarray:
     return np.repeat(np.sqrt(1.0 - alpha)[..., None], 6, axis=-1)
 
 
+def _directivity(end: str, pattern, orientation):
+    """(p, unit orientations) on the host for one end (``"mic"`` or ``"source"``); (None, None) when it is
+    omnidirectional: no pattern, or p = 1 everywhere without an orientation."""
+    if pattern is None:
+        if orientation is not None:
+            raise ValueError(f"image_source_ir: {end}_orientation without a {end}_pattern")
+        return None, None
+    if isinstance(pattern, str):
+        if pattern not in PATTERNS:
+            raise ValueError(f"image_source_ir: {end}_pattern = {pattern!r}; one of {', '.join(PATTERNS)} or a "
+                             "value in [0, 1]")
+        p = np.float64(PATTERNS[pattern])
+    else:
+        p = _host(f"{end}_pattern", pattern)
+        if not (p.size and np.all(np.isfinite(p)) and np.all(p >= 0) and np.all(p <= 1)):
+            raise ValueError(f"image_source_ir: {end}_pattern = {p}; p must be in [0, 1] (1: omni, 0: figure8)")
+    if orientation is None:
+        if np.any(p != 1):
+            raise ValueError(f"image_source_ir: a directional {end}_pattern needs a {end}_orientation")
+        return p, None
+    v = _host(f"{end}_orientation", orientation)
+    if v.ndim == 0 or v.shape[-1] != 3:
+        raise ValueError(f"image_source_ir: {end}_orientation has 3 coordinates, got shape {v.shape}")
+    big = np.abs(v).max(axis=-1, keepdims=True)
+    if not (np.all(np.isfinite(v)) and np.all(big > 0)):
+        raise ValueError(f"image_source_ir: every {end}_orientation must be finite and non-zero")
+    v = v / big  # scaled first, so that the norm neither overflows nor underflows
+    return p, v / np.sqrt((v * v).sum(axis=-1, keepdims=True))
+
+
+def _dir_table(p: np.ndarray, v, shape: tuple):
+    """[*shape, 4] (p, v) of one end, or None when p = 1 everywhere (omnidirectional: no table is passed)."""
+    if p is None or np.all(p == 1):
+        return None
+    v = np.zeros(shape + (3,)) if v is None else v
+    return np.concatenate([np.broadcast_to(p, shape)[..., None], np.broadcast_to(v, shape + (3,))], axis=-1)
+
+
 def _batch(name: str, v: np.ndarray, item_ndim: int, B: int) -> np.ndarray:
     if v.ndim == item_ndim:
         return np.broadcast_to(v, (B,) + v.shape)
@@ -92,7 +143,8 @@ def _batch(name: str, v: np.ndarray, item_ndim: int, B: int) -> np.ndarray:
 
 def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta=None, rt60=None,
                     max_order: int = -1, sound_speed: float = 343.0, high_pass: bool = True, diffuse_after=None,
-                    seed=None, bands=None, air_absorption=None, device="cuda"):
+                    seed=None, bands=None, air_absorption=None, mic_pattern=None, mic_orientation=None,
+                    source_pattern=None, source_orientation=None, device="cuda"):
     """Impulse responses [B, C, length] of shoebox rooms by the image-source method, as an ``AudioSignal`` at
     ``sample_rate``.
 
@@ -111,7 +163,13 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
     [K] or [B, K] (``sabine_beta`` per band) and ``air_absorption`` (dB/m, finite, >= 0) [K] or [B, K].  Bands whose
     lower crossover is at or above sample_rate / 2 are checked but not computed.  One launch (two with the tail), the
     crossovers' ``fftconv`` and one launch for their sum when more than one band is computed, then the high-pass.
-    ``bands=None`` is the frequency-flat room, computed as one band."""
+    ``bands=None`` is the frequency-flat room, computed as one band.
+
+    ``mic_pattern`` (a name of ``PATTERNS`` or p in [0, 1]: scalar, [C] or [B, C]) with ``mic_orientation`` ([3],
+    [C, 3] or [B, C, 3], normalised here) makes the microphones directional, and ``source_pattern`` (a name or p:
+    scalar or [B]) with ``source_orientation`` ([3] or [B, 3]) the sources (module docstring; DESIGN.md K20
+    "Directivity").  A pattern other than omni needs its orientation, and an orientation its pattern.  It works with
+    every option above and adds no launch."""
     from ..engine import get_engine
     from .audio_signal import AudioSignal
 
@@ -158,8 +216,14 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
     else:  # the item axis leads a [B, 6, K] beta, a [B, K] rt60 and a [B, K] air absorption
         n_wall = max(wall_h.shape[0] if wall_h.ndim == (3 if rt60 is None else 2) else 1,
                      air_h.shape[0] if air_h is not None and air_h.ndim == 2 else 1)
+    mic_p, mic_v = _directivity("mic", mic_pattern, mic_orientation)
+    src_p, src_v = _directivity("source", source_pattern, source_orientation)
+    n_dir = max(mic_p.shape[0] if mic_p is not None and mic_p.ndim == 2 else 1,
+                mic_v.shape[0] if mic_v is not None and mic_v.ndim == 3 else 1,
+                src_p.shape[0] if src_p is not None and src_p.ndim == 1 else 1,
+                src_v.shape[0] if src_v is not None and src_v.ndim == 2 else 1)
     B = max(room_h.shape[0] if room_h.ndim == 2 else 1, src_h.shape[0] if src_h.ndim == 2 else 1,
-            mics_h.shape[0] if mics_h.ndim == 3 else 1, n_wall, n_tail)
+            mics_h.shape[0] if mics_h.ndim == 3 else 1, n_wall, n_tail, n_dir)
     room_h = _batch("room", room_h, 1, B)
     src_h = _batch("source", src_h, 1, B)
     mics_h = _batch("mics", mics_h, 2, B)
@@ -207,6 +271,21 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
         raise ValueError("image_source_ir: every reflection coefficient beta must be in [0, 1]")
     if bands is None:
         beta_h = beta_h[..., None]  # a frequency-flat room is one band: [B, 6, 1]
+    C = mics_h.shape[1]
+    mic_dir = src_dir = None
+    if mic_p is not None:
+        mp = _batch("mic_pattern", np.broadcast_to(mic_p, (C,)) if mic_p.ndim == 0 else mic_p, 1, B)
+        mv = None if mic_v is None else _batch("mic_orientation", np.broadcast_to(mic_v, (C, 3)) if mic_v.ndim == 1
+                                               else mic_v, 2, B)
+        if mp.shape != (B, C) or (mv is not None and mv.shape != (B, C, 3)):
+            raise ValueError(f"image_source_ir: mic_pattern / mic_orientation must fit {C} microphones: scalar, [C] or "
+                             f"[B, C] / [3], [C, 3] or [B, C, 3], got {mic_p.shape} / "
+                             f"{None if mic_v is None else mic_v.shape}")
+        mic_dir = _dir_table(mp, mv, (B, C))
+    if src_p is not None:
+        sp = _batch("source_pattern", src_p, 0, B)
+        sv = None if src_v is None else _batch("source_orientation", src_v, 1, B)
+        src_dir = _dir_table(sp, sv, (B,))
     dev = torch.device(device)
 
     def upload(a, dtype=np.float64):
@@ -218,5 +297,5 @@ def image_source_ir(room, source, mics, sample_rate: float, length: int, *, beta
         tail = dict(diffuse_after=upload(_batch("diffuse_after", td_h, 0, B)),
                     seed=upload(_batch("seed", sd, 0, B), np.int64))
     ir = get_engine().image_source_ir(*tab, length, sample_rate, sound_speed, max_order, high_pass,
-                                      air=upload(air_h), **tail)
+                                      air=upload(air_h), mic_dir=upload(mic_dir), src_dir=upload(src_dir), **tail)
     return AudioSignal(ir, sample_rate)

@@ -42,6 +42,13 @@
 // once and keeps K' compensated sums per sample, and the rows it writes are r_k - r_{k+1} (k < K' - 1) and r_{K'-1};
 // tail_kernel adds each band's tail the same way.  The crossovers (Engine.fftconv) and band_sum_kernel then form
 // y = r_{K'-1} + sum_k LP_k * (r_k - r_{k+1}) (DESIGN.md K20 "Bands").
+//
+// Directivity (mic_dir [B, C, 4] and / or src_dir [B, 4] given): first-order patterns D(u) = p + (1 - p) u.v.  An image
+// with offset (X, Y, Z) and parities (q, j, k) is also scaled by D_m((X, Y, Z) / d) D_s(-((1-2q) X, (1-2j) Y,
+// (1-2k) Z) / d), in double while it is staged, before its gain is tested for 0; the tail's quadrature weights are
+// scaled by M(u) S(u), M = p_m^2 + (1 - p_m)^2 sum_a v_ma^2 u_a^2 (S likewise), the parts of D_m^2 and of D_s^2
+// averaged over the parity classes that survive an integrand even in every u_a (DESIGN.md K20 "Directivity").  The
+// directional path is a template flag, so the kernels without it are unchanged.
 #include "b2a_common.h"
 
 namespace b2a {
@@ -66,6 +73,8 @@ struct Geo {
   int K, KB;               // bands per item in beta / air (1: frequency-flat); bands computed (the first KB)
   double fs, c;
   float* out;              // [KB, B C, L]: rows k < KB - 1 hold r_k - r_{k+1}, row KB - 1 holds r_{KB-1}
+  const double* mic_dir;   // [B, C, 4] (p, v_x, v_y, v_z) per microphone; null: omnidirectional
+  const double* src_dir;   // [B, 4] the same per item's source; null: omnidirectional
 };
 
 struct __align__(16) Img {
@@ -88,14 +97,16 @@ __device__ __forceinline__ int64_t floor_div2(int64_t a) { return a >= 0 ? a / 2
 // The image sum of one tile for the first NB bands of a row.  The images are enumerated once; each staged image carries
 // the last band's gains in its Img record and the other bands' in bgs, and every band keeps its own compensated sums.
 // A band skips an image whose gain rounds to 0 in float, so band NB - 1 adds exactly the images ism_kernel adds for its
-// beta, in the same order and with the same arithmetic: with one band this is ism_kernel.
-template <int NB>
+// beta, in the same order and with the same arithmetic: with one band this is ism_kernel.  DIR scales every band's
+// gain by the patterns of the row's microphone and the item's source (a null table: p = 1).
+template <int NB, bool DIR>
 __device__ __forceinline__ void ism_tile(const Geo& g) {
   __shared__ float2 tab[TW_MAX + 1];
   __shared__ Img img[CAP];
   __shared__ float2 bgs[NB > 1 ? NB - 1 : 1][CAP];  // bands 0 .. NB - 2: (gs, g0) of the staged images
   __shared__ double wall[6][NB], att[NB];             // beta per wall and band; air absorption per sample of distance
   __shared__ int64_t wtot[WARPS];
+  __shared__ double pat[8];  // DIR: p_m, v_m, p_s, v_s (in shared memory: no registers held across the tile)
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int64_t row = blockIdx.y, b = row / g.C, rows = gridDim.y;
   const int t0 = blockIdx.x * TT, Tw = g.Tw, half = Tw / 2;
@@ -108,6 +119,10 @@ __device__ __forceinline__ void ism_tile(const Geo& g) {
   for (int i = tid; i < 6 * NB; i += NT) wall[i / NB][i % NB] = g.beta[(6 * b + i / NB) * g.K + i % NB];
   // 10^(-a d_m / 20) = exp(-att d), d in samples
   for (int i = tid; i < NB; i += NT) att[i] = g.air ? g.air[b * g.K + i] * (M_LN10 / 20.0) / ks : 0.0;
+  if (DIR && tid < 8) {
+    const double* t = tid < 4 ? g.mic_dir + 4 * row : g.src_dir + 4 * b;
+    pat[tid] = (tid < 4 ? g.mic_dir : g.src_dir) ? t[tid & 3] : (tid & 3) == 0;
+  }
   for (int i = tid; i <= Tw; i += NT) {
     double s, c;
     sincospi((double)(i - half) / Tw, &s, &c);
@@ -199,12 +214,20 @@ __device__ __forceinline__ void ism_tile(const Geo& g) {
         const double Z = Zc + 2.0 * mz * Lz;
         const double d = sqrt(X * X + Y * Y + Z * Z);
         const double fl = floor(d);
+        double dir = 1.0;
+        if (DIR) {  // D_m(u_m) D_s(w): u_m = (X, Y, Z) / d, w the direction the source emitted the ray in
+          const volatile double* pt = pat;  // read at the image, not held in registers across the loop
+          const double um = X * pt[1] + Y * pt[2] + Z * pt[3];                            // d u_m.v_m
+          const double us = -((q ? -X : X) * pt[5] + (j ? -Y : Y) * pt[6] + (k ? -Z : Z) * pt[7]);  // d w.v_s
+          dir = (pt[0] * d + (1.0 - pt[0]) * um) * (pt[4] * d + (1.0 - pt[4]) * us) / (d * d);
+        }
         double gd[NB];
         bool live = false;
 #pragma unroll
         for (int bd = 0; bd < NB; ++bd) {
           gd[bd] = pxy[bd] * ipow(wall[4][bd], mz - k) * ipow(wall[5][bd], mz) / d;
           if (g.air) gd[bd] *= exp(-att[bd] * d);
+          if (DIR) gd[bd] *= dir;
           live = live || (float)gd[bd] != 0.f;
         }
         Img im;
@@ -274,11 +297,14 @@ __device__ __forceinline__ void ism_tile(const Geo& g) {
   }
 }
 
-__global__ void __launch_bounds__(NT) ism_kernel(const Geo g) { ism_tile<1>(g); }
+__global__ void __launch_bounds__(NT) ism_kernel(const Geo g) { ism_tile<1, false>(g); }
+__global__ void __launch_bounds__(NT) ism_dir_kernel(const Geo g) { ism_tile<1, true>(g); }
 
 // one CTA per SM is enough to let ptxas keep every band's sums in registers (no spills up to NB = 8)
 template <int NB>
-__global__ void __launch_bounds__(NT, 1) ism_bands_kernel(const Geo g) { ism_tile<NB>(g); }
+__global__ void __launch_bounds__(NT, 1) ism_bands_kernel(const Geo g) { ism_tile<NB, false>(g); }
+template <int NB>
+__global__ void __launch_bounds__(NT, 1) ism_bands_dir_kernel(const Geo g) { ism_tile<NB, true>(g); }
 
 
 constexpr int QK = 32;                // tanh-sinh: 2 QK + 1 points per dimension, steps of 3 / QK
@@ -299,9 +325,14 @@ __device__ __forceinline__ int node_of(double n, double tau, double lr) { return
 // Adds the tail of every computed band to the rows ism_tile wrote: band k's envelope is E(n; beta_k) exp(-2 att_k n)
 // (the air's 10^(-a_k (c n / fs) / 10), added to ln E at the sample, exactly), its noise xi(seed, c, n) is shared by the
 // bands, so row KB - 1 gets v_{KB-1} and row k < KB - 1 gets v_k - v_{k+1}.  The bands are walked from the last one
-// down, each with the node evaluation of the flat tail; with one band this is the flat tail.
-__global__ void __launch_bounds__(NT) tail_kernel(const Geo g) {
+// down, each with the node evaluation of the flat tail; with one band this is the flat tail.  DIR weights the point
+// (z, phi) by M S = (ma[z] + mb[z] mc[phi]) (sa[z] + sb[z] sc[phi]): with u_x^2 = (1 - z^2) cos^2 phi,
+// u_y^2 = (1 - z^2) sin^2 phi, u_z^2 = z^2, ma = p^2 + (1 - p)^2 v_z^2 z^2, mb = (1 - p)^2 (1 - z^2),
+// mc = v_x^2 cos^2 phi + v_y^2 sin^2 phi (the microphone's pattern; sa, sb, sc the source's).
+template <bool DIR>
+__device__ __forceinline__ void tail_tile(const Geo& g) {
   __shared__ double qa[QM], qr[QM], qw[QM], pb[QM], pw[QM];  // z: lambda_z z, sqrt(1 - z^2), weight; azimuth
+  __shared__ double dw[DIR ? 6 : 1][QM];                     // DIR: ma, mb, mc, sa, sb, sc
   __shared__ double nn[NK], nf[NK], nd[NK];                  // node, ln of the direction mean, its derivative
   __shared__ double part[WARPS][2];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -315,6 +346,21 @@ __global__ void __launch_bounds__(NT) tail_kernel(const Geo g) {
   const double scale = g.c / (4.0 * M_PI * g.room[3 * b] * g.room[3 * b + 1] * g.room[3 * b + 2] * g.fs);
   const int first = max(t0, start);
   const double lr = log(GROW);
+  if (DIR) {  // the patterns' tables; the first band with a tail synchronises before reading them
+    for (int i = tid; i < 2 * QM; i += NT) {
+      const int e = i / QM, t = i - e * QM;  // end: 0 the microphone, 1 the source
+      const double* d = e ? g.src_dir : g.mic_dir;
+      const double* pv = d ? d + 4 * (e ? b : row) : nullptr;
+      const double p = pv ? pv[0] : 1.0, a = (1.0 - p) * (1.0 - p);
+      const double vx = pv ? pv[1] : 0.0, vy = pv ? pv[2] : 0.0, vz = pv ? pv[3] : 0.0;
+      const double h = 3.0 / QK, s = (t - QK) * h, x = 0.5 * (1.0 + tanh(0.5 * M_PI * sinh(s)));
+      double sn, co;
+      sincospi(0.5 * x, &sn, &co);
+      dw[3 * e][t] = p * p + a * vz * vz * x * x;
+      dw[3 * e + 1][t] = a * fmax(0.0, 1.0 - x * x);
+      dw[3 * e + 2][t] = vx * vx * co * co + vy * vy * sn * sn;
+    }
+  }
 
   // this thread's samples first + tid + NT s: the Box-Muller radius and cosine of each
   const uint64_t key = mix64(mix64(g.seed[b]) + (uint64_t)c);
@@ -364,7 +410,8 @@ __global__ void __launch_bounds__(NT) tail_kernel(const Geo g) {
         for (int q = tid; q < QN; q += NT) {
           const int i = q / QM, j = q - i * QM;
           const double sg = qa[i] + qr[i] * pb[j] - m;
-          const double e = qw[i] * pw[j] * exp(-n * sg);
+          double e = qw[i] * pw[j] * exp(-n * sg);
+          if (DIR) e *= (dw[0][i] + dw[1][i] * dw[2][j]) * (dw[3][i] + dw[4][i] * dw[5][j]);
           s0 += e, s1 += e * sg;
         }
 #pragma unroll
@@ -415,6 +462,9 @@ __global__ void __launch_bounds__(NT) tail_kernel(const Geo g) {
   }
 }
 
+__global__ void __launch_bounds__(NT) tail_kernel(const Geo g) { tail_tile<false>(g); }
+__global__ void __launch_bounds__(NT) tail_dir_kernel(const Geo g) { tail_tile<true>(g); }
+
 // y = r_last + conv_0 + conv_1 + ... (the crossovers' outputs, added in band order), one row per blockIdx.y.  The
 // crossovers run on the FFT engine, whose rounding spreads over whole blocks, so the samples before the first one any
 // band can reach are written as the exact zeros they are: every image is at least as far as the direct path d, so
@@ -449,6 +499,7 @@ static Geo geo(const double* room, const double* src, const double* mics, const 
                double fs, double c, int max_order, float* out) {
   Geo g;
   g.room = room, g.src = src, g.mics = mics, g.beta = beta, g.td = nullptr, g.seed = nullptr, g.air = nullptr;
+  g.mic_dir = nullptr, g.src_dir = nullptr;
   g.C = C, g.L = (int)L, g.K = 1, g.KB = 1, g.max_order = max_order, g.Tw = 2 * (int)floor(0.004 * fs + 0.5), g.fs = fs, g.c = c, g.out = out;
   return g;
 }
@@ -461,8 +512,11 @@ static int bands_kept(int K, double fs) {
 }
 
 template <int NB>
-static void launch_bands(const dim3& grid, const Geo& g, void* stream) {
-  B2A_LAUNCH(ism_bands_kernel<NB>, grid, dim3(NT), 0, stream, g);
+static void launch_bands(const dim3& grid, const Geo& g, bool dir, void* stream) {
+  if (dir)
+    B2A_LAUNCH(ism_bands_dir_kernel<NB>, grid, dim3(NT), 0, stream, g);
+  else
+    B2A_LAUNCH(ism_bands_kernel<NB>, grid, dim3(NT), 0, stream, g);
 }
 
 extern "C" int b2a_rir_bands_kept(int K, double fs) {
@@ -470,9 +524,10 @@ extern "C" int b2a_rir_bands_kept(int K, double fs) {
   return bands_kept(K, fs);
 }
 
-extern "C" int b2a_rir_f32(const double* room, const double* src, const double* mics, const double* beta,
-                           const double* air, const double* t_d, const uint64_t* seed, int64_t B, int C, int K,
-                           int64_t L, double fs, double c, int max_order, float* out, void* stream) {
+extern "C" int b2a_rir_directional_f32(const double* room, const double* src, const double* mics, const double* beta,
+                                       const double* air, const double* t_d, const uint64_t* seed,
+                                       const double* mic_dir, const double* src_dir, int64_t B, int C, int K, int64_t L,
+                                       double fs, double c, int max_order, float* out, void* stream) {
   B2A_REQUIRE(room && src && mics && beta && out, B2A_E_INVALID, "rir: null pointer");
   B2A_REQUIRE(B >= 1 && C >= 1 && L >= 1, B2A_E_INVALID, "rir: bad shape B=%lld C=%d L=%lld", (long long)B, C,
               (long long)L);
@@ -487,23 +542,40 @@ extern "C" int b2a_rir_f32(const double* room, const double* src, const double* 
   B2A_REQUIRE(!t_d || max_order == -1, B2A_E_INVALID, "rir: max_order=%d with a diffuse tail", max_order);
   Geo g = geo(room, src, mics, beta, C, L, fs, c, max_order, out);
   g.air = air, g.td = t_d, g.seed = seed, g.K = K, g.KB = bands_kept(K, fs);
+  g.mic_dir = mic_dir, g.src_dir = src_dir;
+  const bool dir = mic_dir || src_dir;
   const dim3 grid((unsigned)((L + TT - 1) / TT), (unsigned)(B * C));
   switch (g.KB) {
-    case 1: B2A_LAUNCH(ism_kernel, grid, dim3(NT), 0, stream, g); break;
-    case 2: launch_bands<2>(grid, g, stream); break;
-    case 3: launch_bands<3>(grid, g, stream); break;
-    case 4: launch_bands<4>(grid, g, stream); break;
-    case 5: launch_bands<5>(grid, g, stream); break;
-    case 6: launch_bands<6>(grid, g, stream); break;
-    case 7: launch_bands<7>(grid, g, stream); break;
-    default: launch_bands<8>(grid, g, stream); break;
+    case 1:
+      if (dir)
+        B2A_LAUNCH(ism_dir_kernel, grid, dim3(NT), 0, stream, g);
+      else
+        B2A_LAUNCH(ism_kernel, grid, dim3(NT), 0, stream, g);
+      break;
+    case 2: launch_bands<2>(grid, g, dir, stream); break;
+    case 3: launch_bands<3>(grid, g, dir, stream); break;
+    case 4: launch_bands<4>(grid, g, dir, stream); break;
+    case 5: launch_bands<5>(grid, g, dir, stream); break;
+    case 6: launch_bands<6>(grid, g, dir, stream); break;
+    case 7: launch_bands<7>(grid, g, dir, stream); break;
+    default: launch_bands<8>(grid, g, dir, stream); break;
   }
   B2A_CUDA_OK(cudaGetLastError());
   if (t_d) {
-    B2A_LAUNCH(tail_kernel, grid, dim3(NT), 0, stream, g);
+    if (dir)
+      B2A_LAUNCH(tail_dir_kernel, grid, dim3(NT), 0, stream, g);
+    else
+      B2A_LAUNCH(tail_kernel, grid, dim3(NT), 0, stream, g);
     B2A_CUDA_OK(cudaGetLastError());
   }
   return B2A_OK;
+}
+
+extern "C" int b2a_rir_f32(const double* room, const double* src, const double* mics, const double* beta,
+                           const double* air, const double* t_d, const uint64_t* seed, int64_t B, int C, int K,
+                           int64_t L, double fs, double c, int max_order, float* out, void* stream) {
+  return b2a_rir_directional_f32(room, src, mics, beta, air, t_d, seed, nullptr, nullptr, B, C, K, L, fs, c, max_order,
+                                 out, stream);
 }
 
 extern "C" int b2a_rir_band_sum_f32(const double* src, const double* mics, const double* t_d, int64_t B, int C,

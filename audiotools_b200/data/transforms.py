@@ -592,7 +592,15 @@ class SyntheticRoomImpulseResponse(BaseTransform):
     convolution's smallest hop, so below 20.48 kHz the default 0.05 s becomes 1024 samples), and the signal is
     convolved with the path, crossfading between neighbouring waypoints.  With ``diffuse_after`` all waypoints of an item share its seed, so their tails are the same noise under
     slightly different envelopes and a crossfade loses no tail power.  A smaller ``waypoint_hop`` reduces the comb
-    filtering a crossfade makes when the delay changes by more than a sample between waypoints."""
+    filtering a crossfade makes when the delay changes by more than a sample between waypoints.
+
+    ``mic_pattern`` and ``source_pattern`` (a name of ``core.room.PATTERNS`` or p in [0, 1]) make the microphones and
+    the sources directional (``image_source_ir(..., mic_pattern=, source_pattern=)``, DESIGN.md K20 "Directivity").
+    Only then more draws follow all the ones above: with ``mic_pattern`` the azimuth of the microphones
+    (``mic_azimuth``, radians, default ``uniform(0, 2 pi)``), all of them pointing horizontally that way
+    (``mic_orientation``); then with ``source_pattern`` the source's yaw (``source_yaw``, radians, default
+    ``uniform(-pi/2, pi/2)``), the source pointing horizontally toward the array's centre turned by the yaw
+    (``source_orientation``).  A moving source keeps its orientation along its path."""
     _bypass_pays = False  # FFT convolution
 
     DEFAULT_ROOM = (("uniform", 3.0, 10.0), ("uniform", 3.0, 8.0), ("uniform", 2.4, 4.0))
@@ -601,8 +609,23 @@ class SyntheticRoomImpulseResponse(BaseTransform):
                  mic_spacing: tuple = ("uniform", 0.05, 0.2), max_order: int = -1, duration: float = None,
                  high_pass: bool = True, name: str = None, prob: float = 1.0, use_original_phase: bool = False,
                  diffuse_after=None, bands: int = None, band_rt60=None, air_absorption=None, source_speed=None,
-                 waypoint_hop: float = 0.05):
+                 waypoint_hop: float = 0.05, mic_pattern=None, source_pattern=None,
+                 mic_azimuth: tuple = ("uniform", 0.0, 2.0 * np.pi),
+                 source_yaw: tuple = ("uniform", -0.5 * np.pi, 0.5 * np.pi)):
         super().__init__(name=name, prob=prob)
+        from ..core.room import PATTERNS
+
+        for end, pat in (("mic", mic_pattern), ("source", source_pattern)):
+            if pat is None:  # omnidirectional: no draw is made, so no key is expected
+                self.keys = [k for k in self.keys if k != f"{end}_orientation"]
+            elif isinstance(pat, str) and pat not in PATTERNS:
+                raise ValueError(f"SyntheticRoomImpulseResponse: {end}_pattern = {pat!r}; one of "
+                                 f"{', '.join(PATTERNS)} or a value in [0, 1]")
+            elif not isinstance(pat, str) and not (np.ndim(pat) == 0 and 0.0 <= float(pat) <= 1.0):
+                raise ValueError(f"SyntheticRoomImpulseResponse: {end}_pattern = {pat!r}; a name or one value in "
+                                 "[0, 1], shared by every item")
+        self.mic_pattern, self.source_pattern = mic_pattern, source_pattern
+        self.mic_azimuth, self.source_yaw = mic_azimuth, source_yaw
         if source_speed is None:  # a static source: neither draw is made, so neither key is expected
             self.keys = [k for k in self.keys if k not in ("end", "speed")]
         if diffuse_after is None:  # no tail: neither draw is made, so neither key is expected
@@ -678,10 +701,18 @@ class SyntheticRoomImpulseResponse(BaseTransform):
                 raise ValueError(f"SyntheticRoomImpulseResponse: source_speed drew {speed} m/s; speeds must be "
                                  "finite and >= 0")
             out["speed"] = np.float64(speed)
+        if self.mic_pattern is not None:
+            az = float(util.sample_from_dist(self.mic_azimuth, state))
+            out["mic_orientation"] = np.array([np.cos(az), np.sin(az), 0.0])
+        if self.source_pattern is not None:
+            yaw = float(util.sample_from_dist(self.source_yaw, state))
+            to = mics.mean(axis=0) - source
+            ang = np.arctan2(to[1], to[0]) + yaw
+            out["source_orientation"] = np.array([np.cos(ang), np.sin(ang), 0.0])
         return out
 
     def _transform(self, signal, room, rt60, source, mics, diffuse_after=None, seed=None, band_rt60=None, end=None,
-                   speed=None, _bypass=None):
+                   speed=None, mic_orientation=None, source_orientation=None, _bypass=None):
         from ..core.room import image_source_ir
 
         sr, T = signal.sample_rate, signal.signal_length
@@ -689,17 +720,22 @@ class SyntheticRoomImpulseResponse(BaseTransform):
         seconds = self.duration if self.duration is not None else float(util.host_view(walls).max())
         length = max(1, min(T, int(np.ceil(seconds * sr))))
         bands = {} if self.bands is None else dict(bands=self.bands, air_absorption=self.air_absorption)
+        B, C = signal.batch_size, signal.num_channels
+        if mic_orientation is not None:  # one azimuth per item, shared by its microphones: [B, C, 3]
+            mic_orientation = np.broadcast_to(_host_values(mic_orientation).reshape(-1, 1, 3), (B, C, 3))
+        if source_orientation is not None:
+            source_orientation = _host_values(source_orientation).reshape(-1, 3)
         if end is None:
             ir = image_source_ir(room, source, mics, sr, length, rt60=walls, max_order=self.max_order,
                                  high_pass=self.high_pass, diffuse_after=diffuse_after, seed=seed,
-                                 device=signal.device, **bands)
+                                 device=signal.device, mic_pattern=self.mic_pattern, mic_orientation=mic_orientation,
+                                 source_pattern=self.source_pattern, source_orientation=source_orientation, **bands)
             return signal.apply_ir(ir, use_original_phase=self.use_original_phase, _bypass=_bypass)
         from ..engine import Engine
 
         hop = max(Engine.MOVING_IR_MIN_HOP, int(round(self.waypoint_hop * sr)))
         K = (T - 1) // hop + 1
         path = self.path(source, end, speed, K, hop / sr)  # [B, K, 3]
-        B, C = signal.batch_size, signal.num_channels
 
         def per_waypoint(v, nd: int, dtype=np.float64):  # each item's value [..nd dims], repeated for its waypoints
             if v is None:
@@ -712,6 +748,7 @@ class SyntheticRoomImpulseResponse(BaseTransform):
         room_k, mics_k = per_waypoint(room, 1), per_waypoint(mics, 2)
         walls_k = per_waypoint(walls, 0 if band_rt60 is None else 1)
         td_k, seed_k = per_waypoint(diffuse_after, 0), per_waypoint(seed, 0, np.int64)
+        mo_k, so_k = per_waypoint(mic_orientation, 2), per_waypoint(source_orientation, 1)
         step = max(1, MAX_ROWS // (C * (self.bands or 1)))  # items per call: items x microphones x bands <= MAX_ROWS
         irs = []
         for i in range(0, B * K, step):
@@ -720,7 +757,10 @@ class SyntheticRoomImpulseResponse(BaseTransform):
                                        max_order=self.max_order, high_pass=self.high_pass,
                                        diffuse_after=None if td_k is None else td_k[s],
                                        seed=None if seed_k is None else seed_k[s], device=signal.device,
-                                       **bands).audio_data)
+                                       mic_pattern=self.mic_pattern,
+                                       mic_orientation=None if mo_k is None else mo_k[s],
+                                       source_pattern=self.source_pattern,
+                                       source_orientation=None if so_k is None else so_k[s], **bands).audio_data)
         irs = torch.cat(irs).reshape(B, K, C, length)
         return signal.apply_moving_ir(irs, hop, use_original_phase=self.use_original_phase, _bypass=_bypass)
 

@@ -841,8 +841,9 @@ class Engine:
                         length: int, sample_rate: float, sound_speed: float = 343.0, max_order: int = -1,
                         high_pass: bool = True, air: Optional[torch.Tensor] = None,
                         diffuse_after: Optional[torch.Tensor] = None,
-                        seed: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Shoebox-room impulse responses by the image-source method (``b2a_rir_f32``, DESIGN.md K20) -> [B, C, length]
+                        seed: Optional[torch.Tensor] = None, mic_dir: Optional[torch.Tensor] = None,
+                        src_dir: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Shoebox-room impulse responses by the image-source method (``b2a_rir_directional_f32``, DESIGN.md K20) -> [B, C, length]
         float32.  room [B, 3], src [B, 3], mics [B, C, 3] (metres), beta [B, 6, K] per wall and octave band (K = 1: a
         frequency-flat room) and ``air`` [B, K] dB/m or None are float64 tensors on the device, already checked
         (``core.room.image_source_ir``).  ``high_pass`` applies Allen & Berkley's 100 Hz high-pass as one second-order
@@ -852,7 +853,11 @@ class Engine:
         ceil(diffuse_after sample_rate) only and adds a diffuse tail after them; ``max_order`` must be -1 then.  One
         launch, two with the tail.
 
-        ``b2a_rir_f32`` writes the K' kept bands' differences r_k - r_{k+1} and the last band r_{K'-1}; when K' > 1 the
+        ``mic_dir`` (float64 [B, C, 4]) and ``src_dir`` (float64 [B, 4]) give the microphones and the sources
+        first-order patterns (p, v_x, v_y, v_z), p in [0, 1] and v a unit vector, already checked; None is
+        omnidirectional (DESIGN.md K20 "Directivity").  They add no launch and no host sync.
+
+        ``b2a_rir_directional_f32`` writes the K' kept bands' differences r_k - r_{k+1} and the last band r_{K'-1}; when K' > 1 the
         differences go through the zero-phase crossovers LP_k (``fftconv``, zero padding) and ``b2a_rir_band_sum_f32``
         adds them to the last band: y = r_{K'-1} + sum_k LP_k * (r_k - r_{k+1}), exactly 0 before the first sample the
         direct path (or the tail) reaches through the crossovers."""
@@ -877,16 +882,22 @@ class Engine:
                                  "order")
             if tuple(diffuse_after.shape) != (B,) or tuple(seed.shape) != (B,):
                 raise ValueError(f"image_source_ir: diffuse_after and seed must be [{B}]")
+        if mic_dir is not None and tuple(mic_dir.shape) != (B, C, 4):
+            raise ValueError(f"image_source_ir: mic_dir must be [{B}, {C}, 4], got {tuple(mic_dir.shape)}")
+        if src_dir is not None and tuple(src_dir.shape) != (B, 4):
+            raise ValueError(f"image_source_ir: src_dir must be [{B}, 4], got {tuple(src_dir.shape)}")
         room, src, mics, beta = (self._prep(t, n, torch.float64) for t, n in
                                  ((room, "room"), (src, "source"), (mics, "mics"), (beta, "beta")))
         air = None if air is None else self._prep(air, "air", torch.float64)
         td = None if diffuse_after is None else self._prep(diffuse_after, "diffuse_after", torch.float64)
         sd = None if seed is None else self._prep(seed, "seed", torch.int64)
+        md = None if mic_dir is None else self._prep(mic_dir, "mic_dir", torch.float64)
+        sdir = None if src_dir is None else self._prep(src_dir, "src_dir", torch.float64)
         L = int(length)
         bands = torch.empty(kept, B, C, L, dtype=torch.float32, device=room.device)
-        self._call(self.lib.b2a_rir_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), _dptr(air), _dptr(td),
-                   _dptr(sd), B, C, K, L, float(sample_rate), float(sound_speed), int(max_order), _dptr(bands),
-                   self._stream(room))
+        self._call(self.lib.b2a_rir_directional_f32, _dptr(room), _dptr(src), _dptr(mics), _dptr(beta), _dptr(air),
+                   _dptr(td), _dptr(sd), _dptr(md), _dptr(sdir), B, C, K, L, float(sample_rate), float(sound_speed),
+                   int(max_order), _dptr(bands), self._stream(room))
         if kept == 1:
             out = bands[0]
         else:

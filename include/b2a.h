@@ -438,6 +438,20 @@ int b2a_rir_bands_kept(int K, double fs);
 int b2a_rir_f32(const double* room, const double* src, const double* mics, const double* beta, const double* air,
                 const double* t_d, const uint64_t* seed, int64_t B, int C, int K, int64_t L, double fs, double c,
                 int max_order, float* out, void* stream);
+/* b2a_rir_f32 with first-order directivity (DESIGN.md K20, "Directivity"); with both tables null it is
+ * b2a_rir_f32, bit for bit and through the same kernels.  mic_dir [B, C, 4] and src_dir [B, 4] (float64 on the device,
+ * each null for an omnidirectional end) hold (p, v_x, v_y, v_z): the pattern p in [0, 1] and a unit orientation v.  Its
+ * amplitude gain for a unit direction u is D(u) = p + (1 - p) u.v (p = 1: omni, 1/2: cardioid, 0: figure-eight; it
+ * may be negative).  An image with offset (X, Y, Z) = image - microphone and parities (q, j, k) (odd numbers of
+ * reflections on the x, y, z walls) is scaled by D_m((X, Y, Z) / d) D_s(-((1-2q) X, (1-2j) Y, (1-2k) Z) / d), the
+ * microphone's pattern at the direction the sound arrives from and the source's at the direction it left in, the same
+ * in every band; the tail's envelope becomes the expected energy of those scaled arrivals.  The tables are not read on
+ * the host, so their sizes and the p and unit-vector conditions are the caller's (core/room.py checks them).  The
+ * same launches as b2a_rir_f32. */
+int b2a_rir_directional_f32(const double* room, const double* src, const double* mics, const double* beta,
+                            const double* air, const double* t_d, const uint64_t* seed, const double* mic_dir,
+                            const double* src_dir, int64_t B, int C, int K, int64_t L, double fs, double c,
+                            int max_order, float* out, void* stream);
 
 /* y[b, c] = bands[n_conv, b, c] + sum_{k < n_conv} conv[k, b, c] (added in k order): the crossover outputs of the
  * octave-band differences added to the last band (bands [n_conv + 1, B, C, L] from b2a_rir_f32, conv [n_conv, B,
